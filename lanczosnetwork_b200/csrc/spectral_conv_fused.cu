@@ -327,10 +327,12 @@ struct SpectralPolicy {
   const int tid, r;
   const int N, K, S, E1, H, XP;           // hot parameters in registers
   int Din;                                // input width of the current layer
+  // Shared memory, in this order.  Tables comes first so that everything behind Xs is one
+  // contiguous region that is dead after the last layer's epilogue (the fused readout's scratch).
+  Tables* tb;
   float* Xs;                // X rows [RMAX][XP]; reused for V Z + the finished output rows
   float* UZ;                // U rows (graph,k) [RMAX][XP] during step 0, Z afterwards
   float* Qs;                // [RMAX][K]
-  Tables* tb;
   float* Ev;                // [LB][RMAX] staged ELL values
   uint8_t* Ei;              // [LB][RMAX] staged ELL columns as tile-local row indices
   float fr[FR];             // this (graph, k) row's filter coefficients f[k, 0..S)
@@ -341,12 +343,11 @@ struct SpectralPolicy {
   __device__ SpectralPolicy(const Params& p_, uint8_t* smem, int tid_)
       : p(p_), tid(tid_), r(tid_ & 127), N(p_.N), K(p_.K), S(p_.S), E1(p_.E1),
         H(p_.H), XP((p_.Din[0] > p_.H ? p_.Din[0] : p_.H) + 4), Din(p_.Din[0]) {
-    Xs = reinterpret_cast<float*>(smem);
+    tb = reinterpret_cast<Tables*>(smem);
+    Xs = reinterpret_cast<float*>(smem + tables_bytes());
     UZ = Xs + (size_t)RMAX * XP;
     Qs = UZ + (size_t)RMAX * XP;
-    uint8_t* t8 = reinterpret_cast<uint8_t*>(Qs + (size_t)RMAX * K);
-    tb = reinterpret_cast<Tables*>(t8);
-    Ev = reinterpret_cast<float*>(t8 + tables_bytes());
+    Ev = Qs + (size_t)RMAX * K;
     Ei = reinterpret_cast<uint8_t*>(Ev + (size_t)p.LB * RMAX);
   }
   static size_t smem_fixed(int Din, int K, int H) {
@@ -354,6 +355,16 @@ struct SpectralPolicy {
     return (size_t)2 * RMAX * W * 4 + (size_t)RMAX * K * 4 + tables_bytes() + 16;
   }
   static size_t ell_line_bytes() { return (size_t)RMAX * 5; }
+  // UZ, Qs, Ev and Ei: free once the last layer's output rows are in Xs
+  static size_t dead_bytes(int Din, int K, int H, int lb) {
+    const int W = (Din > H ? Din : H) + 4;
+    return (size_t)RMAX * (W + K) * 4 + (size_t)lb * ell_line_bytes();
+  }
+  // scratch of readout(), laid out from UZ: Wr, Yr, cx and the node masks of up to GMAX graphs
+  static size_t readout_bytes(int H, int P, int N) {
+    const size_t P1 = (size_t)P + 1, PQ = (P1 + 3) / 4, yr = (RMAX + 1) * P1;
+    return (4 * PQ * (H + 4) + yr + ((4 - (yr & 3)) & 3) + H) * 4 + (size_t)GMAX * N;
+  }
 
   // ------------------------------------------------------------------------------------------
   __device__ void build_tables(int m_tile) {
@@ -656,15 +667,18 @@ struct SpectralPolicy {
     tcg::producers_sync();
   }
 
+  // Rows of UZ and Xs are XP = max(Din0, H) + 4 floats long, which a 16-column chunk can overrun
+  // when H % 16 != 0: only the float4 pieces below column H are written (H % 4 == 0, so a piece
+  // is either wholly inside the row or wholly outside it).
   __device__ __forceinline__ void store(int sub, int col, float (&x)[tcg::EW]) {
     if (col >= H) return;
     if ((sub & 1) == 0) {
-      // drain Z[row, col:col+32] to shared memory (overwrites U, which is dead by now)
+      // drain Z[row, col:col+16] to shared memory (overwrites U, which is dead by now)
       if (r < tb->Ztot) {
         float4* z4 = reinterpret_cast<float4*>(UZ + (size_t)r * XP + col);
 #pragma unroll
         for (int q = 0; q < tcg::EW / 4; ++q)
-          z4[q] = make_float4(x[4 * q + 0], x[4 * q + 1], x[4 * q + 2], x[4 * q + 3]);
+          if (col + 4 * q < H) z4[q] = make_float4(x[4 * q + 0], x[4 * q + 1], x[4 * q + 2], x[4 * q + 3]);
       }
       return;
     }
@@ -674,27 +688,17 @@ struct SpectralPolicy {
     const float* bias = p.bias ? p.bias + (sub >> 1) * H : nullptr;
 #pragma unroll
     for (int q = 0; q < tcg::EW / 4; ++q) {
+      if (col + 4 * q >= H) break;
       float y[4] = {x[4 * q + 0], x[4 * q + 1], x[4 * q + 2], x[4 * q + 3]};
       if (S > 0) {                                  // + (V Z)[row, col + 4q ..], from pre_epilogue()
         const float4 t = o4[q];
         y[0] += t.x; y[1] += t.y; y[2] += t.z; y[3] += t.w;
       }
-      if (col + 4 * q + 3 < H) {
-        if (bias) {
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + col) + q);
-          y[0] += b4.x; y[1] += b4.y; y[2] += b4.z; y[3] += b4.w;
-        }
-        if (relu) { y[0] = fmaxf(y[0], 0.f); y[1] = fmaxf(y[1], 0.f); y[2] = fmaxf(y[2], 0.f); y[3] = fmaxf(y[3], 0.f); }
-      } else {
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int c = col + 4 * q + u;
-          if (c < H) {
-            if (bias) y[u] += __ldg(bias + c);
-            if (relu) y[u] = fmaxf(y[u], 0.f);
-          }
-        }
+      if (bias) {
+        const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + col) + q);
+        y[0] += b4.x; y[1] += b4.y; y[2] += b4.z; y[3] += b4.w;
       }
+      if (relu) { y[0] = fmaxf(y[0], 0.f); y[1] = fmaxf(y[1], 0.f); y[2] = fmaxf(y[2], 0.f); y[3] = fmaxf(y[3], 0.f); }
       o4[q] = make_float4(y[0], y[1], y[2], y[3]);   // finished row chunk = next layer's X row
     }
   }
@@ -919,6 +923,13 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
   }
   int lb = (int)((227 * 1024 - smem) / SpectralPolicy::ell_line_bytes());
   if (lb > 255) lb = 255;
+  // The readout scratch (at most 56 KiB: P = 48, H = 128, N = 128) fits the dead region (at least
+  // 93 KiB: Din or H = 128, K = 32) at every shape accepted above; the check keeps it that way.
+  if (d.score && SpectralPolicy::readout_bytes(d.H, d.P, d.N) > SpectralPolicy::dead_bytes(dmax, d.K, d.H, lb)) {
+    lnb::set_err("%s: fused readout (P=%d, H=%d, N=%d) does not fit the free shared memory", who, d.P,
+                 d.H, d.N);
+    return LNB_ERR_UNSUPPORTED;
+  }
   smem += (size_t)lb * SpectralPolicy::ell_line_bytes();
   CUtensorMap map_hi, map_lo;
   int rc = tcg::make_weight_map(&map_hi, d.W_hi, d.num_layers * d.H, d.Kw, who);
