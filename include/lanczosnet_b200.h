@@ -114,7 +114,15 @@ int lnb_linear_tf32x3_grouped(lnb_stream_t stream, const float* A, const float* 
  *   gext [B,2] = {n_eff, k_eff}: operators / Q are identically zero beyond these extents;
  *   tiles [4B+2]: tiles[0] = T, tiles[1+t] = first graph of packed tile t (next-fit:
  *                sum n_eff <= 128, sum ceil4(k_eff) <= 128, <= 32 graphs), tiles[1+T] = B;
- *                entries [B+2, 4B+2) are scratch of the assignment kernel;
+ *                for B >= 2 the tile SCHEDULE the fused kernels run follows at S = tiles + B + 2
+ *                (at most 2B + 2 ints; the rest of [B+2, 4B+2) is scratch): S[0] = T',
+ *                S[1+t] = first slot of tile t, S[1+T'] = B, S[T'+2+slot] = graph id.  Rule:
+ *                first-fit decreasing -- graphs by n_eff descending, k_eff descending, index
+ *                ascending, each into the lowest tile where sum n_eff <= 128, sum k_eff <= 128
+ *                (unpadded) and <= 32 graphs still hold (data.host_tile_schedule).  Shapes the
+ *                fused kernels do not run (K > 32, n_eff > 128) and batches of more than 7113
+ *                graphs (beyond the assignment kernel's shared memory) get the next-fit tiles in
+ *                graph order instead; with B <= 1 the fused kernels run the table;
  *   rowmap [B*K], nrows [1] (both optional, NULL to skip): the compact Ritz row list of
  *                lnb_ritz_rowmap, produced by the same pass;
  *   flags bit 0: store 1.0 for every non-zero (the `L[L != 0] = 1.0` of model/gcnfp.py:83).
@@ -163,16 +171,16 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
  *   hdr[0] = 0x4c4e4231 ("LNB1"), hdr[1] = B, hdr[2] = K, hdr[3] = off(sizes [B] i32),
  *   hdr[4] = off(node_ptr [B+1] i32), hdr[5] = off(edge_ptr [B+1] i32), hdr[6] = off(D [B,K] f32),
  *   hdr[7] = off(node_feat [sum n] i32), hdr[8] = off(V_rows [sum n, K] f32),
- *   hdr[9] = off(edges [sum E][4] u8), hdr[10] = total bytes, hdr[11] = off(tiles [B+2] i32),
+ *   hdr[9] = off(edges [sum E][4] u8), hdr[10] = total bytes,
+ *   hdr[11] = off(tiles [3B+4] i32: the next-fit table [B+2], then the tile schedule [2B+2]),
  *   hdr[12] = off(krow_ptr [B+1] i32) (both 0 when absent); hdr[3..6], hdr[11], hdr[12] depend on (B, K)
- *   only, so D and the tile table sit at fixed addresses of a reused buffer (lnb_ritz_power_table and
+ *   only, so D and the tiles sit at fixed addresses of a reused buffer (lnb_ritz_power_table and
  *   lnb_spectral_stack_forward read them there).
  * The kernel derives its input pointers from the header on the device.  flags bit 1
- * (LNB_PACKED_HOST_TILES): the host knows every graph's extents, so it ships the packed-tile table
- * (same next-fit rule as lnb_graph_prepare: consecutive graphs, sum n <= 128, sum ceil4(k_eff) <= 128,
- * <= 32 graphs) and the prefix sums krow_ptr of k_eff; the kernel expands the Ritz row list itself and
- * NO tile-assignment launch follows (the `tiles` argument is then unused: pass the blob's segment to
- * the stack kernel). */
+ * (LNB_PACKED_HOST_TILES): the host knows every graph's extents, so it ships the tiles (the same
+ * next-fit table and first-fit-decreasing schedule as lnb_graph_prepare, in the same layout) and the
+ * prefix sums krow_ptr of k_eff; the kernel expands the Ritz row list itself and NO tile-assignment
+ * launch follows (the `tiles` argument is then unused: pass the blob's segment to the stack kernel). */
 #define LNB_PACKED_HOST_TILES 2
 int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, const double* inv_sqrt_deg,
                                     int B, int N, int E1, int K, int flags, float* ell_val,

@@ -5,10 +5,11 @@
 //
 // Tiles are PACKED: lnb_graph_prepare measures every graph's real extent (n_eff rows/columns
 // of the operators that are not identically zero, k_eff non-zero Ritz vectors) and assigns
-// consecutive graphs to 128-row tiles by next-fit (sum n_eff <= 128, sum ceil4(k_eff) <= 128,
-// <= 32 graphs).  A QM8-shaped batch of 1024 molecules (16 real atoms on average, padded to 26)
-// becomes ~137 tiles -- about one wave of the 132 SMs -- instead of 256 fixed-slot tiles.  Rows that
-// are pure padding are never multiplied; their (constant) output act(b) is written directly.
+// graphs to 128-row tiles by first-fit decreasing (sum n_eff <= 128, sum k_eff <= 128, <= 32
+// graphs; the tile schedule, below the next-fit table of the C ABI).  A QM8-shaped batch of 1024
+// molecules (16 real atoms on average, padded to 26) becomes 128-129 tiles -- one wave of the 132
+// SMs -- instead of 256 fixed-slot tiles (next-fit over consecutive graphs: 142-143, two waves).
+// Rows that are pure padding are never multiplied; their (constant) output act(b) is written directly.
 // Dropping exact zeros is exact, so the result equals the dense reference for arbitrary inputs.
 //
 // Two accumulator lifetimes ("steps") per tile:
@@ -120,6 +121,48 @@ graph_prepare_kernel(const float* __restrict__ L, const float* __restrict__ Q, i
   if (tid < 2) gext[b * 2 + tid] = s_ext[tid];
 }
 
+// (n_eff, k_eff) classes of the schedule's counting sort: n_eff <= RMAX, k_eff <= KMAX
+constexpr int SCH_KC = KMAX + 1;
+constexpr int SCH_NCLS = (RMAX + 1) * SCH_KC;
+
+// Exclusive prefix sum over the 1024 threads of a block; `total` = sum of all values.
+__device__ __forceinline__ int block_scan_excl(int v, int* ws /* [33] shared */, int& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  if (lane == 31) ws[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    const int w = ws[lane];
+    int s = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += t;
+    }
+    ws[lane] = s - w;
+    if (lane == 31) ws[32] = s;
+  }
+  __syncthreads();
+  const int r = ws[warp] + inc - v;
+  total = ws[32];
+  __syncthreads();
+  return r;
+}
+
+// Schedule = the next-fit tiles in graph order (always valid: next-fit keeps sum ceil4(k_eff) <= 128,
+// so also sum k_eff <= 128).  Reads the finished table; every thread of the block calls it.
+__device__ void identity_schedule(int32_t* __restrict__ tiles, int B, int T) {
+  int32_t* S = tiles + B + 2;
+  for (int i = threadIdx.x; i <= T; i += blockDim.x) S[1 + i] = tiles[1 + i];
+  for (int i = threadIdx.x; i < B; i += blockDim.x) S[T + 2 + i] = i;
+  if (threadIdx.x == 0) S[0] = T;
+}
+
 // Next-fit assignment of consecutive graphs to tiles.  tiles[0] = T, tiles[1 + t] = first graph
 // of tile t, tiles[1 + T] = B.  One CTA, all of it parallel: inclusive prefix sums of the row /
 // Ritz-row counts; for every graph i the end NX[i] of the tile that would start at i (a window of
@@ -127,6 +170,16 @@ graph_prepare_kernel(const float* __restrict__ L, const float* __restrict__ Q, i
 // jumping (round k marks the starts 2^k .. 2^(k+1)-1 hops away and squares the jump table); a
 // prefix sum over the marks numbers the tiles.  The arrays live in shared memory (6 (B+1) ints);
 // batches too large for that use the global scratch and a serial walk.
+//
+// Then, for B >= 2, the schedule the stack kernel runs, at S = tiles + B + 2:
+//   S[0] = T', S[1 + t] = first slot of tile t (t <= T', S[1 + T'] = B), S[T' + 2 + slot] = graph id.
+// Rule (data.host_tile_schedule): first-fit decreasing -- graphs by n_eff descending, k_eff
+// descending, index ascending; each goes into the lowest tile with sum n_eff <= 128, sum k_eff <= 128
+// (unpadded) and <= 32 graphs, or opens a new one.  Identical graphs are placed in bulk, which gives
+// exactly what first-fit gives one at a time: a stable counting sort by class (warps 1..31) runs
+// beside warp 0, which walks the classes in order and gives every tile, lowest first, as many graphs
+// of the class as still fit.  Batches outside the shared-memory path, with K > KMAX or with an
+// n_eff > 128 (shapes the stack kernel does not run) get the next-fit tiles in graph order instead.
 template <bool in_smem>
 __global__ void __launch_bounds__(1024)
 tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __restrict__ tiles,
@@ -135,6 +188,7 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
   extern __shared__ int32_t ta_smem[];
   __shared__ int warp_n[32], warp_k[32], warp_r[32];
   __shared__ int run_n, run_k, run_r;
+  __shared__ int scan_ws[33];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int32_t* PN = in_smem ? ta_smem : scratch;                     // inclusive prefix of n_eff
   int32_t* PK = PN + B;                                          // inclusive prefix of ceil4(k_eff)
@@ -206,7 +260,10 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
       while (i < B) { tiles[1 + T] = i; ++T; i = NX[i]; }
       tiles[0] = T;
       tiles[1 + T] = B;
+      run_n = T;
     }
+    __syncthreads();                                 // the scratch (under the schedule) is dead
+    if (B >= 2) identity_schedule(tiles, B, run_n);
     return;
   }
   int32_t* Ja = NX;
@@ -256,6 +313,176 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
     tiles[0] = run_n;
     tiles[1 + run_n] = B;
   }
+  __syncthreads();                                   // table done; the shared arrays above are dead
+  if (B < 2) return;                                 // no room for a schedule: the kernel runs the table
+  if (K > KMAX) {
+    identity_schedule(tiles, B, run_n);
+    return;
+  }
+  int32_t* S = tiles + B + 2;
+  int32_t* key = ta_smem;                            // [B] class of graph b
+  int32_t* order = key + B;                          // [B] graph ids sorted by class, stable
+  int32_t* tst = order + B;                          // [B] tile state: sum n | sum k << 8 | graphs << 16
+  int32_t* rec_t = tst + B;                          // [B] placement records: tile,
+  int32_t* rec_src = rec_t + B;                      //     first position in `order`,
+  int32_t* rec_sm = rec_src + B;                     //     first slot in the tile | count << 8
+  int32_t* hist = ta_smem + 6 * (B + 1);             // [SCH_NCLS] first position of each class in `order`
+  int32_t* cls = hist + SCH_NCLS;                    // [SCH_NCLS] the non-empty classes, in order
+  for (int i = tid; i < SCH_NCLS; i += 1024) hist[i] = 0;
+  __syncthreads();
+  // class = (128 - n_eff) * 33 + (32 - k_eff): ascending class = n_eff descending, then k_eff descending
+  bool big = false;
+  for (int b = tid; b < B; b += 1024) {
+    const int n = gext[b * 2];
+    big |= n > RMAX;
+    const int c = (RMAX - min(n, RMAX)) * SCH_KC + (KMAX - min(gext[b * 2 + 1], K));
+    key[b] = c;
+    atomicAdd(&hist[c], 1);
+  }
+  if (__syncthreads_or(big)) {
+    identity_schedule(tiles, B, run_n);
+    return;
+  }
+  {
+    constexpr int PER = (SCH_NCLS + 1023) / 1024;
+    int cnt[PER], s = 0, ne = 0;
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+      const int i = tid * PER + j;
+      cnt[j] = i < SCH_NCLS ? hist[i] : 0;
+      s += cnt[j];
+      ne += cnt[j] > 0;
+    }
+    int tot;                                         // graphs (low 16 bits) and classes (high bits) at once
+    const int ex = block_scan_excl(s | (ne << 16), scan_ws, tot);
+    int pos = ex & 0xffff, ci = ex >> 16;
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+      const int i = tid * PER + j;
+      if (i < SCH_NCLS) {
+        hist[i] = pos;
+        if (cnt[j]) cls[ci++] = i;
+        pos += cnt[j];
+      }
+    }
+    if (tid == 0) run_k = tot >> 16;
+  }
+  __syncthreads();
+  const int ncls = run_k;
+  if (warp == 0) {
+    // first-fit of whole classes.  Lane l owns the tiles [l P, l P + P) (P = ceil(T' / 32)): the free
+    // room of its tiles, one warp scan, then each lane fills its own tiles in order.  Placement
+    // records are independent of each other, so they take their index from a shared counter.
+    int T2 = 0;
+    if (lane == 0) run_r = 0;
+    __syncwarp();
+    for (int i0 = 0; i0 < ncls; i0 += 32) {
+      // lane j describes class i0 + j: first position in `order`, count, n_eff, k_eff, and
+      // ceil(2^16 / n), ceil(2^16 / k) for floor(free / n) = free * ceil(2^16 / n) >> 16 (exact for
+      // free, n <= 128), the most graphs an empty tile takes
+      int c_first = 0, c_count = 0, c_n = 1, c_k = 1;
+      if (i0 + lane < ncls) {
+        const int c = cls[i0 + lane];
+        c_first = hist[c];
+        c_count = (i0 + lane + 1 < ncls ? hist[cls[i0 + lane + 1]] : B) - c_first;
+        c_n = RMAX - c / SCH_KC;
+        c_k = KMAX - c % SCH_KC;
+      }
+      const int c_rn = c_n ? (65536 + c_n - 1) / c_n : 0, c_rk = c_k ? (65536 + c_k - 1) / c_k : 0;
+      const int c_ce = max(1, min(GMAX, min(c_n ? RMAX / c_n : GMAX, c_k ? RMAX / c_k : GMAX)));
+      const int nc = min(32, ncls - i0);
+      for (int j = 0; j < nc; ++j) {
+        const int first = __shfl_sync(0xffffffffu, c_first, j), count = __shfl_sync(0xffffffffu, c_count, j);
+        const int n = __shfl_sync(0xffffffffu, c_n, j), k = __shfl_sync(0xffffffffu, c_k, j);
+        const int rn = __shfl_sync(0xffffffffu, c_rn, j), rk = __shfl_sync(0xffffffffu, c_rk, j);
+        const int ce = __shfl_sync(0xffffffffu, c_ce, j);
+        int done = 0;
+        if (T2 > 0) {
+          const int P = (T2 + 31) >> 5, t0 = lane * P, t1 = min(t0 + P, T2);
+          int room = 0;
+          for (int t = t0; t < t1; ++t) {
+            const int st = tst[t];
+            int cap = GMAX - (st >> 16);
+            if (n) cap = min(cap, ((RMAX - (st & 255)) * rn) >> 16);
+            if (k) cap = min(cap, ((RMAX - ((st >> 8) & 255)) * rk) >> 16);
+            room += cap;
+          }
+          int inc = room;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += v;
+          }
+          int left = count - (inc - room);             // graphs still unplaced when this lane's tiles come
+          int src = first + inc - room;
+          for (int t = t0; t < t1 && left > 0 && room > 0; ++t) {
+            const int st = tst[t];
+            int cap = GMAX - (st >> 16);
+            if (n) cap = min(cap, ((RMAX - (st & 255)) * rn) >> 16);
+            if (k) cap = min(cap, ((RMAX - ((st >> 8) & 255)) * rk) >> 16);
+            const int m = min(cap, left);
+            if (m > 0) {
+              const int r = atomicAdd(&run_r, 1);
+              rec_t[r] = t;
+              rec_src[r] = src;
+              rec_sm[r] = (st >> 16) | (m << 8);
+              tst[t] = st + m * n + ((m * k) << 8) + (m << 16);
+              left -= m;
+              src += m;
+            }
+          }
+          done = min(count, __shfl_sync(0xffffffffu, inc, 31));
+        }
+        if (done < count) {                            // the rest opens new tiles, each as full as the limits allow
+          const int rem = count - done, nt = (rem + ce - 1) / ce;
+          const int r0 = lane == 0 ? atomicAdd(&run_r, nt) : 0;
+          const int rb = __shfl_sync(0xffffffffu, r0, 0);
+          for (int q = lane; q < nt; q += 32) {
+            const int m = min(ce, rem - q * ce);
+            rec_t[rb + q] = T2 + q;
+            rec_src[rb + q] = first + done + q * ce;
+            rec_sm[rb + q] = m << 8;
+            tst[T2 + q] = m * n + ((m * k) << 8) + (m << 16);
+          }
+          T2 += nt;
+        }
+        __syncwarp();
+      }
+    }
+    if (lane == 0) run_n = T2;
+  } else {
+    // stable counting sort: warp w gathers the graphs of classes w - 1, w + 30, ... in index order
+    for (int i = warp - 1; i < ncls; i += 31) {
+      const int c = cls[i];
+      int dst = hist[c];
+      const int end = i + 1 < ncls ? hist[cls[i + 1]] : B;
+      for (int b0 = 0; b0 < B && dst < end; b0 += 32) {
+        const int b = b0 + lane;
+        const bool hit = b < B && key[b] == c;
+        const unsigned mk = __ballot_sync(0xffffffffu, hit);
+        if (hit) order[dst + __popc(mk & ((1u << lane) - 1))] = b;
+        dst += __popc(mk);
+      }
+    }
+  }
+  __syncthreads();
+  const int T2 = run_n, nrec = run_r;
+  // first slot of every tile: exclusive prefix of the graph counts
+  int run = 0;
+  for (int t0 = 0; t0 < T2; t0 += 1024) {
+    const int t = t0 + tid;
+    const int c = t < T2 ? tst[t] >> 16 : 0;
+    int tot;
+    const int ex = block_scan_excl(c, scan_ws, tot);
+    if (t < T2) { S[1 + t] = run + ex; tst[t] = run + ex; }
+    run += tot;
+  }
+  if (tid == 0) { S[0] = T2; S[1 + T2] = B; }
+  __syncthreads();
+  for (int r = warp; r < nrec; r += 32) {
+    const int sm = rec_sm[r];
+    if (lane < (sm >> 8)) S[T2 + 2 + tst[rec_t[r]] + (sm & 255) + lane] = order[rec_src[r] + lane];
+  }
 }
 
 // --------------------------------------------------------------------------------------------
@@ -274,8 +501,8 @@ struct SpectralPolicy {
     const uint8_t* ell_idx; // [B, E1, N, N]
     const int32_t* ell_max; // [B, E1]
     const int32_t* gext;    // [B, 2]
-    const int32_t* tiles;   // [B + 2]
-    const float* bias;      // layer l: bias + l * H (may be null)
+    const int32_t* tiles;   // next-fit table [B + 2], then (B >= 2) the schedule the kernel runs
+    const float* bias;     // layer l: bias + l * H (may be null)
     float* out;             // [B, N, H] final state (may be null when the readout is fused)
     // fused readout (model/lanczos_net.py:185-194); score == nullptr disables it
     const float* W_out;     // [P, H]
@@ -292,9 +519,14 @@ struct SpectralPolicy {
     int write_pad;          // also write the constant rows of padded nodes of `out`
     int dbg;                // debug experiment flags (LNB_DBG), 0 in production
   };
+  // tile schedule (tile_assign_kernel): [T', first slot of tile 0 .. T', graph ids]; with B <= 1 there is
+  // no room for it and the next-fit table [T, first graph of tile 0 .. T] is run in graph order
+  static __device__ __forceinline__ const int32_t* schedule(const Params& p) {
+    return p.B >= 2 ? p.tiles + p.B + 2 : p.tiles;
+  }
   // sub = layer * 2 + step  (step 0: Z accumulation, step 1: edge accumulation + epilogue)
   static __device__ __forceinline__ int num_steps(const Params& p, int cta, int ncta) {
-    const int T = __ldg(p.tiles);
+    const int T = __ldg(schedule(p));
     const int mine = T > cta ? (T - cta + ncta - 1) / ncta : 0;
     return (p.S > 0 ? 2 : 1) * p.L * mine;
   }
@@ -313,13 +545,17 @@ struct SpectralPolicy {
     row0 = (sub >> 1) * p.H;
   }
 
+  // Row tables of the tile being run.  Node rows: graph after graph, n_eff rows each; Ritz rows
+  // (Z, U): graph after graph, k_eff rows each (unpadded); quads: groups of 4 rows of one graph.
   struct Tables {
-    int gs, ng, Rtot, Ztot, nquads, nlines;
+    int ng, Rtot, Ztot, nquads, nzquads, nlines;
+    int gid[GMAX];                                  // graph ids of the tile's graphs
     int nbase[GMAX + 1], kbase[GMAX + 1], gn[GMAX], gk[GMAX];
     int cnt_e[EMAX], base_e[EMAX], tmax_e[EMAX];
     uint8_t emax[GMAX][EMAX];
     uint8_t row_g[RMAX], row_n[RMAX], z_g[RMAX], z_k[RMAX];
-    uint8_t q_g[RMAX / 4 + GMAX], q_n0[RMAX / 4 + GMAX];
+    uint8_t q_g[RMAX / 4 + GMAX], q_n0[RMAX / 4 + GMAX];     // node-row quads
+    uint8_t zq_g[RMAX / 4 + GMAX], zq_k0[RMAX / 4 + GMAX];   // Ritz-row quads
     uint8_t line_e[256], line_t[256];
   };
 
@@ -370,36 +606,40 @@ struct SpectralPolicy {
   __device__ void build_tables(int m_tile) {
     // executed by warp 0: lane j <-> j-th graph of the tile
     const int lane = tid & 31;
-    const int gs = __ldg(p.tiles + 1 + m_tile), ge = __ldg(p.tiles + 2 + m_tile);
-    const int ng = ge - gs;
-    int n = 0, k = 0;
+    const int32_t* sc = schedule(p);
+    const int s0 = __ldg(sc + 1 + m_tile), s1 = __ldg(sc + 2 + m_tile);
+    const int ng = s1 - s0;
+    int g = s0 + lane, n = 0, k = 0;
     if (lane < ng) {
-      n = __ldg(p.gext + (gs + lane) * 2);
-      k = __ldg(p.gext + (gs + lane) * 2 + 1);
+      if (p.B >= 2) g = __ldg(sc + __ldg(sc) + 2 + s0 + lane);
+      n = __ldg(p.gext + g * 2);
+      k = __ldg(p.gext + g * 2 + 1);
     }
-    const int kp = (k + 3) & ~3, nq = (n + 3) >> 2;
-    int pn = n, pk = kp, pq = nq;                     // inclusive prefix sums
+    const int nq = (n + 3) >> 2, kq = (k + 3) >> 2;
+    int pn = n, pk = k, pq = nq, pz = kq;              // inclusive prefix sums
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
       const int a = __shfl_up_sync(0xffffffffu, pn, o), bq = __shfl_up_sync(0xffffffffu, pk, o);
-      const int c = __shfl_up_sync(0xffffffffu, pq, o);
-      if (lane >= o) { pn += a; pk += bq; pq += c; }
+      const int c = __shfl_up_sync(0xffffffffu, pq, o), d = __shfl_up_sync(0xffffffffu, pz, o);
+      if (lane >= o) { pn += a; pk += bq; pq += c; pz += d; }
     }
-    const int nb = pn - n, kb = pk - kp, qb = pq - nq;
+    const int nb = pn - n, kb = pk - k, qb = pq - nq, zb = pz - kq;
     if (lane < ng) {
+      tb->gid[lane] = g;
       tb->nbase[lane] = nb; tb->kbase[lane] = kb; tb->gn[lane] = n; tb->gk[lane] = k;
       for (int i = 0; i < n; ++i) { tb->row_g[nb + i] = (uint8_t)lane; tb->row_n[nb + i] = (uint8_t)i; }
-      for (int i = 0; i < kp; ++i) { tb->z_g[kb + i] = (uint8_t)lane; tb->z_k[kb + i] = (uint8_t)i; }
+      for (int i = 0; i < k; ++i) { tb->z_g[kb + i] = (uint8_t)lane; tb->z_k[kb + i] = (uint8_t)i; }
       for (int i = 0; i < nq; ++i) { tb->q_g[qb + i] = (uint8_t)lane; tb->q_n0[qb + i] = (uint8_t)(4 * i); }
+      for (int i = 0; i < kq; ++i) { tb->zq_g[zb + i] = (uint8_t)lane; tb->zq_k0[zb + i] = (uint8_t)(4 * i); }
     }
     const int Rtot = __shfl_sync(0xffffffffu, pn, 31), Ztot = __shfl_sync(0xffffffffu, pk, 31);
-    const int nquads = __shfl_sync(0xffffffffu, pq, 31);
+    const int nquads = __shfl_sync(0xffffffffu, pq, 31), nzquads = __shfl_sync(0xffffffffu, pz, 31);
     // per-channel maximum row length over the tile's graphs, per-graph row lengths
     // (all loads issued before the first reduction: one global round trip instead of E1)
     int em[EMAX];
 #pragma unroll
     for (int e = 0; e < EMAX; ++e)
-      em[e] = (e < E1 && lane < ng) ? __ldg(p.ell_max + (gs + lane) * E1 + e) : 0;
+      em[e] = (e < E1 && lane < ng) ? __ldg(p.ell_max + g * E1 + e) : 0;
 #pragma unroll
     for (int e = 0; e < EMAX; ++e) {
       if (e < E1) {
@@ -412,7 +652,7 @@ struct SpectralPolicy {
     }
     __syncwarp();
     if (lane == 0) {
-      tb->gs = gs; tb->ng = ng; tb->Rtot = Rtot; tb->Ztot = Ztot; tb->nquads = nquads;
+      tb->ng = ng; tb->Rtot = Rtot; tb->Ztot = Ztot; tb->nquads = nquads; tb->nzquads = nzquads;
       tb->nbase[ng] = Rtot; tb->kbase[ng] = Ztot;
       int left = p.LB, base = 0;
       for (int e = 0; e < E1; ++e) {            // staged lines per channel, in channel order
@@ -438,15 +678,15 @@ struct SpectralPolicy {
     if (warp == 0) build_tables(m_tile);
     tcg::producers_sync();
     tm.lap(16);
-    const int gs = tb->gs, Rtot = tb->Rtot;
+    const int Rtot = tb->Rtot;
     // ---- phase A: asynchronous copies of the real rows of X and Q (one warp per row) --------
     int64_t my_id = 0;                           // lane j: embedding id of this warp's j-th row
     if (!p.X && warp + lane * NW < Rtot) {
       const int row = warp + lane * NW;
-      my_id = __ldg(p.node_ids + (int64_t)(gs + tb->row_g[row]) * N + tb->row_n[row]);
+      my_id = __ldg(p.node_ids + (int64_t)tb->gid[tb->row_g[row]] * N + tb->row_n[row]);
     }
     for (int row = warp, j = 0; row < Rtot; row += NW, ++j) {
-      const int64_t src_row = (int64_t)(gs + tb->row_g[row]) * N + tb->row_n[row];
+      const int64_t src_row = (int64_t)tb->gid[tb->row_g[row]] * N + tb->row_n[row];
       const float* xsrc;
       if (p.X) {
         xsrc = p.X + src_row * Din;
@@ -479,7 +719,7 @@ struct SpectralPolicy {
               const int e = tb->line_e[line], t = tb->line_t[line];
               const int g = tb->row_g[rr], n = tb->row_n[rr];
               if (t < tb->emax[g][e]) {
-                const int64_t off = (((int64_t)(gs + g) * E1 + e) * N + t) * N + n;
+                const int64_t off = (((int64_t)tb->gid[g] * E1 + e) * N + t) * N + n;
                 vv[u] = __ldg(p.ell_val + off);
                 ii[u] = tb->nbase[g] + __ldg(p.ell_idx + off);
               }
@@ -498,18 +738,15 @@ struct SpectralPolicy {
     }
     tm.lap(18);
     }  // layer == 0: tile state staged once, reused by every layer
-    const int gs = tb->gs, Ztot = tb->Ztot;
+    const int Ztot = tb->Ztot;
     // this thread's (graph, k) row: filter coefficients of this layer into registers
 #pragma unroll
     for (int i = 0; i < FR; ++i) fr[i] = 0.f;
     if (S > 0 && r < Ztot) {
-      const int g = tb->z_g[r], k = tb->z_k[r];
-      if (k < tb->gk[g]) {                       // rows beyond k_eff multiply zero rows of U
-        const float* f = p.coeff + layer * p.coeff_stride + ((int64_t)(gs + g) * K + k) * S;
+      const float* f = p.coeff + layer * p.coeff_stride + ((int64_t)tb->gid[tb->z_g[r]] * K + tb->z_k[r]) * S;
 #pragma unroll
-        for (int i = 0; i < FR; ++i)
-          if (i < S) fr[i] = __ldg(f + i);
-      }
+      for (int i = 0; i < FR; ++i)
+        if (i < S) fr[i] = __ldg(f + i);
     }
     tm.lap(0);
     sm90::cp_async_wait_all();
@@ -517,10 +754,12 @@ struct SpectralPolicy {
     tm.lap(1);
     if (S == 0) return;
     // ---- phase B: U_g = Q_g^T X_g in 4 x 4 register tiles over (graph,k) rows x columns -----
-    for (int task = tid; task < (Ztot >> 2) * dv; task += tcg::PRODUCER_THREADS) {
+    // (a quad's Q columns past k_eff are zero and its rows there are not stored: they belong to the
+    // next graph)
+    for (int task = tid; task < tb->nzquads * dv; task += tcg::PRODUCER_THREADS) {
       const int dq = task % dv, zq = task / dv;
-      const int g = tb->z_g[4 * zq], k0 = tb->z_k[4 * zq];
-      const int n_g = tb->gn[g], nb = tb->nbase[g];
+      const int g = tb->zq_g[zq], k0 = tb->zq_k0[zq];
+      const int n_g = tb->gn[g], nb = tb->nbase[g], kr = tb->gk[g] - k0;
       float acc[4][4];
 #pragma unroll
       for (int i = 0; i < 4; ++i)
@@ -539,10 +778,11 @@ struct SpectralPolicy {
 #pragma unroll
           for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(qv[i], xv[j], acc[i][j]);
       }
+      float* ud = UZ + (size_t)(tb->kbase[g] + k0) * XP + 4 * dq;
 #pragma unroll
       for (int i = 0; i < 4; ++i)
-        *reinterpret_cast<float4*>(UZ + (size_t)(4 * zq + i) * XP + 4 * dq) =
-            make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+        if (i < kr)
+          *reinterpret_cast<float4*>(ud + (size_t)i * XP) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
     }
     tcg::producers_sync();
     tm.lap(2);
@@ -561,8 +801,7 @@ struct SpectralPolicy {
 #pragma unroll
         for (int i = 0; i < FR; ++i) f = (i == c) ? fr[i] : f;
       } else {
-        const int g = tb->z_g[r], k = tb->z_k[r];
-        f = (k < tb->gk[g]) ? __ldg(p.coeff + (sub >> 1) * p.coeff_stride + ((int64_t)(tb->gs + g) * K + k) * S + c) : 0.f;
+        f = __ldg(p.coeff + (sub >> 1) * p.coeff_stride + ((int64_t)tb->gid[tb->z_g[r]] * K + tb->z_k[r]) * S + c);
       }
       const float4* u4 = reinterpret_cast<const float4*>(UZ + (size_t)r * XP + d0);
 #pragma unroll
@@ -597,7 +836,7 @@ struct SpectralPolicy {
     if (ts < tmax) {                               // lines that did not fit the staging budget
       const int g = tb->row_g[r], n = tb->row_n[r];
       const int my = tb->emax[g][e], nb = tb->nbase[g];
-      const int64_t off0 = (((int64_t)(tb->gs + g) * E1 + e) * N) * N + n;
+      const int64_t off0 = (((int64_t)tb->gid[g] * E1 + e) * N) * N + n;
       for (int t = ts; t < tmax; ++t) {
         float a = 0.f;
         int i = 0;
@@ -640,8 +879,10 @@ struct SpectralPolicy {
       const float* z = UZ + (size_t)tb->kbase[g] * XP + 4 * hq;
       const float* q0 = Qs + (size_t)r0 * K;
       const int r1 = (n0 + 1 < n_g) ? 1 : 0, r2 = (n0 + 2 < n_g) ? 2 : 0, r3 = (n0 + 3 < n_g) ? 3 : 0;
-      // four Ritz indices per trip: Q columns and Z rows in [k_eff, ceil4(k_eff)) are zero
-      for (int k = 0; k < k_g; k += 4) {
+      // four Ritz indices per trip, then the k_eff % 4 last ones: Z rows from k_eff on belong to the
+      // next graph (or lie past Ztot), so none is read
+      int k = 0;
+      for (; k + 4 <= k_g; k += 4) {
         const float4 a0 = *reinterpret_cast<const float4*>(q0 + k);
         const float4 a1 = *reinterpret_cast<const float4*>(q0 + r1 * K + k);
         const float4 a2 = *reinterpret_cast<const float4*>(q0 + r2 * K + k);
@@ -657,6 +898,15 @@ struct SpectralPolicy {
 #pragma unroll
             for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i][kk], zv[j], acc[i][j]);
         }
+      }
+      for (; k < k_g; ++k) {
+        const float av[4] = {q0[k], q0[r1 * K + k], q0[r2 * K + k], q0[r3 * K + k]};
+        const float4 z4 = *reinterpret_cast<const float4*>(z + (size_t)k * XP);
+        const float zv[4] = {z4.x, z4.y, z4.z, z4.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], zv[j], acc[i][j]);
       }
 #pragma unroll
       for (int i = 0; i < 4; ++i)
@@ -712,13 +962,13 @@ struct SpectralPolicy {
     if (ptm) ptm->lap(19);
     const int warp = tid >> 5, lane = tid & 31;
     constexpr int NW = tcg::PRODUCER_THREADS / 32;
-    const int hv = H / 4, gs = tb->gs, Rtot = tb->Rtot;
+    const int hv = H / 4, Rtot = tb->Rtot;
     const float* bias = p.bias ? p.bias + (p.L - 1) * H : nullptr;
     if (p.out) {
       for (int row = warp; row < Rtot; row += NW) {
         const float4* src = reinterpret_cast<const float4*>(Xs + (size_t)row * XP);
         float4* dst = reinterpret_cast<float4*>(
-            p.out + ((int64_t)(gs + tb->row_g[row]) * N + tb->row_n[row]) * H);
+            p.out + ((int64_t)tb->gid[tb->row_g[row]] * N + tb->row_n[row]) * H);
         for (int q4 = lane; q4 < hv; q4 += 32) dst[q4] = src[q4];
       }
       if (p.write_pad) {
@@ -727,7 +977,7 @@ struct SpectralPolicy {
           // i-th padded (graph, node) pair of the tile, found by walking the per-graph pad counts
           int g = 0, rem = i;
           while (rem >= N - tb->gn[g]) { rem -= N - tb->gn[g]; ++g; }
-          float4* dst = reinterpret_cast<float4*>(p.out + ((int64_t)(gs + g) * N + tb->gn[g] + rem) * H);
+          float4* dst = reinterpret_cast<float4*>(p.out + ((int64_t)tb->gid[g] * N + tb->gn[g] + rem) * H);
           for (int q4 = lane; q4 < hv; q4 += 32) {
             float y[4];
 #pragma unroll
@@ -760,8 +1010,10 @@ struct SpectralPolicy {
       cx[h] = (p.relu != 0) ? fmaxf(t, 0.f) : t;
     }
     uint8_t* mk = reinterpret_cast<uint8_t*>(cx + H);   // [ng][N] node masks of the tile's graphs
-    for (int e = tid; e < tb->ng * N; e += tcg::PRODUCER_THREADS)
-      mk[e] = p.mask ? __ldg(p.mask + (int64_t)tb->gs * N + e) : (uint8_t)1;
+    for (int e = tid; e < tb->ng * N; e += tcg::PRODUCER_THREADS) {
+      const int g = e / N;
+      mk[e] = p.mask ? __ldg(p.mask + (int64_t)tb->gid[g] * N + (e - g * N)) : (uint8_t)1;
+    }
     tcg::producers_sync();
     if (ptm) ptm->lap(20);
     const int Rtot = tb->Rtot;
@@ -826,7 +1078,7 @@ struct SpectralPolicy {
         acc += y[P] * y[o];
         ++cnt;
       }
-      p.score[(int64_t)(tb->gs + g) * P + o] = acc / (float)cnt;
+      p.score[(int64_t)tb->gid[g] * P + o] = acc / (float)cnt;
     }
   }
 };
@@ -834,11 +1086,12 @@ struct SpectralPolicy {
 }  // namespace
 
 namespace lnb {
-// tile table + compact Ritz row list from the extents (shared by lnb_graph_prepare and
-// lnb_graph_prepare_sparse); tiles = [4*B + 2] ints: B + 2 table entries followed by 3*B scratch
+// tile table, tile schedule and compact Ritz row list from the extents (shared by lnb_graph_prepare
+// and lnb_graph_prepare_sparse); tiles = [4*B + 2] ints: B + 2 table entries followed by 3*B ints
+// that hold the schedule (2*B + 2 at most; B >= 2) and serve as scratch before it
 void launch_tile_assign(cudaStream_t s, const int32_t* gext, int B, int K, int32_t* tiles,
                         int32_t* rowmap, int32_t* nrows) {
-  const size_t tbytes = (size_t)6 * (B + 1) * sizeof(int32_t);
+  const size_t tbytes = ((size_t)6 * (B + 1) + 2 * SCH_NCLS) * sizeof(int32_t);
   const int tsm = tbytes <= 200 * 1024;
   if (tsm && tbytes > 40 * 1024)
     cudaFuncSetAttribute(tile_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tbytes);

@@ -169,7 +169,7 @@ def packed_offsets(B, K):
   off_edge_ptr = off_node_ptr + _align16(4 * (B + 1))
   off_D = off_edge_ptr + _align16(4 * (B + 1))
   off_tiles = off_D + _align16(4 * B * K)
-  off_krow = off_tiles + _align16(4 * (B + 2))
+  off_krow = off_tiles + _align16(4 * tile_segment_ints(B))
   off_var = off_krow + _align16(4 * (B + 1))
   return off_sizes, off_node_ptr, off_edge_ptr, off_D, off_var, off_tiles, off_krow
 
@@ -202,6 +202,86 @@ def host_tile_table(sizes, k_eff, rows_per_tile=128, graphs_per_tile=32):
   return tiles
 
 
+def tile_segment_ints(B):
+  """Size in ints of the tile segment of a packed batch: the next-fit table [B + 2] followed by the
+  tile schedule [2B + 2] (fixed size, so the segments behind it stay where (B, K) puts them)."""
+  return 3 * B + 4
+
+
+def host_tile_segment(sizes, k_eff):
+  """The tile segment of a packed batch: next-fit table, then the tile schedule (int32 [3B + 4])."""
+  return np.concatenate([host_tile_table(sizes, k_eff), host_tile_schedule(sizes, k_eff)])
+
+
+def host_tile_schedule(sizes, k_eff, rows_per_tile=128, graphs_per_tile=32):
+  """The tile schedule the fused convolution kernel runs (csrc/spectral_conv_fused.cu,
+  tile_assign_kernel): first-fit decreasing.  Graphs are taken by n_eff descending, then k_eff
+  descending, then index ascending; each goes into the lowest-numbered tile where sum n_eff <= 128,
+  sum k_eff <= 128 (not rounded up to 4) and <= 32 graphs still hold, or opens a new tile (a lone graph
+  always fits).  Inside a tile the graphs are listed in placement order.
+
+  Vectorised over classes of identical (n_eff, k_eff): for identical graphs, giving every tile, lowest
+  first, as many as still fit is what first-fit does one graph at a time.
+  Returns int32 [2B+2]: [T', first slot of tile 0 .. T' (the last = B), graph ids in tile order, 0 ...]."""
+  n = np.asarray(sizes, np.int64)
+  k = np.asarray(k_eff, np.int64)
+  B = len(n)
+  out = np.zeros(2 * B + 2, np.int32)
+  if B == 0:
+    return out
+  R, G = rows_per_tile, graphs_per_tile
+  order = np.lexsort((np.arange(B), -k, -n))
+  sn, sk = n[order], k[order]
+  cut = np.flatnonzero((sn[1:] != sn[:-1]) | (sk[1:] != sk[:-1])) + 1
+  bounds = np.concatenate([[0], cut, [B]])
+  tn, tk, tc = (np.zeros(B, np.int64) for _ in range(3))      # per tile: sum n_eff, sum k_eff, graphs
+  rec_t, rec_src, rec_slot, rec_m = [], [], [], []              # placements, in placement order
+  T = 0
+  for first, end in zip(bounds[:-1].tolist(), bounds[1:].tolist()):
+    cn, ck, count = int(sn[first]), int(sk[first]), end - first
+    done = 0
+    if T:
+      cap = G - tc[:T]
+      if cn:
+        cap = np.minimum(cap, (R - tn[:T]) // cn)
+      if ck:
+        cap = np.minimum(cap, (R - tk[:T]) // ck)
+      cap = np.maximum(cap, 0)
+      inc = np.cumsum(cap)
+      m = np.clip(count - (inc - cap), 0, cap)
+      t = np.flatnonzero(m)
+      rec_t.append(t)
+      rec_src.append(first + (inc - cap)[t])
+      rec_slot.append(tc[t].copy())
+      rec_m.append(m[t])
+      tn[:T] += m * cn
+      tk[:T] += m * ck
+      tc[:T] += m
+      done = min(count, int(inc[-1]))
+    if done < count:                                            # new tiles, each as full as the limits allow
+      ce = max(1, min(G, R // cn if cn else G, R // ck if ck else G))
+      rem = count - done
+      nt = -(-rem // ce)
+      m = np.full(nt, ce, np.int64)
+      m[-1] = rem - (nt - 1) * ce
+      t = T + np.arange(nt)
+      rec_t.append(t)
+      rec_src.append(first + done + ce * np.arange(nt))
+      rec_slot.append(np.zeros(nt, np.int64))
+      rec_m.append(m)
+      tn[t], tk[t], tc[t] = m * cn, m * ck, m
+      T += nt
+  rec_t, rec_src, rec_slot, rec_m = (np.concatenate(a) for a in (rec_t, rec_src, rec_slot, rec_m))
+  starts = np.zeros(T + 1, np.int64)
+  starts[1:] = np.cumsum(tc[:T])
+  pos = np.zeros(B, np.int64)
+  pos[PackedMolecules._ranges(rec_src, rec_m)] = PackedMolecules._ranges(starts[rec_t] + rec_slot, rec_m)
+  out[0] = T
+  out[1:T + 2] = starts
+  out[T + 2 + pos] = order
+  return out
+
+
 def ritz_extents(V_rows, node_ptr):
   """k_eff per graph = last non-zero column of its Ritz rows + 1 (what the device measures in
   lnb_graph_prepare); vectorised over the batch (every graph has at least one node)."""
@@ -222,7 +302,7 @@ def pack_sparse(sp):
   off_sizes, off_node_ptr, off_edge_ptr, off_D, off, off_tiles, off_krow = packed_offsets(B, K)
   # extents the device would measure: k_eff = last non-zero column of the graph's Ritz rows + 1
   k_eff = ritz_extents(sp['V_rows'], sp['node_ptr'])
-  tiles = host_tile_table(sp['sizes'], k_eff)
+  tiles = host_tile_segment(sp['sizes'], k_eff)
   krow = np.zeros(B + 1, np.int32)
   krow[1:] = np.cumsum(np.minimum(k_eff, K))
   off_nf = off
@@ -316,7 +396,7 @@ class PackedMolecules(object):
       raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
       blob[off:off + raw.size] = raw
 
-    put(off_tiles, host_tile_table(sizes, k_eff))
+    put(off_tiles, host_tile_segment(sizes, k_eff))
     put(off_krow, krow)
     put(off_sizes, sizes)
     put(off_node_ptr, node_ptr)

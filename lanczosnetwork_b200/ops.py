@@ -262,9 +262,10 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
   ell_max = torch.empty((B, E1), device=dev, dtype=torch.int32)
   gext = torch.empty((B, 2), device=dev, dtype=torch.int32)
   if host_tiles:
-    from .data import packed_offsets
+    from .data import packed_offsets, tile_segment_ints
     off_tiles = packed_offsets(B, K)[5]
-    tiles = blob[off_tiles:off_tiles + 4 * (B + 2)].view(torch.int32)
+    # the next-fit table and, behind it, the tile schedule the stack kernel runs
+    tiles = blob[off_tiles:off_tiles + 4 * tile_segment_ints(B)].view(torch.int32)
   else:
     tiles = torch.empty((4 * B + 2,), device=dev, dtype=torch.int32)
   rowmap = torch.empty((B * K,), device=dev, dtype=torch.int32)
