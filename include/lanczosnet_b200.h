@@ -258,6 +258,26 @@ int lnb_readout(lnb_stream_t stream, const float* state, const float* W_out, con
                 int P, float* score /* [B,P] */);
 
 /* ---------------------------------------------------------------------------------------
+ * Graph attention of the GAT baseline (model/gat.py:145-180), everything of a layer after the
+ * per-head projection.  Channel c = jj*heads + ii (bond channel jj, head ii), C = E1*heads:
+ *   s1[k] = Wh_c[k,:] . a1[c,:] + c1[c],   s2[k] = Wh_c[k,:] . a2[c,:] + c2[c]
+ *   att[i,k] = softmax over i (the ROW index, per column k) of
+ *              leaky_relu(s1[i] + s2[k], 0.2) + bias[b,i,k,jj]
+ *   h_c = att Wh_c + state_bias[c,:]
+ *   last == 0: out[b,n,c*F:(c+1)*F] = ELU(h_c[n,:])           out [B,N,C*F]
+ *   last != 0: out[b,n,:] = (sum over c = 0..C-1 of h_c[n,:]) / C   out [B,N,F]
+ * Wh [B,N,C*F] (column block c = Wh_c), bias [B,N,N,E1] channel innermost (the additive mask the
+ * reference collate builds, dataset/qm8.py:196-219), a1/a2/state_bias [C,F], c1/c2 [C].  fp32 dots in
+ * feature order, max-subtracted softmax with expf, ELU with expm1f; the channel sum runs in a fixed
+ * order, so repeated launches are bit-identical.  Wh, state_bias and out 16-byte aligned.
+ * Envelope: N <= 128, F % 4 == 0, F <= 128, E1 <= 16, heads <= 32 (LNB_ERR_UNSUPPORTED otherwise,
+ * nothing launched).
+ * ------------------------------------------------------------------------------------- */
+int lnb_gat_attention(lnb_stream_t stream, const float* Wh, const float* bias, const float* a1,
+                      const float* a2, const float* c1, const float* c2, const float* state_bias,
+                      int B, int N, int E1, int heads, int F, int last, float* out);
+
+/* ---------------------------------------------------------------------------------------
  * Operator chain on channel 0 of L [B,N,N,E1], per graph, starting from X [B,N,D]:
  *   chebyshev == 0: w_s = L_0 w_{s-1} (w_0 = X), s = 1..steps   (model/dcnn.py:88-92, the short
  *                   diffusion walk of model/lanczos_net.py:164-169);

@@ -41,6 +41,15 @@ def qm8_cheby_net(**model_over):
                                   num_bond_type=6), model=NS(**model))
 
 
+def qm8_gat(**model_over):
+  """config/qm8_gat.yaml"""
+  model = dict(name='GAT', input_dim=64, hidden_dim=[16] * 7, num_layer=7, num_heads=[8] * 7,
+               output_dim=16, dropout=0.0, loss='MSE')
+  model.update(model_over)
+  return NS(seed=1234, dataset=NS(loader_name='QM8Data', name='chemistry', num_atom=70,
+                                  num_bond_type=6), model=NS(**model))
+
+
 def qm8_ada_lanczos_net(**model_over):
   model = dict(name='AdaLanczosNet', short_diffusion_dist=[1, 2, 3],
                long_diffusion_dist=[5, 7, 10, 20, 30], num_eig_vec=20,

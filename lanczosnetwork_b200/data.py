@@ -18,7 +18,7 @@ import numpy as np
 
 __all__ = [
     'check_dist', 'get_laplacian', 'get_graph_laplacian_eigs', 'prepare_graph',
-    'collate', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
+    'collate', 'gat_bias', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
     'synthetic_regression_graphs',
 ]
 
@@ -119,6 +119,19 @@ def collate(samples, num_eigs, num_nodes=None):
     out['label'] = np.concatenate([np.asarray(s['label'], np.float32).reshape(1, -1)
                                    for s in samples], axis=0)
   return out
+
+
+def gat_bias(L):
+  """The additive attention bias the reference collate hands GAT (dataset/qm8.py:196-219), from the
+  collated operators L [B,N,N,E1] of ``collate``, bit for bit: per channel m = I (adj + I) in fp64,
+  every entry > 0 of the padded N x N block set to 1, bias = -1e9 * (1 - m) cast to fp32.  For the
+  non-negative QM8 operators that is -0.0 (note the sign) on edges, on the diagonal and on every
+  padded node's self-loop, and -1e9 elsewhere.  Returns float32 [B,N,N,E1]."""
+  L = np.asarray(L)
+  N = L.shape[1]
+  mt = L.astype(np.float64) + np.eye(N)[None, :, :, None]      # I @ (adj + I) is exact
+  mt[mt > 0.0] = 1.0
+  return (-1e9 * (1.0 - mt)).astype(np.float32)
 
 
 def sparse_collate(samples, num_eigs):

@@ -6,8 +6,8 @@ What it does (see INTEGRATION.md):
   1. registers ``operators._ext`` / ``operators._ext.segment_reduction`` in ``sys.modules`` so
      ``from model import *`` of the reference works without building its THC-era extension
      (model/mpnn.py:6 -> operators/functions/unsorted_segment_sum.py:5);
-  2. rebinds ``LanczosNet`` / ``AdaLanczosNet`` / ``LanczosNetGeneral`` / ``GCN`` inside the runner
-     modules' globals, because the runners resolve the class with ``eval(name)`` in their own
+  2. rebinds the classes of ``DROPIN_CLASSES`` (``LanczosNet``, ``AdaLanczosNet``, ``GCN``, ``GAT``, ...)
+     inside the runner modules' globals, because the runners resolve the class with ``eval(name)`` in their own
      namespace (runner/qm8_runner.py:59,288; runner/graph_runner.py:57,285);
   3. runs the reference ``run_exp.main()`` unchanged.
 """
@@ -18,7 +18,8 @@ import sys
 from . import model as _models
 from .operators import _ext as _ext_pkg
 
-DROPIN_CLASSES = ('LanczosNet', 'AdaLanczosNet', 'LanczosNetGeneral', 'GCN', 'GCNFP', 'DCNN', 'ChebyNet')
+DROPIN_CLASSES = ('LanczosNet', 'AdaLanczosNet', 'LanczosNetGeneral', 'GCN', 'GCNFP', 'DCNN', 'ChebyNet',
+                  'GAT')
 
 
 def register_native_op():
@@ -33,8 +34,8 @@ def register_native_op():
 def patch_namespace(module, training=False):
   """Rebind the class names in ``module``'s globals to the H100 drop-ins.  ``training=True`` (a
   run without ``-t``) rebinds only the classes that have a differentiable training path
-  (currently every class); one without it would keep the reference's trainable class
-  instead of failing on the first ``loss.backward()``."""
+  (every class but ``GAT``, which is inference only); a class without one keeps the reference's
+  trainable class instead of failing on the first ``loss.backward()``."""
   for name in DROPIN_CLASSES:
     if hasattr(module, name):
       cls = getattr(_models, name)

@@ -6,3 +6,4 @@ from .lanczos_net_general import *  # noqa: F401,F403
 from .gcn import *                  # noqa: F401,F403  (SURVEY 8f3: sibling models on the same kernels)
 from .dcnn import *                 # noqa: F401,F403
 from .cheby_net import *            # noqa: F401,F403
+from .gat import *                  # noqa: F401,F403  (inference only)

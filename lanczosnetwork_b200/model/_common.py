@@ -111,8 +111,11 @@ class SpectralNetBase(nn.Module):
             mod.bias.data.zero_()
 
   # ------------------------------------------------------------------------------------------
+  def _param_device(self):
+    return self.filter[0].weight.device
+
   def _device(self):
-    dev = self.filter[0].weight.device
+    dev = self._param_device()
     if dev.type != 'cuda':
       raise RuntimeError(
           '%s runs on CUDA (sm_90a) only -- move the module with .cuda(); there is no CPU '

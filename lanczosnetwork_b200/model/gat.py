@@ -1,0 +1,144 @@
+"""Drop-in for the reference ``model.GAT`` (model/gat.py:8-201): graph attention over the bond channels,
+inference only.  Same constructor fields, parameter names, registration and initialisation order (so
+``torch.manual_seed(s)`` gives the reference's initial weights and its checkpoints load by name), and
+the same ``forward(node_feat, L, label=None, mask=None)``, where ``L`` is the additive attention bias
+the reference collate builds for GAT (``data.gat_bias``).
+
+Per layer the reference runs one Linear / two scorers / softmax / bmm sequence for each of the
+(E+1) * heads channels (model/gat.py:145-180).  Here a layer is two launches: the per-head weights,
+stacked in concat order into one [C*F, Din] matrix, go through the 3xTF32 wgmma dense layer once for
+all B*N rows, and ``lnb_gat_attention`` does the scorers, the column softmax, the aggregation and the
+ELU (or, in the last layer, the mean over channels).  With the embedding gather and the readout that is
+2 + 2 * num_layer launches, captured as one CUDA graph.
+
+Quirk kept on purpose: the reference's ``state_bias`` repeats one inner list for every bond channel
+(model/gat.py:62-70), so every channel of layer t uses ``bias_{ii}_{E}_{t}``; the other
+``bias_{ii}_{jj}_{t}`` are registered and saved but never read.  There is no training path: under
+autograd with trainable parameters the forward raises, and ``dropin.patch_namespace(training=True)``
+keeps the reference class for training runs."""
+import torch
+import torch.nn as nn
+
+from ._common import SpectralNetBase, _opt
+from ..spectral_conv import WeightCache
+from .. import ops
+
+__all__ = ['GAT']
+
+
+def _linear_grid(num_layer, num_channel, num_heads, make):
+  return nn.ModuleList([
+      nn.ModuleList([nn.ModuleList([make(t) for _ in range(num_heads[t])]) for _ in range(num_channel)])
+      for t in range(num_layer)])
+
+
+class GAT(SpectralNetBase):
+
+  def __init__(self, config):
+    super(GAT, self).__init__()
+    m = config.model
+    self.config = config
+    self.input_dim = m.input_dim
+    self.hidden_dim = m.hidden_dim
+    self.output_dim = m.output_dim
+    self.num_layer = m.num_layer
+    self.num_heads = m.num_heads
+    self.dropout = _opt(m, 'dropout', 0.0)
+    self.num_atom = config.dataset.num_atom
+    self.num_edgetype = config.dataset.num_bond_type
+    self._wcache = WeightCache()
+    E1 = self.num_edgetype + 1
+    dims = [self.input_dim] + list(self.hidden_dim) + [self.output_dim]
+
+    self.embedding = nn.Embedding(self.num_atom, self.input_dim)
+    # input width of layer t > 0 is dims[t] * num_heads[t] * (E+1): num_heads of layer t itself,
+    # as the reference constructor has it (model/gat.py:34-38)
+    din = [dims[t] if t == 0 else dims[t] * self.num_heads[t] * E1 for t in range(self.num_layer)]
+    self.filter = _linear_grid(self.num_layer, E1, self.num_heads,
+                               lambda t: nn.Linear(din[t], dims[t + 1], bias=False))
+    self.att_net_1 = _linear_grid(self.num_layer, E1, self.num_heads, lambda t: nn.Linear(dims[t + 1], 1))
+    self.att_net_2 = _linear_grid(self.num_layer, E1, self.num_heads, lambda t: nn.Linear(dims[t + 1], 1))
+    # bias_{ii}_{jj}_{t}, registered on the module itself (first in the state_dict); state_bias[t][jj]
+    # is ONE list shared by every jj, so it ends up holding the jj = E parameters
+    self.state_bias = []
+    for t in range(self.num_layer):
+      shared = [None] * self.num_heads[t]
+      self.state_bias.append([shared] * E1)
+      for jj in range(E1):
+        for ii in range(self.num_heads[t]):
+          shared[ii] = nn.Parameter(torch.zeros(dims[t + 1]))
+          self.register_parameter('bias_%d_%d_%d' % (ii, jj, t), shared[ii])
+    self.att_func = nn.Sequential(nn.Linear(dims[-2], 1), nn.Sigmoid())
+    self.output_func = nn.Sequential(nn.Linear(dims[-2], dims[-1]))
+    loss = m.loss
+    if loss == 'CrossEntropy':
+      self.loss_func = torch.nn.CrossEntropyLoss()
+    elif loss == 'MSE':
+      self.loss_func = torch.nn.MSELoss()
+    elif loss == 'L1':
+      self.loss_func = torch.nn.L1Loss()
+    else:
+      raise ValueError("Non-supported loss function!")
+    self._init_param()
+
+  def _init_param(self):
+    """Xavier-uniform weights and zero biases, in the reference's order (model/gat.py:88-123):
+    att_func, output_func, filter, att_net_1, att_net_2."""
+    linears = list(self.att_func) + list(self.output_func)
+    for grid in (self.filter, self.att_net_1, self.att_net_2):
+      linears += [mod for per_layer in grid for per_channel in per_layer for mod in per_channel]
+    for mod in linears:
+      if isinstance(mod, nn.Linear):
+        nn.init.xavier_uniform_(mod.weight.data)
+        if mod.bias is not None:
+          mod.bias.data.zero_()
+
+  def _param_device(self):
+    return self.embedding.weight.device
+
+  def forward(self, node_feat, L, label=None, mask=None):
+    """
+      node_feat: long B x N (atom ids); L: float B x N x N x (E+1), the attention bias of the GAT
+      collate (data.gat_bias); label: B x P; mask: B x N (uint8 / bool / float).
+      Returns score (B x P) or (score, loss).
+    """
+    dev = self._device()
+    self._check_mode()                    # no training path: raises under autograd
+    score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
+    return self._finish(score, self._to(dev, label))
+
+  def _layer_params(self, t):
+    """Per-layer tensors in concat order c = jj * heads + ii, stacked once per parameter version."""
+    E = self.num_edgetype
+    mods = [(jj, ii) for jj in range(E + 1) for ii in range(self.num_heads[t])]
+    cache = self._wcache
+    w = [self.filter[t][jj][ii].weight for jj, ii in mods]
+    a1, = cache.stacked('att_net_1.%d.weight' % t, [self.att_net_1[t][jj][ii].weight for jj, ii in mods])
+    a2, = cache.stacked('att_net_2.%d.weight' % t, [self.att_net_2[t][jj][ii].weight for jj, ii in mods])
+    c1, = cache.stacked('att_net_1.%d.bias' % t, [self.att_net_1[t][jj][ii].bias for jj, ii in mods])
+    c2, = cache.stacked('att_net_2.%d.bias' % t, [self.att_net_2[t][jj][ii].bias for jj, ii in mods])
+    # every channel reads the bias registered for jj = E (the shared state_bias list)
+    sb, = cache.stacked('state_bias.%d' % t, [getattr(self, 'bias_%d_%d_%d' % (ii, E, t)) for _, ii in mods])
+    return w, a1, a2, c1, c2, sb.view(len(mods), -1)
+
+  def _project(self, x2d, weights, t):
+    """x2d @ [W_0; W_1; ...]^T: every head of every channel in one dense launch."""
+    M, K = x2d.shape
+    if K % 4 == 0:
+      w_hi, w_lo = self._wcache.stacked('filter.%d' % t, weights, split=True)
+      return ops.linear_tf32x3(x2d, w_hi, w_lo)
+    w, = self._wcache.stacked('filter.%d' % t, weights)       # rows not 16-byte multiples: FFMA GEMM
+    out = torch.empty((M, w.shape[0]), device=x2d.device, dtype=torch.float32)
+    ops.bgemm(x2d, (0, 0, K, 1), w, (0, 0, 1, K), out, (0, 0, w.shape[0], 1), 1, 1, M, w.shape[0], K)
+    return out
+
+  def _forward_impl(self, node_feat, L, mask):
+    bias = L.float().contiguous()
+    B, N = node_feat.shape
+    state = ops.embedding_rows(node_feat.long(), self.embedding.weight)
+    for t in range(self.num_layer):
+      w, a1, a2, c1, c2, sb = self._layer_params(t)
+      Wh = self._project(state.reshape(B * N, -1), w, t).view(B, N, -1)
+      state = ops.gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=(t == self.num_layer - 1))
+    head, att = self.output_func[0], self.att_func[0]
+    return ops.readout(state, head.weight, head.bias, att.weight.reshape(-1), att.bias, mask)

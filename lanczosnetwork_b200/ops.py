@@ -14,6 +14,7 @@ from ._lib import GemmDesc, SpectralStack
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
+    'gat_attention', 'gat_attention_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
     'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
@@ -445,6 +446,32 @@ def readout(state, W_out, b_out, w_att, b_att, mask=None):
     _lib.check(_lib.load().lnb_readout(_stream(state), _ptr(state), _ptr(_f32c(W_out)),
                                        _ptr(_f32c(b_out)), _ptr(_f32c(w_att)), _ptr(_f32c(b_att)),
                                        _ptr(mask), B, N, H, P, _ptr(out)), 'lnb_readout')
+  return out
+
+
+def gat_attention_supported(N, F, E1, heads):
+  """Shapes lnb_gat_attention accepts (mirrors its checks)."""
+  return N <= 128 and F % 4 == 0 and F <= 128 and E1 <= 16 and heads <= 32
+
+
+def gat_attention(Wh, bias, a1, a2, c1, c2, state_bias, last=False):
+  """Graph attention of one GAT layer after the projection (see lnb_gat_attention).
+  Wh [B,N,C*F], bias [B,N,N,E1], a1/a2/state_bias [C,F], c1/c2 [C] with C = E1*heads.
+  Returns ELU(h_c) concatenated over c [B,N,C*F], or with ``last`` the mean over c [B,N,F]."""
+  _need_cuda(Wh, bias, a1, a2, c1, c2, state_bias)
+  Wh, bias = _f32c(Wh), _f32c(bias)
+  a1, a2, c1, c2, state_bias = [_f32c(t) for t in (a1, a2, c1, c2, state_bias)]
+  B, N, _, E1 = bias.shape
+  C, F = a1.shape
+  heads = C // E1
+  if heads * E1 != C or tuple(Wh.shape) != (B, N, C * F) or tuple(state_bias.shape) != (C, F):
+    raise ValueError('gat_attention: Wh %s, bias %s, a1 %s, state_bias %s do not agree'
+                     % (tuple(Wh.shape), tuple(bias.shape), tuple(a1.shape), tuple(state_bias.shape)))
+  out = torch.empty((B, N, F if last else C * F), device=Wh.device, dtype=torch.float32)
+  with torch.cuda.device(Wh.device):
+    _lib.check(_lib.load().lnb_gat_attention(
+        _stream(Wh), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
+        B, N, E1, heads, F, int(bool(last)), _ptr(out)), 'lnb_gat_attention')
   return out
 
 

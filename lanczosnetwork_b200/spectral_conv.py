@@ -103,6 +103,16 @@ class WeightCache(object):
       return hi, lo, torch.cat([b.detach() for b in biases], dim=0).contiguous()
     return self._get((name, weights[0].device.index), tag, build, list(weights) + list(biases))
 
+  def stacked(self, name, parts, split=False):
+    """torch.cat(parts, 0) of per-module tensors (e.g. the per-head weights of GAT), rebuilt when any
+    part changes; returns (hi, lo) of its tf32 split when ``split``, else a 1-tuple."""
+    tag = tuple((t.data_ptr(), t._version) for t in parts) + (split,)
+
+    def build():
+      cat = torch.cat([t.detach() for t in parts], dim=0).contiguous()
+      return ops.split_tf32(cat) if split else (cat,)
+    return self._get((name, parts[0].device.index), tag, build, list(parts))
+
   def clear(self):
     self.invalidate()
 
