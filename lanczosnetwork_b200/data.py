@@ -367,9 +367,10 @@ class PackedMolecules(object):
     return np.repeat(starts - (ends - lens), lens) + np.arange(total, dtype=np.int64)
 
   def max_bytes(self, B):
-    """Upper bound of a B-molecule blob (for a reusable pinned staging buffer)."""
-    n = int(np.sort(self.sizes)[-B:].sum())
-    e = int(np.sort(np.diff(self.edge_ptr))[-B:].sum())
+    """Upper bound of the blob of any B molecules, repeats included (for a reusable pinned staging
+    buffer): an index list may repeat the largest molecule B times."""
+    n = B * int(self.sizes.max())
+    e = B * int(np.diff(self.edge_ptr).max())
     return packed_offsets(B, self.K)[4] + _align16(4 * n) + _align16(4 * n * self.K) + _align16(4 * e)
 
   def batch(self, idx, out=None):

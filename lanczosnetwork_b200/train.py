@@ -19,7 +19,8 @@ PyTorch supplies what it supplies everywhere in this package -- tensor memory, s
 tape -- plus the pointwise glue of the adjoint (ReLU masks, sigmoid gate, masked mean, the loss).
 The training forward is the UNFUSED formulation (activations have to exist to be differentiated);
 the one-launch fused stack remains the inference path.  Gradients are checked against
-``torch.autograd`` over the fp64 CPU oracle in tests/test_gpu_train.py.
+``torch.autograd`` over the fp64 CPU oracle in tests/test_gpu_train.py, and function by function
+across the shapes they accept in tests/test_gpu_train_envelope.py.
 """
 import torch
 
@@ -175,7 +176,8 @@ def spectral_messages(V, X, F):
 
 class _Embedding(torch.autograd.Function):
   """state = table[ids] (model/lanczos_net.py:154); the gradient of the table is the scatter-add of
-  the reference's own unsorted_segment_sum op."""
+  the reference's own unsorted_segment_sum op.  An id outside [0, rows) reads a zero row, so its
+  gradient row belongs to no table row: the segment sum skips it."""
 
   @staticmethod
   def forward(ctx, ids, table):
@@ -188,8 +190,7 @@ class _Embedding(torch.autograd.Function):
     (ids,) = ctx.saved_tensors
     D = g.shape[-1]
     flat = g.reshape(1, -1, D).contiguous()
-    seg = ids.reshape(1, -1).clamp(0, ctx.rows - 1)
-    return None, ops.segment_sum_forward(flat, seg, ctx.rows)[0]
+    return None, ops.segment_sum_forward(flat, ids.reshape(1, -1), ctx.rows)[0]
 
 
 def embedding(ids, table):
