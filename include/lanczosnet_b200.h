@@ -215,6 +215,35 @@ typedef struct lnb_spectral_stack {
 int lnb_spectral_stack_forward(lnb_stream_t stream, const lnb_spectral_stack* desc /* host */);
 
 /* ---------------------------------------------------------------------------------------
+ * GraphSAGE (model/graph_sage.py:98-175) on the convolution stack.  With the Mean aggregator the
+ * message of channel e is M_e X with the layer-invariant, count-weighted operator
+ *   M_e[b, n, m] = (nonempty[b, n] != 0) * count(nn_idx[b, n, :, e] == m) / K
+ * lnb_sage_operators writes it dense, [B, N, N, E1] channel innermost (every entry, zeros
+ * included): the layout lnb_graph_prepare reads.  nn_idx [B, N, K, E1] int64 (the collate's
+ * neighbour samples), nonempty [B, N] fp32 (one flag per node).  Ids outside [0, N) contribute
+ * nothing.  Limit: N * E1 ints within shared memory (LNB_ERR_UNSUPPORTED otherwise).
+ *
+ * lnb_sage_stack_forward runs the descriptor of lnb_spectral_stack_forward (same fields, same
+ * shape limits, S must be 0; LNB_ERR_UNSUPPORTED and nothing launched otherwise) with two changes:
+ * every finished layer row y = act(. + b) is replaced by y / (||y||_2 + FLT_EPSILON) (the padded
+ * nodes' constant rows of write_pad and of the readout likewise), and with LNB_SAGE_MAX in flags the
+ * edge messages are the elementwise max over the ELL entries of each row (values ignored, a row
+ * without entries gives 0) instead of the weighted sum.
+ *
+ * lnb_neighbour_max: the Max messages on their own (the training path),
+ *   out[b, n, e*D + f] = max over the ELL entries m of row n of channel e of X[b, m, f]
+ *   argmax[b, n, e, f] = that m (ties: lowest m), -1 for a row without entries (out = 0).
+ * X [B, N, D]; ell_* from lnb_graph_prepare on the operators above; N <= 255.
+ * ------------------------------------------------------------------------------------- */
+#define LNB_SAGE_MAX 1
+int lnb_sage_operators(lnb_stream_t stream, const int64_t* nn_idx, const float* nonempty, int B, int N,
+                       int K, int E1, float* out /* [B,N,N,E1] */);
+int lnb_sage_stack_forward(lnb_stream_t stream, const lnb_spectral_stack* desc /* host */, int flags);
+int lnb_neighbour_max(lnb_stream_t stream, const float* X, const float* ell_val, const uint8_t* ell_idx,
+                      const int32_t* ell_max, int B, int N, int E1, int D, float* out /* [B,N,E1*D] */,
+                      int32_t* argmax /* [B,N,E1,D] */);
+
+/* ---------------------------------------------------------------------------------------
  * Embedding rows (model/lanczos_net.py:154): out[r, :] = table[idx[r], :].
  * ------------------------------------------------------------------------------------- */
 int lnb_embedding_rows(lnb_stream_t stream, const int64_t* idx, const float* table,

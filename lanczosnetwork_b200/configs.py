@@ -50,6 +50,15 @@ def qm8_gat(**model_over):
                                   num_bond_type=6), model=NS(**model))
 
 
+def qm8_graphsage(**model_over):
+  """config/qm8_graphsage.yaml"""
+  model = dict(name='GraphSAGE', input_dim=64, hidden_dim=[128] * 7, output_dim=16, num_sample_neighbors=40,
+               agg_func='Mean', num_layer=7, loss='MSE')
+  model.update(model_over)
+  return NS(seed=1234, dataset=NS(loader_name='QM8Data', name='chemistry', num_atom=70,
+                                  num_bond_type=6), model=NS(**model))
+
+
 def qm8_ada_lanczos_net(**model_over):
   model = dict(name='AdaLanczosNet', short_diffusion_dist=[1, 2, 3],
                long_diffusion_dist=[5, 7, 10, 20, 30], num_eig_vec=20,

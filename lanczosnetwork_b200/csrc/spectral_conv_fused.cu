@@ -486,7 +486,20 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
 }
 
 // --------------------------------------------------------------------------------------------
-struct SpectralPolicy {
+// Layer variants of the stack kernel, fixed at compile time (lnb_sage_stack_forward):
+//   STACK_PLAIN      out = act(E + V Z + b)                          (LanczosNet, GCN, ...)
+//   STACK_SAGE_MEAN  then every finished row divided by (||row||_2 + eps) (model/graph_sage.py:150-153)
+//   STACK_SAGE_MAX   the same, and the edge producer takes the elementwise max over the ELL row
+//                    instead of the weighted sum (the Max aggregator, model/graph_sage.py:141-142)
+constexpr int STACK_PLAIN = 0;
+constexpr int STACK_SAGE_MEAN = 1;
+constexpr int STACK_SAGE_MAX = 2;
+constexpr float SAGE_EPS = 1.1920928955078125e-07f;   // np.finfo(np.float32).eps (graph_sage.py:6)
+
+template <int kVariant>
+struct SpectralPolicyT {
+  static constexpr bool kNormRows = kVariant != STACK_PLAIN;
+  static constexpr bool kMaxAgg = kVariant == STACK_SAGE_MAX;
   static constexpr int kStagesB = 1;      // one W stage and one A stage: shared memory goes to the packed tile
   static constexpr int kStagesA = 1;
   static constexpr int LMAX = 8;          // layers run by one launch
@@ -576,7 +589,7 @@ struct SpectralPolicy {
 
   static __host__ __device__ constexpr size_t tables_bytes() { return (sizeof(Tables) + 15) & ~size_t(15); }
 
-  __device__ SpectralPolicy(const Params& p_, uint8_t* smem, int tid_)
+  __device__ SpectralPolicyT(const Params& p_, uint8_t* smem, int tid_)
       : p(p_), tid(tid_), r(tid_ & 127), N(p_.N), K(p_.K), S(p_.S), E1(p_.E1),
         H(p_.H), XP((p_.Din[0] > p_.H ? p_.Din[0] : p_.H) + 4), Din(p_.Din[0]) {
     tb = reinterpret_cast<Tables*>(smem);
@@ -814,6 +827,10 @@ struct SpectralPolicy {
     // edge type e = c: sparse row of L_e (ELL) times X[:, d0:d0+32]; row = (graph, node)
     if (r >= tb->Rtot) return;
     const int e = c;
+    if constexpr (kMaxAgg) {
+      produce_max(e, d0, v);
+      return;
+    }
     const float* xs = Xs + d0;
     const int ts = tb->cnt_e[e], tmax = tb->tmax_e[e];
     const float* ev = Ev + (size_t)tb->base_e[e] * RMAX + r;
@@ -856,6 +873,83 @@ struct SpectralPolicy {
         }
       }
     }
+  }
+
+  // Max aggregator (STACK_SAGE_MAX): v = elementwise max over X[i, d0:d0+32] for the entries i of
+  // row r of channel e.  The entry values (sample counts / K) are ignored: a non-zero only says the
+  // neighbour was drawn; zero entries are the fill up to the tile's longest row.  A row without
+  // entries (nonempty = 0) gives 0, like the reference's `agg * nonempty_mask`.
+  __device__ __forceinline__ void produce_max(int e, int d0, float (&v)[32]) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = -INFINITY;
+    bool any = false;
+    const float* xs = Xs + d0;
+    const int ts = tb->cnt_e[e], tmax = tb->tmax_e[e];
+    const float* ev = Ev + (size_t)tb->base_e[e] * RMAX + r;
+    const uint8_t* ei = Ei + (size_t)tb->base_e[e] * RMAX + r;
+    for (int t = 0; t < ts; ++t) {
+      if (ev[t * RMAX] == 0.f) continue;
+      const float4* x4 = reinterpret_cast<const float4*>(xs + (size_t)ei[t * RMAX] * XP);
+      any = true;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float4 tt = x4[q];
+        v[4 * q + 0] = fmaxf(v[4 * q + 0], tt.x);
+        v[4 * q + 1] = fmaxf(v[4 * q + 1], tt.y);
+        v[4 * q + 2] = fmaxf(v[4 * q + 2], tt.z);
+        v[4 * q + 3] = fmaxf(v[4 * q + 3], tt.w);
+      }
+    }
+    if (ts < tmax) {                               // lines that did not fit the staging budget
+      const int g = tb->row_g[r], n = tb->row_n[r];
+      const int my = tb->emax[g][e], nb = tb->nbase[g];
+      const int64_t off0 = (((int64_t)tb->gid[g] * E1 + e) * N) * N + n;
+      for (int t = ts; t < tmax && t < my; ++t) {
+        if (__ldg(p.ell_val + off0 + (int64_t)t * N) == 0.f) continue;
+        const int i = nb + __ldg(p.ell_idx + off0 + (int64_t)t * N);
+        const float4* x4 = reinterpret_cast<const float4*>(xs + (size_t)i * XP);
+        any = true;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float4 tt = x4[q];
+          v[4 * q + 0] = fmaxf(v[4 * q + 0], tt.x);
+          v[4 * q + 1] = fmaxf(v[4 * q + 1], tt.y);
+          v[4 * q + 2] = fmaxf(v[4 * q + 2], tt.z);
+          v[4 * q + 3] = fmaxf(v[4 * q + 3], tt.w);
+        }
+      }
+    }
+    if (!any) {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) v[j] = 0.f;
+    }
+  }
+
+  // GraphSAGE row normalisation (model/graph_sage.py:152): y / (||y||_2 + eps), a division like the
+  // reference.  The squares are summed in feature order, so a row equal to act(b) gets exactly the
+  // denominator of pad_den() below.
+  __device__ __forceinline__ void normalize_row(float* row) const {
+    float4* r4 = reinterpret_cast<float4*>(row);
+    float ss = 0.f;
+    for (int h4 = 0; h4 < H / 4; ++h4) {
+      const float4 t = r4[h4];
+      ss = fmaf(t.x, t.x, ss); ss = fmaf(t.y, t.y, ss); ss = fmaf(t.z, t.z, ss); ss = fmaf(t.w, t.w, ss);
+    }
+    const float den = sqrtf(ss) + SAGE_EPS;
+    for (int h4 = 0; h4 < H / 4; ++h4) {
+      const float4 t = r4[h4];
+      r4[h4] = make_float4(t.x / den, t.y / den, t.z / den, t.w / den);
+    }
+  }
+  // denominator of the constant row act(b) of padded nodes (every calling thread computes it alone)
+  __device__ __forceinline__ float pad_den(const float* bias) const {
+    float ss = 0.f;
+    for (int h = 0; h < H; ++h) {
+      float t = bias ? __ldg(bias + h) : 0.f;
+      t = (p.relu != 0) ? fmaxf(t, 0.f) : t;
+      ss = fmaf(t, t, ss);
+    }
+    return sqrtf(ss) + SAGE_EPS;
   }
 
   // After the last k-block of the edge step: (V Z)[row, :] for every real row in 4 x 4 register
@@ -957,6 +1051,11 @@ struct SpectralPolicy {
   // memory, one warp per 512-byte row, plus the constant rows act(b) of padded nodes when
   // requested) and / or the fused readout.  Between layers the state never leaves the SM.
   __device__ void post_epilogue(int sub) {
+    if constexpr (kNormRows) {
+      // thread r stored every chunk of row r itself; the next reader of other rows (next layer's
+      // producers, the write-back and readout below) is behind a producers_sync()
+      if ((sub & 1) != 0 && r < tb->Rtot) normalize_row(Xs + (size_t)r * XP);
+    }
     if ((sub & 1) == 0 || (sub >> 1) != p.L - 1) return;
     tcg::producers_sync();              // every chunk of every row is in shared memory
     if (ptm) ptm->lap(19);
@@ -972,6 +1071,8 @@ struct SpectralPolicy {
         for (int q4 = lane; q4 < hv; q4 += 32) dst[q4] = src[q4];
       }
       if (p.write_pad) {
+        [[maybe_unused]] float den = 1.f;
+        if constexpr (kNormRows) den = pad_den(bias);
         const int npad = tb->ng * N - Rtot;
         for (int i = warp; i < npad; i += NW) {
           // i-th padded (graph, node) pair of the tile, found by walking the per-graph pad counts
@@ -984,6 +1085,7 @@ struct SpectralPolicy {
             for (int u = 0; u < 4; ++u) {
               float t = bias ? __ldg(bias + 4 * q4 + u) : 0.f;
               y[u] = (p.relu != 0) ? fmaxf(t, 0.f) : t;
+              if constexpr (kNormRows) y[u] = y[u] / den;
             }
             dst[q4] = make_float4(y[0], y[1], y[2], y[3]);
           }
@@ -1005,9 +1107,12 @@ struct SpectralPolicy {
       const int o = e / H, h = e - o * H;
       Wr[o * HP + h] = (o < P) ? __ldg(p.W_out + o * H + h) : (o == P ? __ldg(p.w_att + h) : 0.f);
     }
+    [[maybe_unused]] float den = 1.f;
+    if constexpr (kNormRows) den = pad_den(bias_last);
     for (int h = tid; h < H; h += tcg::PRODUCER_THREADS) {
       float t = bias_last ? __ldg(bias_last + h) : 0.f;
       cx[h] = (p.relu != 0) ? fmaxf(t, 0.f) : t;
+      if constexpr (kNormRows) cx[h] = cx[h] / den;
     }
     uint8_t* mk = reinterpret_cast<uint8_t*>(cx + H);   // [ng][N] node masks of the tile's graphs
     for (int e = tid; e < tb->ng * N; e += tcg::PRODUCER_THREADS) {
@@ -1082,6 +1187,7 @@ struct SpectralPolicy {
     }
   }
 };
+using SpectralPolicy = SpectralPolicyT<STACK_PLAIN>;
 
 }  // namespace
 
@@ -1138,13 +1244,16 @@ int lnb_graph_prepare(lnb_stream_t stream, const float* L, const float* Q, int B
   return lnb::finish_launch("graph_prepare");
 }
 
+// one launcher for every variant of the stack kernel
+extern "C++" {
+template <class Pol>
 static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const char* who) {
   LNB_REQUIRE((d.X || (d.node_ids && d.emb_table)) && d.Q && d.ell_val && d.ell_idx && d.ell_max &&
                   d.gext && d.tiles && d.W_hi && d.W_lo && (d.out_state || d.score) &&
                   (d.coeff || d.S == 0),
               "%s: null pointer", who);
   LNB_REQUIRE(d.B >= 0 && d.N >= 1 && d.E1 >= 1 && d.K >= 1 && d.S >= 0 && d.H >= 1 &&
-                  d.num_layers >= 1 && d.num_layers <= SpectralPolicy::LMAX,
+                  d.num_layers >= 1 && d.num_layers <= Pol::LMAX,
               "%s: bad dims", who);
   LNB_REQUIRE(!d.score || (d.W_out && d.b_out && d.w_att && d.b_att && d.P >= 1 && d.P <= 48),
               "%s: readout needs W_out, b_out, w_att, b_att and 1 <= P <= 48", who);
@@ -1167,31 +1276,31 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
     return LNB_ERR_ARG;
   }
   if (d.B == 0) return LNB_OK;
-  size_t smem = tcg::core_smem(SpectralPolicy::kStagesB, SpectralPolicy::kStagesA) + 1024 +
-                SpectralPolicy::smem_fixed(dmax, d.K, d.H);
+  size_t smem = tcg::core_smem(Pol::kStagesB, Pol::kStagesA) + 1024 +
+                Pol::smem_fixed(dmax, d.K, d.H);
   if (smem > 227 * 1024) {
     lnb::set_err("%s: tile state (Din=%d, K=%d, H=%d) needs %zu B of shared memory", who, dmax, d.K,
                  d.H, smem);
     return LNB_ERR_UNSUPPORTED;
   }
-  int lb = (int)((227 * 1024 - smem) / SpectralPolicy::ell_line_bytes());
+  int lb = (int)((227 * 1024 - smem) / Pol::ell_line_bytes());
   if (lb > 255) lb = 255;
   // The readout scratch (at most 56 KiB: P = 48, H = 128, N = 128) fits the dead region (at least
   // 93 KiB: Din or H = 128, K = 32) at every shape accepted above; the check keeps it that way.
-  if (d.score && SpectralPolicy::readout_bytes(d.H, d.P, d.N) > SpectralPolicy::dead_bytes(dmax, d.K, d.H, lb)) {
+  if (d.score && Pol::readout_bytes(d.H, d.P, d.N) > Pol::dead_bytes(dmax, d.K, d.H, lb)) {
     lnb::set_err("%s: fused readout (P=%d, H=%d, N=%d) does not fit the free shared memory", who, d.P,
                  d.H, d.N);
     return LNB_ERR_UNSUPPORTED;
   }
-  smem += (size_t)lb * SpectralPolicy::ell_line_bytes();
+  smem += (size_t)lb * Pol::ell_line_bytes();
   CUtensorMap map_hi, map_lo;
   int rc = tcg::make_weight_map(&map_hi, d.W_hi, d.num_layers * d.H, d.Kw, who);
   if (rc != LNB_OK) return rc;
   rc = tcg::make_weight_map(&map_lo, d.W_lo, d.num_layers * d.H, d.Kw, who);
   if (rc != LNB_OK) return rc;
-  auto kern = tcg::tc_gemm_kernel<SpectralPolicy>;
+  auto kern = tcg::tc_gemm_kernel<Pol>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  SpectralPolicy::Params p{};
+  typename Pol::Params p{};
   p.X = d.X; p.node_ids = d.node_ids; p.emb = d.emb_table; p.Q = d.Q;
   p.coeff = d.coeff; p.coeff_stride = d.coeff_layer_stride;
   p.ell_val = d.ell_val; p.ell_idx = d.ell_idx; p.ell_max = d.ell_max; p.gext = d.gext; p.tiles = d.tiles;
@@ -1209,9 +1318,23 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
   return lnb::finish_launch(who);
 }
 
+}  // extern "C++"
+
 int lnb_spectral_stack_forward(lnb_stream_t stream, const lnb_spectral_stack* desc) {
   LNB_REQUIRE(desc, "spectral_stack_forward: null descriptor");
-  return launch_stack(stream, *desc, "spectral_stack_forward");
+  return launch_stack<SpectralPolicy>(stream, *desc, "spectral_stack_forward");
+}
+
+int lnb_sage_stack_forward(lnb_stream_t stream, const lnb_spectral_stack* desc, int flags) {
+  LNB_REQUIRE(desc, "sage_stack_forward: null descriptor");
+  LNB_REQUIRE((flags & ~LNB_SAGE_MAX) == 0, "sage_stack_forward: unknown flags %d", flags);
+  if (desc->S != 0) {
+    lnb::set_err("sage_stack_forward: S=%d, the GraphSAGE stack has no long scales (S must be 0)", desc->S);
+    return LNB_ERR_UNSUPPORTED;
+  }
+  if (flags & LNB_SAGE_MAX)
+    return launch_stack<SpectralPolicyT<STACK_SAGE_MAX>>(stream, *desc, "sage_stack_forward");
+  return launch_stack<SpectralPolicyT<STACK_SAGE_MEAN>>(stream, *desc, "sage_stack_forward");
 }
 
 int lnb_spectral_conv_fused(lnb_stream_t stream, const float* X, const float* Q, const float* coeff,
@@ -1225,7 +1348,7 @@ int lnb_spectral_conv_fused(lnb_stream_t stream, const float* X, const float* Q,
   d.W_hi = W_hi; d.W_lo = W_lo; d.Kw = (S + E1) * Din; d.bias = bias;
   d.Din[0] = Din; d.num_layers = 1; d.out_state = out; d.write_pad = write_pad;
   d.B = B; d.N = N; d.E1 = E1; d.K = K; d.S = S; d.H = H; d.relu = relu;
-  return launch_stack(stream, d, "spectral_conv_fused");
+  return launch_stack<SpectralPolicy>(stream, d, "spectral_conv_fused");
 }
 
 }  // extern "C"

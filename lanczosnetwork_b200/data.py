@@ -18,7 +18,7 @@ import numpy as np
 
 __all__ = [
     'check_dist', 'get_laplacian', 'get_graph_laplacian_eigs', 'prepare_graph',
-    'collate', 'gat_bias', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
+    'collate', 'gat_bias', 'sage_collate', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
     'synthetic_regression_graphs',
 ]
 
@@ -132,6 +132,42 @@ def gat_bias(L):
   mt = L.astype(np.float64) + np.eye(N)[None, :, :, None]      # I @ (adj + I) is exact
   mt[mt > 0.0] = 1.0
   return (-1e9 * (1.0 - mt)).astype(np.float32)
+
+
+def sage_collate(samples, num_sample_neighbors, npr):
+  """The GraphSAGE branch of the reference collate (dataset/qm8.py:57-90,137-166): the same
+  ``npr.choice`` calls in the same order (graph, then channel -- simple graph first, then the bond
+  types --, then node), so the same ``np.random.RandomState`` gives an identical batch.  A node with
+  at least K neighbours draws K of them without replacement, one with fewer draws K with replacement,
+  one without any keeps the zero fill (node 0); ``nonempty`` is 1 once any channel has a neighbour.
+
+  Returns numpy arrays: node_feat (B,N) int64, node_mask (B,N) uint8, nn_idx (B,N,K,E+1) int64,
+  nonempty_mask (B,N,1) float32, label (B,P) float32 if present."""
+  K = int(num_sample_neighbors)
+  sizes = np.array([s['L_simple_4'].shape[0] for s in samples])
+  B, N = len(samples), int(sizes.max())
+  E = samples[0]['L_multi'].shape[2]
+  node_feat = np.zeros((B, N), np.int64)
+  nonempty = np.zeros((B, N, 1))
+  nn_idx = np.zeros((B, N, K, E + 1))
+  for ii, s in enumerate(samples):
+    node_feat[ii, :sizes[ii]] = s['node_feat']
+    for jj in range(E + 1):
+      tmp_L = s['L_simple_4'] if jj == 0 else s['L_multi'][:, :, jj - 1]
+      for nn in range(tmp_L.shape[0]):
+        nn_list = np.nonzero(tmp_L[nn, :])[0]
+        if len(nn_list) >= K:
+          nn_idx[ii, nn, :, jj] = npr.choice(nn_list, size=K, replace=False)
+          nonempty[ii, nn] = 1
+        elif len(nn_list) > 0:
+          nn_idx[ii, nn, :, jj] = npr.choice(nn_list, size=K, replace=True)
+          nonempty[ii, nn] = 1
+  out = {'node_feat': node_feat, 'node_mask': (np.arange(N)[None, :] < sizes[:, None]).astype(np.uint8),
+         'nn_idx': nn_idx.astype(np.int64), 'nonempty_mask': nonempty.astype(np.float32)}
+  if 'label' in samples[0]:
+    out['label'] = np.concatenate([np.asarray(s['label'], np.float32).reshape(1, -1)
+                                   for s in samples], axis=0)
+  return out
 
 
 def sparse_collate(samples, num_eigs):

@@ -6,7 +6,7 @@ What it does (see INTEGRATION.md):
   1. registers ``operators._ext`` / ``operators._ext.segment_reduction`` in ``sys.modules`` so
      ``from model import *`` of the reference works without building its THC-era extension
      (model/mpnn.py:6 -> operators/functions/unsorted_segment_sum.py:5);
-  2. rebinds the classes of ``DROPIN_CLASSES`` (``LanczosNet``, ``AdaLanczosNet``, ``GCN``, ``GAT``, ...)
+  2. rebinds the classes of ``DROPIN_CLASSES`` (``LanczosNet``, ``AdaLanczosNet``, ``GCN``, ``GAT``, ``GraphSAGE``, ...)
      inside the runner modules' globals, because the runners resolve the class with ``eval(name)`` in their own
      namespace (runner/qm8_runner.py:59,288; runner/graph_runner.py:57,285);
   3. runs the reference ``run_exp.main()`` unchanged.
@@ -19,7 +19,7 @@ from . import model as _models
 from .operators import _ext as _ext_pkg
 
 DROPIN_CLASSES = ('LanczosNet', 'AdaLanczosNet', 'LanczosNetGeneral', 'GCN', 'GCNFP', 'DCNN', 'ChebyNet',
-                  'GAT')
+                  'GAT', 'GraphSAGE')
 
 
 def register_native_op():

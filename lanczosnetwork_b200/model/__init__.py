@@ -7,3 +7,4 @@ from .gcn import *                  # noqa: F401,F403  (SURVEY 8f3: sibling mode
 from .dcnn import *                 # noqa: F401,F403
 from .cheby_net import *            # noqa: F401,F403
 from .gat import *                  # noqa: F401,F403  (inference only)
+from .graph_sage import *        # noqa: F401,F403  (Mean / Max aggregators)

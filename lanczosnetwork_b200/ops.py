@@ -14,7 +14,7 @@ from ._lib import GemmDesc, SpectralStack
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
-    'gat_attention', 'gat_attention_supported',
+    'gat_attention', 'gat_attention_supported', 'sage_operators', 'neighbour_max',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
     'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
@@ -322,15 +322,54 @@ def spectral_conv_fused(X, Q, coeff, prep, w_hi, w_lo, bias, relu=True, write_pa
   return out
 
 
+def sage_operators(nn_idx, nonempty):
+  """GraphSAGE's count-weighted operators (lnb_sage_operators): nn_idx [B,N,K,E1] int64 neighbour
+  samples, nonempty [B,N] or [B,N,1] -> M [B,N,N,E1] fp32 with M[b,n,m,e] = nonempty * count / K."""
+  _need_cuda(nn_idx, nonempty)
+  nn_idx = nn_idx.contiguous().long()
+  nonempty = _f32c(nonempty)
+  B, N, K, E1 = nn_idx.shape
+  if nonempty.numel() != B * N:
+    raise ValueError('sage_operators: nonempty %s does not match nn_idx %s'
+                     % (tuple(nonempty.shape), tuple(nn_idx.shape)))
+  out = torch.empty((B, N, N, E1), device=nn_idx.device, dtype=torch.float32)
+  with torch.cuda.device(nn_idx.device):
+    _lib.check(_lib.load().lnb_sage_operators(_stream(nn_idx), _ptr(nn_idx), _ptr(nonempty), B, N, K, E1,
+                                              _ptr(out)), 'lnb_sage_operators')
+  return out
+
+
+def neighbour_max(X, prep):
+  """Max messages of GraphSAGE (lnb_neighbour_max): X [B,N,D], prep = graph_prepare(M, ...) ->
+  (msg [B,N,E1*D] channel-major, argmax [B,N,E1,D] int32 node index, -1 for empty rows)."""
+  ell_val, ell_idx, ell_max = prep[0], prep[1], prep[2]
+  _need_cuda(X, ell_val)
+  X = _f32c(X)
+  B, N, D = X.shape
+  E1 = ell_val.shape[1]
+  out = torch.empty((B, N, E1 * D), device=X.device, dtype=torch.float32)
+  arg = torch.empty((B, N, E1, D), device=X.device, dtype=torch.int32)
+  with torch.cuda.device(X.device):
+    _lib.check(_lib.load().lnb_neighbour_max(_stream(X), _ptr(X), _ptr(ell_val), _ptr(ell_idx),
+                                             _ptr(ell_max), B, N, E1, D, _ptr(out), _ptr(arg)),
+               'lnb_neighbour_max')
+  return out, arg
+
+
+SAGE_MAX = 1        # LNB_SAGE_MAX
+
+
 def spectral_stack_forward(prep, Q, w_hi, w_lo, bias, dins, H, S, coeff=None, coeff_stride=0,
                            X=None, node_ids=None, emb=None, want_state=False, write_pad=True,
-                           readout=None, mask=None, relu=True):
+                           readout=None, mask=None, relu=True, sage=None):
   """All convolution layers (+ optional embedding gather and readout) in one persistent kernel.
 
   prep = graph_prepare(L, Q); w_hi/w_lo [len(dins)*H, Kw] stacked split weights, bias
   [len(dins)*H]; dins = input width per layer; coeff = tensor whose layer l block starts at
   element l*coeff_stride (None when S == 0); X [B,N,dins[0]] or node_ids [B,N] + emb;
   readout = (W_out [P,H], b_out [P], w_att [H], b_att [1]) -> score [B,P].
+  sage = None runs lnb_spectral_stack_forward; 'Mean' / 'Max' run the GraphSAGE variant
+  (lnb_sage_stack_forward: rows L2-normalised after every layer, Max aggregation for 'Max').
   Returns (state or None, score or None)."""
   ell_val, ell_idx, ell_max, gext, tiles = prep
   _need_cuda(Q, w_hi, w_lo, bias, coeff, X, node_ids, emb, mask)
@@ -375,8 +414,15 @@ def spectral_stack_forward(prep, Q, w_hi, w_lo, bias, dins, H, S, coeff=None, co
   d.num_layers, d.Kw, d.write_pad = len(dins), int(w_hi.shape[1]), int(bool(write_pad))
   d.B, d.N, d.E1, d.K, d.S, d.H, d.relu = B, N, E1, K, int(S), int(H), int(bool(relu))
   with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_spectral_stack_forward(_stream(Q), ctypes.byref(d)),
-               'lnb_spectral_stack_forward')
+    if sage is None:
+      _lib.check(_lib.load().lnb_spectral_stack_forward(_stream(Q), ctypes.byref(d)),
+                 'lnb_spectral_stack_forward')
+    else:
+      if sage not in ('Mean', 'Max'):
+        raise ValueError('spectral_stack_forward: sage=%r (Mean or Max)' % (sage,))
+      _lib.check(_lib.load().lnb_sage_stack_forward(_stream(Q), ctypes.byref(d),
+                                                    SAGE_MAX if sage == 'Max' else 0),
+                 'lnb_sage_stack_forward')
   return state, score
 
 

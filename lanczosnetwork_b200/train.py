@@ -27,7 +27,8 @@ import torch
 from . import ops
 
 __all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
-           'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'GraphedStep']
+           'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
+           'GraphedStep']
 
 
 def _pad_cols(x, mult=4):
@@ -293,6 +294,57 @@ def cheby_train(model, node_ids, L, mask):
     msgs = ([operator_messages(L, state, 1, E1 - 1)] if E1 > 1 else []) + scale
     lin = model.filter[t]
     state = dense(torch.cat(msgs, dim=2).reshape(B * N, -1), lin.weight, lin.bias, True).reshape(B, N, -1)
+    if model.training and model.dropout > 0.0:
+      state = torch.nn.functional.dropout(state, model.dropout, True)
+  return gated_readout(model, state, mask)
+
+
+class _NeighbourMax(torch.autograd.Function):
+  """msg[b, n, e*D + f] = max over the neighbours m drawn for row n of channel e of X[b, m, f]: the Max
+  aggregator of model/graph_sage.py:141-146 (a row with nonempty = 0 gives 0).  ``prep`` is
+  ops.graph_prepare of the count-weighted operators (ops.sage_operators): their ELL rows list the
+  distinct neighbours drawn.  The gradient goes to the argmax node (ties: lowest index), scatter-added
+  per feature with the library's segment sum."""
+
+  @staticmethod
+  def forward(ctx, X, prep):
+    msg, arg = ops.neighbour_max(X, prep)
+    ctx.save_for_backward(arg)
+    ctx.dims = tuple(X.shape)
+    return msg
+
+  @staticmethod
+  def backward(ctx, g):
+    (arg,) = ctx.saved_tensors
+    B, N, D = ctx.dims
+    b = torch.arange(B, device=g.device).view(B, 1, 1, 1)
+    f = torch.arange(D, device=g.device).view(1, 1, 1, D)
+    seg = torch.where(arg >= 0, (b * N + arg.long()) * D + f, -1)       # -1: empty row, skipped
+    gx = ops.segment_sum_forward(g.reshape(1, -1, 1), seg.reshape(1, -1), B * N * D)
+    return gx.view(B, N, D), None
+
+
+def neighbour_max(X, prep):
+  return _NeighbourMax.apply(X.float(), prep)
+
+
+def sage_train(model, node_ids, M, mask, prep=None):
+  """Differentiable GraphSAGE (model/graph_sage.py:98-175): embedding -> num_layer - 1 layers of
+  [messages of every channel] -> Linear + ReLU -> row / (||row|| + eps) -> dropout -> gated readout
+  with the head filter[num_layer].  Mean messages are M_e X on the count-weighted operators M
+  [B,N,N,E1] (ops.sage_operators); Max messages come from ``neighbour_max`` on the ELL lists of M
+  (``prep``, built here when not given)."""
+  M = M.float().contiguous()
+  state = embedding(node_ids, model.embedding.weight)
+  B, N = state.shape[0], state.shape[1]
+  if model.agg_func_name == 'Max' and prep is None and model.num_layer > 1:
+    prep = ops.graph_prepare(M, torch.zeros((B, N, 4), device=M.device, dtype=torch.float32))
+  for t in range(model.num_layer - 1):
+    msg = neighbour_max(state, prep) if model.agg_func_name == 'Max' else operator_messages(M, state)
+    lin = model.filter[t]
+    y = dense(msg.reshape(B * N, -1), lin.weight, lin.bias, True)
+    y = y / (torch.norm(y, 2, dim=1, keepdim=True) + _EPS)
+    state = y.reshape(B, N, -1)
     if model.training and model.dropout > 0.0:
       state = torch.nn.functional.dropout(state, model.dropout, True)
   return gated_readout(model, state, mask)
