@@ -307,6 +307,28 @@ int lnb_gat_attention(lnb_stream_t stream, const float* Wh, const float* bias, c
                       int B, int N, int E1, int heads, int F, int last, float* out);
 
 /* ---------------------------------------------------------------------------------------
+ * GGNN propagation step after the message MLPs (model/ggnn.py:143-171), one persistent 3xTF32 wgmma
+ * launch over all B*N rows:
+ *   agg[b,n, e*D:(e+1)*D] = sum over the non-zeros m of row n of channel e of  w * M[b*N+m, e*D:(e+1)*D]
+ *                           w = 1 (avg == 0, 'sum') or 1 / (nnz + FLT_EPSILON) (avg != 0, 'avg')
+ *   G = [agg | h] W^T + bias;   r = sigmoid(G_r), z = sigmoid(G_z), n = tanh(G_nin + r * G_nh)
+ *   out = (h - n) * z + n                                                 (torch's GRUCell)
+ * The operators enter only through their non-zero pattern (A_e = L_e != 0, the reference's in-place
+ * binarisation): ell_* are the ELL rows of lnb_graph_prepare over L [B,N,N,E1].  The aggregated
+ * messages are computed in the producer warps of the GEMM and never written out.
+ * M [B*N, E1*D] (column block e = channel e), h and out [B*N, D] (out must not alias h).
+ * W_hi / W_lo: tf32 split of the re-laid-out gate matrix [4D, (E1+1)*D] whose row (u/4)*16 + g*4 + u%4
+ * is gate g of hidden unit u, g = r, z, n_in, n_h:  r = [W_ir | W_hr], z = [W_iz | W_hz],
+ * n_in = [W_in | 0], n_h = [0 | W_hn] (weight_ih / weight_hh of torch.nn.GRUCell); bias [4D] in the same
+ * order: b_ir + b_hr, b_iz + b_hz, b_in, b_hn.  M, h, out, W 16-byte aligned.
+ * Envelope: 1 <= N <= 255, D % 32 == 0, 32 <= D <= 128, 1 <= E1 <= 16 (LNB_ERR_UNSUPPORTED otherwise,
+ * nothing launched).  Summation order is fixed: repeated launches are bit-identical.
+ * ------------------------------------------------------------------------------------- */
+int lnb_ggnn_update(lnb_stream_t stream, const float* M, const float* h, const float* ell_val,
+                    const uint8_t* ell_idx, const int32_t* ell_max, const float* W_hi, const float* W_lo,
+                    const float* bias, int B, int N, int D, int E1, int avg, float* out);
+
+/* ---------------------------------------------------------------------------------------
  * Operator chain on channel 0 of L [B,N,N,E1], per graph, starting from X [B,N,D]:
  *   chebyshev == 0: w_s = L_0 w_{s-1} (w_0 = X), s = 1..steps   (model/dcnn.py:88-92, the short
  *                   diffusion walk of model/lanczos_net.py:164-169);

@@ -19,7 +19,7 @@ from . import model as _models
 from .operators import _ext as _ext_pkg
 
 DROPIN_CLASSES = ('LanczosNet', 'AdaLanczosNet', 'LanczosNetGeneral', 'GCN', 'GCNFP', 'DCNN', 'ChebyNet',
-                  'GAT', 'GraphSAGE')
+                  'GAT', 'GraphSAGE', 'GGNN')
 
 
 def register_native_op():

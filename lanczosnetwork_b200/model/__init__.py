@@ -8,3 +8,4 @@ from .dcnn import *                 # noqa: F401,F403
 from .cheby_net import *            # noqa: F401,F403
 from .gat import *                  # noqa: F401,F403  (inference only)
 from .graph_sage import *        # noqa: F401,F403  (Mean / Max aggregators)
+from .ggnn import *              # noqa: F401,F403

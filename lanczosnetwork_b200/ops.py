@@ -14,7 +14,8 @@ from ._lib import GemmDesc, SpectralStack
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
-    'gat_attention', 'gat_attention_supported', 'sage_operators', 'neighbour_max',
+    'gat_attention', 'gat_attention_supported', 'sage_operators', 'neighbour_max', 'ggnn_update',
+    'ggnn_update_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
     'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
@@ -518,6 +519,35 @@ def gat_attention(Wh, bias, a1, a2, c1, c2, state_bias, last=False):
     _lib.check(_lib.load().lnb_gat_attention(
         _stream(Wh), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
         B, N, E1, heads, F, int(bool(last)), _ptr(out)), 'lnb_gat_attention')
+  return out
+
+
+def ggnn_update_supported(N, D, E1):
+  """Shapes lnb_ggnn_update accepts (mirrors its checks)."""
+  return 1 <= N <= 255 and D % 32 == 0 and 32 <= D <= 128 and 1 <= E1 <= 16
+
+
+def ggnn_update(M, h, prep, w_hi, w_lo, bias, avg, out=None):
+  """One GGNN propagation step after the message MLPs (see lnb_ggnn_update): the GRU cell of
+  [A_0 M_0 | ... | A_{E1-1} M_{E1-1} | h] with A_e the 0/1 pattern of channel e (row-normalised when
+  ``avg``), gathered through the ELL rows of ``prep`` (graph_prepare of the operators [B,N,N,E1]).
+  M [B*N, E1*D], h [B*N, D]; w_hi / w_lo / bias: the re-laid-out gate matrix [4D, (E1+1)*D] and its
+  bias [4D] (model.ggnn.gru_gate_matrix).  Returns h' [B*N, D] (written to ``out`` when given)."""
+  _need_cuda(M, h, w_hi, w_lo, bias, out)
+  M, h, bias = _f32c(M), _f32c(h), _f32c(bias)
+  ell_val, ell_idx, ell_max = prep[0], prep[1], prep[2]
+  B, E1, N = ell_val.shape[0], ell_val.shape[1], ell_val.shape[2]
+  D = h.shape[1]
+  if (tuple(h.shape) != (B * N, D) or tuple(M.shape) != (B * N, E1 * D) or
+      tuple(w_hi.shape) != (4 * D, (E1 + 1) * D) or tuple(bias.shape) != (4 * D,)):
+    raise ValueError('ggnn_update: M %s, h %s, W %s, bias %s do not agree with B=%d N=%d E1=%d'
+                     % (tuple(M.shape), tuple(h.shape), tuple(w_hi.shape), tuple(bias.shape), B, N, E1))
+  if out is None:
+    out = torch.empty_like(h)
+  with torch.cuda.device(h.device):
+    _lib.check(_lib.load().lnb_ggnn_update(
+        _stream(h), _ptr(M), _ptr(h), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi), _ptr(w_lo),
+        _ptr(bias), B, N, D, E1, int(bool(avg)), _ptr(out)), 'lnb_ggnn_update')
   return out
 
 

@@ -113,6 +113,12 @@ class WeightCache(object):
       return ops.split_tf32(cat) if split else (cat,)
     return self._get((name, parts[0].device.index), tag, build, list(parts))
 
+  def derived(self, name, sources, build):
+    """Tensors ``build()`` computes from the parameters ``sources`` (e.g. a re-laid-out weight matrix
+    and its tf32 split), rebuilt when any source changes; returns build()'s tuple."""
+    tag = tuple((t.data_ptr(), t._version) for t in sources)
+    return self._get((name, sources[0].device.index), tag, build, list(sources))
+
   def clear(self):
     self.invalidate()
 

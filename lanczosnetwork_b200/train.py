@@ -28,7 +28,7 @@ from . import ops
 
 __all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
            'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
-           'GraphedStep']
+           'ggnn_train', 'GraphedStep']
 
 
 def _pad_cols(x, mult=4):
@@ -241,11 +241,14 @@ def ritz_stack_train(model, state, node_ids, L, D, V, mask):
   return gated_readout(model, state, mask)
 
 
-def gated_readout(model, state, mask):
+def gated_readout(model, state, mask, head=None):
   """Gated masked-mean readout shared by all models (lanczos_net.py:185-194): the two Linears in the
-  library's dense kernel, the pointwise gate / mean on the autograd tape."""
+  library's dense kernel, the pointwise gate / mean on the autograd tape.  ``head`` is the output
+  Linear, by default ``model.filter[model.num_layer]`` (GGNN passes its ``output_func[0]``)."""
   B, N = state.shape[0], state.shape[1]
-  head, att = model.filter[model.num_layer], model.att_func[0]
+  if head is None:
+    head = model.filter[model.num_layer]
+  att = model.att_func[0]
   flat = state.reshape(B * N, -1)
   y = dense(flat, head.weight, head.bias, False).reshape(B, N, -1)
   gate = torch.sigmoid(dense(flat, att.weight, att.bias, False)).reshape(B, N, 1)
@@ -348,6 +351,50 @@ def sage_train(model, node_ids, M, mask, prep=None):
     if model.training and model.dropout > 0.0:
       state = torch.nn.functional.dropout(state, model.dropout, True)
   return gated_readout(model, state, mask)
+
+
+def ggnn_train(model, node_ids, L, mask):
+  """Differentiable GGNN (model/ggnn.py:122-197): embedding -> input_func -> num_prop steps of
+  [per-channel message MLP -> A_e m_e -> GRU / RNN cell -> dropout] -> gated readout with the head
+  ``output_func``.  A_e is the 0/1 pattern of L_e, row-normalised by (nnz + float32 eps) for ``avg``;
+  both are new tensors (the caller's L is not modified).  The first message layers of all channels run
+  as one dense layer against their weights concatenated on the tape."""
+  A = (L != 0).float()
+  if model.aggregate_type == 'avg':
+    A = A / (A.sum(dim=2, keepdim=True) + _EPS)
+  A = A.contiguous()
+  B, N, E1 = A.shape[0], A.shape[1], A.shape[3]
+  x = embedding(node_ids, model.embedding.weight).reshape(B * N, -1)
+  lin = model.input_func[0]
+  h = dense(x, lin.weight, lin.bias, False)
+  D = h.shape[1]
+  first = [seq[0] for seq in model.msg_func]
+  w1 = torch.cat([l.weight for l in first], dim=0)
+  b1 = torch.cat([l.bias for l in first], dim=0)
+  hw = first[0].weight.shape[0]
+  cell = model.update_func
+  for _ in range(model.num_prop):
+    hid = dense(h, w1, b1, True)                                               # [B*N, E1 * 128]
+    agg = []
+    for e in range(E1):
+      second = model.msg_func[e][2]
+      m_e = dense(hid[:, e * hw:(e + 1) * hw], second.weight, second.bias, False)
+      agg.append(operator_messages(A, m_e.reshape(B, N, D), e, 1))
+    agg = torch.cat(agg, dim=2).reshape(B * N, E1 * D)
+    gi = dense(agg, cell.weight_ih, cell.bias_ih, False)
+    gh = dense(h, cell.weight_hh, cell.bias_hh, False)
+    if model.update_func_name == 'GRU':                                        # torch's GRUCell
+      i_r, i_z, i_n = gi.chunk(3, dim=1)
+      h_r, h_z, h_n = gh.chunk(3, dim=1)
+      r = torch.sigmoid(i_r + h_r)
+      z = torch.sigmoid(i_z + h_z)
+      n = torch.tanh(i_n + r * h_n)
+      h = (h - n) * z + n
+    else:                                                                      # RNNCell, relu
+      h = torch.relu(gi + gh)
+    if model.training and model.dropout > 0.0:
+      h = torch.nn.functional.dropout(h, model.dropout, True)
+  return gated_readout(model, h.reshape(B, N, D), mask, head=model.output_func[0])
 
 
 class _BMM(torch.autograd.Function):
