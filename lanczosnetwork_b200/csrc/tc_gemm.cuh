@@ -14,8 +14,8 @@
 // leaves 168 registers per thread for the 128 accumulator registers of a consumer):
 //   warps 0-3       producers (thread r <-> tile row r), then epilogue (Policy::store)
 //   warps 4-11      two consumer warpgroups: warpgroup c owns tile rows [64 c, 64 c + 64) and
-//                   keeps [D_main | D_corr] (64 x 256 fp32) in registers; per k-step one
-//                   m64n256k8 wgmma against [W_hi ; W_lo] and one m64n128k8 for A_lo * W_hi.
+//                   keeps D_main and D_corr (64 x 128 fp32 each) in registers; per k-step three
+//                   m64n128k8 wgmma: A_hi W_hi -> D_main, A_hi W_lo -> D_corr, A_lo W_hi -> D_corr.
 //                   One lane of warp 4 also issues the W tile loads (TMA), kStagesB k-blocks ahead.
 // The accumulators reach the epilogue through shared memory: once a step's last k-block is
 // multiplied the A ring is dead, and the consumers drain [D_main + D_corr] into it in column
@@ -288,11 +288,12 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
           sm90::wgmma_fence();
 #pragma unroll
           for (int k = 0; k < BK / 8; ++k) {
-            // [D_main | D_corr] += A_hi [W_hi ; W_lo]^T (N = 256),  D_corr += A_lo W_hi^T
-            sm90::wgmma_n256(d, sm90::wgmma_desc_kmajor_sw128(a_hi + 32 * k),
-                             sm90::wgmma_desc_kmajor_sw128(b + 32 * k), (kb | k) != 0 ? 1u : 0u);
-            sm90::wgmma_n128_hi(d, sm90::wgmma_desc_kmajor_sw128(a_lo + 32 * k),
-                                sm90::wgmma_desc_kmajor_sw128(b + 32 * k), 1u);
+            const uint64_t ah = sm90::wgmma_desc_kmajor_sw128(a_hi + 32 * k);
+            const uint64_t wh = sm90::wgmma_desc_kmajor_sw128(b + 32 * k);
+            const uint32_t acc = (kb | k) != 0 ? 1u : 0u;
+            sm90::wgmma_n128(d, ah, wh, acc);                                                  // D_main += A_hi W_hi^T
+            sm90::wgmma_n128_hi(d, ah, sm90::wgmma_desc_kmajor_sw128(b + TILE_B_BYTES + 32 * k), acc);  // D_corr += A_hi W_lo^T
+            sm90::wgmma_n128_hi(d, sm90::wgmma_desc_kmajor_sw128(a_lo + 32 * k), wh, 1u);     // D_corr += A_lo W_hi^T
           }
           sm90::wgmma_commit();
           sm90::wgmma_wait_all();
