@@ -13,11 +13,13 @@
 // Dropping exact zeros is exact, so the result equals the dense reference for arbitrary inputs.
 //
 // Two accumulator lifetimes ("steps") per tile:
-//   step 0  Z = sum_s (f_s . U) W_s^T      rows = (graph, Ritz index): the producer only scales
-//           rows of U_g = V_g^T X_g (shared memory) by the filter coefficient; Z is drained to
-//           shared memory;
+//   step 0  Z = sum_s (f_s . U) W_s^T      rows = (graph, Ritz index), k-blocks d-block-major: at
+//           the first k-block of a d-block the producer thread of row (g, k) computes its 32
+//           columns of U_g = V_g^T X_g into registers, then scales them by f_s for every s; Z is
+//           drained into the A ring and stays there;
 //   step 1  E = sum_e (L_e X) W_e^T        rows = (graph, node): sparse ELL rows of the operators
-//           times X; epilogue: out = act(E + V Z + b), written back as full 512-byte rows.
+//           times X, accumulated on top of V Z, which the consumers compute from the Z in the A
+//           ring before the first MMA; epilogue: out = act(acc + b).
 // Algebra: sum_s V diag(f_s) V^T X W_s^T = V [ sum_s diag(f_s) (V^T X) W_s^T ].
 #include "tc_gemm.cuh"
 
@@ -500,8 +502,9 @@ template <int kVariant>
 struct SpectralPolicyT {
   static constexpr bool kNormRows = kVariant != STACK_PLAIN;
   static constexpr bool kMaxAgg = kVariant == STACK_SAGE_MAX;
-  static constexpr int kStagesB = 1;      // one W stage and one A stage: shared memory goes to the packed tile
-  static constexpr int kStagesA = 1;
+  static constexpr bool kLongScales = kVariant == STACK_PLAIN;    // GraphSAGE runs S = 0: no step 0
+  static constexpr int kStagesB = 2;      // k-block i + 1 is produced and its W tile loaded during MMA i
+  static constexpr int kStagesA = 2;      // 64 KB: also holds Z (Ztot <= 128 rows x H <= 128) in one pass
   static constexpr int LMAX = 8;          // layers run by one launch
   struct Params {
     const float* X;         // [B, N, Din0] input state, or nullptr with node_ids/emb (embedding)
@@ -553,13 +556,19 @@ struct SpectralPolicyT {
   static __device__ __forceinline__ int num_kblocks(const Params& p, int sub) {
     return ((sub & 1) == 0 ? p.S : p.E1) * p.Din[sub >> 1] / tcg::BK;
   }
+  // step 0 runs its k-blocks d-block-major (kb = dblk * S + s), so one U block serves S k-blocks
   static __device__ __forceinline__ void w_coords(const Params& p, int sub, int kb, int& col0, int& row0) {
-    col0 = ((sub & 1) == 0 ? 0 : p.S * p.Din[sub >> 1]) + kb * tcg::BK;
+    const int Din = p.Din[sub >> 1];
+    col0 = (sub & 1) == 0 ? (kb % p.S) * Din + (kb / p.S) * tcg::BK : p.S * Din + kb * tcg::BK;
     row0 = (sub >> 1) * p.H;
   }
+  // Z of step 0 stays in the A ring for the edge step's acc_init()
+  static __device__ __forceinline__ bool drain_kept(const Params&, int sub) { return kLongScales && (sub & 1) == 0; }
+  // row pitch (floats) of the X rows in shared memory
+  static __host__ __device__ __forceinline__ int x_pitch(int Din0, int H) { return (Din0 > H ? Din0 : H) + 4; }
 
   // Row tables of the tile being run.  Node rows: graph after graph, n_eff rows each; Ritz rows
-  // (Z, U): graph after graph, k_eff rows each (unpadded); quads: groups of 4 rows of one graph.
+  // (Z): graph after graph, k_eff rows each (unpadded); quads: groups of 4 rows of one graph.
   struct Tables {
     int ng, Rtot, Ztot, nquads, nzquads, nlines;
     int gid[GMAX];                                  // graph ids of the tile's graphs
@@ -576,40 +585,35 @@ struct SpectralPolicyT {
   const int tid, r;
   const int N, K, S, E1, H, XP;           // hot parameters in registers
   int Din;                                // input width of the current layer
-  // Shared memory, in this order.  Tables comes first so that everything behind Xs is one
-  // contiguous region that is dead after the last layer's epilogue (the fused readout's scratch).
+  // Shared memory, in this order (acc_init() finds Tables and Qs the same way)
   Tables* tb;
-  float* Xs;                // X rows [RMAX][XP]; reused for V Z + the finished output rows
-  float* UZ;                // U rows (graph,k) [RMAX][XP] during step 0, Z afterwards
+  float* Xs;                // X rows [RMAX][XP]; the finished output rows are the next layer's X
   float* Qs;                // [RMAX][K]
   float* Ev;                // [LB][RMAX] staged ELL values
   uint8_t* Ei;              // [LB][RMAX] staged ELL columns as tile-local row indices
   float fr[FR];             // this (graph, k) row's filter coefficients f[k, 0..S)
+  float u[tcg::BK];         // step 0: this (graph, k) row's U columns of the current d-block
+  float* ring;              // the skeleton's A ring: the fused readout's scratch
   tcg::PhaseTimer* ptm = nullptr;   // profiling aid: the current step's timer
 
   static __host__ __device__ constexpr size_t tables_bytes() { return (sizeof(Tables) + 15) & ~size_t(15); }
 
   __device__ SpectralPolicyT(const Params& p_, uint8_t* smem, int tid_)
       : p(p_), tid(tid_), r(tid_ & 127), N(p_.N), K(p_.K), S(p_.S), E1(p_.E1),
-        H(p_.H), XP((p_.Din[0] > p_.H ? p_.Din[0] : p_.H) + 4), Din(p_.Din[0]) {
+        H(p_.H), XP(x_pitch(p_.Din[0], p_.H)), Din(p_.Din[0]) {
     tb = reinterpret_cast<Tables*>(smem);
     Xs = reinterpret_cast<float*>(smem + tables_bytes());
-    UZ = Xs + (size_t)RMAX * XP;
-    Qs = UZ + (size_t)RMAX * XP;
+    Qs = Xs + (size_t)RMAX * XP;
     Ev = Qs + (size_t)RMAX * K;
     Ei = reinterpret_cast<uint8_t*>(Ev + (size_t)p.LB * RMAX);
+    ring = reinterpret_cast<float*>(tcg::a_ring(smem, kStagesB, kStagesA));
   }
   static size_t smem_fixed(int Din, int K, int H) {
-    const int W = (Din > H ? Din : H) + 4;
-    return (size_t)2 * RMAX * W * 4 + (size_t)RMAX * K * 4 + tables_bytes() + 16;
+    return (size_t)RMAX * x_pitch(Din, H) * 4 + (size_t)RMAX * K * 4 + tables_bytes() + 16;
   }
   static size_t ell_line_bytes() { return (size_t)RMAX * 5; }
-  // UZ, Qs, Ev and Ei: free once the last layer's output rows are in Xs
-  static size_t dead_bytes(int Din, int K, int H, int lb) {
-    const int W = (Din > H ? Din : H) + 4;
-    return (size_t)RMAX * (W + K) * 4 + (size_t)lb * ell_line_bytes();
-  }
-  // scratch of readout(), laid out from UZ: Wr, Yr, cx and the node masks of up to GMAX graphs
+  // scratch of readout(), laid out from the start of the A ring: Wr, Yr, cx and the node masks of
+  // up to GMAX graphs
   static size_t readout_bytes(int H, int P, int N) {
     const size_t P1 = (size_t)P + 1, PQ = (P1 + 3) / 4, yr = (RMAX + 1) * P1;
     return (4 * PQ * (H + 4) + yr + ((4 - (yr & 3)) & 3) + H) * 4 + (size_t)GMAX * N;
@@ -765,65 +769,48 @@ struct SpectralPolicyT {
     sm90::cp_async_wait_all();
     tcg::producers_sync();
     tm.lap(1);
-    if (S == 0) return;
-    // ---- phase B: U_g = Q_g^T X_g in 4 x 4 register tiles over (graph,k) rows x columns -----
-    // (a quad's Q columns past k_eff are zero and its rows there are not stored: they belong to the
-    // next graph)
-    for (int task = tid; task < tb->nzquads * dv; task += tcg::PRODUCER_THREADS) {
-      const int dq = task % dv, zq = task / dv;
-      const int g = tb->zq_g[zq], k0 = tb->zq_k0[zq];
-      const int n_g = tb->gn[g], nb = tb->nbase[g], kr = tb->gk[g] - k0;
-      float acc[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-      const float* xs = Xs + (size_t)nb * XP + 4 * dq;
-      const float* qs = Qs + (size_t)nb * K + k0;
-#pragma unroll 4
-      for (int nn = 0; nn < n_g; ++nn) {
-        const float4 x4 = *reinterpret_cast<const float4*>(xs + (size_t)nn * XP);
-        const float4 q4 = *reinterpret_cast<const float4*>(qs + (size_t)nn * K);
-        const float qv[4] = {q4.x, q4.y, q4.z, q4.w};
-        const float xv[4] = {x4.x, x4.y, x4.z, x4.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(qv[i], xv[j], acc[i][j]);
-      }
-      float* ud = UZ + (size_t)(tb->kbase[g] + k0) * XP + 4 * dq;
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (i < kr)
-          *reinterpret_cast<float4*>(ud + (size_t)i * XP) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-    }
-    tcg::producers_sync();
-    tm.lap(2);
   }
 
   __device__ __forceinline__ void produce(int sub, int kb, float (&v)[32]) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = 0.f;
-    const int j0 = kb * tcg::BK;
-    const int c = j0 / Din, d0 = j0 - c * Din;
-    if ((sub & 1) == 0) {
-      // row = (graph, Ritz index): f[k, s] * U[row, d0:d0+32]
+    if (kLongScales && (sub & 1) == 0) {
+      // row = (graph, Ritz index): f[k, s] * U[row, d0:d0+32], kb = dblk * S + s
       if (r >= tb->Ztot) return;
+      const int s = kb % S;
+      if (s == 0) {
+        // U[(g, k), d0:d0+32] = sum_n Q_g[n, k] X_g[n, d0:d0+32]: every thread of graph g reads the
+        // same X row (a broadcast), consecutive Q entries
+        const int g = tb->z_g[r], n_g = tb->gn[g], nb = tb->nbase[g];
+        const float* xs = Xs + (size_t)nb * XP + (kb / S) * tcg::BK;
+        const float* qs = Qs + (size_t)nb * K + tb->z_k[r];
+#pragma unroll
+        for (int j = 0; j < tcg::BK; ++j) u[j] = 0.f;
+#pragma unroll 2
+        for (int n = 0; n < n_g; ++n) {
+          const float q = qs[(size_t)n * K];
+          const float4* x4 = reinterpret_cast<const float4*>(xs + (size_t)n * XP);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float4 t = x4[j];
+            u[4 * j + 0] = fmaf(q, t.x, u[4 * j + 0]); u[4 * j + 1] = fmaf(q, t.y, u[4 * j + 1]);
+            u[4 * j + 2] = fmaf(q, t.z, u[4 * j + 2]); u[4 * j + 3] = fmaf(q, t.w, u[4 * j + 3]);
+          }
+        }
+      }
       float f = 0.f;
       if (S <= FR) {
 #pragma unroll
-        for (int i = 0; i < FR; ++i) f = (i == c) ? fr[i] : f;
+        for (int i = 0; i < FR; ++i) f = (i == s) ? fr[i] : f;
       } else {
-        f = __ldg(p.coeff + (sub >> 1) * p.coeff_stride + ((int64_t)tb->gid[tb->z_g[r]] * K + tb->z_k[r]) * S + c);
+        f = __ldg(p.coeff + (sub >> 1) * p.coeff_stride + ((int64_t)tb->gid[tb->z_g[r]] * K + tb->z_k[r]) * S + s);
       }
-      const float4* u4 = reinterpret_cast<const float4*>(UZ + (size_t)r * XP + d0);
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 t = u4[q];
-        v[4 * q + 0] = f * t.x; v[4 * q + 1] = f * t.y; v[4 * q + 2] = f * t.z; v[4 * q + 3] = f * t.w;
-      }
+      for (int j = 0; j < tcg::BK; ++j) v[j] = f * u[j];
       return;
     }
+    const int j0 = kb * tcg::BK;
+    const int c = j0 / Din, d0 = j0 - c * Din;
     // edge type e = c: sparse row of L_e (ELL) times X[:, d0:d0+32]; row = (graph, node)
     if (r >= tb->Rtot) return;
     const int e = c;
@@ -952,81 +939,51 @@ struct SpectralPolicyT {
     return sqrtf(ss) + SAGE_EPS;
   }
 
-  // After the last k-block of the edge step: (V Z)[row, :] for every real row in 4 x 4 register
-  // tiles into the (now dead) X buffer; overlaps with the tensor core draining its queue.
+  // The edge step's store() overwrites rows of X that other producers may still be reading.
   __device__ void pre_epilogue(int sub) {
     if ((sub & 1) == 0) return;
     tcg::producers_sync();              // every producer is done reading X
     if (ptm) ptm->lap(22);              // (profiling) wait for the slowest producer group
-    if (S == 0) return;
-    const int hv = H / 4;
-    for (int task = tid; task < tb->nquads * hv; task += tcg::PRODUCER_THREADS) {
-      const int hq = task % hv, q = task / hv;
-      const int g = tb->q_g[q], n0 = tb->q_n0[q];
-      const int n_g = tb->gn[g], k_g = tb->gk[g];
-      const int r0 = tb->nbase[g] + n0;
-      float acc[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-      const float* z = UZ + (size_t)tb->kbase[g] * XP + 4 * hq;
-      const float* q0 = Qs + (size_t)r0 * K;
-      const int r1 = (n0 + 1 < n_g) ? 1 : 0, r2 = (n0 + 2 < n_g) ? 2 : 0, r3 = (n0 + 3 < n_g) ? 3 : 0;
-      // four Ritz indices per trip, then the k_eff % 4 last ones: Z rows from k_eff on belong to the
-      // next graph (or lie past Ztot), so none is read
-      int k = 0;
-      for (; k + 4 <= k_g; k += 4) {
-        const float4 a0 = *reinterpret_cast<const float4*>(q0 + k);
-        const float4 a1 = *reinterpret_cast<const float4*>(q0 + r1 * K + k);
-        const float4 a2 = *reinterpret_cast<const float4*>(q0 + r2 * K + k);
-        const float4 a3 = *reinterpret_cast<const float4*>(q0 + r3 * K + k);
-        const float av[4][4] = {{a0.x, a0.y, a0.z, a0.w}, {a1.x, a1.y, a1.z, a1.w},
-                                {a2.x, a2.y, a2.z, a2.w}, {a3.x, a3.y, a3.z, a3.w}};
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const float4 z4 = *reinterpret_cast<const float4*>(z + (size_t)(k + kk) * XP);
-          const float zv[4] = {z4.x, z4.y, z4.z, z4.w};
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i][kk], zv[j], acc[i][j]);
-        }
-      }
-      for (; k < k_g; ++k) {
-        const float av[4] = {q0[k], q0[r1 * K + k], q0[r2 * K + k], q0[r3 * K + k]};
-        const float4 z4 = *reinterpret_cast<const float4*>(z + (size_t)k * XP);
-        const float zv[4] = {z4.x, z4.y, z4.z, z4.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], zv[j], acc[i][j]);
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (n0 + i < n_g)
-          *reinterpret_cast<float4*>(Xs + (size_t)(r0 + i) * XP + 4 * hq) =
-              make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-    }
-    tcg::producers_sync();
   }
 
-  // Rows of UZ and Xs are XP = max(Din0, H) + 4 floats long, which a 16-column chunk can overrun
-  // when H % 16 != 0: only the float4 pieces below column H are written (H % 4 == 0, so a piece
-  // is either wholly inside the row or wholly outside it).
-  __device__ __forceinline__ void store(int sub, int col, float (&x)[tcg::EW]) {
-    if (col >= H) return;
-    if ((sub & 1) == 0) {
-      // drain Z[row, col:col+16] to shared memory (overwrites U, which is dead by now)
-      if (r < tb->Ztot) {
-        float4* z4 = reinterpret_cast<float4*>(UZ + (size_t)r * XP + col);
+  // Consumers, before the first MMA of an edge step: D_main = (V Z) for the rows of this thread's
+  // fragment (Z of the layer, left in the A ring by step 0's drain: row (graph, k), swizzled like
+  // any drain pass), D_corr = 0.  Reads the tile's Tables and Qs, which the producers staged
+  // before they produced step 0.
+  static __device__ __forceinline__ bool acc_init(const Params& p, const uint8_t* smem, const float* zr,
+                                                  int sub, int row0, int cl, float (&d)[128]) {
+    if (!kLongScales || (sub & 1) == 0 || p.S == 0) return false;
+    const Tables* tb = reinterpret_cast<const Tables*>(smem);
+    const int K = p.K;
+    const float* Qs = reinterpret_cast<const float*>(smem + tables_bytes()) + (size_t)RMAX * x_pitch(p.Din[0], p.H);
+    const int Rtot = tb->Rtot;
 #pragma unroll
-        for (int q = 0; q < tcg::EW / 4; ++q)
-          if (col + 4 * q < H) z4[q] = make_float4(x[4 * q + 0], x[4 * q + 1], x[4 * q + 2], x[4 * q + 3]);
+    for (int i = 0; i < 128; ++i) d[i] = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      if (row >= Rtot) continue;
+      const int g = tb->row_g[row], k_g = tb->gk[g], zb = tb->kbase[g];
+      const float* q = Qs + (size_t)row * K;
+      // Ritz index order, like the reference's V (Z): rows past k_eff belong to the next graph
+      for (int k = 0; k < k_g; ++k) {
+        const float a = q[k];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float2 t = *reinterpret_cast<const float2*>(zr + tcg::stg_index(zb + k, 8 * j + cl, tcg::BN));
+          d[4 * j + 2 * h] = fmaf(a, t.x, d[4 * j + 2 * h]);
+          d[4 * j + 2 * h + 1] = fmaf(a, t.y, d[4 * j + 2 * h + 1]);
+        }
       }
-      return;
     }
-    if (r >= tb->Rtot) return;
+    return true;
+  }
+
+  // Edge steps only (step 0's drain is kept).  Rows of Xs are XP = max(Din0, H) + 4 floats long,
+  // which a 16-column chunk can overrun when H % 16 != 0: only the float4 pieces below column H are
+  // written (H % 4 == 0, so a piece is either wholly inside the row or wholly outside it).
+  __device__ __forceinline__ void store(int sub, int col, float (&x)[tcg::EW]) {
+    if (col >= H || r >= tb->Rtot) return;
     float4* o4 = reinterpret_cast<float4*>(Xs + (size_t)r * XP + col);
     const bool relu = p.relu != 0;
     const float* bias = p.bias ? p.bias + (sub >> 1) * H : nullptr;
@@ -1034,10 +991,6 @@ struct SpectralPolicyT {
     for (int q = 0; q < tcg::EW / 4; ++q) {
       if (col + 4 * q >= H) break;
       float y[4] = {x[4 * q + 0], x[4 * q + 1], x[4 * q + 2], x[4 * q + 3]};
-      if (S > 0) {                                  // + (V Z)[row, col + 4q ..], from pre_epilogue()
-        const float4 t = o4[q];
-        y[0] += t.x; y[1] += t.y; y[2] += t.z; y[3] += t.w;
-      }
       if (bias) {
         const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + col) + q);
         y[0] += b4.x; y[1] += b4.y; y[2] += b4.z; y[3] += b4.w;
@@ -1100,7 +1053,7 @@ struct SpectralPolicyT {
   // act(b_last); they count only where the mask says so (or when there is no mask).
   __device__ void readout(const float* bias_last) {
     const int P = p.P, P1 = p.P + 1, PQ = (P1 + 3) >> 2, HP = H + 4;
-    float* Wr = UZ;                                  // [4 PQ][HP]  W_out rows, w_att, zero rows (Z is dead)
+    float* Wr = ring;                                // [4 PQ][HP]  W_out rows, w_att, zero rows (the ring is idle)
     float* Yr = Wr + (size_t)4 * PQ * HP;            // [RMAX + 1][P1]  per-row outputs; last = pad row
     float* cx = Yr + (size_t)(RMAX + 1) * P1 + ((4 - ((RMAX + 1) * P1 & 3)) & 3);   // [H], 16 B aligned
     for (int e = tid; e < 4 * PQ * H; e += tcg::PRODUCER_THREADS) {
@@ -1285,9 +1238,9 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
   }
   int lb = (int)((227 * 1024 - smem) / Pol::ell_line_bytes());
   if (lb > 255) lb = 255;
-  // The readout scratch (at most 56 KiB: P = 48, H = 128, N = 128) fits the dead region (at least
-  // 93 KiB: Din or H = 128, K = 32) at every shape accepted above; the check keeps it that way.
-  if (d.score && Pol::readout_bytes(d.H, d.P, d.N) > Pol::dead_bytes(dmax, d.K, d.H, lb)) {
+  // The readout scratch (at most 56 KiB: P = 48, H = 128, N = 128) fits the A ring (64 KiB), which
+  // is idle after the last drain, at every shape accepted above; the check keeps it that way.
+  if (d.score && Pol::readout_bytes(d.H, d.P, d.N) > (size_t)Pol::kStagesA * tcg::STAGE_A_BYTES) {
     lnb::set_err("%s: fused readout (P=%d, H=%d, N=%d) does not fit the free shared memory", who, d.P,
                  d.H, d.N);
     return LNB_ERR_UNSUPPORTED;

@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "sm90.cuh"
 #include <stdlib.h>
+#include <type_traits>
 
 namespace tcg {
 
@@ -48,6 +49,11 @@ __host__ __device__ constexpr int pass_cols(int stages_a) {
   return stages_a * STAGE_A_BYTES / (BM * 4) < BN ? stages_a * STAGE_A_BYTES / (BM * 4) : BN;
 }
 
+// The A ring, from the policy's shared memory (which follows the skeleton's)
+__device__ __forceinline__ uint8_t* a_ring(uint8_t* policy_smem, int stages_b, int stages_a) {
+  return policy_smem - core_smem(stages_b, stages_a) + stages_b * STAGE_B_BYTES;
+}
+
 struct Core {
   uint8_t* Bst;        // [kStagesB][hi 16 KB | lo 16 KB]   W tiles
   uint8_t* Ast;        // [kStagesA][hi 16 KB | lo 16 KB]   A k-blocks; drain buffer of the epilogue
@@ -57,6 +63,7 @@ struct Core {
   uint64_t* a_empty;   // [kStagesA]  one arrival per consumer warp
   uint64_t* stg_full;  // [1]         drain pass written (every consumer thread)
   uint64_t* stg_empty; // [1]         drain pass read (every producer thread)
+  uint64_t* kept_read; // [1]         a drain kept in the A ring has been read (one arrival per consumer warp)
 };
 
 __device__ __forceinline__ Core carve(uint8_t* base, int stages_b, int stages_a) {
@@ -70,13 +77,14 @@ __device__ __forceinline__ Core carve(uint8_t* base, int stages_b, int stages_a)
   c.a_empty = c.a_full + MAX_A_STAGES;
   c.stg_full = c.a_empty + MAX_A_STAGES;
   c.stg_empty = c.stg_full + 1;
+  c.kept_read = c.stg_empty + 1;
   return c;
 }
 
 // Optional phase timers (profiling aid): when a buffer is registered with lnb_debug_set_prof,
 // thread 0 of every CTA accumulates clock64() deltas per phase into prof[cta*32 + phase]
 // (slots 8 / 9: k-loop / accumulator wait of odd sub-steps, 10: post_epilogue):
-//   0 staging issue  1 staging wait  2 U = V^T X   (policy)   3 k-loop  4 pre_epilogue
+//   0 staging issue  1 staging wait (policy)  3 k-loop  4 pre_epilogue
 //   5 wait for the accumulator  7 epilogue store
 __device__ unsigned long long* g_prof = nullptr;
 
@@ -122,6 +130,22 @@ __device__ __forceinline__ int stg_index(int row, int col, int pw) {
 //   void post_epilogue(int sub)                           after the step's last store()
 //   void store(int sub, int col, float (&x)[EW])          accumulator columns [col, col+EW) of
 //                                                         this thread's row (main + corr summed)
+// Optional pair (a policy whose step starts from the previous step's result; without it every
+// accumulator starts at zero):
+//   static bool drain_kept(const Params&, int sub)        the step's drain ([D_main + D_corr], one pass)
+//                                                         stays in the A ring: the producers read none of
+//                                                         it, and write the next step's first k-block only
+//                                                         after every consumer warp has run acc_init();
+//                                                         that step and the next have k-blocks
+//   static bool acc_init(const Params&, const uint8_t* policy_smem, const float* ring, int sub,
+//                        int row0, int cl, float (&d)[128])
+//                                                         consumers, before the step's first MMA: true
+//                                                         when it set the fragment d (rows row0 and
+//                                                         row0 + 8, columns 8 j + cl + {0, 1}); the
+//                                                         MMAs then add to it
+template <class P, class = void> struct HasAccInit : std::false_type {};
+template <class P> struct HasAccInit<P, std::void_t<decltype(&P::acc_init)>> : std::true_type {};
+
 template <class Policy>
 __global__ void __launch_bounds__(THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
@@ -135,6 +159,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
   static_assert(SB >= 1 && SB <= MAX_B_STAGES && SA >= 1 && SA <= MAX_A_STAGES, "ring depths");
   constexpr int PW = pass_cols(SA);                 // columns per drain pass
   constexpr int NPASS = BN / PW;
+  constexpr bool kAccInit = HasAccInit<Policy>::value;
+  static_assert(!kAccInit || NPASS == 1, "a drain kept in the A ring must fit it in one pass");
   Core c = carve(base, SB, SA);
   uint8_t* policy_smem = base + core_smem(SB, SA);
   float* stg = reinterpret_cast<float*>(c.Ast);
@@ -162,6 +188,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
     }
     sm90::mbar_init(c.stg_full, CONSUMER_THREADS);
     sm90::mbar_init(c.stg_empty, PRODUCER_THREADS);
+    sm90::mbar_init(c.kept_read, CONSUMER_THREADS / 32);
     sm90::fence_barrier_init();
   }
   __syncthreads();
@@ -172,10 +199,14 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
     Policy pol(p, policy_smem, tid);
     uint32_t cnt = 0;                                // k-blocks produced so far
     uint32_t npass = 0;                              // drain passes read so far
+    uint32_t nkept = 0;                              // drains kept in the A ring so far
+    bool after_kept = false;                         // the previous step's drain is in the A ring
     for (int it = 0; it < nsteps; ++it) {
       int m_tile, sub;
       Policy::decode(p, cta, ncta, it, m_tile, sub);
       const int nkb = Policy::num_kblocks(p, sub);
+      bool kept = false;
+      if constexpr (kAccInit) kept = Policy::drain_kept(p, sub);
       PhaseTimer tm;
       tm.start(cta, tid);
       pol.step_begin(m_tile, sub, 0, tm);
@@ -183,6 +214,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
         float v[32];
         if (!(p.dbg & 8)) pol.produce(sub, kb, v);
         const uint32_t sa = cnt % SA;
+        if (kAccInit && kb == 0 && after_kept) {     // the consumers have read the kept drain
+          sm90::mbar_wait(c.kept_read, nkept & 1u);
+          ++nkept;
+        }
         sm90::mbar_wait(&c.a_empty[sa], ((cnt / SA) & 1u) ^ 1u);
         if (!(p.dbg & 1)) {
           uint8_t* hi = c.Ast + sa * STAGE_A_BYTES + r * 128;
@@ -208,7 +243,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
       tm.lap(4);
       // ---- epilogue: the consumers drain the accumulators in passes of PW columns ----
 #pragma unroll 1
-      for (int q = 0; q < NPASS; ++q, ++npass) {
+      for (int q = 0; q < (kept ? 0 : NPASS); ++q, ++npass) {
         sm90::mbar_wait(c.stg_full, npass & 1u);
         if (q == 0) tm.lap((sub & 1) ? 9 : 5);
 #pragma unroll 1
@@ -227,6 +262,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
       producers_sync();                              // every row is read before the A ring is rewritten
       pol.post_epilogue(sub);
       tm.lap(10);
+      after_kept = kept;
     }
   } else {
     // ================================ MMA consumers ========================================
@@ -234,6 +270,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
     const int wq = warp & 3;
     float d[128];                                    // [D_main (64 x 128) | D_corr (64 x 128)]
     uint32_t cnt = 0, npass = 0;
+    bool after_kept = false;                         // the previous step's drain is in the A ring
+    const int row0 = wg * 64 + wq * 16 + (lane >> 2), cl = 2 * (lane & 3);
     // W loads (warp CONSUMER_WARP0 only): the cursor walks the k-blocks of all steps in order;
     // the load of k-block i waits until every consumer warp has released k-block i - kStagesB
     const bool issuer = warp == CONSUMER_WARP0;
@@ -273,7 +311,18 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
       int m_tile, sub;
       Policy::decode(p, cta, ncta, it, m_tile, sub);
       const int nkb = Policy::num_kblocks(p, sub);
-      if (nkb == 0) {
+      bool kept = false;
+      if constexpr (kAccInit) {
+        kept = Policy::drain_kept(p, sub);
+        if (!Policy::acc_init(p, policy_smem, stg, sub, row0, cl, d)) {
+#pragma unroll
+          for (int i = 0; i < 128; ++i) d[i] = 0.f;
+        }
+        if (after_kept) {                            // this warp is done reading the kept drain
+          __syncwarp();
+          if (lane == 0) sm90::mbar_arrive(c.kept_read);
+        }
+      } else {
 #pragma unroll
         for (int i = 0; i < 128; ++i) d[i] = 0.f;
       }
@@ -290,15 +339,14 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
           for (int k = 0; k < BK / 8; ++k) {
             const uint64_t ah = sm90::wgmma_desc_kmajor_sw128(a_hi + 32 * k);
             const uint64_t wh = sm90::wgmma_desc_kmajor_sw128(b + 32 * k);
-            const uint32_t acc = (kb | k) != 0 ? 1u : 0u;
-            sm90::wgmma_n128(d, ah, wh, acc);                                                  // D_main += A_hi W_hi^T
-            sm90::wgmma_n128_hi(d, ah, sm90::wgmma_desc_kmajor_sw128(b + TILE_B_BYTES + 32 * k), acc);  // D_corr += A_hi W_lo^T
+            sm90::wgmma_n128(d, ah, wh, 1u);                                                   // D_main += A_hi W_hi^T
+            sm90::wgmma_n128_hi(d, ah, sm90::wgmma_desc_kmajor_sw128(b + TILE_B_BYTES + 32 * k), 1u);   // D_corr += A_hi W_lo^T
             sm90::wgmma_n128_hi(d, sm90::wgmma_desc_kmajor_sw128(a_lo + 32 * k), wh, 1u);     // D_corr += A_lo W_hi^T
           }
           sm90::wgmma_commit();
           sm90::wgmma_wait_all();
         }
-        __syncwarp();
+        __syncwarp();                                // stage released as soon as its MMAs retire
         if (lane == 0) {
           sm90::mbar_arrive(&c.a_empty[sa]);
           sm90::mbar_arrive(&c.b_empty[sb]);
@@ -306,10 +354,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
         if (issuer) load_next();
       }
       consumers_sync();                              // both warpgroups are done reading the A ring
-      const int row0 = wg * 64 + wq * 16 + (lane >> 2), cl = 2 * (lane & 3);
+      // A kept drain needs no hand-over: the producers read the last drain before they wrote this
+      // step's k-blocks, and they write no more until kept_read
 #pragma unroll
-      for (int q = 0; q < NPASS; ++q, ++npass) {
-        sm90::mbar_wait(c.stg_empty, (npass & 1u) ^ 1u);
+      for (int q = 0; q < NPASS; ++q, npass += kept ? 0 : 1) {
+        if (!kept) sm90::mbar_wait(c.stg_empty, (npass & 1u) ^ 1u);
 #pragma unroll
         for (int i = 0; i < 64; i += 2) {
           const int col = 8 * (i / 4) + cl, row = row0 + 8 * ((i / 2) % 2);
@@ -317,8 +366,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
             *reinterpret_cast<float2*>(stg + stg_index(row, col - q * PW, PW)) =
                 make_float2(d[i] + d[i + 64], d[i + 1] + d[i + 65]);
         }
-        sm90::mbar_arrive(c.stg_full);
+        if (!kept) sm90::mbar_arrive(c.stg_full);
       }
+      if (kept) consumers_sync();                    // the next acc_init() reads rows of both halves
+      after_kept = kept;
     }
   }
 

@@ -293,7 +293,7 @@ def fused_conv_supported(N, Din, K, H, n_short, dense_filter, S=8, E1=7):
   if (n_short or dense_filter or N > 128 or Din % 32 or K > 32 or K % 4 or H % 4 or H > 128 or
       E1 > 16):
     return False
-  smem = 2 * 32768 + 256 + 1024 + 2 * 128 * (max(Din, H) + 4) * 4 + 128 * K * 4 + 4096
+  smem = 4 * 32768 + 256 + 1024 + 128 * (max(Din, H) + 4) * 4 + 128 * K * 4 + 4096
   return smem <= 227 * 1024
 
 
