@@ -94,13 +94,19 @@ def split_tf32(x):
 
 
 def linear_tf32x3(x, w_hi, w_lo, bias=None, relu=False, out=None):
-  """act(x @ W^T + bias) on the tensor cores (wgmma, 3xTF32).  x [M,K], w_hi/w_lo [N,K]."""
+  """act(x @ W^T + bias) on the tensor cores (wgmma, 3xTF32).  x [M,K], w_hi/w_lo [N,K]; ``out``, when
+  given, must be a contiguous float32 [M,N] tensor on x's device."""
   _need_cuda(x, w_hi, w_lo, bias)
   x = _f32c(x)
   M, K = x.shape
   N = w_hi.shape[0]
   if out is None:
     out = torch.empty((M, N), device=x.device, dtype=torch.float32)
+  elif (out.dtype != torch.float32 or tuple(out.shape) != (M, N) or not out.is_contiguous() or
+        out.device != x.device):
+    raise ValueError('linear_tf32x3: out must be a contiguous float32 [%d, %d] tensor on %s; got %s %s%s on %s'
+                     % (M, N, x.device, out.dtype, tuple(out.shape),
+                        '' if out.is_contiguous() else ' (not contiguous)', out.device))
   tiles = ((M + 127) // 128) * ((N + 127) // 128)
   nkb = (K + 31) // 32
   splits = 1
@@ -134,16 +140,22 @@ def _sm_count(device):
 
 
 def _splitk_workspace(device, nfloats, ntiles):
-  """Per-device split-K scratch: partial tiles + per-tile arrival counters (zero between launches;
-  launches on one stream are ordered, so one buffer per device and stream is enough)."""
+  """Split-K scratch of the current stream on ``device``: partial tiles + per-tile arrival counters
+  (zero between launches; launches on one stream are ordered, so one pair per device and stream is
+  enough).  linear_tf32x3 never asks for more than tiles * splits <= SM count partial tiles, so the
+  pair is allocated once at that size and never replaced: it lives as long as the process, because
+  a captured CUDA graph binds its pointers.  Graphs captured on the same stream share it, so their
+  replays must not run concurrently with each other or with launches on that stream."""
   key = (device.index, torch.cuda.current_stream(device).cuda_stream)
-  ws, counters = _SPLITK_WS.get(key, (None, None))
-  if ws is None or ws.numel() < nfloats or counters.numel() < ntiles:
-    ws = torch.empty((max(nfloats, ws.numel() if ws is not None else 0),), device=device,
-                     dtype=torch.float32)
-    counters = torch.zeros((max(ntiles, 256),), device=device, dtype=torch.int32)
-    _SPLITK_WS[key] = (ws, counters)
-  return ws, counters
+  pair = _SPLITK_WS.get(key)
+  if pair is None:
+    sms = _sm_count(device)
+    pair = (torch.empty((sms * 128 * 128,), device=device, dtype=torch.float32),
+            torch.zeros((max(sms, 256),), device=device, dtype=torch.int32))
+    _SPLITK_WS[key] = pair
+  ws, counters = pair
+  assert nfloats <= ws.numel() and ntiles <= counters.numel(), (nfloats, ws.numel(), ntiles)
+  return pair
 
 
 def linear_tf32x3_grouped(x, w_hi, w_lo, bias, groups, relu=False):
