@@ -329,6 +329,62 @@ int lnb_ggnn_update(lnb_stream_t stream, const float* M, const float* h, const f
                     const float* bias, int B, int N, int D, int E1, int avg, float* out);
 
 /* ---------------------------------------------------------------------------------------
+ * MPNN propagation step with the edge-network messages (model/mpnn.py:131-191), one persistent 3xTF32
+ * wgmma launch over all B*N rows.  Receiver i, neighbour j, channel e, A_e = (L_e != 0):
+ *   S_e[i]  = w_i * sum over the non-zeros j of row i of channel e of relu(P_e[j] + Q_e[i])   (64 wide)
+ *   deg[i,e] = w_i * nnz_e(i)           w_i = 1 (avg == 0, 'sum') or 1 / (nnz_e(i) + FLT_EPSILON) (avg != 0)
+ *   G = [S_0 | ... | S_{E1-1} | deg, zero padded to 32 | h] W^T + bias, then the GRU cell of
+ *   lnb_ggnn_update: out = (h - n) * z + n.
+ * PQ [B*N, E1*128]: per channel the 64 columns of P_e = h W1a_e^T, then the 64 of Q_e = h W1b_e^T + b1_e
+ * (the first edge layer split at the neighbour / receiver halves of its input [h_j | h_i]).
+ * W_hi / W_lo: tf32 split of the gate matrix [4D, 64*E1 + 32 + D] laid out as in lnb_ggnn_update, whose
+ * input part is the folded F = [W_ih,e W2_e]_e | [W_ih,e b2_e]_e (zero padded to 64*E1 + 32 columns).
+ * ell_*: lnb_graph_prepare of L [B,N,N,E1].  h and out [B*N, D] (out must not alias h).  PQ, h, out, W
+ * 16-byte aligned.  S is computed in the producer warps and never written out.
+ * Envelope: 1 <= N <= 255, D % 32 == 0, 32 <= D <= 128, 1 <= E1 <= 16 (LNB_ERR_UNSUPPORTED otherwise,
+ * nothing launched).  Summation order is fixed: repeated launches are bit-identical.
+ * ------------------------------------------------------------------------------------- */
+int lnb_mpnn_update(lnb_stream_t stream, const float* PQ, const float* h, const float* ell_val,
+                    const uint8_t* ell_idx, const int32_t* ell_max, const float* W_hi, const float* W_lo,
+                    const float* bias, int B, int N, int D, int E1, int avg, float* out);
+
+/* ---------------------------------------------------------------------------------------
+ * Training path of lnb_mpnn_update: S [B*N, E1*64] (column block e = S_e) with the producer's
+ * arithmetic, and its adjoint
+ *   gQ_e[i] = w_i sum_j A_e[i,j] [P_e[j] + Q_e[i] > 0] gS_e[i]
+ *   gP_e[j] = sum_i A_e[i,j] w_i [P_e[j] + Q_e[i] > 0] gS_e[i]
+ * written as gPQ [B*N, E1*128] in the layout of PQ.  ellT_* are lnb_graph_prepare of the transposed
+ * operators L.transpose(1, 2) (operators need not be symmetric).  One thread per output element, sums
+ * in ELL order, no atomics: deterministic.  Envelope: 1 <= N <= 255, 1 <= E1 <= 16
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ * ------------------------------------------------------------------------------------- */
+int lnb_mpnn_edge_aggregate(lnb_stream_t stream, const float* PQ, const float* ell_val, const uint8_t* ell_idx,
+                            const int32_t* ell_max, int B, int N, int E1, int avg, float* S);
+int lnb_mpnn_edge_aggregate_backward(lnb_stream_t stream, const float* PQ, const float* gS, const float* ell_val,
+                                     const uint8_t* ell_idx, const int32_t* ell_max, const float* ellT_val,
+                                     const uint8_t* ellT_idx, const int32_t* ellT_max, int B, int N, int E1,
+                                     int avg, float* gPQ);
+
+/* ---------------------------------------------------------------------------------------
+ * Set2Vec readout + output_func of MPNN (model/set2set.py:60-100, model/mpnn.py:198-207), every graph
+ * of the batch in one launch.  Per graph, over its set (nodes with mask != 0, or all N when mask is
+ * NULL), hidden [2D] = 0, mem [D] = 0, and `steps` times:
+ *   f, i, o = sigmoid, c = tanh of the gate rows of Wg hidden + bg (blocks forget, input, output, memory)
+ *   mem = f * mem + i * c;  h = o * tanh(mem);  u = h W1;  e_n = tanh(u + x_n) . W2
+ *   a = max-subtracted softmax of e over the set;  read = sum_n a_n x_n (0 for an empty set)
+ *   hidden = [h | read]
+ * then score[b] = W_out hidden + b_out.
+ * X [B,N,D]; mask [B,N] uint8 or NULL; WgT [2D, 4D] = the four gate Linear weights stacked [4D, 2D] and
+ * transposed; bg [4D]; W1 [D, D] used as [in, out]; W2 [D]; W_out [P, 2D]; b_out [P]; score [B,P].
+ * fp32, every sum in a fixed order: repeated launches are bit-identical.
+ * Envelope: 1 <= N <= 128, D % 32 == 0, 32 <= D <= 128, 1 <= P <= 128 (LNB_ERR_UNSUPPORTED otherwise,
+ * nothing launched).
+ * ------------------------------------------------------------------------------------- */
+int lnb_set2vec(lnb_stream_t stream, const float* X, const uint8_t* mask, const float* WgT, const float* bg,
+                const float* W1, const float* W2, const float* W_out, const float* b_out, int B, int N, int D,
+                int P, int steps, float* score);
+
+/* ---------------------------------------------------------------------------------------
  * Operator chain on channel 0 of L [B,N,N,E1], per graph, starting from X [B,N,D]:
  *   chebyshev == 0: w_s = L_0 w_{s-1} (w_0 = X), s = 1..steps   (model/dcnn.py:88-92, the short
  *                   diffusion walk of model/lanczos_net.py:164-169);

@@ -96,6 +96,15 @@ SIGNATURES = {
                                   c_int, c_int, c_int, c_int, c_int, c_int, c_f32p]),
     'lnb_ggnn_update': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p,
                                 c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int, c_f32p]),
+    'lnb_mpnn_update': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p,
+                                c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int, c_f32p]),
+    'lnb_mpnn_edge_aggregate': (c_int, [c_stream, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_int, c_int,
+                                        c_int, c_int, c_f32p]),
+    'lnb_mpnn_edge_aggregate_backward':
+        (c_int, [c_stream, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p, ctypes.c_void_p,
+                 ctypes.c_void_p, c_int, c_int, c_int, c_int, c_f32p]),
+    'lnb_set2vec': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
+                            c_int, c_int, c_int, c_int, c_int, c_f32p]),
     'lnb_operator_chain': (c_int, [c_stream, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int, c_int,
                                    ctypes.POINTER(c_int), c_f32p, c_i64, c_i64, c_int]),
     'lnb_graph_messages': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int,

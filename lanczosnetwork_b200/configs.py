@@ -68,6 +68,15 @@ def qm8_ggnn(**model_over):
                                   num_bond_type=6), model=NS(**model))
 
 
+def qm8_mpnn(**model_over):
+  """config/qm8_mpnn.yaml"""
+  model = dict(name='MPNN', num_prop=7, input_dim=64, hidden_dim=128, update_func='GRU', output_dim=16,
+               msg_func='MLP', num_step_set2vec=10, aggregate_type='avg', num_layer=1, loss='MSE')
+  model.update(model_over)
+  return NS(seed=1234, dataset=NS(loader_name='QM8Data', name='chemistry', num_atom=70,
+                                  num_bond_type=6), model=NS(**model))
+
+
 def qm8_ada_lanczos_net(**model_over):
   model = dict(name='AdaLanczosNet', short_diffusion_dist=[1, 2, 3],
                long_diffusion_dist=[5, 7, 10, 20, 30], num_eig_vec=20,

@@ -8,8 +8,9 @@ What it does (see INTEGRATION.md):
      (model/mpnn.py:6 -> operators/functions/unsorted_segment_sum.py:5);
   2. rebinds the classes of ``DROPIN_CLASSES`` (``LanczosNet``, ``AdaLanczosNet``, ``GCN``, ``GAT``, ``GraphSAGE``, ...)
      inside the runner modules' globals, because the runners resolve the class with ``eval(name)`` in their own
-     namespace (runner/qm8_runner.py:59,288; runner/graph_runner.py:57,285);
-  3. runs the reference ``run_exp.main()`` unchanged.
+     namespace (runner/qm8_runner.py:59,288; runner/graph_runner.py:57,285), plus the classes of
+     ``OPT_IN_CLASSES`` named with ``--opt-in NAME`` (repeatable; e.g. ``--opt-in MPNN``);
+  3. runs the reference ``run_exp.main()`` unchanged (``--opt-in`` is removed from its argv).
 """
 import importlib
 import os
@@ -20,6 +21,8 @@ from .operators import _ext as _ext_pkg
 
 DROPIN_CLASSES = ('LanczosNet', 'AdaLanczosNet', 'LanczosNetGeneral', 'GCN', 'GCNFP', 'DCNN', 'ChebyNet',
                   'GAT', 'GraphSAGE', 'GGNN')
+# drop-ins that replace the reference class only when asked for (patch_namespace(opt_in=...), --opt-in)
+OPT_IN_CLASSES = ('MPNN',)
 
 
 def register_native_op():
@@ -31,12 +34,20 @@ def register_native_op():
     setattr(ops_pkg, '_ext', _ext_pkg)
 
 
-def patch_namespace(module, training=False):
-  """Rebind the class names in ``module``'s globals to the H100 drop-ins.  ``training=True`` (a
-  run without ``-t``) rebinds only the classes that have a differentiable training path
-  (every class but ``GAT``, which is inference only); a class without one keeps the reference's
+def _check_opt_in(opt_in):
+  unknown = [n for n in opt_in if n not in OPT_IN_CLASSES]
+  if unknown:
+    raise ValueError('dropin: %s not in OPT_IN_CLASSES %s' % (', '.join(map(repr, unknown)), OPT_IN_CLASSES))
+  return tuple(opt_in)
+
+
+def patch_namespace(module, training=False, opt_in=()):
+  """Rebind the class names in ``module``'s globals to the H100 drop-ins: those of ``DROPIN_CLASSES``
+  and those of ``opt_in`` (names from ``OPT_IN_CLASSES``; any other name is a ValueError).
+  ``training=True`` (a run without ``-t``) rebinds only the classes that have a differentiable training
+  path (every class but ``GAT``, which is inference only); a class without one keeps the reference's
   trainable class instead of failing on the first ``loss.backward()``."""
-  for name in DROPIN_CLASSES:
+  for name in DROPIN_CLASSES + _check_opt_in(opt_in):
     if hasattr(module, name):
       cls = getattr(_models, name)
       if training and not hasattr(cls, '_train_impl'):
@@ -46,13 +57,14 @@ def patch_namespace(module, training=False):
 
 
 def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.graph_runner'),
-            compat=False, training=False):
+            compat=False, training=False, opt_in=()):
   """Returns the list of patched modules.  ``reference_root`` is put on sys.path if given.
   ``compat=True`` first installs the shims of ``lanczosnetwork_b200.compat`` (missing easydict /
   tensorboardX, PyYAML >= 6, numpy >= 2) so the 2019 checkout imports under a current stack.
   Raises ImportError when NO runner module could be imported and patched: the runners resolve
   the model class by name in their own namespace, so a silent miss would run the reference's
-  classes while claiming the drop-in."""
+  classes while claiming the drop-in.  ``opt_in``: see patch_namespace."""
+  opt_in = _check_opt_in(opt_in)
   if compat:
     from . import compat as _compat
     _compat.install()
@@ -63,7 +75,7 @@ def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.gr
   register_native_op()
   patched = []
   ref_model = importlib.import_module('model')
-  patched.append(patch_namespace(ref_model, training))
+  patched.append(patch_namespace(ref_model, training, opt_in))
   errors = []
   for name in runner_modules:
     try:
@@ -71,7 +83,7 @@ def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.gr
     except ImportError as exc:      # e.g. tensorboardX absent: that runner cannot be used anyway
       errors.append('%s: %s' % (name, exc))
       continue
-    patched.append(patch_namespace(mod, training))
+    patched.append(patch_namespace(mod, training, opt_in))
   if runner_modules and len(patched) == 1:
     raise ImportError('dropin.install: no runner module could be imported, nothing would call the '
                       'H100 classes (%s); pass compat=True for the shims of '
@@ -84,7 +96,14 @@ def main(argv=None):
   if not argv:
     raise SystemExit(__doc__)
   root = argv.pop(0)
-  install(root, compat=True, training=('-t' not in argv and '--test' not in argv))
+  opt_in = []
+  while '--opt-in' in argv:
+    i = argv.index('--opt-in')
+    if i + 1 >= len(argv):
+      raise SystemExit('--opt-in needs a class name (one of %s)' % (OPT_IN_CLASSES,))
+    opt_in.append(argv[i + 1])
+    del argv[i:i + 2]
+  install(root, compat=True, training=('-t' not in argv and '--test' not in argv), opt_in=opt_in)
   os.chdir(root)
   sys.argv = ['run_exp.py'] + argv
   run_exp = importlib.import_module('run_exp')

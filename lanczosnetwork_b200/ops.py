@@ -15,7 +15,8 @@ __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'sage_operators', 'neighbour_max', 'ggnn_update',
-    'ggnn_update_supported',
+    'ggnn_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
+    'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'set2vec', 'set2vec_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
     'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
@@ -560,6 +561,113 @@ def ggnn_update(M, h, prep, w_hi, w_lo, bias, avg, out=None):
     _lib.check(_lib.load().lnb_ggnn_update(
         _stream(h), _ptr(M), _ptr(h), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi), _ptr(w_lo),
         _ptr(bias), B, N, D, E1, int(bool(avg)), _ptr(out)), 'lnb_ggnn_update')
+  return out
+
+
+MPNN_EDGE_HIDDEN = 64      # width of the edge network's hidden layer, fixed in the reference (model/mpnn.py:60)
+
+
+def mpnn_update_supported(N, D, E1):
+  """Shapes lnb_mpnn_update accepts (mirrors its checks)."""
+  return 1 <= N <= 255 and D % 32 == 0 and 32 <= D <= 128 and 1 <= E1 <= 16
+
+
+def mpnn_update(PQ, h, prep, w_hi, w_lo, bias, avg, out=None):
+  """One MPNN propagation step with the edge-network messages (see lnb_mpnn_update): the GRU cell of
+  [S_0 | ... | S_{E1-1} | deg | h] against the folded gate matrix, S_e gathered through the ELL rows of
+  ``prep`` (graph_prepare of the operators [B,N,N,E1]).  PQ [B*N, E1*128] (per channel 64 P columns, then
+  64 Q columns), h [B*N, D]; w_hi / w_lo / bias: the gate matrix [4D, 64*E1 + 32 + D] and its bias [4D]
+  (model.mpnn.MPNN._step_params).  Returns h' [B*N, D] (written to ``out`` when given)."""
+  _need_cuda(PQ, h, w_hi, w_lo, bias, out)
+  PQ, h, bias = _f32c(PQ), _f32c(h), _f32c(bias)
+  ell_val, ell_idx, ell_max = prep[0], prep[1], prep[2]
+  B, E1, N = ell_val.shape[0], ell_val.shape[1], ell_val.shape[2]
+  D = h.shape[1]
+  K = MPNN_EDGE_HIDDEN * E1 + 32 + D
+  if (tuple(h.shape) != (B * N, D) or tuple(PQ.shape) != (B * N, E1 * 2 * MPNN_EDGE_HIDDEN) or
+      tuple(w_hi.shape) != (4 * D, K) or tuple(bias.shape) != (4 * D,)):
+    raise ValueError('mpnn_update: PQ %s, h %s, W %s, bias %s do not agree with B=%d N=%d E1=%d'
+                     % (tuple(PQ.shape), tuple(h.shape), tuple(w_hi.shape), tuple(bias.shape), B, N, E1))
+  if out is None:
+    out = torch.empty_like(h)
+  with torch.cuda.device(h.device):
+    _lib.check(_lib.load().lnb_mpnn_update(
+        _stream(h), _ptr(PQ), _ptr(h), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi), _ptr(w_lo),
+        _ptr(bias), B, N, D, E1, int(bool(avg)), _ptr(out)), 'lnb_mpnn_update')
+  return out
+
+
+def mpnn_edge_aggregate_supported(N, E1):
+  """Shapes lnb_mpnn_edge_aggregate and its backward accept (mirrors their checks)."""
+  return 1 <= N <= 255 and 1 <= E1 <= 16
+
+
+def _check_pq(who, PQ, prep):
+  B, E1, N = prep[0].shape[0], prep[0].shape[1], prep[0].shape[2]
+  if tuple(PQ.shape) != (B * N, E1 * 2 * MPNN_EDGE_HIDDEN):
+    raise ValueError('%s: PQ %s does not agree with B=%d N=%d E1=%d' % (who, tuple(PQ.shape), B, N, E1))
+  return B, N, E1
+
+
+def mpnn_edge_aggregate(PQ, prep, avg):
+  """S [B*N, E1*64] of lnb_mpnn_edge_aggregate: S_e[i] = w_i sum_j A_e[i,j] relu(P_e[j] + Q_e[i])."""
+  _need_cuda(PQ)
+  PQ = _f32c(PQ)
+  B, N, E1 = _check_pq('mpnn_edge_aggregate', PQ, prep)
+  S = torch.empty((B * N, E1 * MPNN_EDGE_HIDDEN), device=PQ.device, dtype=torch.float32)
+  with torch.cuda.device(PQ.device):
+    _lib.check(_lib.load().lnb_mpnn_edge_aggregate(
+        _stream(PQ), _ptr(PQ), _ptr(prep[0]), _ptr(prep[1]), _ptr(prep[2]), B, N, E1, int(bool(avg)), _ptr(S)),
+               'lnb_mpnn_edge_aggregate')
+  return S
+
+
+def mpnn_edge_aggregate_backward(PQ, gS, prep, prep_t, avg):
+  """gPQ [B*N, E1*128] (lnb_mpnn_edge_aggregate_backward); prep_t = graph_prepare of the transposed
+  operators."""
+  _need_cuda(PQ, gS)
+  PQ, gS = _f32c(PQ), _f32c(gS)
+  B, N, E1 = _check_pq('mpnn_edge_aggregate_backward', PQ, prep)
+  if tuple(gS.shape) != (B * N, E1 * MPNN_EDGE_HIDDEN) or tuple(prep_t[0].shape) != tuple(prep[0].shape):
+    raise ValueError('mpnn_edge_aggregate_backward: gS %s / transposed ELL %s do not agree with B=%d N=%d E1=%d'
+                     % (tuple(gS.shape), tuple(prep_t[0].shape), B, N, E1))
+  gPQ = torch.empty_like(PQ)
+  with torch.cuda.device(PQ.device):
+    _lib.check(_lib.load().lnb_mpnn_edge_aggregate_backward(
+        _stream(PQ), _ptr(PQ), _ptr(gS), _ptr(prep[0]), _ptr(prep[1]), _ptr(prep[2]), _ptr(prep_t[0]),
+        _ptr(prep_t[1]), _ptr(prep_t[2]), B, N, E1, int(bool(avg)), _ptr(gPQ)), 'lnb_mpnn_edge_aggregate_backward')
+  return gPQ
+
+
+def set2vec_supported(N, D, P):
+  """Shapes lnb_set2vec accepts (mirrors its checks)."""
+  return 1 <= N <= 128 and D % 32 == 0 and 32 <= D <= 128 and 1 <= P <= 128
+
+
+def set2vec(X, mask, WgT, bg, W1, W2, W_out, b_out, steps):
+  """Set2Vec readout + output Linear of every graph (see lnb_set2vec).  X [B,N,D]; mask [B,N] (any dtype,
+  non-zero = in the set) or None for all nodes; WgT [2D,4D] the stacked gate weights (forget, input,
+  output, memory) transposed; bg [4D]; W1 [D,D] as [in, out]; W2 [D] (or [D,1]); W_out [P,2D]; b_out [P].
+  Returns score [B,P]."""
+  _need_cuda(X, mask, WgT, bg, W1, W2, W_out, b_out)
+  X = _f32c(X)
+  B, N, D = X.shape
+  P = W_out.shape[0]
+  WgT, bg, W1, W2, W_out, b_out = [_f32c(t) for t in (WgT, bg, W1, W2, W_out, b_out)]
+  if (tuple(WgT.shape) != (2 * D, 4 * D) or tuple(bg.shape) != (4 * D,) or tuple(W1.shape) != (D, D) or
+      W2.numel() != D or tuple(W_out.shape) != (P, 2 * D) or tuple(b_out.shape) != (P,)):
+    raise ValueError('set2vec: WgT %s, bg %s, W1 %s, W2 %s, W_out %s, b_out %s do not agree with D=%d'
+                     % (tuple(WgT.shape), tuple(bg.shape), tuple(W1.shape), tuple(W2.shape), tuple(W_out.shape),
+                        tuple(b_out.shape), D))
+  if mask is not None:
+    mask = (mask != 0).to(torch.uint8).contiguous()
+    if tuple(mask.shape) != (B, N):
+      raise ValueError('set2vec: mask %s does not match X %s' % (tuple(mask.shape), tuple(X.shape)))
+  out = torch.empty((B, P), device=X.device, dtype=torch.float32)
+  with torch.cuda.device(X.device):
+    _lib.check(_lib.load().lnb_set2vec(
+        _stream(X), _ptr(X), _ptr(mask), _ptr(WgT), _ptr(bg), _ptr(W1), _ptr(W2), _ptr(W_out), _ptr(b_out),
+        B, N, D, P, int(steps), _ptr(out)), 'lnb_set2vec')
   return out
 
 

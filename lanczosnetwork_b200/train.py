@@ -28,7 +28,7 @@ from . import ops
 
 __all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
            'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
-           'ggnn_train', 'GraphedStep']
+           'ggnn_train', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'GraphedStep']
 
 
 def _pad_cols(x, mult=4):
@@ -395,6 +395,110 @@ def ggnn_train(model, node_ids, L, mask):
     if model.training and model.dropout > 0.0:
       h = torch.nn.functional.dropout(h, model.dropout, True)
   return gated_readout(model, h.reshape(B, N, D), mask, head=model.output_func[0])
+
+
+class _EdgeAggregate(torch.autograd.Function):
+  """S_e[i] = w_i sum_j A_e[i,j] relu(P_e[j] + Q_e[i]) from PQ [B*N, E1*128] (lnb_mpnn_edge_aggregate); the
+  adjoint gathers over the ELL rows of the operators and of their transposes (``prep_t``), without atomics."""
+
+  @staticmethod
+  def forward(ctx, PQ, prep, prep_t, avg):
+    PQ = PQ.contiguous()
+    ctx.save_for_backward(PQ)
+    ctx.prep, ctx.prep_t, ctx.avg = prep, prep_t, avg
+    return ops.mpnn_edge_aggregate(PQ, prep, avg)
+
+  @staticmethod
+  def backward(ctx, gS):
+    (PQ,) = ctx.saved_tensors
+    return ops.mpnn_edge_aggregate_backward(PQ, gS.contiguous(), ctx.prep, ctx.prep_t, ctx.avg), None, None, None
+
+
+def edge_aggregate(PQ, prep, prep_t, avg):
+  return _EdgeAggregate.apply(PQ.float(), prep, prep_t, bool(avg))
+
+
+def set2vec_train(model, X, mask):
+  """Set2Vec (model/set2set.py:60-100) of every graph at once, then output_func: the Linears in the
+  library's dense kernel, the attention over each graph's set as a softmax with the nodes outside the set
+  filled with -inf (an empty set reads 0).  X [B,N,D]."""
+  s2v = model.att_func
+  B, N, D = X.shape
+  lin = [seq[0] for seq in s2v.LSTM.gates()]
+  wg = torch.cat([l.weight for l in lin], dim=0)
+  bg = torch.cat([l.bias for l in lin], dim=0)
+  inset = (torch.ones((B, N), device=X.device, dtype=torch.bool) if mask is None
+           else (mask != 0).reshape(B, N))
+  hidden = X.new_zeros((B, 2 * D))
+  mem = X.new_zeros((B, D))
+  for _ in range(s2v.num_step_encoder):
+    f, i, o, c = dense(hidden, wg, bg, False).chunk(4, dim=1)
+    mem = torch.sigmoid(f) * mem + torch.sigmoid(i) * torch.tanh(c)
+    h = torch.sigmoid(o) * torch.tanh(mem)
+    u = dense(h, s2v.W_1.t(), None, False)
+    energy = dense(torch.tanh(u.unsqueeze(1) + X).reshape(B * N, D), s2v.W_2.t(), None, False).reshape(B, N)
+    energy = energy.masked_fill(~inset, float('-inf'))
+    top = energy.detach().max(dim=1, keepdim=True)[0]
+    top = torch.where(torch.isfinite(top), top, torch.zeros_like(top))
+    a = torch.exp(energy - top)
+    total = a.sum(dim=1, keepdim=True)
+    a = a / torch.where(total > 0, total, torch.ones_like(total))
+    read = bmm(a.unsqueeze(1), X).reshape(B, D)
+    hidden = torch.cat([h, read], dim=1)
+  head = model.output_func[0]
+  return dense(hidden, head.weight, head.bias, False)
+
+
+def mpnn_train(model, node_ids, L, mask):
+  """Differentiable MPNN (model/mpnn.py:110-212): embedding -> input_func -> num_prop steps of [messages
+  -> GRU cell -> dropout] -> Set2Vec -> output_func.  ``MLP`` messages: PQ = dense(h, [W1a_e ; W1b_e]),
+  S = edge_aggregate(PQ), agg_e = S_e W2_e^T + (w nnz_e) b2_e; ``embedding`` messages: A_e (h E_e) as in
+  ggnn_train.  A_e is the 0/1 pattern of L_e (row-normalised by nnz + float32 eps for ``avg``); the
+  caller's L is not modified."""
+  A = (L != 0).float()
+  nnz = A.sum(dim=2)                                                           # [B,N,E1]
+  avg = model.aggregate_type == 'avg'
+  B, N, E1 = A.shape[0], A.shape[1], A.shape[3]
+  x = embedding(node_ids, model.node_embedding.weight).reshape(B * N, -1)
+  lin = model.input_func[0]
+  h = dense(x, lin.weight, lin.bias, False)
+  D = h.shape[1]
+  cell = model.update_func
+  if model.msg_func_name == 'MLP':
+    zeros = torch.zeros((B, N, 4), device=L.device, dtype=torch.float32)
+    prep = ops.graph_prepare(L, zeros, binarize=True)
+    prep_t = ops.graph_prepare(L.transpose(1, 2), zeros, binarize=True)
+    deg = (nnz * (1.0 / (nnz + _EPS)) if avg else nnz).reshape(B * N, E1)     # w_i nnz_e(i)
+    first = [seq[0] for seq in model.edge_func]
+    second = [seq[2] for seq in model.edge_func]
+    w_pq = torch.cat([w for l in first for w in (l.weight[:, :D], l.weight[:, D:])], dim=0)
+    b_pq = torch.cat([b for l in first for b in (torch.zeros_like(l.bias), l.bias)], dim=0)
+    hw = first[0].weight.shape[0]
+  else:
+    if avg:
+      A = A / (nnz.unsqueeze(2) + _EPS)
+    A = A.contiguous()
+    w_msg = model.edge_embedding.weight.view(E1, D, D).transpose(1, 2).reshape(E1 * D, D)    # stacked E_e^T
+  for _ in range(model.num_prop):
+    if model.msg_func_name == 'MLP':
+      S = edge_aggregate(dense(h, w_pq, b_pq, False), prep, prep_t, avg)       # [B*N, E1*64]
+      agg = torch.cat([dense(S[:, e * hw:(e + 1) * hw], second[e].weight, None, False) +
+                       deg[:, e:e + 1] * second[e].bias for e in range(E1)], dim=1)
+    else:
+      msg = dense(h, w_msg, None, False)
+      agg = torch.cat([operator_messages(A, msg[:, e * D:(e + 1) * D].reshape(B, N, D), e, 1)
+                       for e in range(E1)], dim=2).reshape(B * N, E1 * D)
+    gi = dense(agg, cell.weight_ih, cell.bias_ih, False)
+    gh = dense(h, cell.weight_hh, cell.bias_hh, False)
+    i_r, i_z, i_n = gi.chunk(3, dim=1)
+    h_r, h_z, h_n = gh.chunk(3, dim=1)
+    r = torch.sigmoid(i_r + h_r)
+    z = torch.sigmoid(i_z + h_z)
+    n = torch.tanh(i_n + r * h_n)
+    h = (h - n) * z + n
+    if model.training and model.dropout > 0.0:
+      h = torch.nn.functional.dropout(h, model.dropout, True)
+  return set2vec_train(model, h.reshape(B, N, D), mask)
 
 
 class _BMM(torch.autograd.Function):
