@@ -329,6 +329,32 @@ int lnb_ggnn_update(lnb_stream_t stream, const float* M, const float* h, const f
                     const float* bias, int B, int N, int D, int E1, int avg, float* out);
 
 /* ---------------------------------------------------------------------------------------
+ * GPNN propagation within clusters and across cuts (model/gpnn.py:192-225), both partition operators in
+ * one persistent 3xTF32 wgmma launch over all B*N rows.  For each active part p (0 = cluster, 1 = cut):
+ *   agg_p[b,n, :] = sum over the non-zeros m of row n of operator p of  w * M_p[b*N+m, :]
+ *                   w = val (avg == 0, 'sum') or val / (rowsum_n + FLT_EPSILON) (avg != 0, 'avg'; the row
+ *                   sum runs over the row's entries in ELL order, the division is correctly rounded)
+ *   G = [agg_p | h_p] W^T + bias, then the GRU cell of lnb_ggnn_update: out_p = (h_p - n) * z + n.
+ * The operator VALUES enter (the L4 partition Laplacians); ell_* are the ELL rows of lnb_graph_prepare
+ * over stack([L_cluster, L_cut], 3) [B,N,N,2], not binarised.  Every one of the B*N rows is computed.
+ * M_p [B*N rows, stride ldm], h_p [stride ldh] and out_p [stride ldo], H columns each.  A part whose
+ * M, h and out are all null is skipped; M and h may alias between the parts.  h_copy [stride ldo] or
+ * null: the first active part also writes its h rows there (block 0 of the [B*N, 3H] input of
+ * state_func, whose blocks 1 and 2 are the outputs).
+ * W_hi / W_lo: tf32 split of gru_gate_matrix of the partition GRUCell, [4H, 2H] (layout of
+ * lnb_ggnn_update with E1 = 1); bias [4H].
+ * Envelope: 1 <= N <= 255, H % 32 == 0, 32 <= H <= 128; pointers 16-byte aligned and ldm, ldh, ldo
+ * multiples of 4, at least H; no output (nor h_copy) may share an element with any h or with each other.
+ * Outside it: LNB_ERR_UNSUPPORTED, nothing launched.  Summation order is fixed: repeated launches are
+ * bit-identical.
+ * ------------------------------------------------------------------------------------- */
+int lnb_gpnn_partition_update(lnb_stream_t stream, const float* M0, const float* h0, float* out0,
+                              const float* M1, const float* h1, float* out1, const float* ell_val,
+                              const uint8_t* ell_idx, const int32_t* ell_max, const float* W_hi,
+                              const float* W_lo, const float* bias, float* h_copy, int B, int N, int H,
+                              int ldm, int ldh, int ldo, int avg);
+
+/* ---------------------------------------------------------------------------------------
  * MPNN propagation step with the edge-network messages (model/mpnn.py:131-191), one persistent 3xTF32
  * wgmma launch over all B*N rows.  Receiver i, neighbour j, channel e, A_e = (L_e != 0):
  *   S_e[i]  = w_i * sum over the non-zeros j of row i of channel e of relu(P_e[j] + Q_e[i])   (64 wide)

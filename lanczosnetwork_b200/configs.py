@@ -68,6 +68,16 @@ def qm8_ggnn(**model_over):
                                   num_bond_type=6), model=NS(**model))
 
 
+def qm8_gpnn(**model_over):
+  """config/qm8_gpnn.yaml"""
+  model = dict(name='GPNN', num_partition=3, num_prop=10, num_prop_cluster=1, num_prop_cut=1, input_dim=64,
+               hidden_dim=128, update_func='GRU', output_dim=16, msg_func='MLP', aggregate_type='avg',
+               num_layer=1, loss='MSE')
+  model.update(model_over)
+  return NS(seed=1234, dataset=NS(loader_name='QM8Data', name='chemistry', num_atom=70,
+                                  num_bond_type=6), model=NS(**model))
+
+
 def qm8_mpnn(**model_over):
   """config/qm8_mpnn.yaml"""
   model = dict(name='MPNN', num_prop=7, input_dim=64, hidden_dim=128, update_func='GRU', output_dim=16,

@@ -18,7 +18,7 @@ import numpy as np
 
 __all__ = [
     'check_dist', 'get_laplacian', 'get_graph_laplacian_eigs', 'prepare_graph',
-    'collate', 'gat_bias', 'sage_collate', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
+    'collate', 'gat_bias', 'partition_operators', 'random_partition_labels', 'sage_collate', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
     'synthetic_regression_graphs',
 ]
 
@@ -132,6 +132,44 @@ def gat_bias(L):
   mt = L.astype(np.float64) + np.eye(N)[None, :, :, None]      # I @ (adj + I) is exact
   mt[mt > 0.0] = 1.0
   return (-1e9 * (1.0 - mt)).astype(np.float32)
+
+
+def partition_operators(L_simple, labels):
+  """GPNN's partition operators (utils/spectral_graph_partition.py:get_L_cluster_cut, applied per graph
+  by the GPNN collate, dataset/qm8.py:127-135), for a whole batch at once.
+
+  L_simple [B, N, N] (or [N, N]): the padded simple-graph operators; labels [B, N] (or [N]): the cluster of
+  every node, padded nodes included.  The adjacency is the off-diagonal non-zero pattern of L_simple;
+  its within-cluster part (both ends in one cluster) and the rest (the cut) each get the L4
+  renormalisation D^-1/2 (I + A) D^-1/2 in fp64, so every node, padded ones too, keeps a self-loop.
+  Returns (L_cluster, L_cut) as float32, the dtype the collate hands the model."""
+  L = np.asarray(L_simple)
+  lab = np.asarray(labels)
+  single = L.ndim == 2
+  if single:
+    L, lab = L[None], lab[None]
+  B, N = L.shape[0], L.shape[1]
+  if L.shape != (B, N, N) or lab.shape != (B, N):
+    raise ValueError('partition_operators: L_simple %s and labels %s do not agree' % (L.shape, lab.shape))
+  off = ~np.eye(N, dtype=bool)[None]
+  adj = ((L != 0) & off).astype(np.float64)
+  same = (lab[:, :, None] == lab[:, None, :]).astype(np.float64)
+  cluster = adj * same
+  cut = adj - cluster
+  out = []
+  for a in (cluster, cut):
+    m = a + np.eye(N)[None]
+    scale = np.power(m.sum(axis=2), -0.5)                  # every row has its self-loop: no zero degree
+    out.append(((scale[:, :, None] * m) * scale[:, None, :]).astype(np.float32))
+  if single:
+    out = [o[0] for o in out]
+  return out[0], out[1]
+
+
+def random_partition_labels(rng, batch_size, num_nodes, num_partition=3):
+  """Seeded stand-in for the spectral clustering of the GPNN collate: a uniformly drawn cluster label per
+  node [B, N] (benchmarks and tests; partition_operators turns them into operators)."""
+  return rng.randint(0, num_partition, size=(batch_size, num_nodes))
 
 
 def sage_collate(samples, num_sample_neighbors, npr):

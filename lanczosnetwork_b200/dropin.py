@@ -6,7 +6,7 @@ What it does (see INTEGRATION.md):
   1. registers ``operators._ext`` / ``operators._ext.segment_reduction`` in ``sys.modules`` so
      ``from model import *`` of the reference works without building its THC-era extension
      (model/mpnn.py:6 -> operators/functions/unsorted_segment_sum.py:5);
-  2. rebinds the classes of ``DROPIN_CLASSES`` (``LanczosNet``, ``AdaLanczosNet``, ``GCN``, ``GAT``, ``GraphSAGE``, ...)
+  2. rebinds the classes of ``DROPIN_CLASSES`` (``LanczosNet``, ``AdaLanczosNet``, ``GCN``, ``GAT``, ``GraphSAGE``, ``GGNN``, ``GPNN``, ...)
      inside the runner modules' globals, because the runners resolve the class with ``eval(name)`` in their own
      namespace (runner/qm8_runner.py:59,288; runner/graph_runner.py:57,285), plus the classes of
      ``OPT_IN_CLASSES`` named with ``--opt-in NAME`` (repeatable; e.g. ``--opt-in MPNN``);
@@ -20,7 +20,7 @@ from . import model as _models
 from .operators import _ext as _ext_pkg
 
 DROPIN_CLASSES = ('LanczosNet', 'AdaLanczosNet', 'LanczosNetGeneral', 'GCN', 'GCNFP', 'DCNN', 'ChebyNet',
-                  'GAT', 'GraphSAGE', 'GGNN')
+                  'GAT', 'GraphSAGE', 'GGNN', 'GPNN')
 # drop-ins that replace the reference class only when asked for (patch_namespace(opt_in=...), --opt-in)
 OPT_IN_CLASSES = ('MPNN',)
 

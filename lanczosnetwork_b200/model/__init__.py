@@ -9,4 +9,5 @@ from .cheby_net import *            # noqa: F401,F403
 from .gat import *                  # noqa: F401,F403  (inference only)
 from .graph_sage import *        # noqa: F401,F403  (Mean / Max aggregators)
 from .ggnn import *              # noqa: F401,F403
+from .gpnn import *              # noqa: F401,F403
 from .mpnn import *              # noqa: F401,F403  (a drop-in by opt-in only, see dropin.OPT_IN_CLASSES)

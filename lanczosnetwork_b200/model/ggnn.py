@@ -56,6 +56,37 @@ def gru_gate_matrix(weight_ih, weight_hh, bias_ih, bias_hh):
   return W, b
 
 
+def ggnn_step_params(cache, msg_func, cell):
+  """Stacked message weights and the re-laid-out gate matrix of one GGNN propagation step (E1 message
+  MLPs ``msg_func``, GRUCell ``cell``), split once per parameter version through ``cache``."""
+  first = [seq[0] for seq in msg_func]
+  second = [seq[2] for seq in msg_func]
+  w1_hi, w1_lo, b1 = cache.split_stacked('msg_func.0', [l.weight for l in first], [l.bias for l in first])
+  w2_hi, w2_lo, b2 = cache.split_stacked('msg_func.2', [l.weight for l in second], [l.bias for l in second])
+  return (w1_hi, w1_lo, b1), (w2_hi, w2_lo, b2), cached_gates(cache, 'update_func.gates', cell)
+
+
+def cached_gates(cache, name, cell):
+  """(hi, lo, bias) of gru_gate_matrix of the GRUCell ``cell``, rebuilt through ``cache`` when its
+  parameters change."""
+  def build():
+    W, b = gru_gate_matrix(cell.weight_ih.detach(), cell.weight_hh.detach(), cell.bias_ih.detach(),
+                           cell.bias_hh.detach())
+    return ops.split_tf32(W) + (b,)
+  return cache.derived(name, [cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh], build)
+
+
+def ggnn_step(h, prep, params, avg, out):
+  """One GGNN propagation step in three launches (the E1 first message layers stacked, the grouped
+  second layers, lnb_ggnn_update); ``params`` from ggnn_step_params, ``prep`` the binarised ELL rows.
+  h' goes to ``out``, which must not alias h."""
+  (w1_hi, w1_lo, b1), (w2_hi, w2_lo, b2), (g_hi, g_lo, g_b) = params
+  E1 = prep[0].shape[1]
+  hid = ops.linear_tf32x3(h, w1_hi, w1_lo, b1, relu=True)              # [B*N, E1*128]
+  msg = ops.linear_tf32x3_grouped(hid, w2_hi, w2_lo, b2, E1)           # [B*N, E1*D]
+  return ops.ggnn_update(msg, h, prep, g_hi, g_lo, g_b, avg, out=out)
+
+
 class GGNN(SpectralNetBase):
 
   def __init__(self, config):
@@ -162,21 +193,7 @@ class GGNN(SpectralNetBase):
             ops.ggnn_update_supported(N, self.hidden_dim, E1))
 
   def _step_params(self):
-    """Stacked message weights and the re-laid-out gate matrix, split once per parameter version."""
-    cache = self._wcache
-    first = [seq[0] for seq in self.msg_func]
-    second = [seq[2] for seq in self.msg_func]
-    w1_hi, w1_lo, b1 = cache.split_stacked('msg_func.0', [l.weight for l in first], [l.bias for l in first])
-    w2_hi, w2_lo, b2 = cache.split_stacked('msg_func.2', [l.weight for l in second], [l.bias for l in second])
-    cell = self.update_func
-
-    def build():
-      W, b = gru_gate_matrix(cell.weight_ih.detach(), cell.weight_hh.detach(), cell.bias_ih.detach(),
-                             cell.bias_hh.detach())
-      return ops.split_tf32(W) + (b,)
-    g_hi, g_lo, g_b = cache.derived('update_func.gates',
-                                    [cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh], build)
-    return (w1_hi, w1_lo, b1), (w2_hi, w2_lo, b2), (g_hi, g_lo, g_b)
+    return ggnn_step_params(self._wcache, self.msg_func, self.update_func)
 
   def _forward_impl(self, node_feat, L, mask):
     B, N = node_feat.shape
@@ -191,12 +208,10 @@ class GGNN(SpectralNetBase):
     h = ops.linear_tf32x3(x, w_hi, w_lo, lin.bias)
     # ELL rows of the 0/1 operators; no Ritz vectors (an all-zero block)
     prep = ops.graph_prepare(L, torch.zeros((B, N, 4), device=L.device, dtype=torch.float32), binarize=True)
-    (w1_hi, w1_lo, b1), (w2_hi, w2_lo, b2), (g_hi, g_lo, g_b) = self._step_params()
+    params = self._step_params()
     spare = torch.empty_like(h)
     avg = self.aggregate_type == 'avg'
     for _ in range(self.num_prop):
-      hid = ops.linear_tf32x3(h, w1_hi, w1_lo, b1, relu=True)              # [B*N, E1*128]
-      msg = ops.linear_tf32x3_grouped(hid, w2_hi, w2_lo, b2, E1)           # [B*N, E1*D]
-      h, spare = ops.ggnn_update(msg, h, prep, g_hi, g_lo, g_b, avg, out=spare), h
+      h, spare = ggnn_step(h, prep, params, avg, out=spare), h
     head, att = self.output_func[0], self.att_func[0]
     return ops.readout(h.view(B, N, D), head.weight, head.bias, att.weight.reshape(-1), att.bias, mask)

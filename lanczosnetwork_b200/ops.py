@@ -15,7 +15,7 @@ __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'sage_operators', 'neighbour_max', 'ggnn_update',
-    'ggnn_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
+    'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
     'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'set2vec', 'set2vec_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
     'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
@@ -562,6 +562,65 @@ def ggnn_update(M, h, prep, w_hi, w_lo, bias, avg, out=None):
         _stream(h), _ptr(M), _ptr(h), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi), _ptr(w_lo),
         _ptr(bias), B, N, D, E1, int(bool(avg)), _ptr(out)), 'lnb_ggnn_update')
   return out
+
+
+def gpnn_partition_update_supported(N, H):
+  """Shapes lnb_gpnn_partition_update accepts (mirrors its checks)."""
+  return 1 <= N <= 255 and H % 32 == 0 and 32 <= H <= 128
+
+
+def _rows_view(who, t, rows, H):
+  """(tensor, row stride) of a float32 CUDA [rows, H] view whose rows may be strided (a column block)."""
+  if t.dtype != torch.float32 or t.dim() != 2 or tuple(t.shape) != (rows, H) or t.stride(1) != 1:
+    raise ValueError('%s: expected a float32 [%d, %d] view with unit column stride, got %s %s stride %s'
+                     % (who, rows, H, t.dtype, tuple(t.shape), t.stride()))
+  return t, t.stride(0)
+
+
+def gpnn_partition_update(parts, prep, w_hi, w_lo, bias, avg, h_copy=None):
+  """GPNN propagation within clusters and across cuts (see lnb_gpnn_partition_update), both parts in one
+  launch.  ``parts``: two entries, (M, h, out) for the cluster and the cut operator, or None to skip that
+  part; M, h, out are float32 [B*N, H] views (rows may be strided, e.g. column blocks of the [B*N, 3H]
+  input of state_func; one row stride each for all M, all h and all outputs).  M and h may be the same
+  tensors for both parts; no output may overlap an h.  ``prep``: graph_prepare of
+  stack([L_cluster, L_cut], 3), not binarised.  w_hi / w_lo / bias: gru_gate_matrix of the partition
+  GRUCell [4H, 2H], [4H].  ``h_copy``: optional [B*N, H] view with the outputs' row stride that receives
+  the h rows of the first active part.  Returns ``parts``' outputs."""
+  ell_val, ell_idx, ell_max = prep[0], prep[1], prep[2]
+  B, two, N = ell_val.shape[0], ell_val.shape[1], ell_val.shape[2]
+  if two != 2 or len(parts) != 2:
+    raise ValueError('gpnn_partition_update: needs the ELL rows of the two partition operators and two parts')
+  live = [pt for pt in parts if pt is not None]
+  if not live:
+    raise ValueError('gpnn_partition_update: no active part')
+  H = live[0][1].shape[1]
+  rows = B * N
+  _need_cuda(w_hi, w_lo, bias, h_copy, *[t for pt in live for t in pt])
+  bias = _f32c(bias)
+  if tuple(w_hi.shape) != (4 * H, 2 * H) or tuple(w_lo.shape) != (4 * H, 2 * H) or tuple(bias.shape) != (4 * H,):
+    raise ValueError('gpnn_partition_update: W %s, bias %s do not agree with H=%d'
+                     % (tuple(w_hi.shape), tuple(bias.shape), H))
+  ptrs, strides = [], {'M': set(), 'h': set(), 'out': set()}
+  for pt in parts:
+    if pt is None:
+      ptrs += [None, None, None]
+      continue
+    for key, t in zip(('M', 'h', 'out'), pt):
+      _, ld = _rows_view('gpnn_partition_update: %s' % key, t, rows, H)
+      strides[key].add(ld)
+      ptrs.append(t)
+  if h_copy is not None:
+    strides['out'].add(_rows_view('gpnn_partition_update: h_copy', h_copy, rows, H)[1])
+  if any(len(s) != 1 for s in strides.values()):
+    raise ValueError('gpnn_partition_update: one row stride each for M, h and out, got %s' % strides)
+  ldm, ldh, ldo = strides['M'].pop(), strides['h'].pop(), strides['out'].pop()
+  dev = live[0][1].device
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_gpnn_partition_update(
+        _stream(live[0][1]), *[_ptr(t) for t in ptrs], _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi),
+        _ptr(w_lo), _ptr(bias), _ptr(h_copy), B, N, H, ldm, ldh, ldo, int(bool(avg))),
+               'lnb_gpnn_partition_update')
+  return [None if pt is None else pt[2] for pt in parts]
 
 
 MPNN_EDGE_HIDDEN = 64      # width of the edge network's hidden layer, fixed in the reference (model/mpnn.py:60)

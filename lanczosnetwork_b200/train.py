@@ -28,7 +28,7 @@ from . import ops
 
 __all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
            'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
-           'ggnn_train', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'GraphedStep']
+           'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'GraphedStep']
 
 
 def _pad_cols(x, mult=4):
@@ -353,45 +353,98 @@ def sage_train(model, node_ids, M, mask, prep=None):
   return gated_readout(model, state, mask)
 
 
+def recurrent_cell(kind, cell, x, h):
+  """The update cell of GGNN / GPNN on the tape: torch's GRUCell (``kind == 'GRU'``) or the relu RNNCell,
+  with both products in the library's dense kernel."""
+  gi = dense(x, cell.weight_ih, cell.bias_ih, False)
+  gh = dense(h, cell.weight_hh, cell.bias_hh, False)
+  if kind == 'GRU':                                                            # torch's GRUCell
+    i_r, i_z, i_n = gi.chunk(3, dim=1)
+    h_r, h_z, h_n = gh.chunk(3, dim=1)
+    r = torch.sigmoid(i_r + h_r)
+    z = torch.sigmoid(i_z + h_z)
+    n = torch.tanh(i_n + r * h_n)
+    return (h - n) * z + n
+  return torch.relu(gi + gh)                                                   # RNNCell, relu
+
+
+def _ggnn_operators(L, aggregate_type):
+  """The 0/1 pattern of L, row-normalised by (nnz + float32 eps) for ``avg``: a new tensor."""
+  A = (L != 0).float()
+  if aggregate_type == 'avg':
+    A = A / (A.sum(dim=2, keepdim=True) + _EPS)
+  return A.contiguous()
+
+
+def _ggnn_prop(model, A, h):
+  """One GGNN propagation step (model/ggnn.py:143-171, model/gpnn.py:164-190) of h [B*N, D] over the
+  operators A [B,N,N,E1]: the first message layers of all channels as one dense layer against their weights
+  concatenated on the tape, the second layers, A_e m_e, then ``model.update_func``."""
+  B, N, E1 = A.shape[0], A.shape[1], A.shape[3]
+  D = h.shape[1]
+  first = [seq[0] for seq in model.msg_func]
+  w1 = torch.cat([l.weight for l in first], dim=0)
+  b1 = torch.cat([l.bias for l in first], dim=0)
+  hw = first[0].weight.shape[0]
+  hid = dense(h, w1, b1, True)                                                 # [B*N, E1 * 128]
+  agg = []
+  for e in range(E1):
+    second = model.msg_func[e][2]
+    m_e = dense(hid[:, e * hw:(e + 1) * hw], second.weight, second.bias, False)
+    agg.append(operator_messages(A, m_e.reshape(B, N, D), e, 1))
+  agg = torch.cat(agg, dim=2).reshape(B * N, E1 * D)
+  return recurrent_cell(model.update_func_name, model.update_func, agg, h)
+
+
 def ggnn_train(model, node_ids, L, mask):
   """Differentiable GGNN (model/ggnn.py:122-197): embedding -> input_func -> num_prop steps of
   [per-channel message MLP -> A_e m_e -> GRU / RNN cell -> dropout] -> gated readout with the head
   ``output_func``.  A_e is the 0/1 pattern of L_e, row-normalised by (nnz + float32 eps) for ``avg``;
   both are new tensors (the caller's L is not modified).  The first message layers of all channels run
   as one dense layer against their weights concatenated on the tape."""
-  A = (L != 0).float()
-  if model.aggregate_type == 'avg':
-    A = A / (A.sum(dim=2, keepdim=True) + _EPS)
-  A = A.contiguous()
-  B, N, E1 = A.shape[0], A.shape[1], A.shape[3]
+  A = _ggnn_operators(L, model.aggregate_type)
+  B, N = A.shape[0], A.shape[1]
   x = embedding(node_ids, model.embedding.weight).reshape(B * N, -1)
   lin = model.input_func[0]
   h = dense(x, lin.weight, lin.bias, False)
   D = h.shape[1]
-  first = [seq[0] for seq in model.msg_func]
-  w1 = torch.cat([l.weight for l in first], dim=0)
-  b1 = torch.cat([l.bias for l in first], dim=0)
-  hw = first[0].weight.shape[0]
-  cell = model.update_func
   for _ in range(model.num_prop):
-    hid = dense(h, w1, b1, True)                                               # [B*N, E1 * 128]
-    agg = []
-    for e in range(E1):
-      second = model.msg_func[e][2]
-      m_e = dense(hid[:, e * hw:(e + 1) * hw], second.weight, second.bias, False)
-      agg.append(operator_messages(A, m_e.reshape(B, N, D), e, 1))
-    agg = torch.cat(agg, dim=2).reshape(B * N, E1 * D)
-    gi = dense(agg, cell.weight_ih, cell.bias_ih, False)
-    gh = dense(h, cell.weight_hh, cell.bias_hh, False)
-    if model.update_func_name == 'GRU':                                        # torch's GRUCell
-      i_r, i_z, i_n = gi.chunk(3, dim=1)
-      h_r, h_z, h_n = gh.chunk(3, dim=1)
-      r = torch.sigmoid(i_r + h_r)
-      z = torch.sigmoid(i_z + h_z)
-      n = torch.tanh(i_n + r * h_n)
-      h = (h - n) * z + n
-    else:                                                                      # RNNCell, relu
-      h = torch.relu(gi + gh)
+    h = _ggnn_prop(model, A, h)
+    if model.training and model.dropout > 0.0:
+      h = torch.nn.functional.dropout(h, model.dropout, True)
+  return gated_readout(model, h.reshape(B, N, D), mask, head=model.output_func[0])
+
+
+def gpnn_train(model, node_ids, L, L_cluster, L_cut, mask):
+  """Differentiable GPNN (model/gpnn.py:141-251): embedding -> input_func -> num_prop steps of
+  [num_prop_cluster (num_prop_cut) steps of msg_func[0] -> P m -> partition cell over the cluster (cut)
+  operator, both chains from the same state -> state_func on [state | cluster | cut] -> the GGNN step over
+  the 0/1 pattern of L -> dropout] -> gated readout with the head ``output_func``.  P is the valued
+  partition operator, row-normalised by (rowsum + float32 eps) for ``avg``; all operators are new tensors
+  (the caller's L, L_cluster and L_cut are not modified)."""
+  A = _ggnn_operators(L, model.aggregate_type)
+  P = torch.stack([L_cluster, L_cut], 3).float()
+  if model.aggregate_type == 'avg':
+    P = P / (P.sum(dim=2, keepdim=True) + _EPS)
+  P = P.contiguous()
+  B, N = A.shape[0], A.shape[1]
+  x = embedding(node_ids, model.embedding.weight).reshape(B * N, -1)
+  lin = model.input_func[0]
+  h = dense(x, lin.weight, lin.bias, False)
+  D = h.shape[1]
+  m1, m2 = model.msg_func[0][0], model.msg_func[0][2]
+  s1, s2 = model.state_func[0], model.state_func[2]
+  for _ in range(model.num_prop):
+    chains = []
+    for e, count in enumerate((model.num_prop_cluster, model.num_prop_cut)):
+      s = h
+      for _ in range(count):
+        m = dense(dense(s, m1.weight, m1.bias, True), m2.weight, m2.bias, False)
+        agg = operator_messages(P, m.reshape(B, N, D), e, 1).reshape(B * N, D)
+        s = recurrent_cell(model.update_func_name, model.update_func_partition, agg, s)
+      chains.append(s)
+    s = dense(dense(torch.cat([h] + chains, dim=1), s1.weight, s1.bias, True), s2.weight, s2.bias, False)
+    h = _ggnn_prop(model, A, s)
     if model.training and model.dropout > 0.0:
       h = torch.nn.functional.dropout(h, model.dropout, True)
   return gated_readout(model, h.reshape(B, N, D), mask, head=model.output_func[0])
