@@ -6,7 +6,11 @@
 //   * The S-wide first stage (S <= 8 inputs) is evaluated by the CUDA cores in plain fp32 straight
 //     into the activations of the tile -- a tensor-core step for K = 8 would cost a full
 //     accumulator hand-over for 2 % of the flops.  (S > 8 runs it as an MMA step.)
-//   * The other stages are accumulator lifetimes ("steps") of the 3xTF32 skeleton in tc_gemm.cuh.
+//   * Likewise the S-wide output stage (S <= 8 outputs): the epilogue of stage 2 finishes a row,
+//     and the thread that owns it takes its S dot products with the stage-3 weights in fp32 (a
+//     128-wide MMA for 8 columns would be another full hand-over).  (S > 8 runs it as an MMA step.)
+//   * The other stages are accumulator lifetimes ("steps") of the 3xTF32 skeleton in tc_gemm.cuh:
+//     two per item for S <= 8, four for S > 8.
 //     Activations NEVER leave the SM: they live in shared memory, one row per producer thread;
 //     the epilogue of stage s applies bias + ReLU and overwrites the thread's own row, which the
 //     producers of stage s+1 read back as their k-blocks.
@@ -14,7 +18,7 @@
 
 namespace {
 
-constexpr int S0MAX = 8;                 // first-stage widths the CUDA cores handle
+constexpr int S0MAX = 8;                 // first / output stage widths the CUDA cores handle
 constexpr int AP = tcg::BN + 4;          // row pitch of the activation tile (floats)
 
 struct ChainPolicy {
@@ -24,7 +28,7 @@ struct ChainPolicy {
     const float* table;     // [Rall, S]  powers of the Ritz values
     const int32_t* rowmap;  // [Rall]     compact list of rows to evaluate (nullptr: all rows)
     const int32_t* nrows;   // [1]        number of valid entries in rowmap (nullptr: Rall)
-    const float* W_hi;      // [L * (3*Hd + S), Hd] split weights (the first stage reads hi + lo)
+    const float* W_hi;      // [L * (3*Hd + S), Hd] split weights (the CUDA-core stages read hi + lo)
     const float* W_lo;
     const float* bias_all;  // [L * (3*Hd + S)]
     float* coeff;           // [L, Rall, S]
@@ -32,20 +36,33 @@ struct ChainPolicy {
     int dbg;                // debug experiment flags (LNB_DBG), 0 in production
   };
   // sub = layer * 4 + stage
+  // S <= 8: stages 0 and 3 run on the CUDA cores, S > 8: all four stages are MMA steps
   static __device__ __forceinline__ bool mma0(const Params& p) { return p.S > S0MAX; }
   static __device__ __forceinline__ int first_stage(const Params& p) { return mma0(p) ? 0 : 1; }
+  static __device__ __forceinline__ int steps_per_item(const Params& p) { return mma0(p) ? 4 : 2; }
   static __device__ __forceinline__ int rows(const Params& p) { return p.nrows ? __ldg(p.nrows) : p.Rall; }
   static __device__ __forceinline__ int ntile(const Params& p) { return (rows(p) + tcg::BM - 1) / tcg::BM; }
-  static __device__ __forceinline__ int num_steps(const Params& p, int cta, int ncta) {
-    const int items = ntile(p) * p.L;
-    const int mine = items > cta ? (items - cta + ncta - 1) / ncta : 0;
-    return mine * (4 - first_stage(p));
+  // Items are numbered layer-major, and every CTA runs one contiguous range of them: a CTA's
+  // consecutive items share the layer, so the CUDA-core stages' weights are staged once per
+  // layer change (one or two per CTA) instead of at almost every item.  (All layers' weights sit
+  // in L2 together.)
+  static __device__ __forceinline__ void item_range(const Params& p, int cta, int ncta, int& first,
+                                                    int& count) {
+    const int items = ntile(p) * p.L, base = items / ncta, rem = items % ncta;
+    count = base + (cta < rem ? 1 : 0);
+    first = cta * base + min(cta, rem);
   }
-  // items in layer-major order: CTAs running at the same time share the layer's weights in L2
+  static __device__ __forceinline__ int num_steps(const Params& p, int cta, int ncta) {
+    int first, count;
+    item_range(p, cta, ncta, first, count);
+    return count * steps_per_item(p);
+  }
   static __device__ __forceinline__ void decode(const Params& p, int cta, int ncta, int it,
                                                 int& m_tile, int& sub) {
-    const int per = 4 - first_stage(p), nt = ntile(p);
-    const int item = cta + (it / per) * ncta;
+    const int per = steps_per_item(p), nt = ntile(p);
+    int first, count;
+    item_range(p, cta, ncta, first, count);
+    const int item = first + it / per;
     m_tile = item % nt;
     sub = (item / nt) * 4 + first_stage(p) + it % per;
   }
@@ -65,15 +82,21 @@ struct ChainPolicy {
   float* act;               // [BM][AP] activations, row r <-> producer thread r
   float* W1s;               // [BN][S0MAX] first-stage weights (hi + lo)
   float* b1s;               // [BN]
+  float* W3s;               // [BN][S0MAX] output-stage weights (hi + lo), transposed: W3s[c][s] = W3[s][c]
+  float* b3s;               // [S0MAX]
   int src, cur_layer;
 
-  static size_t smem_bytes() { return ((size_t)tcg::BM * AP + tcg::BN * S0MAX + tcg::BN) * 4; }
+  static size_t smem_bytes() {
+    return ((size_t)tcg::BM * AP + 2 * (tcg::BN * S0MAX) + tcg::BN + S0MAX) * 4;
+  }
 
   __device__ ChainPolicy(const Params& p_, uint8_t* smem, int tid_)
       : p(p_), tid(tid_), r(tid_ & 127), src(-1), cur_layer(-1) {
     act = reinterpret_cast<float*>(smem);
     W1s = act + (size_t)tcg::BM * AP;
     b1s = W1s + tcg::BN * S0MAX;
+    W3s = b1s + tcg::BN;
+    b3s = W3s + tcg::BN * S0MAX;
   }
 
   __device__ void step_begin(int m_tile, int sub, int, tcg::PhaseTimer&) {
@@ -83,15 +106,19 @@ struct ChainPolicy {
     src = i < rows(p) ? (p.rowmap ? __ldg(p.rowmap + i) : i) : -1;
     if (mma0(p)) return;
     // ---- first stage on the CUDA cores: act = ReLU(W1 t + b1) ---------------------------------
-    if (layer != cur_layer) {                             // stage this layer's W1 (hi + lo), b1
+    if (layer != cur_layer) {        // stage this layer's W1, b1 and (for store()) W3, b3 (hi + lo)
       tcg::producers_sync();
-      const int row0 = w_row0(p, layer, 0);
+      const int row0 = w_row0(p, layer, 0), row3 = w_row0(p, layer, 3);
+#pragma unroll 4
       for (int e = tid; e < p.Hd * S0MAX; e += tcg::PRODUCER_THREADS) {
         const int c = e / S0MAX, k = e - c * S0MAX;
         const int64_t o = (int64_t)(row0 + c) * p.Hd + k;
         W1s[e] = (k < p.S) ? __ldg(p.W_hi + o) + __ldg(p.W_lo + o) : 0.f;
+        const int64_t o3 = (int64_t)(row3 + k) * p.Hd + c;
+        W3s[e] = (k < p.S) ? __ldg(p.W_hi + o3) + __ldg(p.W_lo + o3) : 0.f;
       }
       for (int c = tid; c < p.Hd; c += tcg::PRODUCER_THREADS) b1s[c] = __ldg(p.bias_all + row0 + c);
+      if (tid < S0MAX) b3s[tid] = tid < p.S ? __ldg(p.bias_all + row3 + tid) : 0.f;
       tcg::producers_sync();
       cur_layer = layer;
     }
@@ -100,6 +127,7 @@ struct ChainPolicy {
     for (int k = 0; k < S0MAX; ++k)
       tv[k] = (src >= 0 && k < p.S) ? __ldg(p.table + (int64_t)src * p.S + k) : 0.f;
     float* row = act + (size_t)r * AP;
+#pragma unroll 4                                          // four independent 8-FMA chains in flight
     for (int c = 0; c < p.Hd; ++c) {
       const float4* wr = reinterpret_cast<const float4*>(W1s + c * S0MAX);
       const float4 wa = wr[0], wb = wr[1];
@@ -137,6 +165,7 @@ struct ChainPolicy {
       float* dst = act + (size_t)r * AP + col;
 #pragma unroll
       for (int j = 0; j < tcg::EW; ++j) dst[j] = fmaxf(x[j] + __ldg(bias + col + j), 0.f);
+      if (stage == 2 && !mma0(p) && col + tcg::EW >= p.Hd) output_stage(layer);
       return;
     }
     if (src < 0 || col >= p.S) return;
@@ -144,6 +173,34 @@ struct ChainPolicy {
 #pragma unroll
     for (int j = 0; j < tcg::EW; ++j)
       if (col + j < p.S) dst[col + j] = x[j] + __ldg(bias + col + j);
+  }
+
+  // ---- output stage on the CUDA cores (S <= 8): coeff = W3 act + b3 --------------------------
+  // Called by store() once this thread's row of stage 2 is complete; the row is read back from
+  // `act` (written by this thread alone) and summed in ascending column order.
+  __device__ __forceinline__ void output_stage(int layer) {
+    if (src < 0) return;
+    const float4* a4 = reinterpret_cast<const float4*>(act + (size_t)r * AP);
+    float o[S0MAX];
+#pragma unroll
+    for (int s = 0; s < S0MAX; ++s) o[s] = 0.f;
+    for (int c4 = 0; c4 < p.Hd / 4; ++c4) {
+      const float4 a = a4[c4];
+      const float av[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const float4* wr = reinterpret_cast<const float4*>(W3s + (4 * c4 + u) * S0MAX);
+        const float4 wa = wr[0], wb = wr[1];
+        o[0] = fmaf(av[u], wa.x, o[0]); o[1] = fmaf(av[u], wa.y, o[1]);
+        o[2] = fmaf(av[u], wa.z, o[2]); o[3] = fmaf(av[u], wa.w, o[3]);
+        o[4] = fmaf(av[u], wb.x, o[4]); o[5] = fmaf(av[u], wb.y, o[5]);
+        o[6] = fmaf(av[u], wb.z, o[6]); o[7] = fmaf(av[u], wb.w, o[7]);
+      }
+    }
+    float* dst = p.coeff + ((int64_t)layer * p.Rall + src) * p.S;
+#pragma unroll
+    for (int s = 0; s < S0MAX; ++s)
+      if (s < p.S) dst[s] = o[s] + b3s[s];
   }
 };
 

@@ -333,13 +333,19 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
   for (int i = tid; i < SCH_NCLS; i += 1024) hist[i] = 0;
   __syncthreads();
   // class = (128 - n_eff) * 33 + (32 - k_eff): ascending class = n_eff descending, then k_eff descending
+  // A batch has few classes, so the lanes of a warp that share one add to it once.
   bool big = false;
-  for (int b = tid; b < B; b += 1024) {
-    const int n = gext[b * 2];
-    big |= n > RMAX;
-    const int c = (RMAX - min(n, RMAX)) * SCH_KC + (KMAX - min(gext[b * 2 + 1], K));
-    key[b] = c;
-    atomicAdd(&hist[c], 1);
+  for (int b0 = 0; b0 < B; b0 += 1024) {
+    const int b = b0 + tid;
+    int c = -1;
+    if (b < B) {
+      const int n = gext[b * 2];
+      big |= n > RMAX;
+      c = (RMAX - min(n, RMAX)) * SCH_KC + (KMAX - min(gext[b * 2 + 1], K));
+      key[b] = c;
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, c);
+    if (c >= 0 && lane == __ffs(peers) - 1) atomicAdd(&hist[c], __popc(peers));
   }
   if (__syncthreads_or(big)) {
     identity_schedule(tiles, B, run_n);
@@ -372,12 +378,12 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
   __syncthreads();
   const int ncls = run_k;
   if (warp == 0) {
-    // first-fit of whole classes.  Lane l owns the tiles [l P, l P + P) (P = ceil(T' / 32)): the free
-    // room of its tiles, one warp scan, then each lane fills its own tiles in order.  Placement
-    // records are independent of each other, so they take their index from a shared counter.
-    int T2 = 0;
-    if (lane == 0) run_r = 0;
-    __syncwarp();
+    // first-fit of whole classes, 32 tiles at a time: lane l looks at tile t0 + l.  A ballot skips
+    // the chunks where no tile has room for the class; in the others one warp scan of the room
+    // gives every tile, in tile order, the graphs it takes, and a second ballot numbers the
+    // placement records.  A class stops at the chunk that uses it up, so a class that fits in
+    // the first tiles costs one or two chunks however many tiles are open.
+    int T2 = 0, nrec = 0;
     for (int i0 = 0; i0 < ncls; i0 += 32) {
       // lane j describes class i0 + j: first position in `order`, count, n_eff, k_eff, and
       // ceil(2^16 / n), ceil(2^16 / k) for floor(free / n) = free * ceil(2^16 / n) >> 16 (exact for
@@ -398,47 +404,36 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
         const int n = __shfl_sync(0xffffffffu, c_n, j), k = __shfl_sync(0xffffffffu, c_k, j);
         const int rn = __shfl_sync(0xffffffffu, c_rn, j), rk = __shfl_sync(0xffffffffu, c_rk, j);
         const int ce = __shfl_sync(0xffffffffu, c_ce, j);
-        int done = 0;
-        if (T2 > 0) {
-          const int P = (T2 + 31) >> 5, t0 = lane * P, t1 = min(t0 + P, T2);
-          int room = 0;
-          for (int t = t0; t < t1; ++t) {
-            const int st = tst[t];
-            int cap = GMAX - (st >> 16);
-            if (n) cap = min(cap, ((RMAX - (st & 255)) * rn) >> 16);
-            if (k) cap = min(cap, ((RMAX - ((st >> 8) & 255)) * rk) >> 16);
-            room += cap;
-          }
-          int inc = room;
+        int done = 0;                                  // graphs of the class placed so far
+        for (int t0 = 0; t0 < T2 && done < count; t0 += 32) {
+          const int t = t0 + lane;
+          const int st = t < T2 ? tst[t] : GMAX << 16; // past the last open tile: no room
+          int cap = GMAX - (st >> 16);
+          if (n) cap = min(cap, ((RMAX - (st & 255)) * rn) >> 16);
+          if (k) cap = min(cap, ((RMAX - ((st >> 8) & 255)) * rk) >> 16);
+          if (!__ballot_sync(0xffffffffu, cap > 0)) continue;
+          int inc = cap;
 #pragma unroll
           for (int o = 1; o < 32; o <<= 1) {
             const int v = __shfl_up_sync(0xffffffffu, inc, o);
             if (lane >= o) inc += v;
           }
-          int left = count - (inc - room);             // graphs still unplaced when this lane's tiles come
-          int src = first + inc - room;
-          for (int t = t0; t < t1 && left > 0 && room > 0; ++t) {
-            const int st = tst[t];
-            int cap = GMAX - (st >> 16);
-            if (n) cap = min(cap, ((RMAX - (st & 255)) * rn) >> 16);
-            if (k) cap = min(cap, ((RMAX - ((st >> 8) & 255)) * rk) >> 16);
-            const int m = min(cap, left);
-            if (m > 0) {
-              const int r = atomicAdd(&run_r, 1);
-              rec_t[r] = t;
-              rec_src[r] = src;
-              rec_sm[r] = (st >> 16) | (m << 8);
-              tst[t] = st + m * n + ((m * k) << 8) + (m << 16);
-              left -= m;
-              src += m;
-            }
+          const int m = min(cap, count - done - (inc - cap));   // <= 0: the class is used up before tile t
+          const unsigned took = __ballot_sync(0xffffffffu, m > 0);
+          if (m > 0) {
+            const int r = nrec + __popc(took & ((1u << lane) - 1));
+            rec_t[r] = t;
+            rec_src[r] = first + done + inc - cap;
+            rec_sm[r] = (st >> 16) | (m << 8);
+            tst[t] = st + m * n + ((m * k) << 8) + (m << 16);
           }
-          done = min(count, __shfl_sync(0xffffffffu, inc, 31));
+          nrec += __popc(took);
+          done = min(count, done + __shfl_sync(0xffffffffu, inc, 31));
         }
         if (done < count) {                            // the rest opens new tiles, each as full as the limits allow
           const int rem = count - done, nt = (rem + ce - 1) / ce;
-          const int r0 = lane == 0 ? atomicAdd(&run_r, nt) : 0;
-          const int rb = __shfl_sync(0xffffffffu, r0, 0);
+          const int rb = nrec;
+          nrec += nt;
           for (int q = lane; q < nt; q += 32) {
             const int m = min(ce, rem - q * ce);
             rec_t[rb + q] = T2 + q;
@@ -451,7 +446,7 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
         __syncwarp();
       }
     }
-    if (lane == 0) run_n = T2;
+    if (lane == 0) { run_n = T2; run_r = nrec; }
   } else {
     // stable counting sort: warp w gathers the graphs of classes w - 1, w + 30, ... in index order
     for (int i = warp - 1; i < ncls; i += 31) {
