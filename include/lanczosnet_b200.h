@@ -473,6 +473,37 @@ int lnb_tridiag_ritz(lnb_stream_t stream, const float* alpha, const float* beta,
                      int32_t* status /* [B] */);
 
 /* ---------------------------------------------------------------------------------------
+ * Exact eigenpairs of every graph's simple-graph operator, in fp64: the reference's offline
+ * preprocessing (utils/data_helper.py:169-226 dense eigh branch, dataset/get_qm8_data.py:63-83,
+ * truncated / zero padded to K at collate, dataset/qm8.py:265-291) on the device.  Householder
+ * tridiagonalisation, implicit-shift QL with the rotations accumulated, then the back-transform of the
+ * kept columns only.  Graph b's operator is the leading n_b x n_b block, n_b = min(sizes[b], N);
+ * its lower triangle is read (numpy's eigh default).
+ * Outputs: D [B,K] = the eigenvalues by descending |lambda|, equal |lambda| by ascending lambda
+ * (np.argsort(-|w|, kind='mergesort') over eigh's ascending order), the first min(n_b, K) of them,
+ * then 0; the matching unit eigenvectors (columns >= min(n_b, K) and rows >= n_b are 0).  Every output
+ * is one rounding of an fp64 value.  Eigenvectors are defined up to sign and, for a repeated
+ * eigenvalue, up to a rotation inside its eigenspace.  status[b]: bit 0 = QL sweeps exhausted.
+ * One warp per graph for N <= 32, one CTA per graph above; repeated launches are bit-identical.
+ * Envelope: 1 <= N <= 128, 1 <= K <= 128 (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ *
+ * lnb_graph_eigs_sparse: the operator is the fp64 L4 = D^-1/2 (A + I) D^-1/2 of the simple graph
+ *   (A summed over bond types; a bond listed twice with one type counts once), built from the sparse
+ *   records of lnb_graph_prepare_sparse (sizes, node_ptr, edge_ptr, edges with bond types < E,
+ *   1 <= E <= 32, inv_sqrt_deg) with the same fp64 products in the same order, so the solver's input
+ *   is bit for bit the matrix the reference hands eigh.  V_rows [node_ptr[B], K]: the rows of the real
+ *   nodes, the layout lnb_graph_prepare_sparse reads (data.sparse_collate's).
+ * lnb_sym_eigs: the operator is the fp32 A[((b*N + i)*N + j) * elem_stride] (elem_stride = E1 reads
+ *   channel 0 of L [B,N,N,E1] in place), widened to fp64; V [B,N,K] padded.
+ * ------------------------------------------------------------------------------------- */
+int lnb_graph_eigs_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
+                          const int32_t* edge_ptr, const uint8_t* edges, const double* inv_sqrt_deg, int B,
+                          int N, int E, int K, float* D /* [B,K] */, float* V_rows /* [node_ptr[B],K] */,
+                          int32_t* status /* [B] */);
+int lnb_sym_eigs(lnb_stream_t stream, const float* A, int64_t elem_stride, const int32_t* sizes, int B, int N,
+                 int K, float* D /* [B,K] */, float* V /* [B,N,K] */, int32_t* status /* [B] */);
+
+/* ---------------------------------------------------------------------------------------
  * The north-star pipeline in ONE launch: operator -> K-step Lanczos (rules of
  * model/ada_lanczos_net.py:139-247, as lnb_lanczos_tridiag) -> implicit-shift QL on (alpha, beta)
  * -> Ritz vectors V = Q S ordered by descending |theta| (utils/data_helper.py:217-223) -- the pair

@@ -73,18 +73,24 @@ def get_graph_laplacian_eigs(adj, k=100, graph_laplacian_type='L4'):
   return vals[order], vecs[:, order], lap
 
 
-def prepare_graph(adjs, node_feat, label=None):
-  """Per-graph record with the keys the collate step reads."""
+def prepare_graph(adjs, node_feat, label=None, eigs=True):
+  """Per-graph record with the keys the collate step reads.  ``eigs=False`` skips the host eigh: the
+  record then has no ``D_simple`` / ``V_simple`` and the eigenpairs are computed on the device
+  (``sparse_collate(..., eigs=False)`` -> ``LanczosNet.forward_sparse``, or ``ops.sym_eigs``)."""
   adjs = np.asarray(adjs, dtype=np.float64)
   if adjs.ndim == 2:
     adjs = adjs[:, :, None]
-  D, V, L4 = get_graph_laplacian_eigs(adjs.sum(axis=2))
+  if eigs:
+    D, V, L4 = get_graph_laplacian_eigs(adjs.sum(axis=2))
+  else:
+    L4 = get_laplacian(adjs.sum(axis=2))
   L_multi = np.stack([get_laplacian(adjs[:, :, e]) for e in range(adjs.shape[2])], axis=2)
   # bond list {u, v, type}, u <= v, each undirected bond once: the sparse record sparse_collate ships
   edges = np.array([(u, v, c) for c in range(adjs.shape[2])
                     for u, v in zip(*np.nonzero(np.triu(adjs[:, :, c])))], dtype=np.uint8).reshape(-1, 3)
-  rec = {'node_feat': np.asarray(node_feat), 'L_multi': L_multi, 'L_simple_4': L4,
-         'D_simple': D, 'V_simple': V, 'edges': edges}
+  rec = {'node_feat': np.asarray(node_feat), 'L_multi': L_multi, 'L_simple_4': L4, 'edges': edges}
+  if eigs:
+    rec['D_simple'], rec['V_simple'] = D, V
   if label is not None:
     rec['label'] = np.asarray(label)
   return rec
@@ -208,7 +214,7 @@ def sage_collate(samples, num_sample_neighbors, npr):
   return out
 
 
-def sparse_collate(samples, num_eigs):
+def sparse_collate(samples, num_eigs, eigs=True):
   """The same batch as ``collate`` in SPARSE form for the GPU-side batch construction
   (ops.graph_prepare_sparse / LanczosNet.forward_sparse): nothing is padded on the host and the
   dense operators are not shipped at all.
@@ -216,7 +222,9 @@ def sparse_collate(samples, num_eigs):
   Returns numpy arrays: sizes [B] int32, node_ptr [B+1] int32 (prefix sums), node_feat [sum n] int32,
   edge_ptr [B+1] int32, edges [sum E, 4] uint8 = {u, v, bond type, 0}, D [B,K] float32 (truncated /
   zero padded like dataset/qm8.py:268-287), V_rows [sum n, K] float32 (rows of real nodes only),
-  N = batch-max node count (the reference's padding target), num_edgetype, label if present."""
+  N = batch-max node count (the reference's padding target), num_edgetype, label if present.
+  ``eigs=False`` (records of ``prepare_graph(..., eigs=False)`` do): no D and no V_rows, only K = num_eigs;
+  forward_sparse then computes the eigenpairs on the device (ops.graph_eigs_sparse)."""
   sizes = np.array([s['L_simple_4'].shape[0] for s in samples], np.int32)
   B = len(samples)
   node_ptr = np.zeros(B + 1, np.int32)
@@ -225,16 +233,20 @@ def sparse_collate(samples, num_eigs):
   edge_ptr[1:] = np.cumsum([len(s['edges']) for s in samples])
   node_feat = np.concatenate([np.asarray(s['node_feat']).astype(np.int32) for s in samples])
   edges = np.zeros((int(edge_ptr[-1]), 4), np.uint8)
-  D = np.zeros((B, num_eigs), np.float32)
-  V_rows = np.zeros((int(node_ptr[-1]), num_eigs), np.float32)
   for b, s in enumerate(samples):
     edges[edge_ptr[b]:edge_ptr[b + 1], :3] = s['edges']
-    kk = min(num_eigs, s['D_simple'].shape[0])
-    D[b, :kk] = s['D_simple'][:kk]
-    V_rows[node_ptr[b]:node_ptr[b + 1], :kk] = s['V_simple'][:, :kk]
-  out = {'sizes': sizes, 'node_ptr': node_ptr, 'node_feat': node_feat, 'edge_ptr': edge_ptr,
-         'edges': edges, 'D': D, 'V_rows': V_rows, 'N': int(sizes.max()),
-         'num_edgetype': int(samples[0]['L_multi'].shape[2])}
+  out = {'sizes': sizes, 'node_ptr': node_ptr, 'node_feat': node_feat, 'edge_ptr': edge_ptr, 'edges': edges}
+  if eigs:
+    D = np.zeros((B, num_eigs), np.float32)
+    V_rows = np.zeros((int(node_ptr[-1]), num_eigs), np.float32)
+    for b, s in enumerate(samples):
+      kk = min(num_eigs, s['D_simple'].shape[0])
+      D[b, :kk] = s['D_simple'][:kk]
+      V_rows[node_ptr[b]:node_ptr[b + 1], :kk] = s['V_simple'][:, :kk]
+    out['D'], out['V_rows'] = D, V_rows
+  else:
+    out['K'] = int(num_eigs)
+  out['N'], out['num_edgetype'] = int(sizes.max()), int(samples[0]['L_multi'].shape[2])
   if 'label' in samples[0]:
     out['label'] = np.concatenate([np.asarray(s['label'], np.float32).reshape(1, -1)
                                    for s in samples], axis=0)

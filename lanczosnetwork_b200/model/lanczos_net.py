@@ -51,7 +51,10 @@ class LanczosNet(SpectralNetBase):
     padded operators, mask, ELL rows and tile table are built on the device
     (lnb_graph_prepare_sparse); the dense B x N x N x (E+1) tensor of the reference's collate
     (dataset/qm8.py:220-262) is never materialised and never crosses PCIe.  Same scores as
-    ``forward`` on the collated batch, bit for bit.  Returns score or (score, loss)."""
+    ``forward`` on the collated batch, bit for bit.  A batch without ``V_rows`` and ``D``
+    (``data.sparse_collate(..., eigs=False)``: bond lists and K only) gets the reference's eigenpairs
+    from one lnb_graph_eigs_sparse launch in front of the batch construction, inside the same CUDA
+    graph: no host eigh and no eigenvector bytes on the bus.  Returns score or (score, loss)."""
     if self._check_mode():
       raise NotImplementedError('forward_sparse is an inference path; train through forward()')
     dev = self._device()
@@ -65,6 +68,13 @@ class LanczosNet(SpectralNetBase):
                                   extra_key=('packed', B, N, K))
       return self._finish(score, self._to(dev, label))
     N, B = int(batch['N']), int(batch['sizes'].shape[0])
+    if 'V_rows' not in batch and 'D' not in batch:
+      K = int(batch['K'])
+      inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
+                Ragged(batch['edges']))
+      score = self._graph_forward(lambda *a: self._forward_sparse_eigs_impl(N, K, *a), inputs,
+                                  extra_key=('sparse_eigs', N, K))
+      return self._finish(score, self._to(dev, label))
     inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
               Ragged(batch['edges']), Ragged(batch['V_rows'], B * N), batch['D'])
     score = self._graph_forward(lambda *a: self._forward_sparse_impl(N, *a), inputs,
@@ -89,3 +99,10 @@ class LanczosNet(SpectralNetBase):
         binarize=getattr(self, '_binarize_operators', False), want_dense=dense)
     return self._ritz_conv_stack(None, node_ids, L, D.float().contiguous(), V, mask, prep=prep,
                                  dims_hint=(N, E1))
+
+  def _forward_sparse_eigs_impl(self, N, K, sizes, node_ptr, node_feat, edge_ptr, edges):
+    # V_rows has node_feat's rows (the static capacity under graph replay); rows past node_ptr[B] are
+    # written by nobody and read by nobody
+    D, V_rows, _ = ops.graph_eigs_sparse(sizes, node_ptr, edge_ptr, edges, N, K,
+                                         num_edgetype=self.num_edgetype, rows=node_feat.shape[0])
+    return self._forward_sparse_impl(N, sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, D)

@@ -13,7 +13,8 @@ from ._lib import GemmDesc, SpectralStack
 
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
-    'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
+    'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
+    'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'sage_operators', 'neighbour_max', 'ggnn_update',
     'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
     'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'set2vec', 'set2vec_supported',
@@ -298,6 +299,53 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows = rowmap, nrows
   return prep, node_ids, mask, V, L
+
+
+def graph_eigs_sparse(sizes, node_ptr, edge_ptr, edges, N, K, num_edgetype=32, rows=None):
+  """Exact eigenpairs of every molecule's simple-graph L4 from its bond list (lnb_graph_eigs_sparse):
+  what the reference's preprocessing computes with fp64 eigh, truncated / zero padded to K.
+  sizes [B], node_ptr [B+1], edge_ptr [B+1] int32, edges [>= edge_ptr[B], 4] uint8 -- all CUDA, the
+  records of data.sparse_collate; bonds of type >= num_edgetype are ignored.  ``rows``: row count of
+  V_rows, at least node_ptr[B] (default: node_ptr[B], read from the device; rows past it stay unwritten).
+  Returns (D [B,K], V_rows [rows, K] in sparse_collate's layout, status [B] int32)."""
+  _need_cuda(sizes, node_ptr, edge_ptr, edges)
+  assert sizes.dtype == torch.int32 and node_ptr.dtype == torch.int32 and edge_ptr.dtype == torch.int32
+  assert edges.dtype == torch.uint8 and edges.shape[1] == 4 and edges.is_contiguous()
+  dev = sizes.device
+  B = sizes.shape[0]
+  if rows is None:
+    rows = int(node_ptr[-1]) if B else 0
+  D = torch.empty((B, int(K)), device=dev, dtype=torch.float32)
+  V_rows = torch.empty((int(rows), int(K)), device=dev, dtype=torch.float32)
+  status = torch.empty((B,), device=dev, dtype=torch.int32)
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_graph_eigs_sparse(
+        _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(edge_ptr), _ptr(edges), _ptr(_inv_sqrt_deg_table(dev)),
+        B, int(N), int(num_edgetype), int(K), _ptr(D), _ptr(V_rows), _ptr(status)), 'lnb_graph_eigs_sparse')
+  return D, V_rows, status
+
+
+def sym_eigs(A, sizes, K):
+  """Exact eigenpairs of the leading sizes[b] x sizes[b] block of every symmetric operator (lnb_sym_eigs),
+  ordered and padded like the reference's preprocessing.  A: [B,N,N] or [B,N,N,E1] (channel 0 is read
+  in place); sizes [B] (any integer dtype).  Returns (D [B,K], V [B,N,K], status [B] int32)."""
+  _need_cuda(A, sizes)
+  if A.dim() == 4:
+    A = A[..., 0]
+  if A.dtype != torch.float32:
+    A = A.float()
+  B, N = A.shape[0], A.shape[1]
+  es = A.stride(2)
+  if es < 1 or tuple(A.stride()) != (N * N * es, N * es, es):
+    A, es = A.contiguous(), 1
+  sizes = sizes.to(torch.int32).contiguous()
+  D = torch.empty((B, int(K)), device=A.device, dtype=torch.float32)
+  V = torch.empty((B, N, int(K)), device=A.device, dtype=torch.float32)
+  status = torch.empty((B,), device=A.device, dtype=torch.int32)
+  with torch.cuda.device(A.device):
+    _lib.check(_lib.load().lnb_sym_eigs(_stream(A), _ptr(A), int(es), _ptr(sizes), B, N, int(K), _ptr(D), _ptr(V),
+                                        _ptr(status)), 'lnb_sym_eigs')
+  return D, V, status
 
 
 def fused_conv_supported(N, Din, K, H, n_short, dense_filter, S=8, E1=7):

@@ -17,12 +17,17 @@ MAE": K Lanczos steps from one start vector span a Krylov space, so
 
 ``tools/study_online_eigs.py`` measures all three effects and what they do to LanczosNet's scores
 (profiles/r2_online_eigs_study.md).
+
+``exact_eigenpairs`` is the other provider: an fp64 Householder + QL eigensolver on the device
+(lnb_sym_eigs) that reproduces the reference's preprocessing itself -- every eigenpair, the top K by
+|lambda| in the reference's order -- so a checkpoint trained on the reference's inputs sees the same
+inputs.
 """
 import torch
 
 from . import ops
 
-__all__ = ['online_ritz_pairs']
+__all__ = ['online_ritz_pairs', 'exact_eigenpairs']
 
 
 def online_ritz_pairs(L, mask, num_eigs, q1=None, generator=None):
@@ -39,3 +44,24 @@ def online_ritz_pairs(L, mask, num_eigs, q1=None, generator=None):
     q1 = torch.randn(B, N, device=A.device, generator=generator)
   out = ops.lanczos_ritz(A, mask, q1, int(num_eigs), want_T=False, want_Q=False, proper=True)
   return out['theta'], out['V'], {'idx': out['idx'], 'status': out['status']}
+
+
+def exact_eigenpairs(L, sizes_or_mask, num_eigs):
+  """(D [B,K], V [B,N,K], info) from channel 0 of the padded operator tensor L [B,N,N,E+1] (or a
+  [B,N,N] operator), ready for ``LanczosNet.forward`` / ``LanczosNetGeneral.forward``.
+
+  Unlike ``online_ritz_pairs`` this REPRODUCES the reference's preprocessing (dense fp64 eigh,
+  utils/data_helper.py:169-226, truncated / zero padded at collate, dataset/qm8.py:265-291): the
+  eigenvalues of the leading n_b x n_b block by descending |lambda| (ties by ascending lambda), the
+  first min(n_b, K), then zeros; repeated eigenvalues keep their whole eigenspace.  The eigenvectors
+  match the reference's up to sign and up to a rotation inside a repeated eigenvalue's eigenspace,
+  which the models do not see.  The solver reads the fp32 operator; the reference decomposed it in fp64
+  before the cast, so eigenvalues agree to about 1e-7.
+
+  sizes_or_mask: [B] real node counts, or a [B,N] node mask whose real nodes lead (the reference's
+  padding).  info: dict(status [B] int32, bit 0 = QL did not converge)."""
+  s = sizes_or_mask
+  if s.dim() == 2:
+    s = (s != 0).sum(dim=1)
+  D, V, status = ops.sym_eigs(L, s.to(L.device), int(num_eigs))
+  return D, V, {'status': status}
