@@ -267,21 +267,10 @@ int lnb_ritz_filter_mlp(lnb_stream_t stream, const float* table, const int32_t* 
     return LNB_ERR_UNSUPPORTED;
   }
   if (Rall == 0) return LNB_OK;
-  const int wrows = L * (3 * Hd + S);
-  CUtensorMap map_hi, map_lo;
-  int rc = tcg::make_weight_map(&map_hi, W_hi, wrows, Hd, "ritz_filter_mlp");
-  if (rc != LNB_OK) return rc;
-  rc = tcg::make_weight_map(&map_lo, W_lo, wrows, Hd, "ritz_filter_mlp");
-  if (rc != LNB_OK) return rc;
   const size_t smem = tcg::core_smem(ChainPolicy::kStagesB, ChainPolicy::kStagesA) + 1024 + ChainPolicy::smem_bytes();
-  auto kern = tcg::tc_gemm_kernel<ChainPolicy>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   ChainPolicy::Params p{table, rowmap, nrows, W_hi, W_lo, bias_all, coeff, Rall, L, S, Hd, tcg::debug_flags()};
-  const int items = lnb::ceil_div(Rall, tcg::BM) * L;
-  const int grid = items < tcg::sm_count() ? items : tcg::sm_count();
-  kern<<<grid, tcg::THREADS, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
-  lnb::count_launch();
-  return lnb::finish_launch("ritz_filter_mlp");
+  return tcg::launch<ChainPolicy>(stream, W_hi, W_lo, L * (3 * Hd + S), Hd, smem, lnb::ceil_div(Rall, tcg::BM) * L, p,
+                                  "ritz_filter_mlp");
 }
 
 }  // extern "C"

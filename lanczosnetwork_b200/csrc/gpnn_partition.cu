@@ -5,75 +5,48 @@
 // msg_func[0] and the GRU weights of update_func_partition (input width H).  Unlike lnb_ggnn_update the
 // operator VALUES enter: the partition operators are L4 Laplacians D^-1/2 (I + A_part) D^-1/2.
 //
-// A policy of the persistent 3xTF32 wgmma skeleton (tc_gemm.cuh) over plain 128-row tiles of the B*N
-// rows.  Work items are (row tile, part, column tile), column tiles innermost: the items of one row
-// tile run on neighbouring CTAs at the same time, so the gathers of both parts share L2.  The GEMM is
-//     G[r, :] = [agg_p(r) | h_p(r)] @ W^T,     W = gru_gate_matrix of update_func_partition [4H, 2H]
-// and its A operand is produced by the CUDA-core warps: the first H/32 k-blocks are the weighted sum of
-// the M_p rows of node n's neighbours, gathered through the ELL rows of lnb_graph_prepare over
-// stack([L_cluster, L_cut], 3) (not binarised); the rest are the row of h_p.  The epilogue is the GRU
-// cell of lnb_ggnn_update (same interleaved gate rows).  The output of part p goes to out_p with row
-// stride ldo (a column block of the [B*N, 3H] input of state_func), and the first active part can copy
-// its h row into h_copy (block 0 of that input) from the values its epilogue already loads.
-#include <float.h>
-
-#include "tc_gemm.cuh"
+// The GRU step of gru_step.cuh with H/32 message k-blocks, over work items (row tile, part, column
+// tile): the items of one row tile run on neighbouring CTAs at the same time, so the gathers of both
+// parts share L2.  W is the gru_gate_matrix of update_func_partition [4H, 2H].  The message k-blocks
+// are the weighted sum of the M_p rows of node n's neighbours, gathered through the ELL rows of
+// lnb_graph_prepare over stack([L_cluster, L_cut], 3) (not binarised).  The output of part p goes to
+// out_p with row stride ldo (a column block of the [B*N, 3H] input of state_func), and the first
+// active part can copy its h row into h_copy (block 0 of that input) from the values its epilogue
+// already loads.
+#include "gru_step.cuh"
 
 namespace {
 
 constexpr int GP_HMAX = 128, GP_NMAX = 255;
 constexpr int GP_PARTS = 2;                   // cluster, cut
 
-struct GpnnPartitionPolicy {
-  static constexpr int kStagesB = 3;
-  static constexpr int kStagesA = 2;
-  struct Params {
-    const float* M[GP_PARTS];    // [rows, ldm] messages of part slot s (may alias between slots)
-    const float* h[GP_PARTS];    // [rows, ldh] state of part slot s (may alias between slots)
-    float* out[GP_PARTS];        // [rows, ldo]
-    int op[GP_PARTS];            // operator channel (0 cluster, 1 cut) of part slot s
-    const float* ell_val;        // [B, 2, N, N]  t-major ELL rows (lnb_graph_prepare)
-    const uint8_t* ell_idx;      // [B, 2, N, N]
-    const int32_t* ell_max;      // [B, 2]
-    const float* bias;           // [4H] interleaved like the rows of W
-    float* h_copy;               // [rows, ldo] or null: slot 0 writes its h row here
-    int rows, N, H, avg, nparts, ldm, ldh, ldo;
-    int dbg;
-  };
-  static __device__ __forceinline__ int n_tiles(const Params& p) { return 4 * p.H / tcg::BN; }
-  static __device__ __forceinline__ int num_steps(const Params& p, int cta, int ncta) {
-    const int t = ((p.rows + tcg::BM - 1) / tcg::BM) * p.nparts * n_tiles(p);
-    return t > cta ? (t - cta + ncta - 1) / ncta : 0;
-  }
-  // sub = slot * n_tiles + column tile; the items of one row tile are consecutive
-  static __device__ __forceinline__ void decode(const Params& p, int cta, int ncta, int it, int& m_tile,
-                                                int& sub) {
-    const int item = cta + it * ncta, per = p.nparts * n_tiles(p);
-    m_tile = item / per;
-    sub = item - m_tile * per;
-  }
-  static __device__ __forceinline__ int num_kblocks(const Params& p, int) { return 2 * p.H / tcg::BK; }
-  static __device__ __forceinline__ void w_coords(const Params& p, int sub, int kb, int& col0, int& row0) {
-    col0 = kb * tcg::BK;
-    row0 = (sub % n_tiles(p)) * tcg::BN;
-  }
+struct GpnnPartitionParams {
+  const float* M[GP_PARTS];    // [rows, ldm] messages of part slot s (may alias between slots)
+  const float* h[GP_PARTS];    // [rows, ldh] state of part slot s (may alias between slots)
+  float* out[GP_PARTS];        // [rows, ldo]
+  int op[GP_PARTS];            // operator channel (0 cluster, 1 cut) of part slot s
+  const float* ell_val;        // [B, 2, N, N]  t-major ELL rows (lnb_graph_prepare)
+  const uint8_t* ell_idx;      // [B, 2, N, N]
+  const int32_t* ell_max;      // [B, 2]
+  const float* bias;           // [4H] interleaved like the rows of W
+  float* h_copy;               // [rows, ldo] or null: slot 0 writes its h row here
+  int rows, N, D, avg, nparts, ldm, ldh, ldo;   // D = H
+  int dbg;
+};
 
-  const Params& p;
-  const int r;
-  int row, b, n, slot, cnt;
-  int64_t line;
-  float denom;
-  bool row_ok;
+struct GpnnPartitionPolicy : gru::Step<GpnnPartitionPolicy, GpnnPartitionParams> {
+  using Step::Step;
+  static __device__ __forceinline__ int parts(const Params& p) { return p.nparts; }
+  // sub = slot * n_tiles + column tile
+  static __device__ __forceinline__ int col_tile(const Params& p, int sub) { return sub % n_tiles(p); }
+  static __device__ __forceinline__ int msg_kblocks(const Params& p) { return p.D / tcg::BK; }
 
-  __device__ GpnnPartitionPolicy(const Params& p_, uint8_t*, int tid)
-      : p(p_), r(tid & 127), row(0), b(0), n(0), slot(0), cnt(0), line(0), denom(1.f), row_ok(false) {}
+  int slot = 0, cnt = 0;
+  int64_t line = 0;
+  float denom = 1.f;
 
-  __device__ __forceinline__ void step_begin(int m_tile, int sub, int, tcg::PhaseTimer&) {
-    row = m_tile * tcg::BM + r;
-    row_ok = row < p.rows;
+  __device__ __forceinline__ void begin_row(int sub) {
     slot = sub / n_tiles(p);
-    b = row_ok ? row / p.N : 0;
-    n = row_ok ? row - b * p.N : 0;
     cnt = 0;
     denom = 1.f;
     if (!row_ok) return;
@@ -92,21 +65,10 @@ struct GpnnPartitionPolicy {
     denom = sum + FLT_EPSILON;
   }
 
-  __device__ __forceinline__ void produce(int, int kb, float (&v)[32]) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = 0.f;
-    if (!row_ok) return;
-    const int c0 = kb * tcg::BK;
-    if (c0 >= p.H) {                                   // the h columns
-      const float4* src = reinterpret_cast<const float4*>(p.h[slot] + (int64_t)row * p.ldh + (c0 - p.H));
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 t = __ldg(src + j);
-        v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
-      }
-      return;
-    }
-    const float* mb = p.M[slot] + (int64_t)b * p.N * p.ldm + c0;
+  __device__ __forceinline__ const float* h_row() const { return p.h[slot] + (int64_t)row * p.ldh; }
+
+  __device__ __forceinline__ void produce_msg(int kb, float (&v)[32]) {
+    const float* mb = p.M[slot] + (int64_t)b * p.N * p.ldm + kb * tcg::BK;
 #pragma unroll 2
     for (int t = 0; t < cnt; ++t) {
       const float val = __ldg(p.ell_val + line + (int64_t)t * p.N);
@@ -124,49 +86,12 @@ struct GpnnPartitionPolicy {
     }
   }
 
-  __device__ __forceinline__ void pre_epilogue(int) {}
-
-  static __device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
-
-  __device__ __forceinline__ void store(int sub, int col, const float (&x)[tcg::EW]) {
-    if (!row_ok) return;
-    const int w0 = (sub % n_tiles(p)) * tcg::BN + col; // first W row of this unit
-    const int u0 = w0 / 4;                             // its first hidden unit
-    const float4 hv = __ldg(reinterpret_cast<const float4*>(p.h[slot] + (int64_t)row * p.ldh + u0));
-    const float hp[4] = {hv.x, hv.y, hv.z, hv.w};
-    float o[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float rg = sigmoid(x[i] + __ldg(p.bias + w0 + i));
-      const float zg = sigmoid(x[4 + i] + __ldg(p.bias + w0 + 4 + i));
-      const float gin = x[8 + i] + __ldg(p.bias + w0 + 8 + i);
-      const float ghn = x[12 + i] + __ldg(p.bias + w0 + 12 + i);
-      const float ng = tanhf(gin + rg * ghn);
-      o[i] = (hp[i] - ng) * zg + ng;
-    }
+  __device__ __forceinline__ void write_row(int u0, const float (&o)[4], const float4& hv) {
     const int64_t off = (int64_t)row * p.ldo + u0;
     *reinterpret_cast<float4*>(p.out[slot] + off) = make_float4(o[0], o[1], o[2], o[3]);
     if (slot == 0 && p.h_copy) *reinterpret_cast<float4*>(p.h_copy + off) = hv;
   }
-
-  __device__ __forceinline__ void post_epilogue(int) {}
 };
-
-constexpr size_t SMEM_BYTES =
-    tcg::core_smem(GpnnPartitionPolicy::kStagesB, GpnnPartitionPolicy::kStagesA) + 1024 + 16;
-
-// The phase-timer pointer lives in each translation unit's copy of tcg::g_prof: mirror the buffer
-// registered with lnb_debug_set_prof into this one when it changes (profiling only).
-unsigned long long* g_prof_mirrored = nullptr;
-
-int sync_prof_buffer() {
-  unsigned long long* buf = lnb::prof_buffer();
-  if (buf == g_prof_mirrored) return LNB_OK;
-  cudaError_t e = cudaMemcpyToSymbol(tcg::g_prof, &buf, sizeof(buf));
-  if (e != cudaSuccess) { lnb::set_err("gpnn_partition_update: %s", cudaGetErrorString(e)); return (int)e; }
-  g_prof_mirrored = buf;
-  return LNB_OK;
-}
 
 // Do the element sets {a + i*lda + j} and {b + i*ldb + j} (0 <= i < rows, 0 <= j < width) intersect?
 // Exact for equal strides (column blocks of one matrix), conservative otherwise.
@@ -237,23 +162,12 @@ int lnb_gpnn_partition_update(lnb_stream_t stream, const float* M0, const float*
       return LNB_ERR_UNSUPPORTED;
     }
   }
-  int rc = sync_prof_buffer();
-  if (rc != LNB_OK) return rc;
-  CUtensorMap map_hi, map_lo;
-  rc = tcg::make_weight_map(&map_hi, W_hi, 4 * H, 2 * H, "gpnn_partition_update");
-  if (rc != LNB_OK) return rc;
-  rc = tcg::make_weight_map(&map_lo, W_lo, 4 * H, 2 * H, "gpnn_partition_update");
-  if (rc != LNB_OK) return rc;
-  auto kern = tcg::tc_gemm_kernel<GpnnPartitionPolicy>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
   p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.bias = bias; p.h_copy = h_copy;
-  p.rows = rows; p.N = N; p.H = H; p.avg = avg ? 1 : 0; p.nparts = np;
+  p.rows = rows; p.N = N; p.D = H; p.avg = avg ? 1 : 0; p.nparts = np;
   p.ldm = ldm; p.ldh = ldh; p.ldo = ldo; p.dbg = tcg::debug_flags();
-  const int tiles = lnb::ceil_div(rows, tcg::BM) * np * (4 * H / tcg::BN);
-  const int grid = tiles < tcg::sm_count() ? tiles : tcg::sm_count();
-  kern<<<grid, tcg::THREADS, SMEM_BYTES, (cudaStream_t)stream>>>(map_hi, map_lo, p);
-  lnb::count_launch();
-  return lnb::finish_launch("gpnn_partition_update");
+  return tcg::launch<GpnnPartitionPolicy>(stream, W_hi, W_lo, 4 * H, 2 * H, GpnnPartitionPolicy::SMEM_BYTES,
+                                          lnb::ceil_div(rows, tcg::BM) * np * (4 * H / tcg::BN), p,
+                                          "gpnn_partition_update");
 }
 
 }  // extern "C"

@@ -170,13 +170,6 @@ static int launch_linear(lnb_stream_t stream, const float* A, const float* W_hi,
   LNB_REQUIRE(((uintptr_t)A & 15) == 0 && ((uintptr_t)W_hi & 15) == 0 && ((uintptr_t)W_lo & 15) == 0,
               "%s: A / W must be 16-byte aligned", who);
   if (M == 0) return LNB_OK;
-  CUtensorMap map_hi, map_lo;
-  int rc = tcg::make_weight_map(&map_hi, W_hi, groups * N, K, who);
-  if (rc != LNB_OK) return rc;
-  rc = tcg::make_weight_map(&map_lo, W_lo, groups * N, K, who);
-  if (rc != LNB_OK) return rc;
-  auto kern = tcg::tc_gemm_kernel<RowLoadPolicy>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
   const int nkb = lnb::ceil_div(K, tcg::BK);
   LNB_REQUIRE(splits >= 1 && splits <= 16 && (splits == 1 || (ws && counters)),
               "%s: split-K needs 1 <= splits <= 16, a workspace and counters", who);
@@ -184,10 +177,7 @@ static int launch_linear(lnb_stream_t stream, const float* A, const float* W_hi,
               "%s: %d splits leave an empty k range for K=%d", who, splits, K);
   RowLoadPolicy::Params p{A, bias, C, M, N, K, relu, groups, tcg::debug_flags(), splits, ws, counters};
   const int tiles = lnb::ceil_div(M, tcg::BM) * lnb::ceil_div(N, tcg::BN) * groups * splits;
-  const int grid = tiles < tcg::sm_count() ? tiles : tcg::sm_count();
-  kern<<<grid, tcg::THREADS, SMEM_BYTES, (cudaStream_t)stream>>>(map_hi, map_lo, p);
-  lnb::count_launch();
-  return lnb::finish_launch(who);
+  return tcg::launch<RowLoadPolicy>(stream, W_hi, W_lo, groups * N, K, SMEM_BYTES, tiles, p, who);
 }
 
 extern "C" {

@@ -9,19 +9,15 @@
 //     gi = [S_0 | ... | S_{E1-1} | deg] F^T + b_ih,   F = [W_ih,e W2_e]_e | [W_ih,e b2_e]_e,
 //     deg[i, e] = w_i nnz_e(i)
 //
-// lnb_mpnn_update is a policy of the persistent 3xTF32 wgmma skeleton (tc_gemm.cuh) over plain 128-row
-// tiles of the B*N rows.  Its A operand is produced by the CUDA-core warps:
+// lnb_mpnn_update is the GRU step of gru_step.cuh with these k-blocks, produced by the CUDA-core warps:
 //     k-blocks 0 .. 2 E1 - 1    32 columns of S_e (e = kb / 2): the producer thread of row i holds its own
 //                               32 Q values and, for each non-zero j of its ELL row, adds P_e[j], applies
 //                               the ReLU and accumulates with weight w_i
 //     k-block 2 E1              the degree block: column e holds w_i nnz_e(i), the rest are zero
 //     k-blocks past it          the row of h
-// and the epilogue is the GRU cell of lnb_ggnn_update (same interleaved gate rows).  S never exists in
-// HBM.  lnb_mpnn_edge_aggregate writes S with the same arithmetic for the training path, and
-// lnb_mpnn_edge_aggregate_backward is its adjoint.
-#include <float.h>
-
-#include "tc_gemm.cuh"
+// S never exists in HBM.  lnb_mpnn_edge_aggregate writes S with the same arithmetic for the training
+// path, and lnb_mpnn_edge_aggregate_backward is its adjoint.
+#include "gru_step.cuh"
 
 namespace {
 
@@ -29,96 +25,38 @@ constexpr int MP_DMAX = 128, MP_NMAX = 255, MP_E1MAX = 16;
 constexpr int MP_H = 64;                  // edge-network hidden width (model/mpnn.py:60)
 constexpr int MP_PQ = 2 * MP_H;           // PQ columns per channel: 64 P, then 64 Q
 
-// non-zeros of ELL row `line` (t-major, stride N): the leading entries with a non-zero value
-__device__ __forceinline__ int ell_count(const float* ell_val, int64_t line, int len, int N) {
-  int cnt = 0;
-  while (cnt < len && __ldg(ell_val + line + (int64_t)cnt * N) != 0.f) ++cnt;
-  return cnt;
-}
+struct MpnnUpdateParams {
+  const float* PQ;         // [rows, E1*128]
+  const float* h;          // [rows, D]
+  const float* ell_val;    // [B, E1, N, N]  t-major ELL rows (lnb_graph_prepare)
+  const uint8_t* ell_idx;  // [B, E1, N, N]
+  const int32_t* ell_max;  // [B, E1]
+  const float* bias;       // [4D] interleaved like the rows of W
+  float* out;              // [rows, D]
+  int rows, N, D, E1, avg;
+  int dbg;
+};
 
-// avg: the reference's sum / (rowsum(A) + eps) on the 0/1 operator -- one correctly rounded reciprocal
-__device__ __forceinline__ float row_weight(int cnt, int avg) {
-  return avg ? __frcp_rn((float)cnt + FLT_EPSILON) : 1.f;
-}
+struct MpnnUpdatePolicy : gru::Step<MpnnUpdatePolicy, MpnnUpdateParams> {
+  using Step::Step;
+  static __device__ __forceinline__ int msg_kblocks(const Params& p) { return 2 * p.E1 + 1; }
 
-struct MpnnUpdatePolicy {
-  static constexpr int kStagesB = 3;
-  static constexpr int kStagesA = 2;
-  struct Params {
-    const float* PQ;         // [rows, E1*128]
-    const float* h;          // [rows, D]
-    const float* ell_val;    // [B, E1, N, N]  t-major ELL rows (lnb_graph_prepare)
-    const uint8_t* ell_idx;  // [B, E1, N, N]
-    const int32_t* ell_max;  // [B, E1]
-    const float* bias;       // [4D] interleaved like the rows of W
-    float* out;              // [rows, D]
-    int rows, N, D, E1, avg;
-    int dbg;
-  };
-  static __device__ __forceinline__ int n_tiles(const Params& p) { return 4 * p.D / tcg::BN; }
-  static __device__ __forceinline__ int num_steps(const Params& p, int cta, int ncta) {
-    const int t = ((p.rows + tcg::BM - 1) / tcg::BM) * n_tiles(p);
-    return t > cta ? (t - cta + ncta - 1) / ncta : 0;
-  }
-  // consecutive items = the column tiles of one row tile: they run side by side and share the gathers in L2
-  static __device__ __forceinline__ void decode(const Params& p, int cta, int ncta, int it, int& m_tile,
-                                                int& sub) {
-    const int item = cta + it * ncta, nt = n_tiles(p);
-    m_tile = item / nt;
-    sub = item - m_tile * nt;
-  }
-  static __device__ __forceinline__ int num_kblocks(const Params& p, int) {
-    return 2 * p.E1 + 1 + p.D / tcg::BK;
-  }
-  static __device__ __forceinline__ void w_coords(const Params&, int sub, int kb, int& col0, int& row0) {
-    col0 = kb * tcg::BK;
-    row0 = sub * tcg::BN;
-  }
-
-  const Params& p;
-  const int r;
-  int row, b, n;
-  bool row_ok;
-
-  __device__ MpnnUpdatePolicy(const Params& p_, uint8_t*, int tid)
-      : p(p_), r(tid & 127), row(0), b(0), n(0), row_ok(false) {}
-
-  __device__ __forceinline__ void step_begin(int m_tile, int, int, tcg::PhaseTimer&) {
-    row = m_tile * tcg::BM + r;
-    row_ok = row < p.rows;
-    b = row_ok ? row / p.N : 0;
-    n = row_ok ? row - b * p.N : 0;
-  }
-
-  __device__ __forceinline__ void produce(int, int kb, float (&v)[32]) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = 0.f;
-    if (!row_ok) return;
-    if (kb > 2 * p.E1) {                                  // the h columns
-      const int j0 = (kb - 2 * p.E1 - 1) * tcg::BK;
-      const float4* src = reinterpret_cast<const float4*>(p.h + (int64_t)row * p.D + j0);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 t = __ldg(src + j);
-        v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
-      }
-      return;
-    }
+  __device__ __forceinline__ void produce_msg(int kb, float (&v)[32]) {
     if (kb == 2 * p.E1) {                                 // degree block: w_i nnz_e(i)
       for (int e = 0; e < p.E1; ++e) {
         const int64_t line = ((int64_t)(b * p.E1 + e) * p.N) * p.N + n;
-        const int cnt = ell_count(p.ell_val, line, __ldg(p.ell_max + b * p.E1 + e), p.N);
+        const int cnt = gru::ell_count(p.ell_val, line, __ldg(p.ell_max + b * p.E1 + e), p.N);
 #pragma unroll
         for (int j = 0; j < MP_E1MAX; ++j)
-          if (j == e) v[j] = row_weight(cnt, p.avg) * (float)cnt;
+          if (j == e) v[j] = gru::row_weight(cnt, p.avg) * (float)cnt;
       }
       return;
     }
     const int e = kb >> 1, c0 = (kb & 1) * 32;
     const int64_t line = ((int64_t)(b * p.E1 + e) * p.N) * p.N + n;
-    const int cnt = ell_count(p.ell_val, line, __ldg(p.ell_max + b * p.E1 + e), p.N);
+    const int cnt = gru::ell_count(p.ell_val, line, __ldg(p.ell_max + b * p.E1 + e), p.N);
     if (cnt == 0) return;
-    const float w = row_weight(cnt, p.avg);
+    const float w = gru::row_weight(cnt, p.avg);
     const int ld = p.E1 * MP_PQ;
     float q[32];
     const float4* qs = reinterpret_cast<const float4*>(p.PQ + (int64_t)row * ld + e * MP_PQ + MP_H + c0);
@@ -141,47 +79,7 @@ struct MpnnUpdatePolicy {
       }
     }
   }
-
-  __device__ __forceinline__ void pre_epilogue(int) {}
-
-  static __device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
-
-  __device__ __forceinline__ void store(int sub, int col, const float (&x)[tcg::EW]) {
-    if (!row_ok) return;
-    const int w0 = sub * tcg::BN + col;                // first W row of this unit
-    const int u0 = w0 / 4;                             // its first hidden unit
-    const float4 hv = __ldg(reinterpret_cast<const float4*>(p.h + (int64_t)row * p.D + u0));
-    const float hp[4] = {hv.x, hv.y, hv.z, hv.w};
-    float o[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float rg = sigmoid(x[i] + __ldg(p.bias + w0 + i));
-      const float zg = sigmoid(x[4 + i] + __ldg(p.bias + w0 + 4 + i));
-      const float gin = x[8 + i] + __ldg(p.bias + w0 + 8 + i);
-      const float ghn = x[12 + i] + __ldg(p.bias + w0 + 12 + i);
-      const float ng = tanhf(gin + rg * ghn);
-      o[i] = (hp[i] - ng) * zg + ng;
-    }
-    *reinterpret_cast<float4*>(p.out + (int64_t)row * p.D + u0) = make_float4(o[0], o[1], o[2], o[3]);
-  }
-
-  __device__ __forceinline__ void post_epilogue(int) {}
 };
-
-constexpr size_t SMEM_BYTES = tcg::core_smem(MpnnUpdatePolicy::kStagesB, MpnnUpdatePolicy::kStagesA) + 1024 + 16;
-
-// The phase-timer pointer lives in each translation unit's copy of tcg::g_prof: mirror the buffer
-// registered with lnb_debug_set_prof into this one when it changes (profiling only).
-unsigned long long* g_prof_mirrored = nullptr;
-
-int sync_prof_buffer() {
-  unsigned long long* buf = lnb::prof_buffer();
-  if (buf == g_prof_mirrored) return LNB_OK;
-  cudaError_t e = cudaMemcpyToSymbol(tcg::g_prof, &buf, sizeof(buf));
-  if (e != cudaSuccess) { lnb::set_err("mpnn_update: %s", cudaGetErrorString(e)); return (int)e; }
-  g_prof_mirrored = buf;
-  return LNB_OK;
-}
 
 // ---- training path: S and its adjoint, one thread per (row, channel, hidden column) --------------
 struct EdgeAggParams {
@@ -208,8 +106,8 @@ __global__ void edge_aggregate_kernel(const EdgeAggParams p) {
   const int b = row / p.N, n = row - b * p.N;
   const int ld = p.E1 * MP_PQ;
   const int64_t line = ((int64_t)(b * p.E1 + e) * p.N) * p.N + n;
-  const int cnt = ell_count(p.ell_val, line, __ldg(p.ell_max + b * p.E1 + e), p.N);
-  const float w = row_weight(cnt, p.avg);
+  const int cnt = gru::ell_count(p.ell_val, line, __ldg(p.ell_max + b * p.E1 + e), p.N);
+  const float w = gru::row_weight(cnt, p.avg);
   const float q = __ldg(p.PQ + (int64_t)row * ld + e * MP_PQ + MP_H + c);
   const float* pc = p.PQ + (int64_t)b * p.N * ld + e * MP_PQ + c;
   float v = 0.f;
@@ -237,8 +135,8 @@ __global__ void edge_aggregate_backward_kernel(const EdgeAggParams p) {
   const float* Qc = Pc + MP_H;
   const float* gc = p.gS + (int64_t)b * p.N * lds + e * MP_H + c;
   // gQ of row n
-  const int cnt = ell_count(p.ell_val, base + n, len, p.N);
-  const float w = row_weight(cnt, p.avg);
+  const int cnt = gru::ell_count(p.ell_val, base + n, len, p.N);
+  const float w = gru::row_weight(cnt, p.avg);
   const float qn = __ldg(Qc + (int64_t)n * ld), gn = __ldg(gc + (int64_t)n * lds);
   float gq = 0.f;
   for (int t = 0; t < cnt; ++t) {
@@ -247,12 +145,12 @@ __global__ void edge_aggregate_backward_kernel(const EdgeAggParams p) {
   }
   // gP of row n: the receivers i with A[i, n] != 0
   const float pn = __ldg(Pc + (int64_t)n * ld);
-  const int cntT = ell_count(p.ellT_val, base + n, __ldg(p.ellT_max + b * p.E1 + e), p.N);
+  const int cntT = gru::ell_count(p.ellT_val, base + n, __ldg(p.ellT_max + b * p.E1 + e), p.N);
   float gp = 0.f;
   for (int t = 0; t < cntT; ++t) {
     const int i = __ldg(p.ellT_idx + base + n + (int64_t)t * p.N);
     if (pn + __ldg(Qc + (int64_t)i * ld) > 0.f) {
-      const float wi = row_weight(ell_count(p.ell_val, base + i, len, p.N), p.avg);
+      const float wi = gru::row_weight(gru::ell_count(p.ell_val, base + i, len, p.N), p.avg);
       gp = fmaf(wi, __ldg(gc + (int64_t)i * lds), gp);
     }
   }
@@ -295,23 +193,10 @@ int lnb_mpnn_update(lnb_stream_t stream, const float* PQ, const float* h, const 
   LNB_REQUIRE((int64_t)B * N * E1 * MP_PQ <= 0x7fffffff, "mpnn_update: B*N too large");
   const int rows = B * N;
   if (rows == 0) return LNB_OK;
-  int rc = sync_prof_buffer();
-  if (rc != LNB_OK) return rc;
-  const int K = MP_H * E1 + 32 + D;
-  CUtensorMap map_hi, map_lo;
-  rc = tcg::make_weight_map(&map_hi, W_hi, 4 * D, K, "mpnn_update");
-  if (rc != LNB_OK) return rc;
-  rc = tcg::make_weight_map(&map_lo, W_lo, 4 * D, K, "mpnn_update");
-  if (rc != LNB_OK) return rc;
-  auto kern = tcg::tc_gemm_kernel<MpnnUpdatePolicy>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
   MpnnUpdatePolicy::Params p{PQ, h, ell_val, ell_idx, ell_max, bias, out, rows, N, D, E1, avg ? 1 : 0,
                              tcg::debug_flags()};
-  const int tiles = lnb::ceil_div(rows, tcg::BM) * (4 * D / tcg::BN);
-  const int grid = tiles < tcg::sm_count() ? tiles : tcg::sm_count();
-  kern<<<grid, tcg::THREADS, SMEM_BYTES, (cudaStream_t)stream>>>(map_hi, map_lo, p);
-  lnb::count_launch();
-  return lnb::finish_launch("mpnn_update");
+  return tcg::launch<MpnnUpdatePolicy>(stream, W_hi, W_lo, 4 * D, MP_H * E1 + 32 + D, MpnnUpdatePolicy::SMEM_BYTES,
+                                       lnb::ceil_div(rows, tcg::BM) * (4 * D / tcg::BN), p, "mpnn_update");
 }
 
 int lnb_mpnn_edge_aggregate(lnb_stream_t stream, const float* PQ, const float* ell_val, const uint8_t* ell_idx,

@@ -31,4 +31,13 @@ const char* lnb_last_error(void) { return lnb::err_buf(); }
 
 int64_t lnb_launch_count(void) { return lnb::g_launches; }
 
+// Profiling aid: register (or clear with NULL) a device buffer of SMs x 32 uint64 phase timers.  The
+// skeleton kernels read it through their translation unit's copy of the pointer (tcg::g_prof), which
+// tcg::launch updates with a synchronous copy at the first launch after a change.  That launch must
+// not be inside a stream capture, and until it runs, replays of captured graphs see the old buffer.
+int lnb_debug_set_prof(unsigned long long* buf) {
+  lnb::set_prof_buffer(buf);
+  return LNB_OK;
+}
+
 }  // extern "C"

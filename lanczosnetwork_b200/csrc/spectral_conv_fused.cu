@@ -1158,14 +1158,6 @@ void launch_tile_assign(cudaStream_t s, const int32_t* gext, int B, int K, int32
 
 extern "C" {
 
-// profiling aid: register (or clear with NULL) a device buffer of SMs x 32 uint64 phase timers
-int lnb_debug_set_prof(unsigned long long* buf) {
-  cudaError_t e = cudaMemcpyToSymbol(tcg::g_prof, &buf, sizeof(buf));
-  if (e != cudaSuccess) { lnb::set_err("debug_set_prof: %s", cudaGetErrorString(e)); return (int)e; }
-  lnb::set_prof_buffer(buf);
-  return LNB_OK;
-}
-
 int lnb_graph_prepare(lnb_stream_t stream, const float* L, const float* Q, int B, int N, int E1,
                       int K, float* ell_val, uint8_t* ell_idx, int32_t* ell_max, int32_t* gext,
                       int32_t* tiles /* [4*B + 2]: B + 2 tile table followed by 3*B scratch */,
@@ -1241,13 +1233,6 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
     return LNB_ERR_UNSUPPORTED;
   }
   smem += (size_t)lb * Pol::ell_line_bytes();
-  CUtensorMap map_hi, map_lo;
-  int rc = tcg::make_weight_map(&map_hi, d.W_hi, d.num_layers * d.H, d.Kw, who);
-  if (rc != LNB_OK) return rc;
-  rc = tcg::make_weight_map(&map_lo, d.W_lo, d.num_layers * d.H, d.Kw, who);
-  if (rc != LNB_OK) return rc;
-  auto kern = tcg::tc_gemm_kernel<Pol>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   typename Pol::Params p{};
   p.X = d.X; p.node_ids = d.node_ids; p.emb = d.emb_table; p.Q = d.Q;
   p.coeff = d.coeff; p.coeff_stride = d.coeff_layer_stride;
@@ -1260,10 +1245,7 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
   p.LB = lb; p.write_pad = d.write_pad; p.dbg = tcg::debug_flags();
   // the tile count lives in device memory (no host sync): one persistent CTA per SM, bounded by
   // the worst case of one graph per tile
-  const int grid = d.B < tcg::sm_count() ? d.B : tcg::sm_count();
-  kern<<<grid, tcg::THREADS, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
-  lnb::count_launch();
-  return lnb::finish_launch(who);
+  return tcg::launch<Pol>(stream, d.W_hi, d.W_lo, d.num_layers * d.H, d.Kw, smem, d.B, p, who);
 }
 
 }  // extern "C++"

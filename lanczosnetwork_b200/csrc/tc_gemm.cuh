@@ -81,9 +81,9 @@ __device__ __forceinline__ Core carve(uint8_t* base, int stages_b, int stages_a)
   return c;
 }
 
-// Optional phase timers (profiling aid): when a buffer is registered with lnb_debug_set_prof,
-// thread 0 of every CTA accumulates clock64() deltas per phase into prof[cta*32 + phase]
-// (slots 8 / 9: k-loop / accumulator wait of odd sub-steps, 10: post_epilogue):
+// Optional phase timers (profiling aid): when a buffer is registered with lnb_debug_set_prof (launch()
+// points g_prof at it), thread 0 of every CTA accumulates clock64() deltas per phase into
+// prof[cta*32 + phase] (slots 8 / 9: k-loop / accumulator wait of odd sub-steps, 10: post_epilogue):
 //   0 staging issue  1 staging wait (policy)  3 k-loop  4 pre_epilogue
 //   5 wait for the accumulator  7 epilogue store
 __device__ unsigned long long* g_prof = nullptr;
@@ -460,6 +460,40 @@ inline int sm_count() {
   if (cudaGetDevice(&dev) == cudaSuccess)
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
   return n > 0 ? n : 132;
+}
+
+// g_prof is defined in this header, so every translation unit has its own copy.  Each points its
+// copy at the buffer registered with lnb_debug_set_prof when that has changed since its last launch
+// (a synchronous copy; with no buffer ever registered nothing is copied).
+static unsigned long long* g_prof_mirrored = nullptr;
+
+static int sync_prof_buffer(const char* who) {
+  unsigned long long* buf = lnb::prof_buffer();
+  if (buf == g_prof_mirrored) return LNB_OK;
+  cudaError_t e = cudaMemcpyToSymbol(g_prof, &buf, sizeof(buf));
+  if (e != cudaSuccess) { lnb::set_err("%s: %s", who, cudaGetErrorString(e)); return (int)e; }
+  g_prof_mirrored = buf;
+  return LNB_OK;
+}
+
+// Launches tc_gemm_kernel<Pol> on min(items, SMs) persistent CTAs with `smem` bytes of dynamic shared
+// memory; W_hi / W_lo are the split row-major [w_rows, w_cols] weights the TMA streams.
+template <class Pol>
+static int launch(lnb_stream_t stream, const float* W_hi, const float* W_lo, int w_rows, int w_cols,
+                  size_t smem, int items, const typename Pol::Params& p, const char* who) {
+  CUtensorMap map_hi, map_lo;
+  int rc = make_weight_map(&map_hi, W_hi, w_rows, w_cols, who);
+  if (rc != LNB_OK) return rc;
+  rc = make_weight_map(&map_lo, W_lo, w_rows, w_cols, who);
+  if (rc != LNB_OK) return rc;
+  rc = sync_prof_buffer(who);
+  if (rc != LNB_OK) return rc;
+  auto kern = tc_gemm_kernel<Pol>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  const int grid = items < sm_count() ? items : sm_count();
+  kern<<<grid, THREADS, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
+  lnb::count_launch();
+  return lnb::finish_launch(who);
 }
 
 }  // namespace tcg

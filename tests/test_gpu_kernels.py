@@ -738,6 +738,59 @@ def test_spectral_stack_equals_layer_by_layer():
                              rtol=1e-5, atol=1e-6)
 
 
+def test_phase_timers_reach_every_skeleton_launch_site():
+  """With a buffer registered by lnb_debug_set_prof, a launch of the dense layer, the filter-MLP chain,
+  the convolution stack and a GRU update each adds its CTAs' cycle totals (PhaseTimer slot 12) to it;
+  once the buffer is cleared, launches leave it alone."""
+  import ctypes
+  from lanczosnetwork_b200 import _lib
+  d = dev()
+  g = torch.Generator().manual_seed(21)
+  rnd = lambda *s: torch.randn(*s, generator=g).to(d)
+  x = rnd(300, 128)
+  lin_hi, lin_lo = ops().split_tf32(rnd(128, 128) / 12)
+  S, Hd, L = 8, 128, 2
+  table, ch_b = rnd(200, S), rnd(L * (3 * Hd + S))
+  ch_hi, ch_lo = ops().split_tf32(rnd(L * (3 * Hd + S), Hd) / 12)
+  X, Lop, V, coeff, W, bias = [t.to(d) for t in _conv_case(5, 26, 64, 128, 20, 8, 7, 21)]
+  prep = ops().graph_prepare(Lop, V)
+  st_hi, st_lo = ops().split_tf32(W)
+  B, N, D, E1 = 3, 26, 32, 2
+  gg_prep = ops().graph_prepare(Lop[:B, :, :, :E1].contiguous(), torch.zeros((B, N, 4), device=d), binarize=True)
+  M, h, gg_b = rnd(B * N, E1 * D), rnd(B * N, D), rnd(4 * D)
+  gg_hi, gg_lo = ops().split_tf32(rnd(4 * D, (E1 + 1) * D) / 12)
+  launches = {
+      'dense layer': lambda: ops().linear_tf32x3(x, lin_hi, lin_lo),
+      'filter-MLP chain': lambda: ops().ritz_filter_mlp(table, ch_hi, ch_lo, ch_b, L),
+      'convolution stack': lambda: ops().spectral_conv_fused(X, V, coeff, prep, st_hi, st_lo, bias, True),
+      'GGNN update': lambda: ops().ggnn_update(M, h, gg_prep, gg_hi, gg_lo, gg_b, True),
+  }
+  nsm = torch.cuda.get_device_properties(d).multi_processor_count
+  buf = torch.zeros(nsm * 32, dtype=torch.int64, device=d)
+  lib = _lib.load()
+
+  def cycles():
+    torch.cuda.synchronize()
+    return int(buf.view(nsm, 32)[:, 12].sum())
+
+  _lib.check(lib.lnb_debug_set_prof(ctypes.c_void_p(buf.data_ptr())), 'lnb_debug_set_prof')
+  try:
+    for name, run in launches.items():
+      before = cycles()
+      run()
+      assert cycles() > before, name
+  finally:
+    _lib.check(lib.lnb_debug_set_prof(None), 'lnb_debug_set_prof')
+    for run in launches.values():        # each kernel's copy of the pointer is cleared at its next launch
+      run()
+    torch.cuda.synchronize()
+  kept = buf.clone()
+  for run in launches.values():
+    run()
+  torch.cuda.synchronize()
+  assert torch.equal(buf, kept)
+
+
 @pytest.mark.parametrize('cheby', [False, True])
 def test_operator_chain_matches_step_by_step(cheby):
   """lnb_operator_chain (power chain of model/dcnn.py:88-92, Chebyshev chain of

@@ -15,8 +15,9 @@ from lanczosnetwork_b200 import build
 
 LOG = os.path.join(build.HERE, 'build.log')
 SKELETON = '_ZN3tcg14tc_gemm_kernel'
-# one instantiation per policy: dense layer, filter-MLP chain, GGNN update, three stack variants
-POLICIES = {'linear_tf32x3': 1, 'filter_mlp_chain': 1, 'ggnn_update': 1, 'spectral_conv_fused': 3}
+# one instantiation per policy: dense layer, filter-MLP chain, the three GRU updates, three stack variants
+POLICIES = {'linear_tf32x3': 1, 'filter_mlp_chain': 1, 'ggnn_update': 1, 'mpnn_update': 1, 'gpnn_partition': 1,
+            'spectral_conv_fused': 3}
 MAX_REGISTERS = 168          # 384 threads, one CTA per SM
 MAX_SPILL_STORES = 128       # bytes; the stack kernel's producers keep a few values on the stack
 
