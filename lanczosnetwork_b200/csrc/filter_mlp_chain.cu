@@ -3,27 +3,30 @@
 // the B*K rows of Ritz-value powers).
 //
 // An item is (128-row tile, layer): four Linear stages S -> Hd -> Hd -> Hd -> S.
-//   * The S-wide first stage (S <= 8 inputs) is evaluated by the CUDA cores in plain fp32 straight
-//     into the activations of the tile -- a tensor-core step for K = 8 would cost a full
-//     accumulator hand-over for 2 % of the flops.  (S > 8 runs it as an MMA step.)
-//   * Likewise the S-wide output stage (S <= 8 outputs): the epilogue of stage 2 finishes a row,
-//     and the thread that owns it takes its S dot products with the stage-3 weights in fp32 (a
-//     128-wide MMA for 8 columns would be another full hand-over).  (S > 8 runs it as an MMA step.)
-//   * The other stages are accumulator lifetimes ("steps") of the 3xTF32 skeleton in tc_gemm.cuh:
+//   * The hidden stages are accumulator lifetimes ("steps") of the 3xTF32 skeleton in tc_gemm.cuh:
 //     two per item for S <= 8, four for S > 8.
-//     Activations NEVER leave the SM: they live in shared memory, one row per producer thread;
-//     the epilogue of stage s applies bias + ReLU and overwrites the thread's own row, which the
-//     producers of stage s+1 read back as their k-blocks.
+//   * The S-wide first stage (S <= 8 inputs) is evaluated by the CUDA cores in plain fp32 inside
+//     produce(): k-block kb of stage 1 is columns [32 kb, 32 kb + 32) of ReLU(W1 t + b1), computed
+//     in registers from the row's powers and written straight into the operand ring -- a tensor-core
+//     step for K = 8 would cost a full accumulator hand-over for 2 % of the flops.  (S > 8 runs it
+//     as an MMA step whose producers read the powers.)
+//   * Every later hidden stage takes its operand from the previous step's accumulators: the
+//     consumers apply bias + ReLU to their fragments and write the next step's k-blocks themselves
+//     (operand_from_acc), so activations never leave the registers and the tensor cores' operand
+//     ring.
+//   * The S-wide output stage (S <= 8 outputs) runs in the epilogue of the last hidden stage: the
+//     thread that owns a row applies bias + ReLU to each 16-column chunk of the drain and folds it
+//     into its S dot products with the stage-3 weights, in ascending column order (a 128-wide MMA
+//     for 8 columns would be another full hand-over).  (S > 8 runs it as an MMA step.)
 #include "tc_gemm.cuh"
 
 namespace {
 
 constexpr int S0MAX = 8;                 // first / output stage widths the CUDA cores handle
-constexpr int AP = tcg::BN + 4;          // row pitch of the activation tile (floats)
 
 struct ChainPolicy {
   static constexpr int kStagesB = 2;
-  static constexpr int kStagesA = 2;
+  static constexpr int kStagesA = 4;     // one A stage per k-block of a 128-wide consumer-written operand
   struct Params {
     const float* table;     // [Rall, S]  powers of the Ritz values
     const int32_t* rowmap;  // [Rall]     compact list of rows to evaluate (nullptr: all rows)
@@ -76,66 +79,77 @@ struct ChainPolicy {
     col0 = kb * tcg::BK;
     row0 = w_row0(p, sub >> 2, sub & 3);
   }
+  // Every hidden stage after the item's first MMA step multiplies the previous step's activations,
+  // written into the A ring by the consumers: ReLU(acc + b), the operations the epilogue used to
+  // apply before the producers read the row back.  b is the layer's bias of step sub's stage,
+  // staged in shared memory by step_begin.
+  static __device__ __forceinline__ bool operand_from_acc(const Params& p, int sub) {
+    return (sub & 3) > first_stage(p);
+  }
+  static __device__ __forceinline__ float acc_operand(const Params&, const uint8_t* policy_smem, int sub, int col,
+                                                      float x) {
+    const float* bs = reinterpret_cast<const float*>(policy_smem) + BS_OFF;
+    return fmaxf(x + bs[(sub & 3) * tcg::BN + col], 0.f);
+  }
 
   const Params& p;
   const int tid, r;
-  float* act;               // [BM][AP] activations, row r <-> producer thread r
+  // shared memory (floats): W1s | W3s | bs | b3s
+  static constexpr int BS_OFF = 2 * tcg::BN * S0MAX;
   float* W1s;               // [BN][S0MAX] first-stage weights (hi + lo)
-  float* b1s;               // [BN]
   float* W3s;               // [BN][S0MAX] output-stage weights (hi + lo), transposed: W3s[c][s] = W3[s][c]
+  float* bs;                // [3][BN]     biases of stages 0, 1, 2 (b1 = bs[0])
   float* b3s;               // [S0MAX]
   int src, cur_layer;
+  float tv[S0MAX];          // this row's powers (first stage, S <= 8)
+  float o[S0MAX];           // this row's output-stage sums (S <= 8)
 
   static size_t smem_bytes() {
-    return ((size_t)tcg::BM * AP + 2 * (tcg::BN * S0MAX) + tcg::BN + S0MAX) * 4;
+    return (BS_OFF + 3 * tcg::BN + S0MAX) * 4;
   }
 
   __device__ ChainPolicy(const Params& p_, uint8_t* smem, int tid_)
       : p(p_), tid(tid_), r(tid_ & 127), src(-1), cur_layer(-1) {
-    act = reinterpret_cast<float*>(smem);
-    W1s = act + (size_t)tcg::BM * AP;
-    b1s = W1s + tcg::BN * S0MAX;
-    W3s = b1s + tcg::BN;
-    b3s = W3s + tcg::BN * S0MAX;
+    W1s = reinterpret_cast<float*>(smem);
+    W3s = W1s + tcg::BN * S0MAX;
+    bs = W1s + BS_OFF;
+    b3s = bs + 3 * tcg::BN;
   }
 
-  __device__ void step_begin(int m_tile, int sub, int, tcg::PhaseTimer&) {
+  __device__ void step_begin(int m_tile, int sub, int, tcg::PhaseTimer& tm) {
     const int layer = sub >> 2;
     if ((sub & 3) != first_stage(p)) return;
     const int i = m_tile * tcg::BM + r;
     src = i < rows(p) ? (p.rowmap ? __ldg(p.rowmap + i) : i) : -1;
-    if (mma0(p)) return;
-    // ---- first stage on the CUDA cores: act = ReLU(W1 t + b1) ---------------------------------
-    if (layer != cur_layer) {        // stage this layer's W1, b1 and (for store()) W3, b3 (hi + lo)
+    // Stage this layer's hidden biases (read by the consumers' hand-overs and by store()) and, for
+    // S <= 8, W1 and W3 (hi + lo) and b3.  The consumers read the previous layer's biases for the
+    // last time before the drain these producers have read by now.
+    if (layer != cur_layer) {
       tcg::producers_sync();
       const int row0 = w_row0(p, layer, 0), row3 = w_row0(p, layer, 3);
+      if (!mma0(p)) {
 #pragma unroll 4
-      for (int e = tid; e < p.Hd * S0MAX; e += tcg::PRODUCER_THREADS) {
-        const int c = e / S0MAX, k = e - c * S0MAX;
-        const int64_t o = (int64_t)(row0 + c) * p.Hd + k;
-        W1s[e] = (k < p.S) ? __ldg(p.W_hi + o) + __ldg(p.W_lo + o) : 0.f;
-        const int64_t o3 = (int64_t)(row3 + k) * p.Hd + c;
-        W3s[e] = (k < p.S) ? __ldg(p.W_hi + o3) + __ldg(p.W_lo + o3) : 0.f;
+        for (int e = tid; e < p.Hd * S0MAX; e += tcg::PRODUCER_THREADS) {
+          const int c = e / S0MAX, k = e - c * S0MAX;
+          const int64_t o1 = (int64_t)(row0 + c) * p.Hd + k;
+          W1s[e] = (k < p.S) ? __ldg(p.W_hi + o1) + __ldg(p.W_lo + o1) : 0.f;
+          const int64_t o3 = (int64_t)(row3 + k) * p.Hd + c;
+          W3s[e] = (k < p.S) ? __ldg(p.W_hi + o3) + __ldg(p.W_lo + o3) : 0.f;
+        }
+        if (tid < S0MAX) b3s[tid] = tid < p.S ? __ldg(p.bias_all + row3 + tid) : 0.f;
       }
-      for (int c = tid; c < p.Hd; c += tcg::PRODUCER_THREADS) b1s[c] = __ldg(p.bias_all + row0 + c);
-      if (tid < S0MAX) b3s[tid] = tid < p.S ? __ldg(p.bias_all + row3 + tid) : 0.f;
+      for (int e = tid; e < 3 * tcg::BN; e += tcg::PRODUCER_THREADS) {
+        const int st = e / tcg::BN, c = e - st * tcg::BN;
+        bs[e] = c < p.Hd ? __ldg(p.bias_all + row0 + st * p.Hd + c) : 0.f;
+      }
       tcg::producers_sync();
       cur_layer = layer;
+      tm.lap(1);
     }
-    float tv[S0MAX];
+    if (mma0(p)) return;
 #pragma unroll
     for (int k = 0; k < S0MAX; ++k)
       tv[k] = (src >= 0 && k < p.S) ? __ldg(p.table + (int64_t)src * p.S + k) : 0.f;
-    float* row = act + (size_t)r * AP;
-#pragma unroll 4                                          // four independent 8-FMA chains in flight
-    for (int c = 0; c < p.Hd; ++c) {
-      const float4* wr = reinterpret_cast<const float4*>(W1s + c * S0MAX);
-      const float4 wa = wr[0], wb = wr[1];
-      float a = b1s[c];
-      a = fmaf(tv[0], wa.x, a); a = fmaf(tv[1], wa.y, a); a = fmaf(tv[2], wa.z, a); a = fmaf(tv[3], wa.w, a);
-      a = fmaf(tv[4], wb.x, a); a = fmaf(tv[5], wb.y, a); a = fmaf(tv[6], wb.z, a); a = fmaf(tv[7], wb.w, a);
-      row[c] = fmaxf(a, 0.f);
-    }
   }
 
   __device__ __forceinline__ void produce(int sub, int kb, float (&v)[32]) {
@@ -145,58 +159,52 @@ struct ChainPolicy {
         v[j] = (src >= 0 && j < p.S) ? __ldg(p.table + (int64_t)src * p.S + j) : 0.f;
       return;
     }
-    const float4* a4 = reinterpret_cast<const float4*>(act + (size_t)r * AP + kb * tcg::BK);
+    // ---- first stage on the CUDA cores (S <= 8): columns [32 kb, 32 kb + 32) of ReLU(W1 t + b1) ----
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 t = a4[q];
-      v[4 * q + 0] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+    for (int j = 0; j < 32; ++j) {
+      const int c = kb * tcg::BK + j;
+      const float4* wr = reinterpret_cast<const float4*>(W1s + c * S0MAX);
+      const float4 wa = wr[0], wb = wr[1];
+      float a = bs[c];
+      a = fmaf(tv[0], wa.x, a); a = fmaf(tv[1], wa.y, a); a = fmaf(tv[2], wa.z, a); a = fmaf(tv[3], wa.w, a);
+      a = fmaf(tv[4], wb.x, a); a = fmaf(tv[5], wb.y, a); a = fmaf(tv[6], wb.z, a); a = fmaf(tv[7], wb.w, a);
+      v[j] = fmaxf(a, 0.f);
     }
   }
   __device__ __forceinline__ void pre_epilogue(int) {}
   __device__ __forceinline__ void post_epilogue(int) {}
 
-  // Every produce() of this step precedes the step's stores, and a thread only touches its own
-  // row, so the next stage's input overwrites this stage's in place.
+  // Only the item's last step is drained: stage 3 (S > 8) or stage 2 (S <= 8).
   __device__ __forceinline__ void store(int sub, int col, const float (&x)[tcg::EW]) {
     const int layer = sub >> 2, stage = sub & 3;
-    const float* bias = p.bias_all + w_row0(p, layer, stage);
-    if (stage < 3) {
-      if (col >= p.Hd) return;
-      float* dst = act + (size_t)r * AP + col;
+    if (stage == 3) {
+      if (src < 0 || col >= p.S) return;
+      const float* bias = p.bias_all + w_row0(p, layer, stage);
+      float* dst = p.coeff + ((int64_t)layer * p.Rall + src) * p.S;
 #pragma unroll
-      for (int j = 0; j < tcg::EW; ++j) dst[j] = fmaxf(x[j] + __ldg(bias + col + j), 0.f);
-      if (stage == 2 && !mma0(p) && col + tcg::EW >= p.Hd) output_stage(layer);
+      for (int j = 0; j < tcg::EW; ++j)
+        if (col + j < p.S) dst[col + j] = x[j] + __ldg(bias + col + j);
       return;
     }
-    if (src < 0 || col >= p.S) return;
-    float* dst = p.coeff + ((int64_t)layer * p.Rall + src) * p.S;
+    // ---- output stage on the CUDA cores (S <= 8): coeff = W3 ReLU(acc + b2) + b3 ------------------
+    // The chunks arrive in ascending column order, so every sum runs over the columns in order.
+    if (col >= p.Hd) return;
+    const float* b2 = bs + 2 * tcg::BN;
+    if (col == 0) {
 #pragma unroll
-    for (int j = 0; j < tcg::EW; ++j)
-      if (col + j < p.S) dst[col + j] = x[j] + __ldg(bias + col + j);
-  }
-
-  // ---- output stage on the CUDA cores (S <= 8): coeff = W3 act + b3 --------------------------
-  // Called by store() once this thread's row of stage 2 is complete; the row is read back from
-  // `act` (written by this thread alone) and summed in ascending column order.
-  __device__ __forceinline__ void output_stage(int layer) {
-    if (src < 0) return;
-    const float4* a4 = reinterpret_cast<const float4*>(act + (size_t)r * AP);
-    float o[S0MAX];
-#pragma unroll
-    for (int s = 0; s < S0MAX; ++s) o[s] = 0.f;
-    for (int c4 = 0; c4 < p.Hd / 4; ++c4) {
-      const float4 a = a4[c4];
-      const float av[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const float4* wr = reinterpret_cast<const float4*>(W3s + (4 * c4 + u) * S0MAX);
-        const float4 wa = wr[0], wb = wr[1];
-        o[0] = fmaf(av[u], wa.x, o[0]); o[1] = fmaf(av[u], wa.y, o[1]);
-        o[2] = fmaf(av[u], wa.z, o[2]); o[3] = fmaf(av[u], wa.w, o[3]);
-        o[4] = fmaf(av[u], wb.x, o[4]); o[5] = fmaf(av[u], wb.y, o[5]);
-        o[6] = fmaf(av[u], wb.z, o[6]); o[7] = fmaf(av[u], wb.w, o[7]);
-      }
+      for (int s = 0; s < S0MAX; ++s) o[s] = 0.f;
     }
+#pragma unroll
+    for (int j = 0; j < tcg::EW; ++j) {
+      const float y = fmaxf(x[j] + b2[col + j], 0.f);
+      const float4* wr = reinterpret_cast<const float4*>(W3s + (col + j) * S0MAX);
+      const float4 wa = wr[0], wb = wr[1];
+      o[0] = fmaf(y, wa.x, o[0]); o[1] = fmaf(y, wa.y, o[1]);
+      o[2] = fmaf(y, wa.z, o[2]); o[3] = fmaf(y, wa.w, o[3]);
+      o[4] = fmaf(y, wb.x, o[4]); o[5] = fmaf(y, wb.y, o[5]);
+      o[6] = fmaf(y, wb.z, o[6]); o[7] = fmaf(y, wb.w, o[7]);
+    }
+    if (col + tcg::EW < p.Hd || src < 0) return;
     float* dst = p.coeff + ((int64_t)layer * p.Rall + src) * p.S;
 #pragma unroll
     for (int s = 0; s < S0MAX; ++s)

@@ -19,7 +19,8 @@
 //                   One lane of warp 4 also issues the W tile loads (TMA), kStagesB k-blocks ahead.
 // The accumulators reach the epilogue through shared memory: once a step's last k-block is
 // multiplied the A ring is dead, and the consumers drain [D_main + D_corr] into it in column
-// passes that the producer threads read back row by row.
+// passes that the producer threads read back row by row.  A policy may instead have the consumers
+// turn a step's accumulators straight into the next step's A operand (operand_from_acc below).
 #pragma once
 #include "common.cuh"
 #include "sm90.cuh"
@@ -86,6 +87,7 @@ __device__ __forceinline__ Core carve(uint8_t* base, int stages_b, int stages_a)
 // prof[cta*32 + phase] (slots 8 / 9: k-loop / accumulator wait of odd sub-steps, 10: post_epilogue):
 //   0 staging issue  1 staging wait (policy)  3 k-loop  4 pre_epilogue
 //   5 wait for the accumulator  7 epilogue store
+// Slot 14 is the consumers' operand hand-over (operand_from_acc), timed by the first consumer thread.
 __device__ unsigned long long* g_prof = nullptr;
 
 struct PhaseTimer {          // thread 0 of the CTA only; no-op unless a buffer is registered
@@ -93,6 +95,10 @@ struct PhaseTimer {          // thread 0 of the CTA only; no-op unless a buffer 
   long long t0;
   __device__ __forceinline__ void start(int cta, int tid) {
     buf = (tid == 0 && g_prof) ? g_prof + cta * 32 : nullptr;
+    if (buf) t0 = clock64();
+  }
+  __device__ __forceinline__ void start_if(int cta, bool owner) {   // timed by another thread than 0
+    buf = (owner && g_prof) ? g_prof + cta * 32 : nullptr;
     if (buf) t0 = clock64();
   }
   __device__ __forceinline__ void lap(int slot) {
@@ -143,8 +149,40 @@ __device__ __forceinline__ int stg_index(int row, int col, int pw) {
 //                                                         when it set the fragment d (rows row0 and
 //                                                         row0 + 8, columns 8 j + cl + {0, 1}); the
 //                                                         MMAs then add to it
+// Optional pair (a policy whose step multiplies the previous step's activated result; needs
+// kStagesA * BK >= BN; acc_operand may read policy shared memory that the producers wrote before
+// they produced the previous step's k-blocks, or before an earlier one's):
+//   static bool operand_from_acc(const Params&, int sub)  the step's A k-blocks are written by the
+//                                                         consumers from the previous step's accumulators
+//   static float acc_operand(const Params&, const uint8_t* policy_smem, int sub, int col, float x)
+//                                                         consumers: A value of column col of the next
+//                                                         step, from column col of step sub's result
+//                                                         x = D_main + D_corr
+//   The previous step then has no drain.  After its last wgmma.wait every consumer thread writes
+//   acc_operand() of its fragment, split into tf32 hi / lo, into k-block col / 32 = A stage col / 32
+//   (its own warpgroup's rows, which only its own, retired MMAs read), runs fence.proxy.async, and
+//   the consumers meet at named barrier 2; the step's MMAs then read stages 0 .. nkb - 1 without
+//   a_full waits or a_empty arrivals (the A ring's mbarrier phases count produced k-blocks only).
+//   The producers produce nothing for the step and skip the previous step's drain.  Ordering: the
+//   producers write no A stage again until they have read a drain that follows the step (every
+//   producer thread reads its row, then producers_sync), and the consumers write that drain only
+//   after all of the step's MMAs have retired.  (Consecutive operand_from_acc steps are fine: the
+//   drain is then that of the last of them; a CTA's last step is always drained.)
 template <class P, class = void> struct HasAccInit : std::false_type {};
 template <class P> struct HasAccInit<P, std::void_t<decltype(&P::acc_init)>> : std::true_type {};
+template <class P, class = void> struct HasOperandFromAcc : std::false_type {};
+template <class P> struct HasOperandFromAcc<P, std::void_t<decltype(&P::operand_from_acc)>> : std::true_type {};
+
+// Whether step it + 1 takes its operand from step it's accumulators (operand_from_acc policies only)
+template <class Policy>
+__device__ __forceinline__ bool next_from_acc(const typename Policy::Params& p, int cta, int ncta, int it,
+                                              int nsteps, int& nkb_next) {
+  if (it + 1 >= nsteps) return false;
+  int m_tile, sub;
+  Policy::decode(p, cta, ncta, it + 1, m_tile, sub);
+  nkb_next = Policy::num_kblocks(p, sub);
+  return Policy::operand_from_acc(p, sub);
+}
 
 template <class Policy>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -161,6 +199,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
   constexpr int NPASS = BN / PW;
   constexpr bool kAccInit = HasAccInit<Policy>::value;
   static_assert(!kAccInit || NPASS == 1, "a drain kept in the A ring must fit it in one pass");
+  constexpr bool kOpAcc = HasOperandFromAcc<Policy>::value;
+  static_assert(!kOpAcc || SA * BK >= BN, "an operand written from the accumulators needs one A stage per k-block");
   Core c = carve(base, SB, SA);
   uint8_t* policy_smem = base + core_smem(SB, SA);
   float* stg = reinterpret_cast<float*>(c.Ast);
@@ -204,9 +244,14 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
     for (int it = 0; it < nsteps; ++it) {
       int m_tile, sub;
       Policy::decode(p, cta, ncta, it, m_tile, sub);
-      const int nkb = Policy::num_kblocks(p, sub);
-      bool kept = false;
+      int nkb = Policy::num_kblocks(p, sub);
+      bool kept = false, to_acc = false;
       if constexpr (kAccInit) kept = Policy::drain_kept(p, sub);
+      if constexpr (kOpAcc) {
+        if (Policy::operand_from_acc(p, sub)) nkb = 0;      // the consumers write this step's k-blocks
+        int nkb_next;
+        to_acc = next_from_acc<Policy>(p, cta, ncta, it, nsteps, nkb_next);   // no drain
+      }
       PhaseTimer tm;
       tm.start(cta, tid);
       pol.step_begin(m_tile, sub, 0, tm);
@@ -243,7 +288,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
       tm.lap(4);
       // ---- epilogue: the consumers drain the accumulators in passes of PW columns ----
 #pragma unroll 1
-      for (int q = 0; q < (kept ? 0 : NPASS); ++q, ++npass) {
+      for (int q = 0; q < (kept || to_acc ? 0 : NPASS); ++q, ++npass) {
         sm90::mbar_wait(c.stg_full, npass & 1u);
         if (q == 0) tm.lap((sub & 1) ? 9 : 5);
 #pragma unroll 1
@@ -270,6 +315,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
     const int wq = warp & 3;
     float d[128];                                    // [D_main (64 x 128) | D_corr (64 x 128)]
     uint32_t cnt = 0, npass = 0;
+    uint32_t nacc = 0;                               // k-blocks written by the consumers (not in the A ring's count)
     bool after_kept = false;                         // the previous step's drain is in the A ring
     const int row0 = wg * 64 + wq * 16 + (lane >> 2), cl = 2 * (lane & 3);
     // W loads (warp CONSUMER_WARP0 only): the cursor walks the k-blocks of all steps in order;
@@ -311,7 +357,12 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
       int m_tile, sub;
       Policy::decode(p, cta, ncta, it, m_tile, sub);
       const int nkb = Policy::num_kblocks(p, sub);
-      bool kept = false;
+      bool kept = false, from_acc = false, to_acc = false;
+      int nkb_next = 0;
+      if constexpr (kOpAcc) {
+        from_acc = Policy::operand_from_acc(p, sub);
+        to_acc = next_from_acc<Policy>(p, cta, ncta, it, nsteps, nkb_next);
+      }
       if constexpr (kAccInit) {
         kept = Policy::drain_kept(p, sub);
         if (!Policy::acc_init(p, policy_smem, stg, sub, row0, cl, d)) {
@@ -327,9 +378,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
         for (int i = 0; i < 128; ++i) d[i] = 0.f;
       }
       for (int kb = 0; kb < nkb; ++kb, ++cnt) {
-        const uint32_t sb = cnt % SB, sa = cnt % SA;
+        const uint32_t acnt = cnt - nacc;            // A ring position (cnt without operand_from_acc)
+        const uint32_t sb = cnt % SB, sa = from_acc ? (uint32_t)kb : acnt % SA;
         sm90::mbar_wait(&c.b_full[sb], (cnt / SB) & 1u);
-        sm90::mbar_wait(&c.a_full[sa], (cnt / SA) & 1u);
+        if (!from_acc) sm90::mbar_wait(&c.a_full[sa], (acnt / SA) & 1u);
         if (!(p.dbg & 2)) {
           const uint32_t a_hi = sm90::smem_u32(c.Ast + sa * STAGE_A_BYTES) + wg * 64 * 128;
           const uint32_t a_lo = a_hi + TILE_A_BYTES;
@@ -348,25 +400,54 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
         }
         __syncwarp();                                // stage released as soon as its MMAs retire
         if (lane == 0) {
-          sm90::mbar_arrive(&c.a_empty[sa]);
+          if (!from_acc) sm90::mbar_arrive(&c.a_empty[sa]);
           sm90::mbar_arrive(&c.b_empty[sb]);
         }
         if (issuer) load_next();
       }
+      if (from_acc) nacc += nkb;
+      PhaseTimer ctm;
+      if (to_acc) ctm.start_if(cta, tid == PRODUCER_THREADS);
       consumers_sync();                              // both warpgroups are done reading the A ring
-      // A kept drain needs no hand-over: the producers read the last drain before they wrote this
-      // step's k-blocks, and they write no more until kept_read
+      if (to_acc) {
+        // The next step's operand: k-block kb = A stage kb holds columns [32 kb, 32 kb + 32) of
+        // acc_operand(D_main + D_corr), split as the producers split theirs, in SWIZZLE_128B layout
+        if constexpr (kOpAcc) {
 #pragma unroll
-      for (int q = 0; q < NPASS; ++q, npass += kept ? 0 : 1) {
-        if (!kept) sm90::mbar_wait(c.stg_empty, (npass & 1u) ^ 1u);
-#pragma unroll
-        for (int i = 0; i < 64; i += 2) {
-          const int col = 8 * (i / 4) + cl, row = row0 + 8 * ((i / 2) % 2);
-          if (col >= q * PW && col < (q + 1) * PW)
-            *reinterpret_cast<float2*>(stg + stg_index(row, col - q * PW, PW)) =
-                make_float2(d[i] + d[i + 64], d[i + 1] + d[i + 65]);
+          for (int i = 0; i < 64; i += 2) {
+            const int col = 8 * (i / 4) + cl, row = row0 + 8 * ((i / 2) % 2), kb = i / 16;
+            if (kb < nkb_next) {
+              const float y0 = Policy::acc_operand(p, policy_smem, sub, col, d[i] + d[i + 64]);
+              const float y1 = Policy::acc_operand(p, policy_smem, sub, col + 1, d[i + 1] + d[i + 65]);
+              uint2 h, l;
+              h.x = sm90::tf32_rna_bits(y0); h.y = sm90::tf32_rna_bits(y1);
+              l.x = sm90::tf32_rna_bits(y0 - __uint_as_float(h.x));
+              l.y = sm90::tf32_rna_bits(y1 - __uint_as_float(h.y));
+              uint8_t* dst = c.Ast + kb * STAGE_A_BYTES + row * 128 + (((((col & 31) >> 2) ^ row) & 7) << 4) +
+                             (col & 3) * 4;
+              *reinterpret_cast<uint2*>(dst) = h;
+              *reinterpret_cast<uint2*>(dst + TILE_A_BYTES) = l;
+            }
+          }
+          sm90::fence_proxy_async();                 // visible to the tensor core's operand reads
+          consumers_sync();
+          ctm.lap(14);
         }
-        if (!kept) sm90::mbar_arrive(c.stg_full);
+      } else {
+        // A kept drain needs no hand-over: the producers read the last drain before they wrote this
+        // step's k-blocks, and they write no more until kept_read
+#pragma unroll
+        for (int q = 0; q < NPASS; ++q, npass += kept ? 0 : 1) {
+          if (!kept) sm90::mbar_wait(c.stg_empty, (npass & 1u) ^ 1u);
+#pragma unroll
+          for (int i = 0; i < 64; i += 2) {
+            const int col = 8 * (i / 4) + cl, row = row0 + 8 * ((i / 2) % 2);
+            if (col >= q * PW && col < (q + 1) * PW)
+              *reinterpret_cast<float2*>(stg + stg_index(row, col - q * PW, PW)) =
+                  make_float2(d[i] + d[i + 64], d[i + 1] + d[i + 65]);
+          }
+          if (!kept) sm90::mbar_arrive(c.stg_full);
+        }
       }
       if (kept) consumers_sync();                    // the next acc_init() reads rows of both halves
       after_kept = kept;
