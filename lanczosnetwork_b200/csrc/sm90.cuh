@@ -42,6 +42,30 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// The same wait with its retry loop inside one asm block (block-scoped labels).  Code that waits
+// while a wgmma group is in flight uses these: a C++ loop around try_wait is a divergent branch to
+// ptxas, which then waits for the whole group there (C7518) and serialises every wgmma.
+__device__ __forceinline__ void mbar_wait_uniform(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "LAB_WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@p bra DONE;\n\t"
+      "bra.uni LAB_WAIT;\n\t"
+      "DONE:\n\t}"
+      ::"r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+}
+// Arrive when pred is set: a predicated instruction, not a branch
+__device__ __forceinline__ void mbar_arrive_pred(uint64_t* bar, bool pred) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %1, 0;\n\t"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+      ::"r"(smem_u32(bar)), "r"((uint32_t)pred)
+      : "memory");
+}
+
 // ---- TMA ----------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -73,6 +97,39 @@ __device__ __forceinline__ void cp_async_wait_all() {
 // Generic-proxy writes to shared memory become visible to the async proxy (wgmma operand reads).
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
+// One elected lane of a warp for which `pred` holds (the warp must be converged) arms `bar` for
+// `bytes` and issues two 2-D tiled loads into dst0 / dst1 at the same coordinates; with
+// `skip_load` it only arrives (an experiment: the stage then holds stale data).  The election and
+// the predicate stay inside the asm, so the code around it has no branch.
+template <bool skip_load = false>
+__device__ __forceinline__ void tma_load_2d_pair_elected(bool pred, uint64_t* bar, uint32_t bytes, void* dst0,
+                                                         const CUtensorMap* m0, void* dst1, const CUtensorMap* m1,
+                                                         int32_t c0, int32_t c1) {
+  if constexpr (skip_load) {
+    asm volatile(
+        "{\n\t.reg .pred e, p;\n\t"
+        "elect.sync _|e, 0xffffffff;\n\t"
+        "setp.ne.and.b32 p, %1, 0, e;\n\t"
+        "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+        ::"r"(smem_u32(bar)), "r"((uint32_t)pred)
+        : "memory");
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred e, p;\n\t"
+        "elect.sync _|e, 0xffffffff;\n\t"
+        "setp.ne.and.b32 p, %1, 0, e;\n\t"
+        "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %2;\n\t"
+        "@p cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
+        " [%3], [%4, {%7, %8}], [%0];\n\t"
+        "@p cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
+        " [%5], [%6, {%7, %8}], [%0];\n\t}"
+        ::"r"(smem_u32(bar)), "r"((uint32_t)pred), "r"(bytes), "r"(smem_u32(dst0)),
+          "l"(reinterpret_cast<uint64_t>(m0)), "r"(smem_u32(dst1)), "l"(reinterpret_cast<uint64_t>(m1)),
+          "r"(c0), "r"(c1)
+        : "memory");
+  }
 }
 
 __device__ __forceinline__ bool elect_one() {
@@ -107,6 +164,15 @@ __device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw128(uint32_t smem_addr) 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Pins the accumulator registers in program order: the compiler may otherwise sink their
+// initialisation past wgmma.fence, between the start and end of an MMA group, where ptxas then
+// serialises every wgmma (C7515).  Emits no instruction.
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// every group but the newest has retired
+__device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // Accumulator fragment of an m64nNk8 f32 product held by one warpgroup: d[i] of thread
 // (warp w, lane l) is row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.

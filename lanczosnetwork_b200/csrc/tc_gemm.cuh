@@ -16,7 +16,9 @@
 //   warps 4-11      two consumer warpgroups: warpgroup c owns tile rows [64 c, 64 c + 64) and
 //                   keeps D_main and D_corr (64 x 128 fp32 each) in registers; per k-step three
 //                   m64n128k8 wgmma: A_hi W_hi -> D_main, A_hi W_lo -> D_corr, A_lo W_hi -> D_corr.
-//                   One lane of warp 4 also issues the W tile loads (TMA), kStagesB k-blocks ahead.
+//                   Every consumer warp runs the W cursor and its waits; the elected lane of warp 4
+//                   issues the W tile loads (TMA, predicated inside the asm), kStagesB k-blocks ahead.
+//                   Policies without acc_init keep one MMA group queued (wgmma.wait_group 1).
 // The accumulators reach the epilogue through shared memory: once a step's last k-block is
 // multiplied the A ring is dead, and the consumers drain [D_main + D_corr] into it in column
 // passes that the producer threads read back row by row.  A policy may instead have the consumers
@@ -184,10 +186,16 @@ __device__ __forceinline__ bool next_from_acc(const typename Policy::Params& p, 
   return Policy::operand_from_acc(p, sub);
 }
 
-template <class Policy>
-__global__ void __launch_bounds__(THREADS, 1)
-tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
-               const __grid_constant__ CUtensorMap map_lo, const typename Policy::Params p) {
+// Pipeline experiments (LNB_DBG, profiling only; results are wrong with any bit set): bits of the
+// kernel's kSkip template parameter, so the production kernel has no branch around its MMAs.
+constexpr int SKIP_MMA = 2;      // issue no wgmma
+constexpr int SKIP_TMA = 4;      // load no W tile (b_full is armed without a transfer)
+// Bits 1 (skip the A stores) and 8 (skip produce()) are read from Params::dbg by the producer warps,
+// which issue no wgmma.
+
+template <class Policy, int kSkip>
+__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CUtensorMap& map_lo,
+                                             const typename Policy::Params& p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   // 1024-byte alignment (SWIZZLE_128B) by OFFSETTING the __shared__ array -- keeps the
   // shared address space visible to the compiler (LDS/STS instead of generic LD/ST)
@@ -200,14 +208,22 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
   constexpr bool kAccInit = HasAccInit<Policy>::value;
   static_assert(!kAccInit || NPASS == 1, "a drain kept in the A ring must fit it in one pass");
   constexpr bool kOpAcc = HasOperandFromAcc<Policy>::value;
+  // One MMA group queued across k-blocks.  Not with acc_init(): ptxas (CUDA 12.9) then serialises
+  // every wgmma (C7515) because acc_init's FMAs define the accumulators, even with the operand
+  // fences below; those policies wait for every group, as before.
+  constexpr bool kQueue = !kAccInit;
   static_assert(!kOpAcc || SA * BK >= BN, "an operand written from the accumulators needs one A stage per k-block");
   Core c = carve(base, SB, SA);
   uint8_t* policy_smem = base + core_smem(SB, SA);
   float* stg = reinterpret_cast<float*>(c.Ast);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // 0: producers, 1 / 2: consumer warpgroups; broadcast from lane 0, so ptxas sees a warp-uniform value
+  const int role = __shfl_sync(0xffffffffu, tid / 128, 0);
   const int cta = blockIdx.x, ncta = gridDim.x;
-  const int nsteps = Policy::num_steps(p, cta, ncta);
+  // num_steps may read memory (the stack's schedule): broadcast, so every count the consumers' loops
+  // derive from it is warp-uniform to ptxas as well
+  const int nsteps = __shfl_sync(0xffffffffu, Policy::num_steps(p, cta, ncta), 0);
   unsigned long long prof_ns0 = 0;                  // whole-CTA wall time / cycles (slots 11, 12)
   long long prof_c0 = 0;
   if (tid == 0 && g_prof) {
@@ -233,7 +249,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
   }
   __syncthreads();
 
-  if (warp < CONSUMER_WARP0) {
+  if (role == 0) {
     // ================================ producers + epilogue ================================
     const int r = tid & 127;                         // tile row of this thread
     Policy pol(p, policy_smem, tid);
@@ -311,16 +327,18 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
     }
   } else {
     // ================================ MMA consumers ========================================
-    const int wg = (warp - CONSUMER_WARP0) >> 2;     // rows [64 wg, 64 wg + 64) of the tile
+    const int wg = role - 1;                         // rows [64 wg, 64 wg + 64) of the tile
     const int wq = warp & 3;
     float d[128];                                    // [D_main (64 x 128) | D_corr (64 x 128)]
     uint32_t cnt = 0, npass = 0;
     uint32_t nacc = 0;                               // k-blocks written by the consumers (not in the A ring's count)
     bool after_kept = false;                         // the previous step's drain is in the A ring
     const int row0 = wg * 64 + wq * 16 + (lane >> 2), cl = 2 * (lane & 3);
-    // W loads (warp CONSUMER_WARP0 only): the cursor walks the k-blocks of all steps in order;
-    // the load of k-block i waits until every consumer warp has released k-block i - kStagesB
-    const bool issuer = warp == CONSUMER_WARP0;
+    // W loads: the cursor walks the k-blocks of all steps in order; the load of k-block i waits until
+    // every consumer warp has released k-block i - kStagesB.  Every consumer warp runs the cursor and
+    // the wait, and the elected lane of warp CONSUMER_WARP0 issues the load under a predicate inside
+    // the asm: between two MMA groups no consumer warp takes a path another one does not.
+    const bool w_issuer = warp == CONSUMER_WARP0;
     int l_it = 0, l_kb = 0, l_nkb = -1, l_sub = 0;
     uint32_t l_cnt = 0;
     auto load_next = [&]() {
@@ -337,22 +355,20 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
       int col0, row0;
       Policy::w_coords(p, l_sub, l_kb, col0, row0);
       const uint32_t st = l_cnt % SB;
-      sm90::mbar_wait(&c.b_empty[st], ((l_cnt / SB) & 1u) ^ 1u);
-      if (sm90::elect_one()) {
-        if (p.dbg & 4) {
-          sm90::mbar_arrive(&c.b_full[st]);
-        } else {
-          uint8_t* dst = c.Bst + st * STAGE_B_BYTES;
-          sm90::mbar_arrive_expect_tx(&c.b_full[st], STAGE_B_BYTES);
-          sm90::tma_load_2d(dst, &map_hi, &c.b_full[st], col0, row0);
-          sm90::tma_load_2d(dst + TILE_B_BYTES, &map_lo, &c.b_full[st], col0, row0);
-        }
-      }
-      __syncwarp();
+      sm90::mbar_wait_uniform(&c.b_empty[st], ((l_cnt / SB) & 1u) ^ 1u);
+      uint8_t* dst = c.Bst + st * STAGE_B_BYTES;
+      sm90::tma_load_2d_pair_elected<(kSkip & SKIP_TMA) != 0>(w_issuer, &c.b_full[st], STAGE_B_BYTES, dst, &map_hi,
+                                                               dst + TILE_B_BYTES, &map_lo, col0, row0);
       ++l_kb; ++l_cnt;
     };
-    if (issuer)
-      for (int i = 0; i < SB; ++i) load_next();
+    // releases the W stage sb_rel and, with a_stage, the A stage sa_rel of a k-block whose MMAs have
+    // retired, and loads W kStagesB k-blocks ahead
+    auto release = [&](uint32_t sb_rel, bool a_stage, uint32_t sa_rel) {
+      sm90::mbar_arrive_pred(&c.a_empty[sa_rel], a_stage && lane == 0);
+      sm90::mbar_arrive_pred(&c.b_empty[sb_rel], lane == 0);
+      load_next();
+    };
+    for (int i = 0; i < SB; ++i) load_next();
     for (int it = 0; it < nsteps; ++it) {
       int m_tile, sub;
       Policy::decode(p, cta, ncta, it, m_tile, sub);
@@ -365,6 +381,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
       }
       if constexpr (kAccInit) {
         kept = Policy::drain_kept(p, sub);
+        sm90::wgmma_fence_operand(d);              // acc_init() writes d only after the last step's wait
         if (!Policy::acc_init(p, policy_smem, stg, sub, row0, cl, d)) {
 #pragma unroll
           for (int i = 0; i < 128; ++i) d[i] = 0.f;
@@ -377,15 +394,21 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
 #pragma unroll
         for (int i = 0; i < 128; ++i) d[i] = 0.f;
       }
+      sm90::wgmma_fence_operand(d);
+      // kQueue: one MMA group stays queued: k-block kb is issued before k-block kb - 1 is waited for,
+      // and kb - 1's stages are released once it has retired.  Between two groups there are only
+      // mbarrier waits whose retry loops are inside their asm, predicated arrivals and the W
+      // cursor, whose branches depend on kernel parameters and loop counters alone.
       for (int kb = 0; kb < nkb; ++kb, ++cnt) {
         const uint32_t acnt = cnt - nacc;            // A ring position (cnt without operand_from_acc)
         const uint32_t sb = cnt % SB, sa = from_acc ? (uint32_t)kb : acnt % SA;
-        sm90::mbar_wait(&c.b_full[sb], (cnt / SB) & 1u);
-        if (!from_acc) sm90::mbar_wait(&c.a_full[sa], (acnt / SA) & 1u);
-        if (!(p.dbg & 2)) {
+        sm90::mbar_wait_uniform(&c.b_full[sb], (cnt / SB) & 1u);
+        if (!from_acc) sm90::mbar_wait_uniform(&c.a_full[sa], (acnt / SA) & 1u);
+        if constexpr (!(kSkip & SKIP_MMA)) {
           const uint32_t a_hi = sm90::smem_u32(c.Ast + sa * STAGE_A_BYTES) + wg * 64 * 128;
           const uint32_t a_lo = a_hi + TILE_A_BYTES;
           const uint32_t b = sm90::smem_u32(c.Bst + sb * STAGE_B_BYTES);
+          sm90::wgmma_fence_operand(d);
           sm90::wgmma_fence();
 #pragma unroll
           for (int k = 0; k < BK / 8; ++k) {
@@ -396,15 +419,23 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
             sm90::wgmma_n128_hi(d, sm90::wgmma_desc_kmajor_sw128(a_lo + 32 * k), wh, 1u);     // D_corr += A_lo W_hi^T
           }
           sm90::wgmma_commit();
-          sm90::wgmma_wait_all();
+          if constexpr (kQueue) sm90::wgmma_wait_one();   // k-block kb - 1 has retired
+          else sm90::wgmma_wait_all();
+          sm90::wgmma_fence_operand(d);
         }
-        __syncwarp();                                // stage released as soon as its MMAs retire
-        if (lane == 0) {
-          if (!from_acc) sm90::mbar_arrive(&c.a_empty[sa]);
-          sm90::mbar_arrive(&c.b_empty[sb]);
+        if constexpr (kQueue) {
+          if (kb > 0) release((cnt - 1) % SB, !from_acc, from_acc ? (uint32_t)(kb - 1) : (acnt - 1) % SA);
+        } else {
+          release(sb, !from_acc, sa);
         }
-        if (issuer) load_next();
       }
+      // unconditional, so that on every path ptxas sees no group in flight past this point
+      if constexpr (!(kSkip & SKIP_MMA)) {
+        sm90::wgmma_wait_all();
+        sm90::wgmma_fence_operand(d);
+      }
+      if (kQueue && nkb > 0)                         // the step's last k-block
+        release((cnt - 1) % SB, !from_acc, from_acc ? (uint32_t)(nkb - 1) : (cnt - nacc - 1) % SA);
       if (from_acc) nacc += nkb;
       PhaseTimer ctm;
       if (to_acc) ctm.start_if(cta, tid == PRODUCER_THREADS);
@@ -462,6 +493,21 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
     atomicAdd(&g_prof[cta * 32 + 12], (unsigned long long)(clock64() - prof_c0));
     g_prof[cta * 32 + 13] = prof_ns0;               // CTA start (ns), for launch skew
   }
+}
+
+template <class Policy>
+__global__ void __launch_bounds__(THREADS, 1)
+tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
+               const __grid_constant__ CUtensorMap map_lo, const typename Policy::Params p) {
+  tc_gemm_body<Policy, 0>(map_hi, map_lo, p);
+}
+
+// The skeleton with pipeline parts switched off (kSkip: SKIP_MMA | SKIP_TMA), for LNB_DBG experiments
+template <class Policy, int kSkip>
+__global__ void __launch_bounds__(THREADS, 1)
+tc_gemm_probe_kernel(const __grid_constant__ CUtensorMap map_hi,
+                     const __grid_constant__ CUtensorMap map_lo, const typename Policy::Params p) {
+  tc_gemm_body<Policy, kSkip>(map_hi, map_lo, p);
 }
 
 // Epilogue helper: bias / ReLU / bounds-checked store of EW accumulator columns of one row.
@@ -530,7 +576,8 @@ inline int make_weight_map(CUtensorMap* map, const float* W, int rows, int cols,
 }
 
 // LNB_DBG=<bits>: pipeline experiments (1 skip A stores, 2 skip MMA issue, 4 skip TMA loads,
-// 8 skip produce()).  Results are wrong with any bit set; for profiling only.
+// 8 skip produce()).  Results are wrong with any bit set; for profiling only.  Bits 2 and 4 select a
+// tc_gemm_probe_kernel instantiation in launch(); bits 1 and 8 are read by the producer warps.
 inline int debug_flags() {
   const char* e = getenv("LNB_DBG");
   return e ? atoi(e) : 0;
@@ -569,7 +616,11 @@ static int launch(lnb_stream_t stream, const float* W_hi, const float* W_lo, int
   if (rc != LNB_OK) return rc;
   rc = sync_prof_buffer(who);
   if (rc != LNB_OK) return rc;
-  auto kern = tc_gemm_kernel<Pol>;
+  const int skip = p.dbg & (SKIP_MMA | SKIP_TMA);
+  auto kern = skip == 0                    ? tc_gemm_kernel<Pol>
+              : skip == SKIP_MMA           ? tc_gemm_probe_kernel<Pol, SKIP_MMA>
+              : skip == SKIP_TMA           ? tc_gemm_probe_kernel<Pol, SKIP_TMA>
+                                           : tc_gemm_probe_kernel<Pol, SKIP_MMA | SKIP_TMA>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   const int grid = items < sm_count() ? items : sm_count();
   kern<<<grid, THREADS, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
