@@ -306,6 +306,24 @@ int lnb_gat_attention(lnb_stream_t stream, const float* Wh, const float* bias, c
                       const float* a2, const float* c1, const float* c2, const float* state_bias,
                       int B, int N, int E1, int heads, int F, int last, float* out);
 
+/* Adjoint of lnb_gat_attention for the training path.  Inputs: the forward's Wh, bias, a1, a2, c1, c2,
+ * state_bias and gout = dL/dout (the shape of the forward's out).  Per channel c, with att and
+ * h_c = att Wh_c + state_bias_c recomputed exactly as the forward computes them, and gh = gout_c * ELU'(h_c)
+ * (hidden; ELU'(h) = exp(h) for h <= 0) or gout / C (last):
+ *   gWh[b,k,c*F:(c+1)*F] = sum_i att[i,k] gh[i] + gs1[k] a1[c] + gs2[k] a2[c]        gWh [B,N,C*F]
+ *   gX[i,k] = att[i,k] (gh[i].Wh[k] - sum_i' att[i',k] gh[i'].Wh[k]) * (s1[i] + s2[k] > 0 ? 1 : 0.2)
+ *   gs1[i] = sum_k gX[i,k],  gs2[k] = sum_i gX[i,k]
+ *   gpar[b,c,:] = [sum_k gs1[k] Wh[k] (F) | sum_k gs2[k] Wh[k] (F) | sum_i gh[i] (F) | sum gs1 | sum gs2]
+ * gpar [B, C, 3F+2] holds each graph's share of the gradients of a1, a2, state_bias, c1 and c2: the caller
+ * sums it over B.  The bias gets no gradient.  One CTA per (graph, bond channel, head group); every sum
+ * in a fixed order, no atomics: repeated launches are bit-identical.  gout, Wh, a1, a2, state_bias, gWh
+ * 16-byte aligned.  Envelope: that of lnb_gat_attention (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ */
+int lnb_gat_attention_backward(lnb_stream_t stream, const float* gout, const float* Wh, const float* bias,
+                               const float* a1, const float* a2, const float* c1, const float* c2,
+                               const float* state_bias, int B, int N, int E1, int heads, int F, int last,
+                               float* gWh, float* gpar);
+
 /* ---------------------------------------------------------------------------------------
  * GGNN propagation step after the message MLPs (model/ggnn.py:143-171), one persistent 3xTF32 wgmma
  * launch over all B*N rows:

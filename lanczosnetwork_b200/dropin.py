@@ -9,7 +9,8 @@ What it does (see INTEGRATION.md):
   2. rebinds the classes of ``DROPIN_CLASSES`` (``LanczosNet``, ``AdaLanczosNet``, ``GCN``, ``GAT``, ``GraphSAGE``, ``GGNN``, ``GPNN``, ...)
      inside the runner modules' globals, because the runners resolve the class with ``eval(name)`` in their own
      namespace (runner/qm8_runner.py:59,288; runner/graph_runner.py:57,285), plus the classes of
-     ``OPT_IN_CLASSES`` named with ``--opt-in NAME`` (repeatable; e.g. ``--opt-in MPNN``);
+     ``OPT_IN_CLASSES`` named with ``--opt-in NAME`` (repeatable; e.g. ``--opt-in MPNN``); ``--opt-in GAT``
+     (``TRAINING_OPT_IN_CLASSES``) binds ``TrainableGAT`` under the name ``GAT``, for training and test runs;
   3. runs the reference ``run_exp.main()`` unchanged (``--opt-in`` is removed from its argv).
 """
 import importlib
@@ -23,6 +24,9 @@ DROPIN_CLASSES = ('LanczosNet', 'AdaLanczosNet', 'LanczosNetGeneral', 'GCN', 'GC
                   'GAT', 'GraphSAGE', 'GGNN', 'GPNN')
 # drop-ins that replace the reference class only when asked for (patch_namespace(opt_in=...), --opt-in)
 OPT_IN_CLASSES = ('MPNN',)
+# names whose drop-in becomes its trainable subclass ``Trainable<name>`` when asked for (opt_in=..., --opt-in);
+# without the opt-in they keep their DROPIN_CLASSES behaviour
+TRAINING_OPT_IN_CLASSES = ('GAT',)
 
 
 def register_native_op():
@@ -35,24 +39,30 @@ def register_native_op():
 
 
 def _check_opt_in(opt_in):
-  unknown = [n for n in opt_in if n not in OPT_IN_CLASSES]
+  unknown = [n for n in opt_in if n not in OPT_IN_CLASSES + TRAINING_OPT_IN_CLASSES]
   if unknown:
-    raise ValueError('dropin: %s not in OPT_IN_CLASSES %s' % (', '.join(map(repr, unknown)), OPT_IN_CLASSES))
+    raise ValueError('dropin: %s not in OPT_IN_CLASSES %s or TRAINING_OPT_IN_CLASSES %s'
+                     % (', '.join(map(repr, unknown)), OPT_IN_CLASSES, TRAINING_OPT_IN_CLASSES))
   return tuple(opt_in)
 
 
 def patch_namespace(module, training=False, opt_in=()):
   """Rebind the class names in ``module``'s globals to the H100 drop-ins: those of ``DROPIN_CLASSES``
-  and those of ``opt_in`` (names from ``OPT_IN_CLASSES``; any other name is a ValueError).
-  ``training=True`` (a run without ``-t``) rebinds only the classes that have a differentiable training
-  path (every class but ``GAT``, which is inference only); a class without one keeps the reference's
-  trainable class instead of failing on the first ``loss.backward()``."""
-  for name in DROPIN_CLASSES + _check_opt_in(opt_in):
+  and those of ``opt_in`` (names from ``OPT_IN_CLASSES`` or ``TRAINING_OPT_IN_CLASSES``; any other name
+  is a ValueError).  ``training=True`` (a run without ``-t``) rebinds only the classes that have a
+  differentiable training path (every class but ``GAT``, which is inference only); a class without one
+  keeps the reference's trainable class instead of failing on the first ``loss.backward()``.  A name of
+  ``TRAINING_OPT_IN_CLASSES`` in ``opt_in`` is bound to ``Trainable<name>`` in training and test runs."""
+  opt_in = _check_opt_in(opt_in)
+  for name in DROPIN_CLASSES + tuple(n for n in opt_in if n in OPT_IN_CLASSES):
     if hasattr(module, name):
       cls = getattr(_models, name)
       if training and not hasattr(cls, '_train_impl'):
         continue
       setattr(module, name, cls)
+  for name in opt_in:
+    if name in TRAINING_OPT_IN_CLASSES and hasattr(module, name):
+      setattr(module, name, getattr(_models, 'Trainable' + name))
   return module
 
 
@@ -100,7 +110,7 @@ def main(argv=None):
   while '--opt-in' in argv:
     i = argv.index('--opt-in')
     if i + 1 >= len(argv):
-      raise SystemExit('--opt-in needs a class name (one of %s)' % (OPT_IN_CLASSES,))
+      raise SystemExit('--opt-in needs a class name (one of %s)' % (OPT_IN_CLASSES + TRAINING_OPT_IN_CLASSES,))
     opt_in.append(argv[i + 1])
     del argv[i:i + 2]
   install(root, compat=True, training=('-t' not in argv and '--test' not in argv), opt_in=opt_in)

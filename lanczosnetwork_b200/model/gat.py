@@ -13,9 +13,12 @@ ELU (or, in the last layer, the mean over channels).  With the embedding gather 
 
 Quirk kept on purpose: the reference's ``state_bias`` repeats one inner list for every bond channel
 (model/gat.py:62-70), so every channel of layer t uses ``bias_{ii}_{E}_{t}``; the other
-``bias_{ii}_{jj}_{t}`` are registered and saved but never read.  There is no training path: under
+``bias_{ii}_{jj}_{t}`` are registered and saved but never read.  ``GAT`` has no training path: under
 autograd with trainable parameters the forward raises, and ``dropin.patch_namespace(training=True)``
-keeps the reference class for training runs."""
+keeps the reference class for training runs.  ``TrainableGAT`` (same constructor, parameters and
+checkpoints) adds one: under autograd its forward is ``train.gat_train``, whose attention adjoint is
+``lnb_gat_attention_backward``; the drop-in binds it under the name ``GAT`` by opt-in only
+(``dropin.TRAINING_OPT_IN_CLASSES``, ``--opt-in GAT``)."""
 import torch
 import torch.nn as nn
 
@@ -23,7 +26,7 @@ from ._common import SpectralNetBase, _opt
 from ..spectral_conv import WeightCache
 from .. import ops
 
-__all__ = ['GAT']
+__all__ = ['GAT', 'TrainableGAT']
 
 
 def _linear_grid(num_layer, num_channel, num_heads, make):
@@ -142,3 +145,27 @@ class GAT(SpectralNetBase):
       state = ops.gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=(t == self.num_layer - 1))
     head, att = self.output_func[0], self.att_func[0]
     return ops.readout(state, head.weight, head.bias, att.weight.reshape(-1), att.bias, mask)
+
+
+class TrainableGAT(GAT):
+  """``GAT`` with a training path.  Under ``no_grad`` (or without trainable parameters) the forward is the
+  fused inference path with its CUDA graphs; under autograd it is ``train.gat_train``.  Dropout > 0 in
+  training mode is refused: the reference draws it at three sites per head (the head's input, the
+  attention weights and Wh, model/gat.py:149-163), and per-head input masks rule out the one stacked
+  projection per layer."""
+
+  def forward(self, node_feat, L, label=None, mask=None):
+    if self.training and self.dropout > 0.0:
+      raise NotImplementedError(
+          'TrainableGAT: dropout %g in training mode is not implemented (the reference drops the per-head '
+          'input, the attention weights and Wh); train with dropout 0.0' % self.dropout)
+    dev = self._device()
+    if self._check_mode():
+      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, mask)])
+    else:
+      score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
+    return self._finish(score, self._to(dev, label))
+
+  def _train_impl(self, node_feat, L, mask):
+    from ..train import gat_train
+    return gat_train(self, node_feat, L, mask)

@@ -15,7 +15,8 @@ __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
-    'gat_attention', 'gat_attention_supported', 'sage_operators', 'neighbour_max', 'ggnn_update',
+    'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
+    'sage_operators', 'neighbour_max', 'ggnn_update',
     'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
     'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'set2vec', 'set2vec_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
@@ -581,6 +582,43 @@ def gat_attention(Wh, bias, a1, a2, c1, c2, state_bias, last=False):
         _stream(Wh), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
         B, N, E1, heads, F, int(bool(last)), _ptr(out)), 'lnb_gat_attention')
   return out
+
+
+def gat_attention_backward_supported(N, F, E1, heads):
+  """Shapes lnb_gat_attention_backward accepts (mirrors its checks): the forward's envelope."""
+  return gat_attention_supported(N, F, E1, heads)
+
+
+def gat_attention_backward(gout, Wh, bias, a1, a2, c1, c2, state_bias, out=None, last=False):
+  """Adjoint of ``gat_attention`` (see lnb_gat_attention_backward); ``gout`` is the gradient of its
+  output.  The kernel recomputes the attention and h from the inputs; ``out`` (the forward's output) is
+  optional and only checked against the shapes.
+  Returns (gWh [B,N,C*F], ga1 [C,F], ga2 [C,F], gc1 [C], gc2 [C], gsb [C,F]); the per-graph partials
+  of the parameter gradients are summed over the batch here.  No gradient for the bias (data)."""
+  _need_cuda(gout, Wh, bias, a1, a2, c1, c2, state_bias, out)
+  Wh, bias, gout = _f32c(Wh), _f32c(bias), _f32c(gout)
+  a1, a2, c1, c2, state_bias = [_f32c(t) for t in (a1, a2, c1, c2, state_bias)]
+  B, N, _, E1 = bias.shape
+  C, F = a1.shape
+  heads = C // E1
+  shape = (B, N, F if last else C * F)
+  if (heads * E1 != C or tuple(Wh.shape) != (B, N, C * F) or tuple(state_bias.shape) != (C, F) or
+      tuple(gout.shape) != shape or (out is not None and tuple(out.shape) != shape)):
+    raise ValueError('gat_attention_backward: gout %s, Wh %s, bias %s, a1 %s, state_bias %s, out %s do not agree'
+                     % (tuple(gout.shape), tuple(Wh.shape), tuple(bias.shape), tuple(a1.shape),
+                        tuple(state_bias.shape), None if out is None else tuple(out.shape)))
+  gWh = torch.empty((B, N, C * F), device=Wh.device, dtype=torch.float32)
+  if B == 0:                                                # zero parameter gradients, nothing launched
+    z = torch.zeros((C, F), device=Wh.device, dtype=torch.float32)
+    return gWh, z, z.clone(), z[:, 0].clone(), z[:, 0].clone(), z.clone()
+  gpar = torch.empty((B, C, 3 * F + 2), device=Wh.device, dtype=torch.float32)
+  with torch.cuda.device(Wh.device):
+    _lib.check(_lib.load().lnb_gat_attention_backward(
+        _stream(Wh), _ptr(gout), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
+        B, N, E1, heads, F, int(bool(last)), _ptr(gWh), _ptr(gpar)), 'lnb_gat_attention_backward')
+  g = gpar.sum(dim=0)
+  return (gWh, g[:, :F].contiguous(), g[:, F:2 * F].contiguous(), g[:, 3 * F].contiguous(),
+          g[:, 3 * F + 1].contiguous(), g[:, 2 * F:3 * F].contiguous())
 
 
 def ggnn_update_supported(N, D, E1):

@@ -28,7 +28,8 @@ from . import ops
 
 __all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
            'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
-           'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'GraphedStep']
+           'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'gat_attention',
+           'gat_train', 'GraphedStep']
 
 
 def _pad_cols(x, mult=4):
@@ -552,6 +553,59 @@ def mpnn_train(model, node_ids, L, mask):
     if model.training and model.dropout > 0.0:
       h = torch.nn.functional.dropout(h, model.dropout, True)
   return set2vec_train(model, h.reshape(B, N, D), mask)
+
+
+class _GatAttention(torch.autograd.Function):
+  """One GAT layer after the projection (lnb_gat_attention) and its adjoint (lnb_gat_attention_backward).
+  Only the inputs are saved: the backward recomputes the attention weights ([B, C, N, N], 10 MB per layer
+  at B = 64) and h (ELU'(h) = exp(h) for h <= 0; out + 1 loses it where ELU(h) rounds towards -1)."""
+
+  @staticmethod
+  def forward(ctx, Wh, bias, a1, a2, c1, c2, sb, last):
+    Wh = Wh.contiguous()
+    out = ops.gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=last)
+    ctx.save_for_backward(Wh, bias, a1, a2, c1, c2, sb)
+    ctx.last = last
+    return out
+
+  @staticmethod
+  def backward(ctx, gout):
+    Wh, bias, a1, a2, c1, c2, sb = ctx.saved_tensors
+    gWh, ga1, ga2, gc1, gc2, gsb = ops.gat_attention_backward(gout.contiguous(), Wh, bias, a1, a2, c1, c2, sb,
+                                                              last=ctx.last)
+    return gWh, None, ga1, ga2, gc1, gc2, gsb, None
+
+
+def gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=False):
+  """Differentiable ``ops.gat_attention`` in Wh, a1, a2, c1, c2 and sb; ``bias`` is data."""
+  return _GatAttention.apply(Wh.float(), bias.float().contiguous(), a1.float().contiguous(),
+                             a2.float().contiguous(), c1.float().contiguous(), c2.float().contiguous(),
+                             sb.float().contiguous(), bool(last))
+
+
+def gat_train(model, node_ids, bias, mask):
+  """Differentiable GAT (model/gat.py:125-201) without dropout: embedding -> per layer the head weights
+  of all (E+1) * heads channels stacked in concat order c = jj * heads + ii on the tape, ONE ``dense``
+  projection, a1 / a2 / c1 / c2 stacked likewise, ``gat_attention`` -> gated readout with the head
+  ``output_func``.  Every channel reads ``bias_{ii}_{E}_{t}`` (the reference's shared state_bias list),
+  so that parameter's gradient sums over all E+1 channels and the other ``bias_{ii}_{jj}_{t}`` get
+  none (``grad`` stays None, as in the reference).  ``bias`` is the collate's attention bias
+  [B,N,N,E+1] (data.gat_bias)."""
+  bias = bias.float().contiguous()
+  state = embedding(node_ids, model.embedding.weight)
+  B, N = state.shape[0], state.shape[1]
+  E = model.num_edgetype
+  for t in range(model.num_layer):
+    mods = [(jj, ii) for jj in range(E + 1) for ii in range(model.num_heads[t])]
+    w = torch.cat([model.filter[t][jj][ii].weight for jj, ii in mods], dim=0)          # [C*F, Din]
+    Wh = dense(state.reshape(B * N, -1), w, None, False).reshape(B, N, -1)
+    a1 = torch.cat([model.att_net_1[t][jj][ii].weight for jj, ii in mods], dim=0)       # [C, F]
+    a2 = torch.cat([model.att_net_2[t][jj][ii].weight for jj, ii in mods], dim=0)
+    c1 = torch.cat([model.att_net_1[t][jj][ii].bias for jj, ii in mods], dim=0)         # [C]
+    c2 = torch.cat([model.att_net_2[t][jj][ii].bias for jj, ii in mods], dim=0)
+    sb = torch.stack([getattr(model, 'bias_%d_%d_%d' % (ii, E, t)) for _, ii in mods], dim=0)
+    state = gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=(t == model.num_layer - 1))
+  return gated_readout(model, state, mask, head=model.output_func[0])
 
 
 class _BMM(torch.autograd.Function):
