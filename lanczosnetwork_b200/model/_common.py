@@ -45,18 +45,56 @@ def _opt(obj, name, default):
   return getattr(obj, name) if hasattr(obj, name) else default
 
 
+def loss_function(name):
+  """The loss module of the config's ``model.loss`` (model/lanczos_net.py:64-71 and the other models)."""
+  if name == 'CrossEntropy':
+    return torch.nn.CrossEntropyLoss()
+  elif name == 'MSE':
+    return torch.nn.MSELoss()
+  elif name == 'L1':
+    return torch.nn.L1Loss()
+  raise ValueError("Non-supported loss function!")
+
+
+def init_linears(modules):
+  """Xavier-uniform weights and zero biases of the nn.Linear among ``modules``, in the order given (the
+  reference's order, so a seed gives its initial weights); other modules are skipped."""
+  for mod in modules:
+    if isinstance(mod, nn.Linear):
+      nn.init.xavier_uniform_(mod.weight.data)
+      if mod.bias is not None:
+        mod.bias.data.zero_()
+
+
+def init_cell(cell):
+  """The reference's GRU / RNN cell initialisation: Xavier on weight_hh, then weight_ih, zero biases."""
+  nn.init.xavier_uniform_(cell.weight_hh.data)
+  nn.init.xavier_uniform_(cell.weight_ih.data)
+  if cell.bias:
+    cell.bias_hh.data.zero_()
+    cell.bias_ih.data.zero_()
+
+
 class SpectralNetBase(nn.Module):
   """Common constructor pieces; subclasses define the embedding and the long-scale operator."""
 
-  def _setup_common(self, config, num_edgetype, filter_mlp_in, filter_mlp_hidden):
+  def _setup_fields(self, config, num_edgetype):
+    """The config fields every drop-in keeps; ``num_atom`` where the dataset has atom types."""
     m = config.model
     self.config = config
     self.input_dim = m.input_dim
     self.hidden_dim = m.hidden_dim
     self.output_dim = m.output_dim
     self.num_layer = m.num_layer
-    self.num_edgetype = num_edgetype
     self.dropout = _opt(m, 'dropout', 0.0)
+    if hasattr(config.dataset, 'num_atom'):
+      self.num_atom = config.dataset.num_atom
+    self.num_edgetype = num_edgetype
+    self._wcache = WeightCache()
+
+  def _setup_common(self, config, num_edgetype, filter_mlp_in, filter_mlp_hidden):
+    self._setup_fields(config, num_edgetype)
+    m = config.model
     self.short_diffusion_dist = check_dist(m.short_diffusion_dist)
     self.long_diffusion_dist = check_dist(m.long_diffusion_dist)
     self.max_short_diffusion_dist = max(self.short_diffusion_dist) if self.short_diffusion_dist else None
@@ -66,7 +104,6 @@ class SpectralNetBase(nn.Module):
     self.num_eig_vec = m.num_eig_vec
     self.spectral_filter_kind = m.spectral_filter_kind
     self._filter_mlp_dims = (filter_mlp_in, filter_mlp_hidden)
-    self._wcache = WeightCache()
 
   def _build_layers(self):
     C = self.num_scale_short + self.num_scale_long + self.num_edgetype + 1
@@ -87,15 +124,7 @@ class SpectralNetBase(nn.Module):
 
   def _build_head(self, dims):
     self.att_func = nn.Sequential(nn.Linear(dims[-2], 1), nn.Sigmoid())
-    loss = self.config.model.loss
-    if loss == 'CrossEntropy':
-      self.loss_func = torch.nn.CrossEntropyLoss()
-    elif loss == 'MSE':
-      self.loss_func = torch.nn.MSELoss()
-    elif loss == 'L1':
-      self.loss_func = torch.nn.L1Loss()
-    else:
-      raise ValueError("Non-supported loss function!")
+    self.loss_func = loss_function(self.config.model.loss)
 
   def _init_param(self):
     """Xavier-uniform weights, zero biases for filter / att_func / spectral_filter Linears
@@ -103,12 +132,17 @@ class SpectralNetBase(nn.Module):
     groups = [self.filter, self.att_func]
     if hasattr(self, 'spectral_filter'):
       groups += list(self.spectral_filter)
-    for grp in groups:
-      for mod in grp:
-        if isinstance(mod, nn.Linear):
-          nn.init.xavier_uniform_(mod.weight.data)
-          if mod.bias is not None:
-            mod.bias.data.zero_()
+    init_linears([mod for grp in groups for mod in grp])
+
+  def _forward(self, inputs, label):
+    """The forward of every drop-in: the training path under autograd (``_check_mode``), otherwise the
+    fused inference path ``_forward_impl`` through the CUDA-graph cache; then the loss when labelled."""
+    dev = self._device()
+    if self._check_mode():
+      score = self._train_impl(*[self._to(dev, t) for t in inputs])
+    else:
+      score = self._graph_forward(self._forward_impl, inputs)
+    return self._finish(score, self._to(dev, label))
 
   # ------------------------------------------------------------------------------------------
   def _param_device(self):

@@ -22,7 +22,6 @@ class AdaLanczosNet(SpectralNetBase):
 
   def __init__(self, config):
     super(AdaLanczosNet, self).__init__()
-    self.num_atom = config.dataset.num_atom
     K = config.model.num_eig_vec
     S = len(config.model.long_diffusion_dist)
     self._setup_common(config, config.dataset.num_bond_type, K * K * S, 4096)

@@ -10,8 +10,8 @@ wgmma dense layer; the whole forward is one CUDA-graph replay."""
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
-from ..spectral_conv import WeightCache, dense
+from ._common import SpectralNetBase
+from ..spectral_conv import dense
 from .. import ops
 
 __all__ = ['ChebyNet']
@@ -21,21 +21,12 @@ class ChebyNet(SpectralNetBase):
 
   def __init__(self, config):
     super(ChebyNet, self).__init__()
-    m = config.model
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
-    self.polynomial_order = m.polynomial_order
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
-    self.dropout = _opt(m, 'dropout', 0.0)
+    self._setup_fields(config, config.dataset.num_bond_type)
+    self.polynomial_order = config.model.polynomial_order
     self.short_diffusion_dist, self.long_diffusion_dist = [], []
     self.num_scale_short = self.num_scale_long = 0
     self.num_eig_vec = 0
     self.spectral_filter_kind = None
-    self._wcache = WeightCache()
     dims = [self.input_dim] + list(self.hidden_dim) + [self.output_dim]
     C = self.polynomial_order + self.num_edgetype + 1
     self.filter = nn.ModuleList(
@@ -50,12 +41,7 @@ class ChebyNet(SpectralNetBase):
       node_feat: long B x N (atom ids); L: float B x N x N x (E+1) (channel 0: the rescaled
       simple-graph operator); label: B x P; mask: B x N.  Returns score or (score, loss).
     """
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, mask), label)
 
   def _train_impl(self, node_feat, L, mask):
     from ..train import cheby_train

@@ -12,9 +12,9 @@ forward is one CUDA-graph replay."""
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
+from ._common import SpectralNetBase
 from ..data import check_dist
-from ..spectral_conv import WeightCache, dense, graph_conv_layer_unfused
+from ..spectral_conv import dense, graph_conv_layer_unfused
 from .. import ops
 
 __all__ = ['DCNN']
@@ -25,41 +25,27 @@ class DCNN(SpectralNetBase):
   def __init__(self, config):
     super(DCNN, self).__init__()
     m = config.model
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
+    self._setup_fields(config, config.dataset.num_bond_type)
     self.diffusion_dist = m.diffusion_dist
     self.num_scale = len(self.diffusion_dist)
     self.max_dist = max(self.diffusion_dist)
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
-    self.dropout = _opt(m, 'dropout', 0.0)
     # in the vocabulary of the shared layer: short scales = diffusion_dist, no long scales
     self.short_diffusion_dist = check_dist(list(self.diffusion_dist))
     self.long_diffusion_dist = []
     self.num_scale_short, self.num_scale_long = self.num_scale, 0
     self.num_eig_vec = 0
     self.spectral_filter_kind = None
-    self._wcache = WeightCache()
     dims = self._build_layers()          # Linear(dims[t] * (num_scale + E + 1), dims[t+1])
     self.embedding = nn.Embedding(self.num_atom, self.input_dim)
     self._build_head(dims)
     self._init_param()
-    self._perm = {}
 
   def forward(self, node_feat, L, label=None, mask=None):
     """
       node_feat: long B x N (atom ids); L: float B x N x N x (E+1); label: B x P;
       mask: B x N (uint8 / bool / float).  Returns score (B x P) or (score, loss).
     """
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, mask), label)
 
   def _train_impl(self, node_feat, L, mask):
     from ..train import dcnn_train
@@ -69,13 +55,10 @@ class DCNN(SpectralNetBase):
     """The reference concatenates edge types first and diffusion scales last (dcnn.py:98); the
     shared layer orders scales first: permute the weight columns once per parameter version."""
     w = self.filter[t].weight
-    key = (w.data_ptr(), w._version)
-    hit = self._perm.get(t)
-    if hit is None or hit[0] != key:
-      split = (self.num_edgetype + 1) * (w.shape[1] // (self.num_scale + self.num_edgetype + 1))
-      hit = (key, torch.cat([w.detach()[:, split:], w.detach()[:, :split]], dim=1).contiguous())
-      self._perm[t] = hit
-    return hit[1]
+    split = (self.num_edgetype + 1) * (w.shape[1] // (self.num_scale + self.num_edgetype + 1))
+    return self._wcache.derived(
+        'filter.%d.scales_first' % t, [w],
+        lambda: (torch.cat([w.detach()[:, split:], w.detach()[:, :split]], dim=1).contiguous(),))[0]
 
   def _forward_impl(self, node_feat, L, mask):
     L = L.float().contiguous()

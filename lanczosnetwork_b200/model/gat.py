@@ -22,8 +22,7 @@ checkpoints) adds one: under autograd its forward is ``train.gat_train``, whose 
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
-from ..spectral_conv import WeightCache
+from ._common import SpectralNetBase, init_linears, loss_function
 from .. import ops
 
 __all__ = ['GAT', 'TrainableGAT']
@@ -40,16 +39,8 @@ class GAT(SpectralNetBase):
   def __init__(self, config):
     super(GAT, self).__init__()
     m = config.model
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
+    self._setup_fields(config, config.dataset.num_bond_type)
     self.num_heads = m.num_heads
-    self.dropout = _opt(m, 'dropout', 0.0)
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
-    self._wcache = WeightCache()
     E1 = self.num_edgetype + 1
     dims = [self.input_dim] + list(self.hidden_dim) + [self.output_dim]
 
@@ -73,15 +64,7 @@ class GAT(SpectralNetBase):
           self.register_parameter('bias_%d_%d_%d' % (ii, jj, t), shared[ii])
     self.att_func = nn.Sequential(nn.Linear(dims[-2], 1), nn.Sigmoid())
     self.output_func = nn.Sequential(nn.Linear(dims[-2], dims[-1]))
-    loss = m.loss
-    if loss == 'CrossEntropy':
-      self.loss_func = torch.nn.CrossEntropyLoss()
-    elif loss == 'MSE':
-      self.loss_func = torch.nn.MSELoss()
-    elif loss == 'L1':
-      self.loss_func = torch.nn.L1Loss()
-    else:
-      raise ValueError("Non-supported loss function!")
+    self.loss_func = loss_function(m.loss)
     self._init_param()
 
   def _init_param(self):
@@ -90,11 +73,7 @@ class GAT(SpectralNetBase):
     linears = list(self.att_func) + list(self.output_func)
     for grid in (self.filter, self.att_net_1, self.att_net_2):
       linears += [mod for per_layer in grid for per_channel in per_layer for mod in per_channel]
-    for mod in linears:
-      if isinstance(mod, nn.Linear):
-        nn.init.xavier_uniform_(mod.weight.data)
-        if mod.bias is not None:
-          mod.bias.data.zero_()
+    init_linears(linears)
 
   def _param_device(self):
     return self.embedding.weight.device
@@ -105,10 +84,7 @@ class GAT(SpectralNetBase):
       collate (data.gat_bias); label: B x P; mask: B x N (uint8 / bool / float).
       Returns score (B x P) or (score, loss).
     """
-    dev = self._device()
-    self._check_mode()                    # no training path: raises under autograd
-    score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, mask), label)          # no training path: raises under autograd
 
   def _layer_params(self, t):
     """Per-layer tensors in concat order c = jj * heads + ii, stacked once per parameter version."""
@@ -159,12 +135,7 @@ class TrainableGAT(GAT):
       raise NotImplementedError(
           'TrainableGAT: dropout %g in training mode is not implemented (the reference drops the per-head '
           'input, the attention weights and Wh); train with dropout 0.0' % self.dropout)
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, mask), label)
 
   def _train_impl(self, node_feat, L, mask):
     from ..train import gat_train

@@ -6,8 +6,7 @@ fused convolution-stack kernel with no long scales (embedding gather + all layer
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
-from ..spectral_conv import WeightCache
+from ._common import SpectralNetBase
 
 __all__ = ['GCN', 'GCNFP']
 
@@ -16,21 +15,12 @@ class GCN(SpectralNetBase):
 
   def __init__(self, config):
     super(GCN, self).__init__()
-    m = config.model
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
-    self.dropout = _opt(m, 'dropout', 0.0)
+    self._setup_fields(config, config.dataset.num_bond_type)
     # no diffusion scales: the message is the E+1 edge-type products only
     self.short_diffusion_dist, self.long_diffusion_dist = [], []
     self.num_scale_short = self.num_scale_long = 0
     self.num_eig_vec = 0
     self.spectral_filter_kind = None
-    self._wcache = WeightCache()
     dims = self._build_layers()
     self.embedding = nn.Embedding(self.num_atom, self.input_dim)
     self._build_head(dims)
@@ -41,12 +31,7 @@ class GCN(SpectralNetBase):
       node_feat: long B x N (atom ids); L: float B x N x N x (E+1); label: B x P;
       mask: B x N (uint8 / bool / float).  Returns score (B x P) or (score, loss).
     """
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, mask), label)
 
   def _train_impl(self, node_feat, L, mask):
     from ..train import ritz_stack_train

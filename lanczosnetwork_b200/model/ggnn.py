@@ -23,17 +23,14 @@ Differences from the reference, on purpose:
     (W_i x + b_i) + (W_h h + b_h): the same sum in another order.
 ``update_func: RNN`` (relu RNNCell), shapes outside ``lnb_ggnn_update`` and ``input_dim % 4 != 0`` run the
 training formulation of lanczosnetwork_b200.train under no_grad."""
-import numpy as np
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
-from ..spectral_conv import WeightCache
+from ._common import SpectralNetBase, init_cell, init_linears, loss_function
 from .. import ops
 
 __all__ = ['GGNN']
 
-EPS = float(np.finfo(np.float32).eps)          # model/ggnn.py:6
 MSG_HIDDEN = 128                               # width of the message MLPs, fixed in the reference (:59-61)
 
 
@@ -76,6 +73,15 @@ def cached_gates(cache, name, cell):
   return cache.derived(name, [cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh], build)
 
 
+def embed_input(model, node_feat, table):
+  """h = input_func(table[node_feat]) [B*N, D] of GGNN / GPNN / MPNN: the embedding gather and one dense
+  launch."""
+  lin = model.input_func[0]
+  w_hi, w_lo = model._wcache.split('input_func.0', lin.weight)
+  x = ops.embedding_rows(node_feat.long().reshape(-1), table)
+  return ops.linear_tf32x3(x, w_hi, w_lo, lin.bias)
+
+
 def ggnn_step(h, prep, params, avg, out):
   """One GGNN propagation step in three launches (the E1 first message layers stacked, the grouped
   second layers, lnb_ggnn_update); ``params`` from ggnn_step_params, ``prep`` the binarised ELL rows.
@@ -92,20 +98,12 @@ class GGNN(SpectralNetBase):
   def __init__(self, config):
     super(GGNN, self).__init__()
     m = config.model
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
+    self._setup_fields(config, config.dataset.num_bond_type)
     self.num_prop = m.num_prop
-    self.dropout = _opt(m, 'dropout', 0.0)
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
     self.aggregate_type = m.aggregate_type
     self.update_func_name = m.update_func
     assert self.num_layer == 1, "not implemented"
     assert self.aggregate_type in ['avg', 'sum'], 'not implemented'
-    self._wcache = WeightCache()
     E1, D = self.num_edgetype + 1, self.hidden_dim
 
     self.embedding = nn.Embedding(self.num_atom, self.input_dim)
@@ -123,15 +121,7 @@ class GGNN(SpectralNetBase):
     self.att_func = nn.Sequential(nn.Linear(D, 1), nn.Sigmoid())
     self.input_func = nn.Sequential(nn.Linear(self.input_dim, D))
     self.output_func = nn.Sequential(nn.Linear(D, self.output_dim))
-    loss = m.loss
-    if loss == 'CrossEntropy':
-      self.loss_func = torch.nn.CrossEntropyLoss()
-    elif loss == 'MSE':
-      self.loss_func = torch.nn.MSELoss()
-    elif loss == 'L1':
-      self.loss_func = torch.nn.L1Loss()
-    else:
-      raise ValueError("Non-supported loss function!")
+    self.loss_func = loss_function(m.loss)
     self._init_param()
 
   def _init_param(self):
@@ -139,25 +129,11 @@ class GGNN(SpectralNetBase):
     output_func (msg_func is a ModuleList, neither Sequential nor Linear, so it keeps PyTorch's default
     initialisation); then Xavier on weight_hh, weight_ih and zero biases of the GRU / RNN cell, or
     Xavier on the Linear of the MLP update."""
-    for seq in (self.input_func, self.att_func, self.output_func):
-      for mod in seq:
-        if isinstance(mod, nn.Linear):
-          nn.init.xavier_uniform_(mod.weight.data)
-          if mod.bias is not None:
-            mod.bias.data.zero_()
+    init_linears([*self.input_func, *self.att_func, *self.output_func])
     if self.update_func_name in ('GRU', 'RNN'):
-      cell = self.update_func
-      nn.init.xavier_uniform_(cell.weight_hh.data)
-      nn.init.xavier_uniform_(cell.weight_ih.data)
-      if cell.bias:
-        cell.bias_hh.data.zero_()
-        cell.bias_ih.data.zero_()
+      init_cell(self.update_func)
     elif self.update_func_name == 'MLP':
-      for mod in self.update_func:
-        if isinstance(mod, nn.Linear):
-          nn.init.xavier_uniform_(mod.weight.data)
-          if mod.bias is not None:
-            mod.bias.data.zero_()
+      init_linears(self.update_func)
 
   def _param_device(self):
     return self.embedding.weight.device
@@ -174,12 +150,7 @@ class GGNN(SpectralNetBase):
     if self.msg_func is None:
       raise UnboundLocalError("msg_func %r: the reference's propagation reads a message that is never "
                               "assigned (model/ggnn.py:147-154); only 'MLP' runs" % self.config.model.msg_func)
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, mask), label)
 
   def _train_impl(self, node_feat, L, mask):
     from ..train import ggnn_train
@@ -199,15 +170,10 @@ class GGNN(SpectralNetBase):
     B, N = node_feat.shape
     E1 = L.shape[3]
     if not self.fused_supported(N, E1):
-      from ..train import ggnn_train              # RNN update / other shapes: the training formulation
-      return ggnn_train(self, node_feat, L, mask)
+      return self._train_impl(node_feat, L, mask)        # RNN update / other shapes: the training formulation
     D = self.hidden_dim
-    lin = self.input_func[0]
-    w_hi, w_lo = self._wcache.split('input_func.0', lin.weight)
-    x = ops.embedding_rows(node_feat.long().reshape(-1), self.embedding.weight)
-    h = ops.linear_tf32x3(x, w_hi, w_lo, lin.bias)
-    # ELL rows of the 0/1 operators; no Ritz vectors (an all-zero block)
-    prep = ops.graph_prepare(L, torch.zeros((B, N, 4), device=L.device, dtype=torch.float32), binarize=True)
+    h = embed_input(self, node_feat, self.embedding.weight)
+    prep = ops.graph_prepare(L, binarize=True)            # ELL rows of the 0/1 operators
     params = self._step_params()
     spare = torch.empty_like(h)
     avg = self.aggregate_type == 'avg'

@@ -28,18 +28,15 @@ Differences from the reference, on purpose:
   * the GRU gate pre-activations are one dot product over [messages | h] plus b_ih + b_hh.
 ``update_func: RNN`` (relu RNNCell), shapes outside the kernels and ``input_dim % 4 != 0`` run the
 training formulation of lanczosnetwork_b200.train under no_grad."""
-import numpy as np
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
-from .ggnn import MSG_HIDDEN, cached_gates, ggnn_step, ggnn_step_params
-from ..spectral_conv import WeightCache
+from ._common import SpectralNetBase, init_cell, init_linears, loss_function
+from .ggnn import MSG_HIDDEN, cached_gates, embed_input, ggnn_step, ggnn_step_params
 from .. import ops
 
 __all__ = ['GPNN']
 
-EPS = float(np.finfo(np.float32).eps)          # model/gpnn.py:7
 STATE_HIDDEN = 512                             # width of state_func, fixed in the reference (:68-72)
 
 
@@ -48,23 +45,15 @@ class GPNN(SpectralNetBase):
   def __init__(self, config):
     super(GPNN, self).__init__()
     m = config.model
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
+    self._setup_fields(config, config.dataset.num_bond_type)
     self.num_prop = m.num_prop
     self.num_partition = m.num_partition
     self.num_prop_cluster = m.num_prop_cluster
     self.num_prop_cut = m.num_prop_cut
-    self.dropout = _opt(m, 'dropout', 0.0)
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
     self.aggregate_type = m.aggregate_type
     self.update_func_name = m.update_func
     assert self.num_layer == 1, "not implemented"
     assert self.aggregate_type in ['avg', 'sum'], 'not implemented'
-    self._wcache = WeightCache()
     E1, D = self.num_edgetype + 1, self.hidden_dim
 
     self.embedding = nn.Embedding(self.num_atom, self.input_dim)
@@ -86,15 +75,7 @@ class GPNN(SpectralNetBase):
     self.att_func = nn.Sequential(nn.Linear(D, 1), nn.Sigmoid())
     self.input_func = nn.Sequential(nn.Linear(self.input_dim, D))
     self.output_func = nn.Sequential(nn.Linear(D, self.output_dim))
-    loss = m.loss
-    if loss == 'CrossEntropy':
-      self.loss_func = torch.nn.CrossEntropyLoss()
-    elif loss == 'MSE':
-      self.loss_func = torch.nn.MSELoss()
-    elif loss == 'L1':
-      self.loss_func = torch.nn.L1Loss()
-    else:
-      raise ValueError("Non-supported loss function!")
+    self.loss_func = loss_function(m.loss)
     self._init_param()
 
   def _init_param(self):
@@ -103,19 +84,10 @@ class GPNN(SpectralNetBase):
     default initialisation); then, per cell (update_func, update_func_partition), Xavier on weight_hh,
     weight_ih and zero biases (``if m.bias:`` is true).  The MLP update keeps PyTorch's default: the
     reference only re-initialises it when it is a Linear, and it is a Sequential."""
-    for seq in (self.input_func, self.state_func, self.att_func, self.output_func):
-      for mod in seq:
-        if isinstance(mod, nn.Linear):
-          nn.init.xavier_uniform_(mod.weight.data)
-          if mod.bias is not None:
-            mod.bias.data.zero_()
+    init_linears([*self.input_func, *self.state_func, *self.att_func, *self.output_func])
     if self.update_func_name in ('GRU', 'RNN'):
-      for cell in (self.update_func, self.update_func_partition):
-        nn.init.xavier_uniform_(cell.weight_hh.data)
-        nn.init.xavier_uniform_(cell.weight_ih.data)
-        if cell.bias:
-          cell.bias_hh.data.zero_()
-          cell.bias_ih.data.zero_()
+      init_cell(self.update_func)
+      init_cell(self.update_func_partition)
 
   def _param_device(self):
     return self.embedding.weight.device
@@ -133,13 +105,7 @@ class GPNN(SpectralNetBase):
     if self.msg_func is None:
       raise UnboundLocalError("msg_func %r: the reference's propagation reads a message that is never "
                               "assigned (model/gpnn.py:193-200); only 'MLP' runs" % self.config.model.msg_func)
-    dev = self._device()
-    inputs = (node_feat, L, L_cluster, L_cut, mask)
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in inputs])
-    else:
-      score = self._graph_forward(self._forward_impl, inputs)
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, L_cluster, L_cut, mask), label)
 
   def _train_impl(self, node_feat, L, L_cluster, L_cut, mask):
     from ..train import gpnn_train
@@ -201,14 +167,11 @@ class GPNN(SpectralNetBase):
     B, N = node_feat.shape
     E1 = L.shape[3]
     if not self.fused_supported(N, E1):
-      from ..train import gpnn_train              # RNN update / other shapes: the training formulation
-      return gpnn_train(self, node_feat, L, L_cluster, L_cut, mask)
+      return self._train_impl(node_feat, L, L_cluster, L_cut, mask)   # RNN update / other shapes
     H = self.hidden_dim
-    lin = self.input_func[0]
-    w_hi, w_lo = self._wcache.split('input_func.0', lin.weight)
-    x = ops.embedding_rows(node_feat.long().reshape(-1), self.embedding.weight)
-    h = ops.linear_tf32x3(x, w_hi, w_lo, lin.bias)
-    # ELL rows of the 0/1 operators and of the valued partition operators; no Ritz vectors
+    h = embed_input(self, node_feat, self.embedding.weight)
+    # ELL rows of the 0/1 operators and of the valued partition operators; no Ritz vectors, one zero
+    # block for both
     zeros = torch.zeros((B, N, 4), device=L.device, dtype=torch.float32)
     prep = ops.graph_prepare(L, zeros, binarize=True)
     pprep = ops.graph_prepare(torch.stack([L_cluster, L_cut], 3), zeros)

@@ -24,8 +24,7 @@ contribute nothing (the reference raises an IndexError)."""
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
-from ..spectral_conv import WeightCache
+from ._common import SpectralNetBase, init_linears, loss_function
 from .. import ops
 
 __all__ = ['GraphSAGE']
@@ -42,18 +41,10 @@ class GraphSAGE(SpectralNetBase):
           "GraphSAGE drop-in: agg_func 'LSTM' is not implemented; supported aggregators: %s"
           % ', '.join(SUPPORTED_AGGREGATORS))
     super(GraphSAGE, self).__init__()
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
-    self.dropout = _opt(m, 'dropout', 0.0)
+    self._setup_fields(config, config.dataset.num_bond_type)
     self.num_sample_neighbors = m.num_sample_neighbors
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
     assert self.num_layer == len(self.hidden_dim)
     dims = [self.input_dim] + list(self.hidden_dim) + [self.output_dim]
-    self._wcache = WeightCache()
 
     self.embedding = nn.Embedding(self.num_atom, self.input_dim)
     self.agg_func_name = m.agg_func
@@ -62,25 +53,13 @@ class GraphSAGE(SpectralNetBase):
     self.filter = nn.ModuleList(
         [nn.Linear(dims[t] * (self.num_edgetype + 1), dims[t + 1]) for t in range(self.num_layer)] +
         [nn.Linear(dims[-2], dims[-1])])
-    loss = m.loss
-    if loss == 'CrossEntropy':
-      self.loss_func = torch.nn.CrossEntropyLoss()
-    elif loss == 'MSE':
-      self.loss_func = torch.nn.MSELoss()
-    elif loss == 'L1':
-      self.loss_func = torch.nn.L1Loss()
-    else:
-      raise ValueError("Non-supported loss function!")
+    self.loss_func = loss_function(m.loss)
     self._init_param()
 
   def _init_param(self):
     """Xavier-uniform weights and zero biases, att_func first, then filter (graph_sage.py:69-96); the
     embedding keeps nn.Embedding's default N(0, 1)."""
-    for mod in list(self.att_func) + list(self.filter):
-      if isinstance(mod, nn.Linear):
-        nn.init.xavier_uniform_(mod.weight.data)
-        if mod.bias is not None:
-          mod.bias.data.zero_()
+    init_linears([*self.att_func, *self.filter])
 
   def forward(self, node_feat, nn_idx, nonempty_mask, label=None, mask=None):
     """
@@ -88,15 +67,11 @@ class GraphSAGE(SpectralNetBase):
       nonempty_mask: float B x N x 1; label: B x P; mask: B x N (uint8 / bool / float).
       Returns score (B x P) or (score, loss).
     """
-    dev = self._device()
+    self._device()                        # a CPU module refuses before the aggregator is checked
     if self.agg_func is None:
       raise TypeError("GraphSAGE: unknown agg_func %r ('NoneType' object is not callable, as in the "
                       "reference); supported: %s" % (self.agg_func_name, ', '.join(SUPPORTED_AGGREGATORS)))
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, nn_idx, nonempty_mask, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, nn_idx, nonempty_mask, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, nn_idx, nonempty_mask, mask), label)
 
   def _train_impl(self, node_feat, nn_idx, nonempty_mask, mask):
     from ..train import sage_train

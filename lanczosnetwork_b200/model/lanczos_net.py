@@ -15,7 +15,6 @@ class LanczosNet(SpectralNetBase):
 
   def __init__(self, config):
     super(LanczosNet, self).__init__()
-    self.num_atom = config.dataset.num_atom
     self._setup_common(config, config.dataset.num_bond_type,
                        len(config.model.long_diffusion_dist), 128)
     dims = self._build_layers()
@@ -30,12 +29,7 @@ class LanczosNet(SpectralNetBase):
       V: Ritz vectors B x N x K; label: B x P; mask: B x N (uint8 / bool / float).
       Returns score (B x P) or (score, loss) when label is given.
     """
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, D, V, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, D, V, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, D, V, mask), label)
 
   def _train_impl(self, node_feat, L, D, V, mask):
     from ..train import ritz_stack_train

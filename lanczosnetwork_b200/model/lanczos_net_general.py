@@ -27,12 +27,7 @@ class LanczosNetGeneral(SpectralNetBase):
       node_feat: float B x N x D node features; L: B x N x N x (E+1); D: Ritz values B x K;
       V: Ritz vectors B x N x K; label: B x P; mask: B x N.
     """
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, D, V, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, D, V, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, D, V, mask), label)
 
   def _train_impl(self, node_feat, L, D, V, mask):
     from ..train import ritz_stack_train

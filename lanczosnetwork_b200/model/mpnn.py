@@ -25,18 +25,15 @@ Differences from the reference, on purpose:
     another order: the same function, fp32 rounding apart.
 Shapes outside the kernels' envelopes and ``input_dim % 4 != 0`` run the training formulation of
 lanczosnetwork_b200.train under no_grad."""
-import numpy as np
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, _opt
-from .ggnn import gru_gate_matrix
-from ..spectral_conv import WeightCache
+from ._common import SpectralNetBase, init_cell, init_linears, loss_function
+from .ggnn import cached_gates, embed_input, gru_gate_matrix
 from .. import ops
 
 __all__ = ['MPNN']
 
-EPS = float(np.finfo(np.float32).eps)          # model/mpnn.py:8
 EDGE_HIDDEN = ops.MPNN_EDGE_HIDDEN             # model/mpnn.py:60
 
 
@@ -78,21 +75,13 @@ class MPNN(SpectralNetBase):
   def __init__(self, config):
     super(MPNN, self).__init__()
     m = config.model
-    self.config = config
-    self.input_dim = m.input_dim
-    self.hidden_dim = m.hidden_dim
-    self.output_dim = m.output_dim
-    self.num_layer = m.num_layer
+    self._setup_fields(config, config.dataset.num_bond_type)
     self.num_prop = m.num_prop
     self.msg_func_name = m.msg_func
     self.num_step_set2vec = m.num_step_set2vec
-    self.dropout = _opt(m, 'dropout', 0.0)
-    self.num_atom = config.dataset.num_atom
-    self.num_edgetype = config.dataset.num_bond_type
     self.aggregate_type = m.aggregate_type
     assert self.num_layer == 1, 'not implemented'
     assert self.aggregate_type in ['avg', 'sum'], 'not implemented'
-    self._wcache = WeightCache()
     E1, D = self.num_edgetype + 1, self.hidden_dim
 
     self.node_embedding = nn.Embedding(self.num_atom, self.input_dim)
@@ -107,15 +96,7 @@ class MPNN(SpectralNetBase):
       raise ValueError('Non-supported message function')
     self.att_func = Set2Vec(D, self.num_step_set2vec)
     self.output_func = nn.Sequential(nn.Linear(2 * D, self.output_dim))
-    loss = m.loss
-    if loss == 'CrossEntropy':
-      self.loss_func = torch.nn.CrossEntropyLoss()
-    elif loss == 'MSE':
-      self.loss_func = torch.nn.MSELoss()
-    elif loss == 'L1':
-      self.loss_func = torch.nn.L1Loss()
-    else:
-      raise ValueError("Non-supported loss function!")
+    self.loss_func = loss_function(m.loss)
     self._init_param()
 
   def _init_param(self):
@@ -123,18 +104,8 @@ class MPNN(SpectralNetBase):
     (att_func is a Set2Vec, neither Sequential nor Linear: it keeps the initialisation of its own
     constructor; the edge network keeps PyTorch's default), then Xavier on weight_hh, weight_ih and zero
     biases of the GRU."""
-    for seq in (self.input_func, self.output_func):
-      for mod in seq:
-        if isinstance(mod, nn.Linear):
-          nn.init.xavier_uniform_(mod.weight.data)
-          if mod.bias is not None:
-            mod.bias.data.zero_()
-    cell = self.update_func
-    nn.init.xavier_uniform_(cell.weight_hh.data)
-    nn.init.xavier_uniform_(cell.weight_ih.data)
-    if cell.bias:
-      cell.bias_hh.data.zero_()
-      cell.bias_ih.data.zero_()
+    init_linears([*self.input_func, *self.output_func])
+    init_cell(self.update_func)
 
   def _param_device(self):
     return self.node_embedding.weight.device
@@ -145,12 +116,7 @@ class MPNN(SpectralNetBase):
       pattern is read; L is not modified); label: B x P; mask: B x N (uint8 / bool / float; the nodes
       of each graph's Set2Vec set).  Returns score (B x P) or (score, loss).
     """
-    dev = self._device()
-    if self._check_mode():
-      score = self._train_impl(*[self._to(dev, t) for t in (node_feat, L, mask)])
-    else:
-      score = self._graph_forward(self._forward_impl, (node_feat, L, mask))
-    return self._finish(score, self._to(dev, label))
+    return self._forward((node_feat, L, mask), label)
 
   def _train_impl(self, node_feat, L, mask):
     from ..train import mpnn_train
@@ -172,16 +138,11 @@ class MPNN(SpectralNetBase):
     ``embedding`` the stacked E_e^T and the GRU gate matrix."""
     cache, cell = self._wcache, self.update_func
     E1, D = self.num_edgetype + 1, self.hidden_dim
-    gru = [cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh]
     if self.msg_func_name == 'embedding':
       emb = self.edge_embedding.weight
       e_hi, e_lo = cache.derived('edge_embedding.stacked', [emb], lambda: ops.split_tf32(
           emb.detach().view(E1, D, D).transpose(1, 2).reshape(E1 * D, D)))
-
-      def build_gru():
-        W, b = gru_gate_matrix(*[t.detach() for t in gru])
-        return ops.split_tf32(W) + (b,)
-      return (e_hi, e_lo, None), cache.derived('update_func.gates', gru, build_gru)
+      return (e_hi, e_lo, None), cached_gates(cache, 'update_func.gates', cell)
     first = [seq[0] for seq in self.edge_func]
     second = [seq[2] for seq in self.edge_func]
 
@@ -199,6 +160,7 @@ class MPNN(SpectralNetBase):
         F[:, EDGE_HIDDEN * E1 + e] = w_ih[:, e, :] @ l.bias.detach().double()
       W, b = gru_gate_matrix(F.float(), cell.weight_hh.detach(), cell.bias_ih.detach(), cell.bias_hh.detach())
       return ops.split_tf32(W) + (b,)
+    gru = [cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh]
     gates = cache.derived('update_func.mpnn_gates',
                           gru + [l.weight for l in second] + [l.bias for l in second], build_gates)
     return pq, gates
@@ -215,15 +177,10 @@ class MPNN(SpectralNetBase):
     B, N = node_feat.shape
     E1 = L.shape[3]
     if not self.fused_supported(N, E1):
-      from ..train import mpnn_train              # other shapes: the training formulation
-      return mpnn_train(self, node_feat, L, mask)
+      return self._train_impl(node_feat, L, mask)        # other shapes: the training formulation
     D = self.hidden_dim
-    lin = self.input_func[0]
-    w_hi, w_lo = self._wcache.split('input_func.0', lin.weight)
-    x = ops.embedding_rows(node_feat.long().reshape(-1), self.node_embedding.weight)
-    h = ops.linear_tf32x3(x, w_hi, w_lo, lin.bias)
-    # ELL rows of the 0/1 operators; no Ritz vectors (an all-zero block)
-    prep = ops.graph_prepare(L, torch.zeros((B, N, 4), device=L.device, dtype=torch.float32), binarize=True)
+    h = embed_input(self, node_feat, self.node_embedding.weight)
+    prep = ops.graph_prepare(L, binarize=True)            # ELL rows of the 0/1 operators
     (m_hi, m_lo, m_b), (g_hi, g_lo, g_b) = self._step_params()
     spare = torch.empty_like(h)
     avg = self.aggregate_type == 'avg'

@@ -186,10 +186,13 @@ class GraphPrep(tuple):
   nrows = None
 
 
-def graph_prepare(L, Q, binarize=False):
+def graph_prepare(L, Q=None, binarize=False):
   """Per-forward compression of the dense operators L [B,N,N,E1] (ELL rows), the real extents
   of every graph, the packed-tile assignment for the fused convolution kernel and the compact
-  list of non-zero Ritz rows.  Returns GraphPrep(ell_val, ell_idx, ell_max, gext, tiles)."""
+  list of non-zero Ritz rows.  ``Q=None``: no Ritz vectors, an all-zero [B,N,4] block, so the
+  extents come from L alone.  Returns GraphPrep(ell_val, ell_idx, ell_max, gext, tiles)."""
+  if Q is None:
+    Q = torch.zeros((L.shape[0], L.shape[1], 4), device=L.device, dtype=torch.float32)
   _need_cuda(L, Q)
   L, Q = _f32c(L), _f32c(Q)
   B, N, _, E1 = L.shape

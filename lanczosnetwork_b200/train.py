@@ -31,6 +31,8 @@ __all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz
            'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'gat_attention',
            'gat_train', 'GraphedStep']
 
+_EPS = 1.1920928955078125e-07       # np.finfo(np.float32).eps (ada_lanczos_net.py:8)
+
 
 def _pad_cols(x, mult=4):
   k = x.shape[1]
@@ -199,6 +201,58 @@ def embedding(ids, table):
   return _Embedding.apply(ids.long(), table)
 
 
+def _dropout(model, x):
+  """The reference's dropout after every layer / propagation step, on the tape in training mode."""
+  if model.training and model.dropout > 0.0:
+    x = torch.nn.functional.dropout(x, model.dropout, True)
+  return x
+
+
+def _short_walk(L, state, dist):
+  """[L_0^k X for k in dist, ascending k]: the walk over channel 0 (lanczos_net.py:164-169)."""
+  msgs, walk = [], state
+  for step in range(1, max(dist, default=0) + 1):
+    walk = operator_messages(L, walk, 0, 1)
+    if step in dist:
+      msgs.append(walk)
+  return msgs
+
+
+def _conv_layer(model, t, msgs):
+  """Graph-convolution layer t on its messages [B,N,*]: concatenated, Linear ``filter[t]`` + ReLU, dropout."""
+  B, N = msgs[0].shape[0], msgs[0].shape[1]
+  msg = torch.cat(msgs, dim=2) if len(msgs) > 1 else msgs[0]
+  lin = model.filter[t]
+  return _dropout(model, dense(msg.reshape(B * N, -1), lin.weight, lin.bias, True).reshape(B, N, -1))
+
+
+def _filter_mlp(seq, h):
+  """The four-layer spectral filter MLP ``seq`` (Linear, ReLU, ..., Linear) in the dense kernel."""
+  for i in (0, 2, 4, 6):
+    h = dense(h, seq[i].weight, seq[i].bias, i != 6)
+  return h
+
+
+def _input_state(model, node_ids, table):
+  """h = input_func(table[node_ids]) [B*N, D] of GGNN / GPNN / MPNN."""
+  x = embedding(node_ids, table)
+  lin = model.input_func[0]
+  return dense(x.reshape(-1, x.shape[-1]), lin.weight, lin.bias, False)
+
+
+def _row_normalised(A):
+  """A / (rowsum + float32 eps): the ``avg`` aggregation of GGNN, GPNN and MPNN."""
+  return A / (A.sum(dim=2, keepdim=True) + _EPS)
+
+
+def _channel_messages(A, msgs):
+  """[A_e m_e]_e as [B*N, E1*D] for the per-channel messages m_e [B*N, D] (an iterable, consumed in
+  channel order)."""
+  B, N = A.shape[0], A.shape[1]
+  agg = torch.cat([operator_messages(A, m.reshape(B, N, -1), e, 1) for e, m in enumerate(msgs)], dim=2)
+  return agg.reshape(B * N, -1)
+
+
 def ritz_stack_train(model, state, node_ids, L, D, V, mask):
   """Differentiable convolution stack + readout of LanczosNet / LanczosNetGeneral / GCN
   (model/lanczos_net.py:125-199): same math, same parameter tensors as the inference path."""
@@ -207,38 +261,23 @@ def ritz_stack_train(model, state, node_ids, L, D, V, mask):
     state = embedding(node_ids, model.embedding.weight)
   else:
     state = state.float().contiguous()
-  B, N = state.shape[0], state.shape[1]
+  B = state.shape[0]
   S = model.num_scale_long
-  short = list(model.short_diffusion_dist)
   table = None
   if S > 0:
     V = V.float().contiguous()
     table = ops.ritz_power_table(D.float().contiguous(), model.long_diffusion_dist)   # [B,K,S], data
     K = table.shape[1]
   for t in range(model.num_layer):
-    msgs = []
-    if short:                                   # walk <- L0 walk (lanczos_net.py:164-169)
-      walk = state
-      for step in range(1, max(short) + 1):
-        walk = operator_messages(L, walk, 0, 1)
-        if step in short:
-          msgs.append(walk)
+    msgs = _short_walk(L, state, model.short_diffusion_dist)
     if S > 0:
       if model.spectral_filter_kind == 'MLP':
-        seq = model.spectral_filter[t]
-        h = table.reshape(B * K, S)
-        for i in (0, 2, 4, 6):
-          h = dense(h, seq[i].weight, seq[i].bias, i != 6)
-        F = h.reshape(B, K, S)
+        F = _filter_mlp(model.spectral_filter[t], table.reshape(B * K, S)).reshape(B, K, S)
       else:
         F = table
       msgs.append(spectral_messages(V, state, F))
     msgs.append(operator_messages(L, state))
-    msg = torch.cat(msgs, dim=2) if len(msgs) > 1 else msgs[0]
-    lin = model.filter[t]
-    state = dense(msg.reshape(B * N, -1), lin.weight, lin.bias, True).reshape(B, N, -1)
-    if model.training and model.dropout > 0.0:
-      state = torch.nn.functional.dropout(state, model.dropout, True)
+    state = _conv_layer(model, t, msgs)
   return gated_readout(model, state, mask)
 
 
@@ -265,19 +304,9 @@ def dcnn_train(model, node_ids, L, mask):
   L_0^k X for k in diffusion_dist, concatenated EDGES FIRST (:98), Linear + ReLU."""
   L = L.float().contiguous()
   state = embedding(node_ids, model.embedding.weight)
-  B, N = state.shape[0], state.shape[1]
   dist = set(model.diffusion_dist)
   for t in range(model.num_layer):
-    msgs = [operator_messages(L, state)]
-    walk = state
-    for step in range(1, model.max_dist + 1):
-      walk = operator_messages(L, walk, 0, 1)
-      if step in dist:
-        msgs.append(walk)
-    lin = model.filter[t]
-    state = dense(torch.cat(msgs, dim=2).reshape(B * N, -1), lin.weight, lin.bias, True).reshape(B, N, -1)
-    if model.training and model.dropout > 0.0:
-      state = torch.nn.functional.dropout(state, model.dropout, True)
+    state = _conv_layer(model, t, [operator_messages(L, state)] + _short_walk(L, state, dist))
   return gated_readout(model, state, mask)
 
 
@@ -287,7 +316,7 @@ def cheby_train(model, node_ids, L, mask):
   cat(edges + [s_0 .. s_{order-1}] + [X]) (:99), Linear + ReLU."""
   L = L.float().contiguous()
   state = embedding(node_ids, model.embedding.weight)
-  B, N, E1 = state.shape[0], state.shape[1], L.shape[3]
+  E1 = L.shape[3]
   order = model.polynomial_order
   for t in range(model.num_layer):
     scale = [None] * (order + 1)
@@ -295,11 +324,7 @@ def cheby_train(model, node_ids, L, mask):
     scale[0] = operator_messages(L, state, 0, 1)
     for kk in range(1, order):
       scale[kk] = 2.0 * operator_messages(L, scale[kk - 1], 0, 1) - scale[kk - 2]
-    msgs = ([operator_messages(L, state, 1, E1 - 1)] if E1 > 1 else []) + scale
-    lin = model.filter[t]
-    state = dense(torch.cat(msgs, dim=2).reshape(B * N, -1), lin.weight, lin.bias, True).reshape(B, N, -1)
-    if model.training and model.dropout > 0.0:
-      state = torch.nn.functional.dropout(state, model.dropout, True)
+    state = _conv_layer(model, t, ([operator_messages(L, state, 1, E1 - 1)] if E1 > 1 else []) + scale)
   return gated_readout(model, state, mask)
 
 
@@ -342,15 +367,13 @@ def sage_train(model, node_ids, M, mask, prep=None):
   state = embedding(node_ids, model.embedding.weight)
   B, N = state.shape[0], state.shape[1]
   if model.agg_func_name == 'Max' and prep is None and model.num_layer > 1:
-    prep = ops.graph_prepare(M, torch.zeros((B, N, 4), device=M.device, dtype=torch.float32))
+    prep = ops.graph_prepare(M)
   for t in range(model.num_layer - 1):
     msg = neighbour_max(state, prep) if model.agg_func_name == 'Max' else operator_messages(M, state)
     lin = model.filter[t]
     y = dense(msg.reshape(B * N, -1), lin.weight, lin.bias, True)
     y = y / (torch.norm(y, 2, dim=1, keepdim=True) + _EPS)
-    state = y.reshape(B, N, -1)
-    if model.training and model.dropout > 0.0:
-      state = torch.nn.functional.dropout(state, model.dropout, True)
+    state = _dropout(model, y.reshape(B, N, -1))
   return gated_readout(model, state, mask)
 
 
@@ -373,7 +396,7 @@ def _ggnn_operators(L, aggregate_type):
   """The 0/1 pattern of L, row-normalised by (nnz + float32 eps) for ``avg``: a new tensor."""
   A = (L != 0).float()
   if aggregate_type == 'avg':
-    A = A / (A.sum(dim=2, keepdim=True) + _EPS)
+    A = _row_normalised(A)
   return A.contiguous()
 
 
@@ -381,19 +404,14 @@ def _ggnn_prop(model, A, h):
   """One GGNN propagation step (model/ggnn.py:143-171, model/gpnn.py:164-190) of h [B*N, D] over the
   operators A [B,N,N,E1]: the first message layers of all channels as one dense layer against their weights
   concatenated on the tape, the second layers, A_e m_e, then ``model.update_func``."""
-  B, N, E1 = A.shape[0], A.shape[1], A.shape[3]
-  D = h.shape[1]
   first = [seq[0] for seq in model.msg_func]
   w1 = torch.cat([l.weight for l in first], dim=0)
   b1 = torch.cat([l.bias for l in first], dim=0)
   hw = first[0].weight.shape[0]
   hid = dense(h, w1, b1, True)                                                 # [B*N, E1 * 128]
-  agg = []
-  for e in range(E1):
-    second = model.msg_func[e][2]
-    m_e = dense(hid[:, e * hw:(e + 1) * hw], second.weight, second.bias, False)
-    agg.append(operator_messages(A, m_e.reshape(B, N, D), e, 1))
-  agg = torch.cat(agg, dim=2).reshape(B * N, E1 * D)
+  second = [seq[2] for seq in model.msg_func]
+  agg = _channel_messages(A, (dense(hid[:, e * hw:(e + 1) * hw], second[e].weight, second[e].bias, False)
+                              for e in range(A.shape[3])))
   return recurrent_cell(model.update_func_name, model.update_func, agg, h)
 
 
@@ -405,14 +423,10 @@ def ggnn_train(model, node_ids, L, mask):
   as one dense layer against their weights concatenated on the tape."""
   A = _ggnn_operators(L, model.aggregate_type)
   B, N = A.shape[0], A.shape[1]
-  x = embedding(node_ids, model.embedding.weight).reshape(B * N, -1)
-  lin = model.input_func[0]
-  h = dense(x, lin.weight, lin.bias, False)
+  h = _input_state(model, node_ids, model.embedding.weight)
   D = h.shape[1]
   for _ in range(model.num_prop):
-    h = _ggnn_prop(model, A, h)
-    if model.training and model.dropout > 0.0:
-      h = torch.nn.functional.dropout(h, model.dropout, True)
+    h = _dropout(model, _ggnn_prop(model, A, h))
   return gated_readout(model, h.reshape(B, N, D), mask, head=model.output_func[0])
 
 
@@ -426,12 +440,10 @@ def gpnn_train(model, node_ids, L, L_cluster, L_cut, mask):
   A = _ggnn_operators(L, model.aggregate_type)
   P = torch.stack([L_cluster, L_cut], 3).float()
   if model.aggregate_type == 'avg':
-    P = P / (P.sum(dim=2, keepdim=True) + _EPS)
+    P = _row_normalised(P)
   P = P.contiguous()
   B, N = A.shape[0], A.shape[1]
-  x = embedding(node_ids, model.embedding.weight).reshape(B * N, -1)
-  lin = model.input_func[0]
-  h = dense(x, lin.weight, lin.bias, False)
+  h = _input_state(model, node_ids, model.embedding.weight)
   D = h.shape[1]
   m1, m2 = model.msg_func[0][0], model.msg_func[0][2]
   s1, s2 = model.state_func[0], model.state_func[2]
@@ -445,9 +457,7 @@ def gpnn_train(model, node_ids, L, L_cluster, L_cut, mask):
         s = recurrent_cell(model.update_func_name, model.update_func_partition, agg, s)
       chains.append(s)
     s = dense(dense(torch.cat([h] + chains, dim=1), s1.weight, s1.bias, True), s2.weight, s2.bias, False)
-    h = _ggnn_prop(model, A, s)
-    if model.training and model.dropout > 0.0:
-      h = torch.nn.functional.dropout(h, model.dropout, True)
+    h = _dropout(model, _ggnn_prop(model, A, s))
   return gated_readout(model, h.reshape(B, N, D), mask, head=model.output_func[0])
 
 
@@ -513,11 +523,8 @@ def mpnn_train(model, node_ids, L, mask):
   nnz = A.sum(dim=2)                                                           # [B,N,E1]
   avg = model.aggregate_type == 'avg'
   B, N, E1 = A.shape[0], A.shape[1], A.shape[3]
-  x = embedding(node_ids, model.node_embedding.weight).reshape(B * N, -1)
-  lin = model.input_func[0]
-  h = dense(x, lin.weight, lin.bias, False)
+  h = _input_state(model, node_ids, model.node_embedding.weight)
   D = h.shape[1]
-  cell = model.update_func
   if model.msg_func_name == 'MLP':
     zeros = torch.zeros((B, N, 4), device=L.device, dtype=torch.float32)
     prep = ops.graph_prepare(L, zeros, binarize=True)
@@ -530,7 +537,7 @@ def mpnn_train(model, node_ids, L, mask):
     hw = first[0].weight.shape[0]
   else:
     if avg:
-      A = A / (nnz.unsqueeze(2) + _EPS)
+      A = _row_normalised(A)
     A = A.contiguous()
     w_msg = model.edge_embedding.weight.view(E1, D, D).transpose(1, 2).reshape(E1 * D, D)    # stacked E_e^T
   for _ in range(model.num_prop):
@@ -540,18 +547,8 @@ def mpnn_train(model, node_ids, L, mask):
                        deg[:, e:e + 1] * second[e].bias for e in range(E1)], dim=1)
     else:
       msg = dense(h, w_msg, None, False)
-      agg = torch.cat([operator_messages(A, msg[:, e * D:(e + 1) * D].reshape(B, N, D), e, 1)
-                       for e in range(E1)], dim=2).reshape(B * N, E1 * D)
-    gi = dense(agg, cell.weight_ih, cell.bias_ih, False)
-    gh = dense(h, cell.weight_hh, cell.bias_hh, False)
-    i_r, i_z, i_n = gi.chunk(3, dim=1)
-    h_r, h_z, h_n = gh.chunk(3, dim=1)
-    r = torch.sigmoid(i_r + h_r)
-    z = torch.sigmoid(i_z + h_z)
-    n = torch.tanh(i_n + r * h_n)
-    h = (h - n) * z + n
-    if model.training and model.dropout > 0.0:
-      h = torch.nn.functional.dropout(h, model.dropout, True)
+      agg = _channel_messages(A, (msg[:, e * D:(e + 1) * D] for e in range(E1)))
+    h = _dropout(model, recurrent_cell('GRU', model.update_func, agg, h))
   return set2vec_train(model, h.reshape(B, N, D), mask)
 
 
@@ -642,9 +639,6 @@ def bmm(A, Bm):
   return _BMM.apply(A.float(), Bm.float())
 
 
-_EPS = 1.1920928955078125e-07       # np.finfo(np.float32).eps (ada_lanczos_net.py:8)
-
-
 def _gaussian_laplacian_train(x, adj):
   """Learned operator of model/ada_lanczos_net.py:101-137 on the autograd tape: Gaussian kernel of the
   embedding distances (sigma^2 = mean over all N^2 pairs, padded ones included), masked by the
@@ -719,7 +713,6 @@ def ada_train(model, node_ids, L, mask, q1):
   state = embedding(node_ids, model.embedding.weight)
   B, N = state.shape[0], state.shape[1]
   K, S = model.num_eig_vec, model.num_scale_long
-  short = list(model.short_diffusion_dist)
   powers = Q = None
   if S > 0:
     adj = (L[:, :, :, 0] != 0).to(torch.float32)                    # ada_lanczos_net.py:310-311
@@ -733,20 +726,11 @@ def ada_train(model, node_ids, L, mask, q1):
         cur = bmm(cur, T)
     powers = torch.cat(plist, dim=2)                                # [B,K,S*K]: index r, s*K + c (:274)
   for t in range(model.num_layer):
-    msgs = []
-    if short:
-      walk = state
-      for step in range(1, max(short) + 1):
-        walk = operator_messages(L, walk, 0, 1)
-        if step in short:
-          msgs.append(walk)
+    msgs = _short_walk(L, state, model.short_diffusion_dist)
     if S > 0:
       if model.spectral_filter_kind == 'MLP':
-        h = powers.reshape(B, K * S * K)
-        seq = model.spectral_filter[t]
-        for i in (0, 2, 4, 6):
-          h = dense(h, seq[i].weight, seq[i].bias, i != 6)
-        G = h.reshape(B, K, K, S)                                   # index r, c, s (:275)
+        G = _filter_mlp(model.spectral_filter[t], powers.reshape(B, K * S * K))
+        G = G.reshape(B, K, K, S)                                   # index r, c, s (:275)
         G = ((G + G.transpose(1, 2)) * 0.5).permute(0, 3, 1, 2)     # [B,S,K,K]
       else:
         G = torch.stack(plist, dim=1)
@@ -756,10 +740,7 @@ def ada_train(model, node_ids, L, mask, q1):
       M = bmm(Q.unsqueeze(1).expand(B, S, N, K).reshape(B * S, N, K), W)      # [B*S,N,D]
       msgs.append(M.reshape(B, S, N, D).permute(0, 2, 1, 3).reshape(B, N, S * D))
     msgs.append(operator_messages(L, state))
-    lin = model.filter[t]
-    state = dense(torch.cat(msgs, dim=2).reshape(B * N, -1), lin.weight, lin.bias, True).reshape(B, N, -1)
-    if model.training and model.dropout > 0.0:
-      state = torch.nn.functional.dropout(state, model.dropout, True)
+    state = _conv_layer(model, t, msgs)
   return gated_readout(model, state, mask)
 
 
