@@ -347,6 +347,28 @@ int lnb_ggnn_update(lnb_stream_t stream, const float* M, const float* h, const f
                     const float* bias, int B, int N, int D, int E1, int avg, float* out);
 
 /* ---------------------------------------------------------------------------------------
+ * One time step t of GraphSAGE's LSTM aggregator (model/graph_sage.py:131-140) for all R = B*N*E1
+ * sequences of a layer, one persistent 3xTF32 wgmma launch.  Sequence s = (b*N + n)*E1 + e:
+ *   x = state[b*N + m] with m = nn_idx[b, n, t, e]  (a zero row when m is outside [0, N))
+ *   [i f g o] = [x | h[s]] W^T + bias;  c[s] = sigmoid(f) c[s] + sigmoid(i) tanh(g)
+ *   out[s] = sigmoid(o) tanh(c[s])                                       (torch's LSTMCell)
+ * At t = 0, h = c = 0: h is not read (may be null) and c is only written.  On the last step
+ * (t == K - 1) out[s] is multiplied by nonempty[b*N + n], so out read as [B*N, E1*D] is the layer's
+ * message matrix (column block e = channel e).  A sequence of a node with nonempty == 0 gathers nothing
+ * and runs no cell: its out row is written (zero) on the last step only, its c row never.
+ * state [B*N, D], nn_idx int32 [B, N, K, E1], nonempty [B*N], h / c / out [R, D]; c is updated in place,
+ * out must alias neither h (for t > 0) nor c.
+ * W_hi / W_lo: tf32 split of [W_ih | W_hh] [4D, 2D] (torch.nn.LSTMCell) with row (u/4)*16 + g*4 + u%4 =
+ * gate g of hidden unit u, g = i, f, g, o; bias [4D] = b_ih + b_hh in the same order.  state, h, c, out
+ * and W 16-byte aligned.
+ * Envelope: D % 32 == 0, 32 <= D <= 128, 1 <= E1 <= 16, K >= 1, 0 <= t < K (LNB_ERR_UNSUPPORTED for
+ * D / E1 outside it, nothing launched).  Summation order is fixed: repeated launches are bit-identical.
+ * ------------------------------------------------------------------------------------- */
+int lnb_sage_lstm_step(lnb_stream_t stream, const float* state, const int32_t* nn_idx, const float* nonempty,
+                       const float* h, float* c, const float* W_hi, const float* W_lo, const float* bias, int B,
+                       int N, int K, int E1, int D, int t, float* out);
+
+/* ---------------------------------------------------------------------------------------
  * GPNN propagation within clusters and across cuts (model/gpnn.py:192-225), both partition operators in
  * one persistent 3xTF32 wgmma launch over all B*N rows.  For each active part p (0 = cluster, 1 = cut):
  *   agg_p[b,n, :] = sum over the non-zeros m of row n of operator p of  w * M_p[b*N+m, :]

@@ -98,6 +98,8 @@ SIGNATURES = {
                                            c_f32p, c_int, c_int, c_int, c_int, c_int, c_int, c_f32p, c_f32p]),
     'lnb_ggnn_update': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p,
                                 c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int, c_f32p]),
+    'lnb_sage_lstm_step': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
+                                   c_f32p, c_int, c_int, c_int, c_int, c_int, c_int, c_f32p]),
     'lnb_mpnn_update': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p,
                                 c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int, c_f32p]),
     'lnb_gpnn_partition_update': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,

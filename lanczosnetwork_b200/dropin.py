@@ -10,7 +10,9 @@ What it does (see INTEGRATION.md):
      inside the runner modules' globals, because the runners resolve the class with ``eval(name)`` in their own
      namespace (runner/qm8_runner.py:59,288; runner/graph_runner.py:57,285), plus the classes of
      ``OPT_IN_CLASSES`` named with ``--opt-in NAME`` (repeatable; e.g. ``--opt-in MPNN``); ``--opt-in GAT``
-     (``TRAINING_OPT_IN_CLASSES``) binds ``TrainableGAT`` under the name ``GAT``, for training and test runs;
+     (``TRAINING_OPT_IN_CLASSES``) binds ``TrainableGAT`` under the name ``GAT``, and ``--opt-in GraphSAGE``
+     (``LSTM_OPT_IN_CLASSES``) binds ``LSTMGraphSAGE`` (which takes ``agg_func: LSTM``) under the name
+     ``GraphSAGE``, for training and test runs;
   3. runs the reference ``run_exp.main()`` unchanged (``--opt-in`` is removed from its argv).
 """
 import importlib
@@ -27,6 +29,9 @@ OPT_IN_CLASSES = ('MPNN',)
 # names whose drop-in becomes its trainable subclass ``Trainable<name>`` when asked for (opt_in=..., --opt-in);
 # without the opt-in they keep their DROPIN_CLASSES behaviour
 TRAINING_OPT_IN_CLASSES = ('GAT',)
+# names whose drop-in becomes the subclass that also takes the LSTM aggregator, ``LSTM<name>``, when asked for
+# (opt_in=..., --opt-in), for training and test runs; without the opt-in an LSTM config fails in the constructor
+LSTM_OPT_IN_CLASSES = ('GraphSAGE',)
 
 
 def register_native_op():
@@ -39,10 +44,11 @@ def register_native_op():
 
 
 def _check_opt_in(opt_in):
-  unknown = [n for n in opt_in if n not in OPT_IN_CLASSES + TRAINING_OPT_IN_CLASSES]
+  unknown = [n for n in opt_in if n not in OPT_IN_CLASSES + TRAINING_OPT_IN_CLASSES + LSTM_OPT_IN_CLASSES]
   if unknown:
-    raise ValueError('dropin: %s not in OPT_IN_CLASSES %s or TRAINING_OPT_IN_CLASSES %s'
-                     % (', '.join(map(repr, unknown)), OPT_IN_CLASSES, TRAINING_OPT_IN_CLASSES))
+    raise ValueError('dropin: %s not in OPT_IN_CLASSES %s, TRAINING_OPT_IN_CLASSES %s or LSTM_OPT_IN_CLASSES %s'
+                     % (', '.join(map(repr, unknown)), OPT_IN_CLASSES, TRAINING_OPT_IN_CLASSES,
+                        LSTM_OPT_IN_CLASSES))
   return tuple(opt_in)
 
 
@@ -52,7 +58,8 @@ def patch_namespace(module, training=False, opt_in=()):
   is a ValueError).  ``training=True`` (a run without ``-t``) rebinds only the classes that have a
   differentiable training path (every class but ``GAT``, which is inference only); a class without one
   keeps the reference's trainable class instead of failing on the first ``loss.backward()``.  A name of
-  ``TRAINING_OPT_IN_CLASSES`` in ``opt_in`` is bound to ``Trainable<name>`` in training and test runs."""
+  ``TRAINING_OPT_IN_CLASSES`` in ``opt_in`` is bound to ``Trainable<name>``, one of ``LSTM_OPT_IN_CLASSES`` to
+  ``LSTM<name>``, in training and test runs."""
   opt_in = _check_opt_in(opt_in)
   for name in DROPIN_CLASSES + tuple(n for n in opt_in if n in OPT_IN_CLASSES):
     if hasattr(module, name):
@@ -63,6 +70,8 @@ def patch_namespace(module, training=False, opt_in=()):
   for name in opt_in:
     if name in TRAINING_OPT_IN_CLASSES and hasattr(module, name):
       setattr(module, name, getattr(_models, 'Trainable' + name))
+    if name in LSTM_OPT_IN_CLASSES and hasattr(module, name):
+      setattr(module, name, getattr(_models, 'LSTM' + name))
   return module
 
 
@@ -110,7 +119,8 @@ def main(argv=None):
   while '--opt-in' in argv:
     i = argv.index('--opt-in')
     if i + 1 >= len(argv):
-      raise SystemExit('--opt-in needs a class name (one of %s)' % (OPT_IN_CLASSES + TRAINING_OPT_IN_CLASSES,))
+      raise SystemExit('--opt-in needs a class name (one of %s)'
+                       % (OPT_IN_CLASSES + TRAINING_OPT_IN_CLASSES + LSTM_OPT_IN_CLASSES,))
     opt_in.append(argv[i + 1])
     del argv[i:i + 2]
   install(root, compat=True, training=('-t' not in argv and '--test' not in argv), opt_in=opt_in)

@@ -7,7 +7,7 @@ from .gcn import *                  # noqa: F401,F403  (SURVEY 8f3: sibling mode
 from .dcnn import *                 # noqa: F401,F403
 from .cheby_net import *            # noqa: F401,F403
 from .gat import *                  # noqa: F401,F403  (GAT inference only; TrainableGAT by opt-in)
-from .graph_sage import *        # noqa: F401,F403  (Mean / Max aggregators)
+from .graph_sage import *        # noqa: F401,F403  (Mean / Max aggregators; LSTMGraphSAGE adds LSTM)
 from .ggnn import *              # noqa: F401,F403
 from .gpnn import *              # noqa: F401,F403
 from .mpnn import *              # noqa: F401,F403  (a drop-in by opt-in only, see dropin.OPT_IN_CLASSES)

@@ -18,25 +18,28 @@ Semantics kept from the reference:
     0 (the collate's zero fill, dataset/qm8.py:143-163): the operator built from nn_idx does the same;
   * each layer is relu(Linear(msg)) / (||.||_2 + float32 eps), then dropout; padded nodes (nonempty = 0)
     get the constant row relu(b) / (||relu(b)|| + eps), which enters the mean when mask is None.
-``agg_func: LSTM`` is not implemented: the constructor raises NotImplementedError before drawing any
-random number.  An unknown aggregator fails in the forward, as in the reference.  Ids outside [0, N)
-contribute nothing (the reference raises an IndexError)."""
+``GraphSAGE`` does not take ``agg_func: LSTM``: the constructor raises NotImplementedError before drawing
+any random number.  ``LSTMGraphSAGE`` (below; ``--opt-in GraphSAGE`` of lanczosnetwork_b200.dropin) takes
+it.  An unknown aggregator fails in the forward, as in the reference.  Ids outside [0, N) contribute
+nothing (the reference raises an IndexError); under the LSTM aggregator such an id is a zero input row."""
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, init_linears, loss_function
+from ._common import SpectralNetBase, init_cell, init_linears, loss_function
 from .. import ops
 
-__all__ = ['GraphSAGE']
+__all__ = ['GraphSAGE', 'LSTMGraphSAGE', 'lstm_gate_matrix', 'lstm_gate_matrix_inverse']
 
 SUPPORTED_AGGREGATORS = ('Mean', 'Max')
+EPS = 1.1920928955078125e-07       # np.finfo(np.float32).eps (graph_sage.py:6)
 
 
 class GraphSAGE(SpectralNetBase):
+  _takes_lstm = False
 
   def __init__(self, config):
     m = config.model
-    if m.agg_func == 'LSTM':
+    if m.agg_func == 'LSTM' and not self._takes_lstm:
       raise NotImplementedError(
           "GraphSAGE drop-in: agg_func 'LSTM' is not implemented; supported aggregators: %s"
           % ', '.join(SUPPORTED_AGGREGATORS))
@@ -48,7 +51,10 @@ class GraphSAGE(SpectralNetBase):
 
     self.embedding = nn.Embedding(self.num_atom, self.input_dim)
     self.agg_func_name = m.agg_func
-    self.agg_func = {'Mean': torch.mean, 'Max': torch.max}.get(self.agg_func_name)
+    if self.agg_func_name == 'LSTM':            # LSTMGraphSAGE only; each cell draws its default init here
+      self.agg_func = nn.ModuleList([nn.LSTMCell(dims[t], dims[t]) for t in range(self.num_layer - 1)])
+    else:
+      self.agg_func = {'Mean': torch.mean, 'Max': torch.max}.get(self.agg_func_name)
     self.att_func = nn.Sequential(nn.Linear(dims[-2], 1), nn.Sigmoid())
     self.filter = nn.ModuleList(
         [nn.Linear(dims[t] * (self.num_edgetype + 1), dims[t + 1]) for t in range(self.num_layer)] +
@@ -57,9 +63,14 @@ class GraphSAGE(SpectralNetBase):
     self._init_param()
 
   def _init_param(self):
-    """Xavier-uniform weights and zero biases, att_func first, then filter (graph_sage.py:69-96); the
-    embedding keeps nn.Embedding's default N(0, 1)."""
-    init_linears([*self.att_func, *self.filter])
+    """Xavier-uniform weights and zero biases, att_func first, then (LSTM) Xavier on weight_hh, weight_ih
+    and zero biases of every cell, then filter (graph_sage.py:69-96); the embedding keeps nn.Embedding's
+    default N(0, 1)."""
+    init_linears(self.att_func)
+    if self.agg_func_name == 'LSTM':
+      for cell in self.agg_func:
+        init_cell(cell)
+    init_linears(self.filter)
 
   def forward(self, node_feat, nn_idx, nonempty_mask, label=None, mask=None):
     """
@@ -113,3 +124,88 @@ class GraphSAGE(SpectralNetBase):
         emb=self.embedding.weight, readout=(head.weight, head.bias, att.weight.reshape(-1), att.bias),
         mask=mask, sage=self.agg_func_name)
     return score
+
+
+def lstm_gate_matrix(weight_ih, weight_hh, bias_ih, bias_hh):
+  """An nn.LSTMCell as one GEMM over [x | h] (layout of lnb_sage_lstm_step): returns W [4D, 2D] and b [4D]
+  whose row (u // 4) * 16 + g * 4 + u % 4 is gate g (i, f, g, o) of hidden unit u: [W_ih | W_hh] rows
+  g*D + u, and b_ih + b_hh in the same order.  Works on any device."""
+  D = weight_hh.shape[1]
+  W = torch.cat([weight_ih, weight_hh], dim=1)
+  b = bias_ih + bias_hh
+  W = W.reshape(4, D // 4, 4, 2 * D).permute(1, 0, 2, 3).reshape(4 * D, 2 * D).contiguous()
+  b = b.reshape(4, D // 4, 4).permute(1, 0, 2).reshape(4 * D).contiguous()
+  return W, b
+
+
+def lstm_gate_matrix_inverse(W, b):
+  """(weight_ih, weight_hh, b_ih + b_hh) of a matrix from lstm_gate_matrix."""
+  D = W.shape[1] // 2
+  W = W.reshape(D // 4, 4, 4, 2 * D).permute(1, 0, 2, 3).reshape(4 * D, 2 * D)
+  b = b.reshape(D // 4, 4, 4).permute(1, 0, 2).reshape(4 * D)
+  return W[:, :D].contiguous(), W[:, D:].contiguous(), b.contiguous()
+
+
+class LSTMGraphSAGE(GraphSAGE):
+  """GraphSAGE with the reference's three aggregators.  ``Mean`` and ``Max`` behave exactly as in
+  GraphSAGE.  ``LSTM`` builds the reference's ``agg_func`` (one nn.LSTMCell per propagation layer, shared
+  by the E+1 channels) in the reference's construction and initialisation order, so a seed gives its
+  initial weights and its checkpoints load by name.
+
+  LSTM inference per layer ii: K = num_sample_neighbors launches of ``lnb_sage_lstm_step`` (all
+  B*N*(E+1) sequences per launch, the neighbour rows gathered in the producer warps, the cell in the
+  epilogue, the last step writing the message matrix), then ``linear_tf32x3`` + ReLU for filter[ii] and
+  the row normalisation in torch; the embedding gather in front and ``ops.readout`` behind, all replayed
+  as one CUDA graph.  Widths outside the kernel (D % 32 != 0, D > 128) or more than 16 channels run the
+  training formulation (``train.sage_train``) under no_grad.  Training: ``train.lstm_messages``."""
+  _takes_lstm = True
+
+  def _samples(self, nn_idx):
+    K = self.num_sample_neighbors
+    if nn_idx.shape[2] < K:
+      raise ValueError('LSTMGraphSAGE: nn_idx holds %d samples per node, num_sample_neighbors is %d'
+                       % (nn_idx.shape[2], K))
+    return nn_idx[:, :, :K]
+
+  def _train_impl(self, node_feat, nn_idx, nonempty_mask, mask):
+    if self.agg_func_name != 'LSTM':
+      return super(LSTMGraphSAGE, self)._train_impl(node_feat, nn_idx, nonempty_mask, mask)
+    from ..train import sage_train
+    return sage_train(self, node_feat, None, mask, samples=(self._samples(nn_idx), nonempty_mask))
+
+  def lstm_supported(self, E1):
+    """True when every propagation layer runs on lnb_sage_lstm_step (and its filter on the dense kernel)."""
+    dims = [self.embedding.weight.shape[1]] + list(self.hidden_dim[:self.num_layer - 1])
+    return all(ops.sage_lstm_step_supported(dims[t], E1, self.num_sample_neighbors)
+               for t in range(self.num_layer - 1))
+
+  def _gates(self, t):
+    cell = self.agg_func[t]
+
+    def build():
+      W, b = lstm_gate_matrix(cell.weight_ih.detach(), cell.weight_hh.detach(), cell.bias_ih.detach(),
+                              cell.bias_hh.detach())
+      return ops.split_tf32(W) + (b,)
+    return self._wcache.derived('agg_func.%d.gates' % t,
+                                [cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh], build)
+
+  def _forward_impl(self, node_feat, nn_idx, nonempty_mask, mask):
+    if self.agg_func_name != 'LSTM':
+      return super(LSTMGraphSAGE, self)._forward_impl(node_feat, nn_idx, nonempty_mask, mask)
+    B, N = node_feat.shape
+    E1 = nn_idx.shape[3]
+    nn_idx = self._samples(nn_idx)
+    if not self.lstm_supported(E1):
+      from ..train import sage_train                # off the kernel: the training formulation (no_grad)
+      return sage_train(self, node_feat, None, mask, samples=(nn_idx, nonempty_mask))
+    idx = nn_idx.to(torch.int32).contiguous()        # converted once per forward
+    ne = nonempty_mask.reshape(B * N).float().contiguous()
+    state = ops.embedding_rows(node_feat.long().reshape(-1), self.embedding.weight)
+    for t in range(self.num_layer - 1):
+      g_hi, g_lo, g_b = self._gates(t)
+      msg = ops.sage_lstm_messages(state, idx, ne, g_hi, g_lo, g_b)
+      lin = self.filter[t]
+      w_hi, w_lo = self._wcache.split('filter.%d' % t, lin.weight)
+      y = ops.linear_tf32x3(msg, w_hi, w_lo, lin.bias, relu=True)
+      state = y / (torch.norm(y, 2, dim=1, keepdim=True) + EPS)
+    return self._readout(state.view(B, N, -1), mask)

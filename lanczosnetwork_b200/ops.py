@@ -16,7 +16,8 @@ __all__ = [
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
-    'sage_operators', 'neighbour_max', 'ggnn_update',
+    'sage_operators', 'neighbour_max', 'sage_lstm_step', 'sage_lstm_step_supported', 'sage_lstm_messages',
+    'ggnn_update',
     'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
     'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'set2vec', 'set2vec_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
@@ -651,6 +652,59 @@ def ggnn_update(M, h, prep, w_hi, w_lo, bias, avg, out=None):
         _stream(h), _ptr(M), _ptr(h), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi), _ptr(w_lo),
         _ptr(bias), B, N, D, E1, int(bool(avg)), _ptr(out)), 'lnb_ggnn_update')
   return out
+
+
+def sage_lstm_step_supported(D, E1, K):
+  """Shapes lnb_sage_lstm_step accepts (mirrors its checks)."""
+  return D % 32 == 0 and 32 <= D <= 128 and 1 <= E1 <= 16 and K >= 1
+
+
+def sage_lstm_step(state, nn_idx, nonempty, h, c, w_hi, w_lo, bias, t, out):
+  """Step t of GraphSAGE's LSTM aggregator for all B*N*E1 sequences of a layer (see lnb_sage_lstm_step).
+  state [B*N, D]; nn_idx int32 [B, N, K, E1] (contiguous); nonempty float32 [B*N]; h (ignored at t = 0),
+  c (updated in place) and out float32 [B*N*E1, D]; w_hi / w_lo / bias: lstm_gate_matrix of the cell,
+  [4D, 2D] and [4D].  Returns out: h of step t, or on the last step the message matrix viewed [B*N, E1*D]."""
+  _need_cuda(state, nn_idx, nonempty, h, c, w_hi, w_lo, bias, out)
+  B, N, K, E1 = nn_idx.shape
+  D = state.shape[1]
+  R = B * N * E1
+  ok = (nn_idx.dtype == torch.int32 and nn_idx.is_contiguous() and tuple(state.shape) == (B * N, D) and
+        tuple(nonempty.shape) == (B * N,) and tuple(c.shape) == (R, D) and tuple(out.shape) == (R, D) and
+        (h is None or tuple(h.shape) == (R, D)) and tuple(w_hi.shape) == (4 * D, 2 * D) and
+        tuple(bias.shape) == (4 * D,))
+  if not ok:
+    raise ValueError('sage_lstm_step: state %s, nn_idx %s %s, nonempty %s, h %s, c %s, out %s, W %s, bias %s do '
+                     'not agree' % (tuple(state.shape), tuple(nn_idx.shape), nn_idx.dtype, tuple(nonempty.shape),
+                                    None if h is None else tuple(h.shape), tuple(c.shape), tuple(out.shape),
+                                    tuple(w_hi.shape), tuple(bias.shape)))
+  for name, x in (('state', state), ('nonempty', nonempty), ('h', h), ('c', c), ('out', out), ('bias', bias)):
+    if x is not None and (x.dtype != torch.float32 or not x.is_contiguous()):
+      raise ValueError('sage_lstm_step: %s must be a contiguous float32 tensor' % name)
+  with torch.cuda.device(state.device):
+    _lib.check(_lib.load().lnb_sage_lstm_step(
+        _stream(state), _ptr(state), _ptr(nn_idx), _ptr(nonempty), _ptr(h), _ptr(c), _ptr(w_hi), _ptr(w_lo),
+        _ptr(bias), B, N, K, E1, D, int(t), _ptr(out)), 'lnb_sage_lstm_step')
+  return out
+
+
+def sage_lstm_messages(state, nn_idx, nonempty, w_hi, w_lo, bias):
+  """The messages of one LSTM GraphSAGE layer: the K steps of ``sage_lstm_step`` over fresh h / c buffers.
+  state [B*N, D], nn_idx int32 [B, N, K, E1], nonempty float32 [B*N].  Returns [B*N, E1*D], column block e
+  = the final h of channel e times nonempty."""
+  B, N, K, E1 = nn_idx.shape
+  D = state.shape[1]
+  R = B * N * E1
+  state = _f32c(state)
+  c = torch.empty((R, D), device=state.device, dtype=torch.float32)
+  h = torch.empty_like(c)
+  spare = torch.empty_like(c) if K > 1 else None
+  for t in range(K):
+    if t == K - 1:
+      out = torch.empty((B * N, E1 * D), device=state.device, dtype=torch.float32)
+      sage_lstm_step(state, nn_idx, nonempty, h if t else None, c, w_hi, w_lo, bias, t, out.view(R, D))
+      return out
+    sage_lstm_step(state, nn_idx, nonempty, h if t else None, c, w_hi, w_lo, bias, t, spare)
+    h, spare = spare, h
 
 
 def gpnn_partition_update_supported(N, H):

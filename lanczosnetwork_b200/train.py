@@ -28,7 +28,7 @@ from . import ops
 
 __all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
            'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
-           'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'gat_attention',
+           'lstm_messages', 'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'gat_attention',
            'gat_train', 'GraphedStep']
 
 _EPS = 1.1920928955078125e-07       # np.finfo(np.float32).eps (ada_lanczos_net.py:8)
@@ -357,24 +357,83 @@ def neighbour_max(X, prep):
   return _NeighbourMax.apply(X.float(), prep)
 
 
-def sage_train(model, node_ids, M, mask, prep=None):
+def sage_train(model, node_ids, M, mask, prep=None, samples=None):
   """Differentiable GraphSAGE (model/graph_sage.py:98-175): embedding -> num_layer - 1 layers of
   [messages of every channel] -> Linear + ReLU -> row / (||row|| + eps) -> dropout -> gated readout
   with the head filter[num_layer].  Mean messages are M_e X on the count-weighted operators M
   [B,N,N,E1] (ops.sage_operators); Max messages come from ``neighbour_max`` on the ELL lists of M
-  (``prep``, built here when not given)."""
-  M = M.float().contiguous()
+  (``prep``, built here when not given).  LSTM messages (``lstm_messages`` with the cell agg_func[t])
+  read ``samples`` = (nn_idx, nonempty_mask) instead; M is then unused."""
+  lstm = model.agg_func_name == 'LSTM'
+  if not lstm:
+    M = M.float().contiguous()
   state = embedding(node_ids, model.embedding.weight)
   B, N = state.shape[0], state.shape[1]
   if model.agg_func_name == 'Max' and prep is None and model.num_layer > 1:
     prep = ops.graph_prepare(M)
   for t in range(model.num_layer - 1):
-    msg = neighbour_max(state, prep) if model.agg_func_name == 'Max' else operator_messages(M, state)
+    if lstm:
+      msg = lstm_messages(model.agg_func[t], state, *samples)
+    else:
+      msg = neighbour_max(state, prep) if model.agg_func_name == 'Max' else operator_messages(M, state)
     lin = model.filter[t]
     y = dense(msg.reshape(B * N, -1), lin.weight, lin.bias, True)
     y = y / (torch.norm(y, 2, dim=1, keepdim=True) + _EPS)
     state = _dropout(model, y.reshape(B, N, -1))
   return gated_readout(model, state, mask)
+
+
+class _LstmPointwise(torch.autograd.Function):
+  """The pointwise part of torch's LSTMCell: from the pre-activations G = [i f g o] [R, 4D] and c [R, D]
+  (None: zero), c' = sigmoid(f) c + sigmoid(i) tanh(g), h' = sigmoid(o) tanh(c').  Saves G, c and c' only
+  (the gates are recomputed in the backward), so the tape of K steps holds about 6D floats per row and
+  step."""
+
+  @staticmethod
+  def forward(ctx, G, c):
+    i, f, g, o = G.chunk(4, dim=1)
+    si, sf, tg, so = torch.sigmoid(i), torch.sigmoid(f), torch.tanh(g), torch.sigmoid(o)
+    c2 = si * tg if c is None else sf * c + si * tg
+    h2 = so * torch.tanh(c2)
+    ctx.save_for_backward(G, c, c2)
+    return h2, c2
+
+  @staticmethod
+  def backward(ctx, gh, gc2):
+    G, c, c2 = ctx.saved_tensors
+    i, f, g, o = G.chunk(4, dim=1)
+    si, sf, tg, so = torch.sigmoid(i), torch.sigmoid(f), torch.tanh(g), torch.sigmoid(o)
+    tc = torch.tanh(c2)
+    gc = gc2 + gh * so * (1 - tc * tc)
+    gi = gc * tg * si * (1 - si)
+    gf = gc * c * sf * (1 - sf) if c is not None else torch.zeros_like(gi)
+    gg = gc * si * (1 - tg * tg)
+    go = gh * tc * so * (1 - so)
+    return torch.cat([gi, gf, gg, go], dim=1), (gc * sf if c is not None and ctx.needs_input_grad[1] else None)
+
+
+def lstm_messages(cell, state, nn_idx, nonempty):
+  """The LSTM aggregator of one GraphSAGE layer (model/graph_sage.py:131-140) on the tape, for every
+  channel at once: the sequences s = (b*N + n)*E1 + e run ``cell`` (an nn.LSTMCell) over
+  x_t = state[b, nn_idx[b, n, t, e]] from h = c = 0.  The input product is hoisted out of the gather:
+  P = state W_ih^T once per layer, then per step P[ids] (the row gather of ``embedding``, whose adjoint is
+  the segment sum; an id outside [0, N) reads a zero row, like x = 0) + b_ih + b_hh + h W_hh^T and the
+  pointwise cell.  state [B, N, D], nn_idx [B, N, K, E1], nonempty [B, N, 1].  Returns the messages
+  [B*N, E1*D]: the final h of channel e in column block e, times nonempty."""
+  B, N, D = state.shape
+  K, E1 = nn_idx.shape[2], nn_idx.shape[3]
+  P = dense(state.reshape(B * N, D), cell.weight_ih, None, False)                 # [B*N, 4D]
+  bias = cell.bias_ih + cell.bias_hh
+  idx = nn_idx.long()
+  rows = torch.where((idx >= 0) & (idx < N), idx + N * torch.arange(B, device=idx.device).view(B, 1, 1, 1),
+                     torch.full_like(idx, -1))                                     # global rows, -1: zero
+  h = c = None
+  for t in range(K):
+    G = embedding(rows[:, :, t, :].reshape(-1), P) + bias
+    if h is not None:
+      G = G + dense(h, cell.weight_hh, None, False)
+    h, c = _LstmPointwise.apply(G, c)
+  return (h.reshape(B, N, E1 * D) * nonempty.reshape(B, N, 1).to(h.dtype)).reshape(B * N, E1 * D)
 
 
 def recurrent_cell(kind, cell, x, h):
