@@ -125,7 +125,13 @@ int lnb_linear_tf32x3_grouped(lnb_stream_t stream, const float* A, const float* 
  *                graph order instead; with B <= 1 the fused kernels run the table;
  *   rowmap [B*K], nrows [1] (both optional, NULL to skip): the compact Ritz row list of
  *                lnb_ritz_rowmap, produced by the same pass;
- *   flags bit 0: store 1.0 for every non-zero (the `L[L != 0] = 1.0` of model/gcnfp.py:83).
+ *   flags bit 0: store 1.0 for every non-zero (the `L[L != 0] = 1.0` of model/gcnfp.py:83);
+ *   flags bit 2 (LNB_PREP_DEFER_TILES): build the row list (a one-CTA lnb_ritz_rowmap launch) but
+ *                leave `tiles` unwritten; the caller writes it with lnb_tile_assign, on any stream,
+ *                before a fused kernel reads it.  The filter-MLP chain needs only the row list, so
+ *                the placement can run beside the chain instead of in front of it.
+ * lnb_tile_assign: the tile table and schedule of `tiles` from gext alone, exactly as the pass
+ * above writes them (one CTA).
  * Skipping exact zeros / padded rows is exact.  write_pad != 0 also writes the constant rows
  * act(bias) of padded nodes (needed when the full [B,N,H] tensor is read afterwards).
  * Requirements of the fused kernel: N <= 128, Din % 32 == 0, K % 4 == 0, K <= 32, H % 4 == 0,
@@ -135,6 +141,8 @@ int lnb_linear_tf32x3_grouped(lnb_stream_t stream, const float* A, const float* 
 int lnb_graph_prepare(lnb_stream_t stream, const float* L, const float* Q, int B, int N, int E1,
                       int K, float* ell_val, uint8_t* ell_idx, int32_t* ell_max, int32_t* gext,
                       int32_t* tiles, int32_t* rowmap, int32_t* nrows, int flags);
+#define LNB_PREP_DEFER_TILES 4
+int lnb_tile_assign(lnb_stream_t stream, const int32_t* gext, int B, int K, int32_t* tiles);
 int lnb_spectral_conv_fused(lnb_stream_t stream, const float* X, const float* Q, const float* coeff,
                             const float* ell_val, const uint8_t* ell_idx, const int32_t* ell_max,
                             const int32_t* gext, const int32_t* tiles, const float* W_hi,
@@ -155,7 +163,8 @@ int lnb_spectral_conv_fused(lnb_stream_t stream, const float* X, const float* Q,
  * Outputs: everything lnb_graph_prepare emits (same layouts, same bits: ell_val / ell_idx / ell_max /
  * gext / tiles / rowmap / nrows), the padded node_ids [B,N] int64, mask [B,N] uint8 and
  * V [B,N,K] that lnb_spectral_stack_forward reads, and -- only when L_dense != NULL -- the padded dense
- * operators [B,N,N,E1] exactly as the reference's collate builds them.  flags as lnb_graph_prepare.
+ * operators [B,N,N,E1] exactly as the reference's collate builds them.  flags as lnb_graph_prepare
+ * (LNB_PREP_DEFER_TILES included).
  * Limits: N <= 128, 2 <= E1 <= 16, degrees < 255.
  * ------------------------------------------------------------------------------------- */
 int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
@@ -270,12 +279,19 @@ int lnb_ritz_power_table(lnb_stream_t stream, const float* D, int64_t rows, cons
  * {b*K + k : k < k_eff(b)} from the extents of lnb_graph_prepare (rows of zero-padded Ritz pairs
  * multiply zero Ritz vectors downstream and are skipped; their coeff entries stay unwritten).
  * Requirements: S <= 32, hidden % 32 == 0, hidden <= 128 (else LNB_ERR_UNSUPPORTED).
+ * lnb_ritz_filter_mlp_ctas: the same with at most `ctas` persistent CTAs (0: one per SM), e.g. one
+ * SM fewer while lnb_tile_assign holds an SM beside it, so no CTA waits for that SM.  An item's
+ * arithmetic does not depend on the CTA that runs it: coeff is bit-identical for every `ctas`.
  * ------------------------------------------------------------------------------------- */
 int lnb_ritz_rowmap(lnb_stream_t stream, const int32_t* gext, int B, int K, int32_t* rowmap,
                     int32_t* nrows);
 int lnb_ritz_filter_mlp(lnb_stream_t stream, const float* table, const int32_t* rowmap,
                         const int32_t* nrows, const float* W_hi, const float* W_lo,
                         const float* bias_all, int Rall, int L, int S, int Hd, float* coeff);
+int lnb_ritz_filter_mlp_ctas(lnb_stream_t stream, const float* table, const int32_t* rowmap,
+                             const int32_t* nrows, const float* W_hi, const float* W_lo,
+                             const float* bias_all, int Rall, int L, int S, int Hd, float* coeff,
+                             int ctas);
 
 /* ---------------------------------------------------------------------------------------
  * Readout (model/lanczos_net.py:185-194, ada_lanczos_net.py:350-361):

@@ -71,6 +71,7 @@ SIGNATURES = {
     'lnb_graph_prepare': (c_int, [c_stream, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_f32p,
                                   ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                   ctypes.c_void_p, ctypes.c_void_p, c_int]),
+    'lnb_tile_assign': (c_int, [c_stream, ctypes.c_void_p, c_int, c_int, ctypes.c_void_p]),
     'lnb_graph_prepare_sparse': (c_int, [c_stream] + [ctypes.c_void_p] * 7 + [c_int] * 5 +
                                  [ctypes.c_void_p] * 11),
     'lnb_graph_prepare_sparse_packed': (c_int, [c_stream] + [ctypes.c_void_p] * 2 + [c_int] * 5 +
@@ -87,6 +88,8 @@ SIGNATURES = {
     'lnb_ritz_rowmap': (c_int, [c_stream, ctypes.c_void_p, c_int, c_int, ctypes.c_void_p, ctypes.c_void_p]),
     'lnb_ritz_filter_mlp': (c_int, [c_stream, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p, c_f32p,
                                     c_f32p, c_int, c_int, c_int, c_int, c_f32p]),
+    'lnb_ritz_filter_mlp_ctas': (c_int, [c_stream, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p, c_f32p,
+                                         c_f32p, c_int, c_int, c_int, c_int, c_f32p, c_int]),
     'lnb_debug_set_prof': (c_int, [ctypes.c_void_p]),
     'lnb_embedding_rows': (c_int, [c_stream, ctypes.c_void_p, c_f32p, c_i64, c_int, c_int, c_f32p]),
     'lnb_ritz_power_table': (c_int, [c_stream, c_f32p, c_i64, ctypes.POINTER(c_int), c_int, c_f32p]),

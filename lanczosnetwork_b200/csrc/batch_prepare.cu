@@ -201,13 +201,11 @@ static int launch_sparse(lnb_stream_t stream, SparseBatchParams p, int32_t* tile
   if (smem > 48 * 1024)
     cudaFuncSetAttribute(batch_prepare_sparse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   batch_prepare_sparse_kernel<<<p.B, BP_THREADS, smem, s>>>(p);
-  if (p.blob && (p.flags & 2)) {                   // tile table + row-list offsets came with the batch
-    lnb::count_launch(1);
-  } else {
-    lnb::launch_tile_assign(s, p.gext, p.B, p.K, tiles, rowmap, nrows);
-    lnb::count_launch(2);
-  }
-  return lnb::finish_launch("graph_prepare_sparse");
+  lnb::count_launch(1);
+  if (p.blob && (p.flags & 2))                     // tile table + row-list offsets came with the batch
+    return lnb::finish_launch("graph_prepare_sparse");
+  return lnb::launch_tiles_or_rowmap(s, p.flags, p.gext, p.B, p.K, tiles, rowmap, nrows,
+                                     "graph_prepare_sparse");
 }
 
 }  // namespace

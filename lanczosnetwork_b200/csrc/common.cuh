@@ -18,6 +18,10 @@ void set_prof_buffer(unsigned long long* p);
 
 void launch_tile_assign(cudaStream_t s, const int32_t* gext, int B, int K, int32_t* tiles,
                         int32_t* rowmap, int32_t* nrows);   // spectral_conv_fused.cu
+// after a prepare kernel: the tile assignment (with the row list), or with LNB_PREP_DEFER_TILES in
+// flags only the row list (lnb_ritz_rowmap); counts its launch and checks the launches
+int launch_tiles_or_rowmap(cudaStream_t s, int flags, const int32_t* gext, int B, int K,
+                           int32_t* tiles, int32_t* rowmap, int32_t* nrows, const char* who);
 
 inline int finish_launch(const char* what) {
   cudaError_t e = cudaGetLastError();

@@ -1154,6 +1154,18 @@ void launch_tile_assign(cudaStream_t s, const int32_t* gext, int B, int K, int32
   else
     tile_assign_kernel<false><<<1, 1024, 0, s>>>(gext, B, K, tiles, tiles + B + 2, rowmap, nrows);
 }
+
+int launch_tiles_or_rowmap(cudaStream_t s, int flags, const int32_t* gext, int B, int K,
+                           int32_t* tiles, int32_t* rowmap, int32_t* nrows, const char* who) {
+  if (flags & LNB_PREP_DEFER_TILES) {            // the caller runs lnb_tile_assign
+    int rc = lnb::finish_launch(who);
+    if (rc == LNB_OK && rowmap) rc = lnb_ritz_rowmap((lnb_stream_t)s, gext, B, K, rowmap, nrows);
+    return rc;
+  }
+  launch_tile_assign(s, gext, B, K, tiles, rowmap, nrows);
+  count_launch();
+  return finish_launch(who);
+}
 }  // namespace lnb
 
 extern "C" {
@@ -1179,9 +1191,17 @@ int lnb_graph_prepare(lnb_stream_t stream, const float* L, const float* Q, int B
     graph_prepare_kernel<false><<<B, 256, 0, s>>>(L, Q, N, E1, K, ell_val, ell_idx, ell_max, gext,
                                                   flags & 1);
   }
-  lnb::launch_tile_assign(s, gext, B, K, tiles, rowmap, nrows);
-  lnb::count_launch(2);
-  return lnb::finish_launch("graph_prepare");
+  lnb::count_launch(1);
+  return lnb::launch_tiles_or_rowmap(s, flags, gext, B, K, tiles, rowmap, nrows, "graph_prepare");
+}
+
+int lnb_tile_assign(lnb_stream_t stream, const int32_t* gext, int B, int K, int32_t* tiles) {
+  LNB_REQUIRE(gext && tiles, "tile_assign: null pointer");
+  LNB_REQUIRE(B >= 0 && K >= 1, "tile_assign: bad dims B=%d K=%d", B, K);
+  if (B == 0) return LNB_OK;
+  lnb::launch_tile_assign((cudaStream_t)stream, gext, B, K, tiles, nullptr, nullptr);
+  lnb::count_launch();
+  return lnb::finish_launch("tile_assign");
 }
 
 // one launcher for every variant of the stack kernel

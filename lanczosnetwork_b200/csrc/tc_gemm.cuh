@@ -604,11 +604,12 @@ static int sync_prof_buffer(const char* who) {
   return LNB_OK;
 }
 
-// Launches tc_gemm_kernel<Pol> on min(items, SMs) persistent CTAs with `smem` bytes of dynamic shared
-// memory; W_hi / W_lo are the split row-major [w_rows, w_cols] weights the TMA streams.
+// Launches tc_gemm_kernel<Pol> on min(items, SMs, max_ctas if > 0) persistent CTAs with `smem` bytes of
+// dynamic shared memory; W_hi / W_lo are the split row-major [w_rows, w_cols] weights the TMA streams.
 template <class Pol>
 static int launch(lnb_stream_t stream, const float* W_hi, const float* W_lo, int w_rows, int w_cols,
-                  size_t smem, int items, const typename Pol::Params& p, const char* who) {
+                  size_t smem, int items, const typename Pol::Params& p, const char* who,
+                  int max_ctas = 0) {
   CUtensorMap map_hi, map_lo;
   int rc = make_weight_map(&map_hi, W_hi, w_rows, w_cols, who);
   if (rc != LNB_OK) return rc;
@@ -622,7 +623,8 @@ static int launch(lnb_stream_t stream, const float* W_hi, const float* W_lo, int
               : skip == SKIP_TMA           ? tc_gemm_probe_kernel<Pol, SKIP_TMA>
                                            : tc_gemm_probe_kernel<Pol, SKIP_MMA | SKIP_TMA>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  const int grid = items < sm_count() ? items : sm_count();
+  int grid = items < sm_count() ? items : sm_count();
+  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
   kern<<<grid, THREADS, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
   lnb::count_launch();
   return lnb::finish_launch(who);

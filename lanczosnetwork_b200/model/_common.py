@@ -390,10 +390,20 @@ class SpectralNetBase(nn.Module):
       with torch.cuda.stream(side):
         table = ops.ritz_power_table(D, self.long_diffusion_dist)
       table.record_stream(cur)
-      gext = ctx.prep() if (mlp is not None and stack_ok and first == 0) else None
+      gext = ctx.prep(defer_tiles=True) if (mlp is not None and stack_ok and first == 0) else None
       cur.wait_stream(side)
+      ctas = 0
+      if gext is not None and gext.tiles_pending:
+        # the chain reads only the Ritz row list: the tile placement (one CTA) runs on the side
+        # stream beside it and is joined before the stack.  The chain gets one SM fewer, so none of
+        # its CTAs waits behind the placement's SM.
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+          ops.tile_assign(gext, K)
+        ctas = torch.cuda.get_device_properties(D.device).multi_processor_count - 1
       coeffs, table = ritz_filter_coefficients(D, self.long_diffusion_dist, mlp, self._wcache, gext,
-                                               table=table)
+                                               table=table, ctas=ctas)
+      cur.wait_stream(side)
 
     def layer_coeff(t):
       if S == 0:

@@ -90,7 +90,7 @@ class LanczosNet(SpectralNetBase):
     dense = not self._sparse_stack_ok(N, E1, K)
     prep, node_ids, mask, V, L = ops.graph_prepare_sparse(
         sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N, E1,
-        binarize=getattr(self, '_binarize_operators', False), want_dense=dense)
+        binarize=getattr(self, '_binarize_operators', False), want_dense=dense, defer_tiles=True)
     return self._ritz_conv_stack(None, node_ids, L, D.float().contiguous(), V, mask, prep=prep,
                                  dims_hint=(N, E1))
 

@@ -12,7 +12,7 @@ from . import _lib
 from ._lib import GemmDesc, SpectralStack
 
 __all__ = [
-    'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'spectral_conv_fused',
+    'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'tile_assign', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
@@ -182,16 +182,32 @@ def linear_tf32x3_grouped(x, w_hi, w_lo, bias, groups, relu=False):
 
 class GraphPrep(tuple):
   """(ell_val, ell_idx, ell_max, gext, tiles) plus the compact Ritz row list of the same pass
-  (attributes rowmap [B*K] int32, nrows [1] int32; see ritz_rowmap)."""
+  (attributes rowmap [B*K] int32, nrows [1] int32; see ritz_rowmap).  tiles_pending: built with
+  defer_tiles, ``tiles`` is written by tile_assign."""
   rowmap = None
   nrows = None
+  tiles_pending = False
 
 
-def graph_prepare(L, Q=None, binarize=False):
+def tile_assign(prep, K):
+  """Writes the tile table and schedule of a GraphPrep built with defer_tiles (lnb_tile_assign) on
+  the current stream; they equal what graph_prepare without defer_tiles writes."""
+  gext, tiles = prep[3], prep[4]
+  with torch.cuda.device(gext.device):
+    _lib.check(_lib.load().lnb_tile_assign(_stream(gext), _ptr(gext), gext.shape[0], int(K), _ptr(tiles)),
+               'lnb_tile_assign')
+  prep.tiles_pending = False
+
+
+PREP_DEFER_TILES = 4    # LNB_PREP_DEFER_TILES
+
+
+def graph_prepare(L, Q=None, binarize=False, defer_tiles=False):
   """Per-forward compression of the dense operators L [B,N,N,E1] (ELL rows), the real extents
   of every graph, the packed-tile assignment for the fused convolution kernel and the compact
   list of non-zero Ritz rows.  ``Q=None``: no Ritz vectors, an all-zero [B,N,4] block, so the
-  extents come from L alone.  Returns GraphPrep(ell_val, ell_idx, ell_max, gext, tiles)."""
+  extents come from L alone.  ``defer_tiles``: leave the tile assignment to tile_assign, which may
+  run on another stream.  Returns GraphPrep(ell_val, ell_idx, ell_max, gext, tiles)."""
   if Q is None:
     Q = torch.zeros((L.shape[0], L.shape[1], 4), device=L.device, dtype=torch.float32)
   _need_cuda(L, Q)
@@ -210,10 +226,10 @@ def graph_prepare(L, Q=None, binarize=False):
     _lib.check(_lib.load().lnb_graph_prepare(_stream(L), _ptr(L), _ptr(Q), B, N, E1, K,
                                              _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max),
                                              _ptr(gext), _ptr(tiles), _ptr(rowmap), _ptr(nrows),
-                                             1 if binarize else 0),
+                                             (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0)),
                'lnb_graph_prepare')
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
-  prep.rowmap, prep.nrows = rowmap, nrows
+  prep.rowmap, prep.nrows, prep.tiles_pending = rowmap, nrows, bool(defer_tiles) and B > 0
   return prep
 
 
@@ -235,8 +251,9 @@ def _inv_sqrt_deg_table(device):
 
 
 def graph_prepare_sparse(sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N, E1, binarize=False,
-                         want_dense=False):
-  """GPU-side batch construction from sparse records (see lnb_graph_prepare_sparse).
+                         want_dense=False, defer_tiles=False):
+  """GPU-side batch construction from sparse records (see lnb_graph_prepare_sparse); defer_tiles
+  as in graph_prepare.
   sizes [B] int32, node_ptr [B+1] int32, node_feat [>= node_ptr[B]] int32, edge_ptr [B+1] int32,
   edges [>= edge_ptr[B], 4] uint8, V_rows [>= node_ptr[B], K] fp32 -- all CUDA.
   Returns (GraphPrep, node_ids [B,N] int64, mask [B,N] uint8, V [B,N,K], L [B,N,N,E1] or None)."""
@@ -262,11 +279,12 @@ def graph_prepare_sparse(sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N,
     _lib.check(_lib.load().lnb_graph_prepare_sparse(
         _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(node_feat), _ptr(edge_ptr), _ptr(edges),
         _ptr(V_rows), _ptr(_inv_sqrt_deg_table(dev)), B, int(N), int(E1), int(K),
-        1 if binarize else 0, _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(gext), _ptr(tiles),
+        (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0), _ptr(ell_val), _ptr(ell_idx),
+        _ptr(ell_max), _ptr(gext), _ptr(tiles),
         _ptr(rowmap), _ptr(nrows), _ptr(node_ids), _ptr(mask), _ptr(V), _ptr(L)),
                'lnb_graph_prepare_sparse')
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
-  prep.rowmap, prep.nrows = rowmap, nrows
+  prep.rowmap, prep.nrows, prep.tiles_pending = rowmap, nrows, bool(defer_tiles) and B > 0
   return prep, node_ids, mask, V, L
 
 
@@ -505,20 +523,20 @@ def ritz_rowmap(gext, K):
   return rowmap, nrows
 
 
-def ritz_filter_mlp(table, w_hi, w_lo, bias_all, num_layers, rowmap=None, nrows=None):
+def ritz_filter_mlp(table, w_hi, w_lo, bias_all, num_layers, rowmap=None, nrows=None, ctas=0):
   """coeff[l, r, :] = MLP_l(table[r, :]) for all layers in one persistent kernel.
   table [R, S]; w_hi/w_lo [L*(3*Hd+S), Hd] stacked split weights; returns coeff [L, R, S]
-  (rows not listed in rowmap are left unwritten)."""
+  (rows not listed in rowmap are left unwritten).  ctas > 0 caps the persistent grid (same bits)."""
   _need_cuda(table, w_hi, w_lo, bias_all, rowmap, nrows)
   table = _f32c(table)
   R, S = table.shape
   Hd = w_hi.shape[1]
   coeff = torch.empty((num_layers, R, S), device=table.device, dtype=torch.float32)
   with torch.cuda.device(table.device):
-    _lib.check(_lib.load().lnb_ritz_filter_mlp(_stream(table), _ptr(table), _ptr(rowmap),
-                                               _ptr(nrows), _ptr(w_hi), _ptr(w_lo),
-                                               _ptr(bias_all), R, int(num_layers), S, Hd,
-                                               _ptr(coeff)), 'lnb_ritz_filter_mlp')
+    _lib.check(_lib.load().lnb_ritz_filter_mlp_ctas(_stream(table), _ptr(table), _ptr(rowmap),
+                                                    _ptr(nrows), _ptr(w_hi), _ptr(w_lo),
+                                                    _ptr(bias_all), R, int(num_layers), S, Hd,
+                                                    _ptr(coeff), int(ctas)), 'lnb_ritz_filter_mlp')
   return coeff
 
 

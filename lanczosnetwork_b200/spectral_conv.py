@@ -140,7 +140,7 @@ def dense(x2d, weight, bias, relu, cache, name):
   return out
 
 
-def ritz_filter_coefficients(D, powers, mlp_layers, cache, gext=None, table=None):
+def ritz_filter_coefficients(D, powers, mlp_layers, cache, gext=None, table=None, ctas=0):
   """Per-layer multi-scale coefficients of the Ritz values (model/lanczos_net.py:109-113,
   146-149).  The MLP input does not depend on the layer state, so the power table is built once
   and every MLP stage runs for ALL layers in one launch: stage 0 as a dense layer with the
@@ -165,7 +165,7 @@ def ritz_filter_coefficients(D, powers, mlp_layers, cache, gext=None, table=None
       rowmap, nrows = gext.rowmap, gext.nrows
     elif gext is not None:
       rowmap, nrows = ops.ritz_rowmap(gext, K)
-    coeff = ops.ritz_filter_mlp(flat, w_hi, w_lo, bias_all, nl, rowmap, nrows).reshape(nl, B, K, S)
+    coeff = ops.ritz_filter_mlp(flat, w_hi, w_lo, bias_all, nl, rowmap, nrows, ctas).reshape(nl, B, K, S)
     return coeff, table
   if S % 4 == 0 and hd % 4 == 0:
     h = flat
@@ -198,9 +198,13 @@ class GraphContext(object):
     self.binarize = binarize          # operators enter as their non-zero pattern (model/gcnfp.py:83)
     self._prep = None
 
-  def prep(self):
+  def prep(self, defer_tiles=False):
+    """defer_tiles: the caller launches ops.tile_assign itself; otherwise tiles pending from a
+    deferred prepare are assigned here, on the current stream."""
     if self._prep is None:
-      self._prep = ops.graph_prepare(self.L, self.Qv, self.binarize)
+      self._prep = ops.graph_prepare(self.L, self.Qv, self.binarize, defer_tiles)
+    elif getattr(self._prep, 'tiles_pending', False) and not defer_tiles:
+      ops.tile_assign(self._prep, self.Qv.shape[2])
     return self._prep
 
 
