@@ -560,6 +560,33 @@ int lnb_sym_eigs(lnb_stream_t stream, const float* A, int64_t elem_stride, const
                  int K, float* D /* [B,K] */, float* V /* [B,N,K] */, int32_t* status /* [B] */);
 
 /* ---------------------------------------------------------------------------------------
+ * GPNN's graph partition (utils/spectral_graph_partition.py:10-50 as the GPNN collate calls it per
+ * padded graph, dataset/qm8.py:123-136) in one launch.  Per graph b:
+ *   1. the operator: channel 0 of L read in place, L[((b*N + i)*N + j) * elem_stride].  The fp64 L4
+ *      s_i s_j of its off-diagonal non-zero pattern is rebuilt with inv_sqrt_deg [256] (deg = 1 + the
+ *      row's count; a node with a zero diagonal is padding and keeps a zero row); if its fp32 rounding
+ *      is channel 0 bit for bit that fp64 matrix is decomposed (the matrix the reference hands eigsh),
+ *      otherwise the widened fp32 values are and status bit 3 is set;
+ *   2. the P eigenvectors of largest |lambda| of the whole padded N x N (the solver of lnb_sym_eigs);
+ *      bit 1 when |lambda_P| and |lambda_P+1| are within 1e-9 (the reference's choice is then open);
+ *   3. KMeans(n_clusters=P, random_state=seed) as scikit-learn >= 1.4 runs it, in fp64: centring,
+ *      k-means++ with T = 2 + floor(ln P) local trials, Lloyd up to 300 iterations (bit 2 when they run
+ *      out).  draws [lnb_spectral_partition_draws(P)] are the RandomState(seed) draws the seeding makes:
+ *      draws[0] = choice(N, p=ones(N)/N), then uniform(size=T) per further centre;
+ *   4. outputs: labels [B,N] int32 canonical (no edge: -1, the other clusters numbered by first
+ *      appearance); L_cluster, L_cut [B,N,N] fp32 = the fp64 L4 of the within-cluster and of the cut
+ *      part of the pattern (every node keeps its unit self-loop), bit for bit data.partition_operators.
+ * status [B]: bit 0 = QL sweeps exhausted, bits 1-3 as above.  One warp per graph for N <= 32, one CTA
+ * above; repeated launches are bit-identical; no allocation, no synchronisation (capturable).
+ * Envelope: 1 <= N <= 128, 2 <= P <= 16, P < N (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ * lnb_spectral_partition_draws: the draw count for P, 0 outside 2 <= P <= 16.
+ * ------------------------------------------------------------------------------------- */
+int lnb_spectral_partition_draws(int P);
+int lnb_spectral_partition(lnb_stream_t stream, const float* L, int64_t elem_stride, int B, int N, int P,
+                           const double* inv_sqrt_deg /* [256] */, const double* draws, int32_t* labels /* [B,N] */,
+                           float* L_cluster /* [B,N,N] */, float* L_cut /* [B,N,N] */, int32_t* status /* [B] */);
+
+/* ---------------------------------------------------------------------------------------
  * The north-star pipeline in ONE launch: operator -> K-step Lanczos (rules of
  * model/ada_lanczos_net.py:139-247, as lnb_lanczos_tridiag) -> implicit-shift QL on (alpha, beta)
  * -> Ritz vectors V = Q S ordered by descending |theta| (utils/data_helper.py:217-223) -- the pair

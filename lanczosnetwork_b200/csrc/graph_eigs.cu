@@ -1,31 +1,22 @@
 // Exact eigenpairs of one small symmetric operator per graph, in fp64: the reference's offline
 // preprocessing (utils/data_helper.py:169-226 dense eigh branch, called from
 // dataset/get_qm8_data.py:63-83 and truncated / zero padded to K at collate, dataset/qm8.py:265-291)
-// on the device.
-//
-//   1. Householder tridiagonalisation of the leading n x n block (lower triangle, packed in shared
-//      memory; the reflectors overwrite the columns they annihilate, as LAPACK's dsptrd does),
-//   2. implicit-shift QL on the tridiagonal with the rotations accumulated into Z (the pattern of
-//      tridiag_ritz_kernel, in fp64),
-//   3. the reference's ordering: descending |lambda|, ties by ascending lambda (np.argsort(-|w|,
-//      kind='mergesort') over eigh's ascending order), then the first min(n, K),
-//   4. the back-transform Q Z of only those columns, one rounding to fp32 on the way out.
+// on the device.  The solver's stages (Householder, QL, the reference's order, the back-transform of the
+// first min(n, K) columns) are the device routines of graph_eigs.cuh; this file builds the operator and
+// rounds the kept pairs to fp32 on the way out.
 //
 // Work unit: one warp per graph for N <= 32 (four graphs per CTA), one 128-thread CTA per graph
 // above; a thread owns one row of A and of Z.  Every reduction has a fixed order: repeated launches
 // are bit-identical.  Eigenvectors are determined up to sign (and up to a rotation inside a repeated
 // eigenvalue's eigenspace), which no consumer sees: they read V diag(g(D)) V^T.
-#include <float.h>
-
-#include "common.cuh"
+#include "graph_eigs.cuh"
 
 namespace {
 
-constexpr int GE_THREADS = 128;
-constexpr int GE_NMAX = 128;     // same limit as lnb_graph_prepare_sparse
+using namespace eigs;
+
 constexpr int GE_KMAX = 128;
 constexpr int GE_EMAX = 32;      // bond types of the sparse producer (one bit each)
-constexpr int GE_SWEEPS = 60;    // QL sweeps per eigenvalue before status bit 0 is set
 
 struct EigParams {
   // dense producer: A[((b * N + i) * N + j) * es], lower triangle read (eigh's default UPLO='L')
@@ -37,41 +28,6 @@ struct EigParams {
   int B, N, K;
   float* D; float* V; int32_t* status;     // V: [B,N,K] (dense) or [node_ptr[B],K] rows (sparse)
 };
-
-// packed lower triangle, row-major: element (i, j), i >= j
-__device__ __forceinline__ int tri(int i, int j) { return i * (i + 1) / 2 + j; }
-
-__host__ __device__ constexpr int tri_doubles(int N) { return (N * (N + 1) / 2 + 1) & ~1; }
-
-// per graph: packed A, Z [N][N|1], (d, e) per warp, tau / sub / v / w / scale, reduction slots, perm
-__host__ __device__ constexpr size_t graph_doubles(int N, int W) {
-  return (size_t)tri_doubles(N) + (size_t)N * (N | 1) + (size_t)W * 2 * N + 5 * (size_t)N + 8 + (N + 1) / 2;
-}
-
-template <int W>
-__device__ __forceinline__ void gsync() {
-  if (W == 1) __syncwarp(); else __syncthreads();
-}
-
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// sum over the graph's threads in a fixed order (every thread gets the same bits)
-template <int W>
-__device__ __forceinline__ double group_sum(double v, double* red) {
-  v = warp_sum_d(v);
-  if (W == 1) return v;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = red[0];
-#pragma unroll
-  for (int w = 1; w < W; ++w) s += red[w];
-  return s;
-}
 
 template <int W, bool SPARSE>
 __global__ void __launch_bounds__(GE_THREADS)
@@ -85,17 +41,10 @@ graph_eigs_kernel(const EigParams P) {
   const int N = P.N, K = P.K, ZS = N | 1;
   const int b = blockIdx.x * GPC + grp;
 
-  double* Ap = ge_smem + (size_t)grp * graph_doubles(N, W);
-  double* Z = Ap + tri_doubles(N);
-  double* dq = Z + (size_t)N * ZS + (size_t)wg * 2 * N;   // this warp's private (d, e) of the QL
-  double* eq = dq + N;
-  double* taus = Z + (size_t)N * ZS + (size_t)W * 2 * N;
-  double* sub = taus + N;                     // subdiagonal of the tridiagonal
-  double* hv = sub + N;                      // current reflector v (v[j+1] = 1)
-  double* hw = hv + N;                        // w = p - (tau/2)(p.v) v
-  double* sc = hw + N;                        // deg^-1/2 (sparse producer)
-  double* red = sc + N;
-  int* perm = reinterpret_cast<int*>(red + 8);   // perm[r] = column of Z holding the r-th pair
+  const Work w(ge_smem + (size_t)grp * graph_doubles(N, W), N, W, wg);
+  double* Ap = w.Ap();
+  double* Z = w.Z();
+  double* sc = w.sc();
   if (b >= P.B) return;                       // whole groups only: a CTA-wide group has b < B
 
   const int n = min(max(P.sizes[b], 0), N);
@@ -139,143 +88,13 @@ graph_eigs_kernel(const EigParams P) {
   }
   gsync<W>();
 
-  // ---- Householder tridiagonalisation: column j's reflector maps A[j+2:, j] to zero ----------------
-  for (int j = 0; j + 2 < n; ++j) {
-    const double xi = (t > j + 1 && t < n) ? Ap[tri(t, j)] : 0.0;
-    const double sigma = group_sum<W>(xi * xi, red);
-    const double alpha = Ap[tri(j + 1, j)];
-    if (sigma == 0.0) {                         // already reduced: H = I
-      if (t == 0) { taus[j] = 0.0; sub[j] = alpha; }
-      gsync<W>();
-      continue;
-    }
-    const double beta = -copysign(sqrt(alpha * alpha + sigma), alpha);
-    const double tau = (beta - alpha) / beta;
-    const double scal = 1.0 / (alpha - beta);
-    const double vi = (t == j + 1) ? 1.0 : xi * scal;
-    if (t < n) hv[t] = (t > j) ? vi : 0.0;
-    gsync<W>();
-    // p = tau A22 v over the trailing block; row t reads its own row left of the diagonal and its
-    // column below it
-    double p = 0.0;
-    if (t > j && t < n) {
-      for (int k = j + 1; k <= t; ++k) p = fma(Ap[tri(t, k)], hv[k], p);
-      for (int k = t + 1; k < n; ++k) p = fma(Ap[tri(k, t)], hv[k], p);
-      p *= tau;
-    }
-    const double pv = group_sum<W>(p * ((t > j && t < n) ? vi : 0.0), red);
-    const double wi = p - 0.5 * tau * pv * vi;
-    if (t > j && t < n) hw[t] = wi;
-    gsync<W>();
-    if (t > j && t < n) {
-      for (int k = j + 1; k <= t; ++k) Ap[tri(t, k)] -= vi * hw[k] + wi * hv[k];
-      if (t > j + 1) Ap[tri(t, j)] = vi;        // keep the reflector where x was
-    }
-    if (t == 0) { taus[j] = tau; sub[j] = beta; }
-    gsync<W>();
-  }
-
-  // ---- tridiagonal (d, e) into every warp's private copy; Z = I ----------------------------------
-  for (int i = lane; i < n; i += 32) {
-    dq[i] = Ap[tri(i, i)];
-    eq[i] = (i + 2 < n) ? sub[i] : (i + 1 < n ? Ap[tri(i + 1, i)] : 0.0);
-  }
-  gsync<W>();
-  if (t < n)
-    for (int k = 0; k < n; ++k) Z[(size_t)t * ZS + k] = (t == k) ? 1.0 : 0.0;
-  gsync<W>();
-
-  // ---- implicit-shift QL; every warp carries the scalar recurrence, thread t rotates row t of Z ----
-  // an off-diagonal splits below eps * ||T|| (EISPACK tql2's test), not below eps * (|d_m| + |d_m+1|):
-  // where a whole eigenspace sits at the rounding level (the complete graph's eigenvalue 0, n - 1 times)
-  // the pairwise test never fires.  Eigenvalues stay within eps * ||T|| of exact.
-  double tnorm = 0.0;
-  for (int i = lane; i < n; i += 32) tnorm = fmax(tnorm, fabs(dq[i]) + fabs(eq[i]) + (i ? fabs(eq[i - 1]) : 0.0));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) tnorm = fmax(tnorm, __shfl_xor_sync(0xffffffffu, tnorm, o));
-  const double etol = DBL_EPSILON * tnorm;
-  int fail = 0;
-  for (int l = 0; l < n; ++l) {
-    int sweeps = 0;
-    while (true) {
-      int m = l;
-      for (; m < n - 1; ++m)
-        if (fabs(eq[m]) <= etol) break;
-      if (m == l) break;
-      if (++sweeps > GE_SWEEPS) { fail = 1; break; }
-      double g = (dq[l + 1] - dq[l]) / (2.0 * eq[l]);
-      double r = sqrt(g * g + 1.0);
-      g = dq[m] - dq[l] + eq[l] / (g + copysign(r, g));
-      double s = 1.0, c = 1.0, p = 0.0;
-      bool underflow = false;
-      for (int i = m - 1; i >= l; --i) {
-        // every lane carries the recurrence; lane 0 alone stores, after all lanes have read this row
-        const double ei = eq[i], di1 = dq[i + 1], di = dq[i];
-        __syncwarp();
-        const double f = s * ei;
-        const double bb = c * ei;
-        r = sqrt(f * f + g * g);
-        if (r == 0.0) {
-          if (lane == 0) { eq[i + 1] = r; dq[i + 1] = di1 - p; eq[m] = 0.0; }
-          underflow = true;
-          break;
-        }
-        const double ir = 1.0 / r;
-        s = f * ir;
-        c = g * ir;
-        g = di1 - p;
-        const double rr = (di - g) * s + 2.0 * c * bb;
-        p = s * rr;
-        if (lane == 0) { eq[i + 1] = r; dq[i + 1] = g + p; }
-        g = c * rr - bb;
-        if (t < n) {
-          double* zr = Z + (size_t)t * ZS;
-          const double z1 = zr[i + 1], z0 = zr[i];
-          zr[i + 1] = s * z0 + c * z1;
-          zr[i] = c * z0 - s * z1;
-        }
-      }
-      if (!underflow) {
-        const double dl = dq[l];
-        __syncwarp();
-        if (lane == 0) { dq[l] = dl - p; eq[l] = g; eq[m] = 0.0; }
-      }
-      __syncwarp();
-    }
-    if (fail) break;
-  }
-  gsync<W>();
-
-  // ---- the reference's order: descending |lambda|, then ascending lambda, then index --------------
+  tridiagonalize<W>(w, n, t);
+  const int fail = tridiag_ql<W>(w, n, t, lane);
   const int kk = min(n, K);
-  const double* d0 = Z + (size_t)N * ZS;         // warp 0's eigenvalues (all copies are identical)
-  for (int r = t; r < kk; r += GT) perm[r] = r;  // only a NaN operator leaves a rank unfilled
-  gsync<W>();
-  for (int j = t; j < n; j += GT) {
-    const double dj = d0[j], aj = fabs(dj);
-    int rank = 0;
-    for (int i = 0; i < n; ++i) {
-      const double di = d0[i], ai = fabs(di);
-      rank += ((ai > aj) || (ai == aj && (di < dj || (di == dj && i < j)))) ? 1 : 0;
-    }
-    if (rank < kk) perm[rank] = j;
-  }
-  gsync<W>();
-
-  // ---- back-transform of the kept columns only: z <- H_0 ... H_{n-3} z ----------------------------
-  for (int r = t; r < kk; r += GT) {
-    const int col = perm[r];
-    for (int j = n - 3; j >= 0; --j) {
-      const double tau = taus[j];
-      if (tau == 0.0) continue;
-      double s = Z[(size_t)(j + 1) * ZS + col];
-      for (int i = j + 2; i < n; ++i) s = fma(Ap[tri(i, j)], Z[(size_t)i * ZS + col], s);
-      s *= tau;
-      Z[(size_t)(j + 1) * ZS + col] -= s;
-      for (int i = j + 2; i < n; ++i) Z[(size_t)i * ZS + col] -= s * Ap[tri(i, j)];
-    }
-  }
-  gsync<W>();
+  order_pairs<W>(w, n, kk, t);
+  back_transform<W>(w, n, kk, t);
+  const double* d0 = w.d0();
+  const int* perm = w.perm();
 
   // ---- fp32 outputs, zero padded ----------------------------------------------------------------
   for (int r = t; r < K; r += GT) P.D[(int64_t)b * K + r] = (r < kk) ? __double2float_rn(d0[perm[r]]) : 0.f;

@@ -1,6 +1,7 @@
 """Install the H100 drop-ins into an UNMODIFIED checkout of lrjconan/LanczosNetwork.
 
     python -m lanczosnetwork_b200.dropin /path/to/LanczosNetwork -c config/qm8_lanczos_net.yaml -t
+    python -m lanczosnetwork_b200.dropin /path/to/LanczosNetwork -c config/qm8_gpnn.yaml --device-partition
 
 What it does (see INTEGRATION.md):
   1. registers ``operators._ext`` / ``operators._ext.segment_reduction`` in ``sys.modules`` so
@@ -13,11 +14,18 @@ What it does (see INTEGRATION.md):
      (``TRAINING_OPT_IN_CLASSES``) binds ``TrainableGAT`` under the name ``GAT``, and ``--opt-in GraphSAGE``
      (``LSTM_OPT_IN_CLASSES``) binds ``LSTMGraphSAGE`` (which takes ``agg_func: LSTM``) under the name
      ``GraphSAGE``, for training and test runs;
-  3. runs the reference ``run_exp.main()`` unchanged (``--opt-in`` is removed from its argv).
+  3. with ``--device-partition`` (``install(..., device_partition=True)``), rebinds ``spectral_clustering``
+     and ``get_L_cluster_cut`` in the dataset modules' globals (``DATASET_MODULES``) to stand-ins, so the GPNN
+     collate never runs scikit-learn and ships empty [B,0,0] partition operators; the GPNN drop-in then
+     partitions every batch on the device (``ops.spectral_partition``);
+  4. runs the reference ``run_exp.main()`` unchanged (``--opt-in`` and ``--device-partition`` are removed
+     from its argv).
 """
 import importlib
 import os
 import sys
+
+import numpy as np
 
 from . import model as _models
 from .operators import _ext as _ext_pkg
@@ -32,6 +40,8 @@ TRAINING_OPT_IN_CLASSES = ('GAT',)
 # names whose drop-in becomes the subclass that also takes the LSTM aggregator, ``LSTM<name>``, when asked for
 # (opt_in=..., --opt-in), for training and test runs; without the opt-in an LSTM config fails in the constructor
 LSTM_OPT_IN_CLASSES = ('GraphSAGE',)
+# modules whose GPNN collate calls the host partition (dataset/qm8.py:123-136, dataset/graph_data.py)
+DATASET_MODULES = ('dataset.qm8', 'dataset.graph_data')
 
 
 def register_native_op():
@@ -75,14 +85,33 @@ def patch_namespace(module, training=False, opt_in=()):
   return module
 
 
+def _skip_spectral_clustering(L, K, seed=1234):
+  """Stand-in for the collate's spectral_clustering: the partition runs on the device."""
+  return np.zeros(L.shape[0], dtype=np.int32)
+
+
+def _skip_cluster_cut(L, node_label):
+  """Stand-in for the collate's get_L_cluster_cut: empty operators, stacked to [B,0,0] by the collate."""
+  empty = np.zeros((0, 0), dtype=np.float32)
+  return empty, empty.copy()
+
+
+def patch_partition(module):
+  """Rebind ``spectral_clustering`` / ``get_L_cluster_cut`` in ``module``'s globals to the stand-ins."""
+  module.spectral_clustering = _skip_spectral_clustering
+  module.get_L_cluster_cut = _skip_cluster_cut
+  return module
+
+
 def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.graph_runner'),
-            compat=False, training=False, opt_in=()):
+            compat=False, training=False, opt_in=(), device_partition=False):
   """Returns the list of patched modules.  ``reference_root`` is put on sys.path if given.
   ``compat=True`` first installs the shims of ``lanczosnetwork_b200.compat`` (missing easydict /
   tensorboardX, PyYAML >= 6, numpy >= 2) so the 2019 checkout imports under a current stack.
   Raises ImportError when NO runner module could be imported and patched: the runners resolve
   the model class by name in their own namespace, so a silent miss would run the reference's
-  classes while claiming the drop-in.  ``opt_in``: see patch_namespace."""
+  classes while claiming the drop-in.  ``opt_in``: see patch_namespace.  ``device_partition``: see patch_partition (the GPNN collate ships
+  [B,0,0] operators and the GPNN drop-in partitions on the device)."""
   opt_in = _check_opt_in(opt_in)
   if compat:
     from . import compat as _compat
@@ -107,6 +136,9 @@ def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.gr
     raise ImportError('dropin.install: no runner module could be imported, nothing would call the '
                       'H100 classes (%s); pass compat=True for the shims of '
                       'lanczosnetwork_b200.compat' % '; '.join(errors))
+  if device_partition:
+    for name in DATASET_MODULES:
+      patched.append(patch_partition(importlib.import_module(name)))
   return patched
 
 
@@ -123,7 +155,10 @@ def main(argv=None):
                        % (OPT_IN_CLASSES + TRAINING_OPT_IN_CLASSES + LSTM_OPT_IN_CLASSES,))
     opt_in.append(argv[i + 1])
     del argv[i:i + 2]
-  install(root, compat=True, training=('-t' not in argv and '--test' not in argv), opt_in=opt_in)
+  device_partition = '--device-partition' in argv
+  argv = [a for a in argv if a != '--device-partition']
+  install(root, compat=True, training=('-t' not in argv and '--test' not in argv), opt_in=opt_in,
+          device_partition=device_partition)
   os.chdir(root)
   sys.argv = ['run_exp.py'] + argv
   run_exp = importlib.import_module('run_exp')

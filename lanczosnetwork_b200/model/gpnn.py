@@ -25,7 +25,11 @@ Differences from the reference, on purpose:
     their values, as in the reference;
   * ``update_func: MLP`` builds the same parameters as the reference, and the forward raises the
     reference's ``TypeError`` (nn.Sequential called with two arguments, :210) before touching the device;
-  * the GRU gate pre-activations are one dot product over [messages | h] plus b_ih + b_hh.
+  * the GRU gate pre-activations are one dot product over [messages | h] plus b_ih + b_hh;
+  * ``L_cluster`` and ``L_cut`` may be left out (``None``, or both empty ``[B,0,0]`` tensors): the module
+    then partitions every graph on the device (ops.spectral_partition, the collate's spectral clustering
+    with ``num_partition`` clusters) inside its captured forward; on the training path the operators are
+    constants, as the collate's are.
 ``update_func: RNN`` (relu RNNCell), shapes outside the kernels and ``input_dim % 4 != 0`` run the
 training formulation of lanczosnetwork_b200.train under no_grad."""
 import torch
@@ -92,11 +96,12 @@ class GPNN(SpectralNetBase):
   def _param_device(self):
     return self.embedding.weight.device
 
-  def forward(self, node_feat, L, L_cluster, L_cut, label=None, mask=None):
+  def forward(self, node_feat, L, L_cluster=None, L_cut=None, label=None, mask=None):
     """
       node_feat: long B x N (atom ids); L: float B x N x N x (E+1) operators (only their non-zero
       pattern is read; L is not modified); L_cluster, L_cut: float B x N x N partition operators (their
-      values are read); label: B x P; mask: B x N (uint8 / bool / float).
+      values are read), or both None / empty (B x 0 x 0): partitioned on the device from channel 0 of L;
+      label: B x P; mask: B x N (uint8 / bool / float).
       Returns score (B x P) or (score, loss).
     """
     if self.update_func_name == 'MLP':
@@ -105,10 +110,23 @@ class GPNN(SpectralNetBase):
     if self.msg_func is None:
       raise UnboundLocalError("msg_func %r: the reference's propagation reads a message that is never "
                               "assigned (model/gpnn.py:193-200); only 'MLP' runs" % self.config.model.msg_func)
+    absent = [t is None or t.numel() == 0 for t in (L_cluster, L_cut)]
+    if any(absent):
+      if not all(absent):
+        raise ValueError('GPNN.forward: pass both L_cluster and L_cut, or neither (device partition)')
+      L_cluster = L_cut = None
     return self._forward((node_feat, L, L_cluster, L_cut, mask), label)
+
+  def _device_partition(self, L):
+    """(L_cluster, L_cut) of the collate's spectral clustering, computed on the device."""
+    _, L_cluster, L_cut, _ = ops.spectral_partition(L, self.num_partition)
+    return L_cluster, L_cut
 
   def _train_impl(self, node_feat, L, L_cluster, L_cut, mask):
     from ..train import gpnn_train
+    if L_cluster is None:
+      with torch.no_grad():                    # constants, as the collate's operators are
+        L_cluster, L_cut = self._device_partition(L)
     return gpnn_train(self, node_feat, L, L_cluster, L_cut, mask)
 
   def fused_supported(self, N, E1):
@@ -168,6 +186,8 @@ class GPNN(SpectralNetBase):
     E1 = L.shape[3]
     if not self.fused_supported(N, E1):
       return self._train_impl(node_feat, L, L_cluster, L_cut, mask)   # RNN update / other shapes
+    if L_cluster is None:
+      L_cluster, L_cut = self._device_partition(L)
     H = self.hidden_dim
     h = embed_input(self, node_feat, self.embedding.weight)
     # ELL rows of the 0/1 operators and of the valued partition operators; no Ritz vectors, one zero

@@ -14,6 +14,7 @@ from ._lib import GemmDesc, SpectralStack
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'tile_assign', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
+    'spectral_partition', 'partition_draws',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
     'sage_operators', 'neighbour_max', 'sage_lstm_step', 'sage_lstm_step_supported', 'sage_lstm_messages',
@@ -369,6 +370,74 @@ def sym_eigs(A, sizes, K):
     _lib.check(_lib.load().lnb_sym_eigs(_stream(A), _ptr(A), int(es), _ptr(sizes), B, N, int(K), _ptr(D), _ptr(V),
                                         _ptr(status)), 'lnb_sym_eigs')
   return D, V, status
+
+
+PARTITION_MAX_N = 128
+PARTITION_P_RANGE = (2, 16)
+
+
+def partition_draws(N, P, seed=1234):
+  """The draws scikit-learn's k-means++ seeding takes from a fresh ``RandomState(seed)`` for N points and
+  P clusters, as one fp64 numpy array: ``choice(N, p=ones(N)/N)``, then ``uniform(size=2 + int(log P))``
+  per further centre.  They depend on (N, P, seed) only."""
+  import numpy as np
+  rs = np.random.RandomState(seed)
+  T = 2 + int(np.log(P))
+  out = [float(rs.choice(N, p=np.ones(N) / N))]
+  for _ in range(P - 1):
+    out.extend(rs.uniform(size=T).tolist())
+  return np.asarray(out, dtype=np.float64)
+
+
+_PARTITION_DRAWS = {}
+
+
+def _partition_draws_table(device, N, P, seed):
+  """partition_draws on ``device``, cached per (device, N, P, seed); the first call for a key copies the
+  table from the host, so it has to happen outside a CUDA-graph capture (a model's warm-up run does)."""
+  key = (device.index if device.index is not None else torch.cuda.current_device(), int(N), int(P), int(seed))
+  if key not in _PARTITION_DRAWS:
+    if torch.cuda.is_current_stream_capturing():
+      raise RuntimeError('spectral_partition: the k-means++ draw table for N=%d, P=%d, seed=%d is built on '
+                         'the host; call spectral_partition once outside the capture' % (N, P, seed))
+    _PARTITION_DRAWS[key] = torch.from_numpy(partition_draws(N, P, seed)).to(device)
+  return _PARTITION_DRAWS[key]
+
+
+def spectral_partition(L, num_partition, seed=1234):
+  """GPNN's graph partition of every padded graph on the device (lnb_spectral_partition): the reference's
+  ``spectral_clustering(L, num_partition, seed)`` (the P eigenvectors of largest |lambda| of the whole padded
+  simple-graph operator, then KMeans as scikit-learn >= 1.4 runs it) and ``get_L_cluster_cut``.
+  L: [B,N,N,E1] (channel 0 is read in place) or [B,N,N], float32, CUDA.
+  Returns (labels [B,N] int32 canonical: -1 for nodes without an edge, the other clusters numbered by
+  first appearance; L_cluster [B,N,N]; L_cut [B,N,N]; status [B] int32: bit 0 QL sweeps exhausted, bit 1
+  |lambda| tie at the cut, bit 2 Lloyd reached 300 iterations, bit 3 operator not an unweighted L4)."""
+  if L.dim() not in (3, 4) or L.shape[1] != L.shape[2]:
+    raise ValueError('spectral_partition: L must be [B,N,N] or [B,N,N,E1]; got %s' % (tuple(L.shape),))
+  P, N = int(num_partition), int(L.shape[1])
+  assert P < N - 1, 'spectral_partition: num_partition=%d needs more than %d nodes (N=%d)' % (P, P + 1, N)
+  if not (PARTITION_P_RANGE[0] <= P <= PARTITION_P_RANGE[1]) or N > PARTITION_MAX_N:
+    raise ValueError('spectral_partition: N=%d, num_partition=%d outside N <= %d, %d <= num_partition <= %d'
+                     % ((N, P, PARTITION_MAX_N) + PARTITION_P_RANGE))
+  _need_cuda(L)
+  A = L[..., 0] if L.dim() == 4 else L
+  if A.dtype != torch.float32:
+    A = A.float()
+  B = A.shape[0]
+  es = A.stride(2)
+  if es < 1 or tuple(A.stride()) != (N * N * es, N * es, es):
+    A, es = A.contiguous(), 1
+  dev = A.device
+  labels = torch.empty((B, N), device=dev, dtype=torch.int32)
+  L_cluster = torch.empty((B, N, N), device=dev, dtype=torch.float32)
+  L_cut = torch.empty((B, N, N), device=dev, dtype=torch.float32)
+  status = torch.empty((B,), device=dev, dtype=torch.int32)
+  with torch.cuda.device(dev):
+    draws = _partition_draws_table(dev, N, P, seed)
+    _lib.check(_lib.load().lnb_spectral_partition(
+        _stream(A), _ptr(A), int(es), B, N, P, _ptr(_inv_sqrt_deg_table(dev)), _ptr(draws), _ptr(labels),
+        _ptr(L_cluster), _ptr(L_cut), _ptr(status)), 'lnb_spectral_partition')
+  return labels, L_cluster, L_cut, status
 
 
 def fused_conv_supported(N, Din, K, H, n_short, dense_filter, S=8, E1=7):

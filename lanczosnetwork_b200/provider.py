@@ -22,12 +22,15 @@ MAE": K Lanczos steps from one start vector span a Krylov space, so
 (lnb_sym_eigs) that reproduces the reference's preprocessing itself -- every eigenpair, the top K by
 |lambda| in the reference's order -- so a checkpoint trained on the reference's inputs sees the same
 inputs.
+
+``spectral_partition`` is GPNN's graph partition (the collate's spectral clustering and partition
+operators) for loaders that hand the model its operators themselves.
 """
 import torch
 
 from . import ops
 
-__all__ = ['online_ritz_pairs', 'exact_eigenpairs']
+__all__ = ['online_ritz_pairs', 'exact_eigenpairs', 'spectral_partition']
 
 
 def online_ritz_pairs(L, mask, num_eigs, q1=None, generator=None):
@@ -65,3 +68,18 @@ def exact_eigenpairs(L, sizes_or_mask, num_eigs):
     s = (s != 0).sum(dim=1)
   D, V, status = ops.sym_eigs(L, s.to(L.device), int(num_eigs))
   return D, V, {'status': status}
+
+
+def spectral_partition(L, num_partition):
+  """(L_cluster [B,N,N], L_cut [B,N,N], info) for ``GPNN.forward(node_feat, L, L_cluster, L_cut)`` from the
+  padded operator tensor L [B,N,N,E+1] (channel 0 is read) or a [B,N,N] operator, on L's device.
+
+  The reference's GPNN collate (dataset/qm8.py:123-136) as one kernel launch: the P = num_partition
+  eigenvectors of largest |lambda| of each padded graph's operator, KMeans(n_clusters=P, random_state=1234)
+  as scikit-learn >= 1.4 runs it (one k-means++ seeding), then the L4 operators of the within-cluster and
+  the cut edges.  The partitions equal the reference's except where the reference itself is undetermined
+  (an eigenvalue tie at the P-th |lambda|, flagged in status bit 1, or KMeans ties).  ``GPNN.forward``
+  with ``L_cluster=L_cut=None`` runs the same launch inside its captured forward.
+  info: dict(labels [B,N] int32 canonical (-1: no edge), status [B] int32, see ops.spectral_partition)."""
+  labels, L_cluster, L_cut, status = ops.spectral_partition(L, int(num_partition))
+  return L_cluster, L_cut, {'labels': labels, 'status': status}
