@@ -586,6 +586,29 @@ int lnb_spectral_partition(lnb_stream_t stream, const float* L, int64_t elem_str
                            const double* inv_sqrt_deg /* [256] */, const double* draws, int32_t* labels /* [B,N] */,
                            float* L_cluster /* [B,N,N] */, float* L_cut /* [B,N,N] */, int32_t* status /* [B] */);
 
+/* GPNN's graph partition from the sparse records of lnb_graph_prepare_sparse (sizes, edge_ptr, edges;
+ * bond types >= E are ignored, E <= 32): steps 2-3 of lnb_spectral_partition on the fp64 L4 that
+ * lnb_graph_eigs_sparse builds (padded rows zero, as the dense entry sees the collated channel 0), so
+ * labels and status equal lnb_spectral_partition's on the collated L wherever no node pair carries two
+ * bond types (status bit 3 is never set).  Outputs: labels, status, and the ELL rows of the two-channel
+ * operator [L_cluster, L_cut] (ell_val / ell_idx [B,2,N,N], ell_max [B,2], gext [B,2] = {N, 0}) in the
+ * layout and slot order of lnb_graph_prepare over stack([L_cluster, L_cut], 3) with a zero Q, so
+ * lnb_gpnn_partition_update reads them as they are; L_cluster / L_cut [B,N,N] when not NULL (both or
+ * neither).  Same envelope as lnb_spectral_partition (and 1 <= E <= 32); capturable, no allocation. */
+int lnb_spectral_partition_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr,
+                                  const uint8_t* edges, const double* inv_sqrt_deg, int B, int N, int E, int P,
+                                  const double* draws, int32_t* labels /* [B,N] */, int32_t* status /* [B] */,
+                                  float* ell_val, uint8_t* ell_idx, int32_t* ell_max, int32_t* gext,
+                                  float* L_cluster /* [B,N,N] or NULL */, float* L_cut /* [B,N,N] or NULL */);
+
+/* GAT's additive attention bias [B,N,N,E1] fp32 from the sparse records (sizes, edge_ptr, edges of
+ * lnb_graph_prepare_sparse): bit for bit data.gat_bias of the collated operators, i.e. -0.0 (sign
+ * included) on the diagonal of every node (padded ones too) and on every bond of the channel (channel 0:
+ * any bond type < E1 - 1, channel e: type e - 1), -1e9 elsewhere.  Envelope: 1 <= N <= 128,
+ * 2 <= E1 <= 16 (LNB_ERR_UNSUPPORTED otherwise, nothing launched). */
+int lnb_gat_bias_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr, const uint8_t* edges,
+                        int B, int N, int E1, float* bias /* [B,N,N,E1] */);
+
 /* ---------------------------------------------------------------------------------------
  * The north-star pipeline in ONE launch: operator -> K-step Lanczos (rules of
  * model/ada_lanczos_net.py:139-247, as lnb_lanczos_tridiag) -> implicit-shift QL on (alpha, beta)

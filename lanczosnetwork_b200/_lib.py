@@ -132,6 +132,9 @@ SIGNATURES = {
                              ctypes.c_void_p]),
     'lnb_spectral_partition_draws': (c_int, [c_int]),
     'lnb_spectral_partition': (c_int, [c_stream, c_f32p, c_i64, c_int, c_int, c_int] + [ctypes.c_void_p] * 6),
+    'lnb_spectral_partition_sparse': (c_int, [c_stream] + [ctypes.c_void_p] * 4 + [c_int] * 4 +
+                                      [ctypes.c_void_p] * 9),
+    'lnb_gat_bias_sparse': (c_int, [c_stream] + [ctypes.c_void_p] * 3 + [c_int] * 3 + [ctypes.c_void_p]),
     'lnb_tridiag_powers':(c_int, [c_stream, c_f32p, c_int, c_int, ctypes.POINTER(c_int), c_int,
                                    c_f32p]),
     'lnb_symmetrize_filters': (c_int, [c_stream, c_f32p, c_int, c_int, c_int, c_f32p]),

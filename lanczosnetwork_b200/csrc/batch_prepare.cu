@@ -193,6 +193,34 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
   }
 }
 
+// GAT's additive attention bias (data.gat_bias of the collated operators) from the bond lists: -0.0 on the
+// diagonal (padded nodes included) and on every bond of the channel (channel 0: any bond type < E), -1e9
+// elsewhere.  One CTA per graph: the fill, then the bonds overwrite their entries.
+__global__ void __launch_bounds__(BP_THREADS)
+gat_bias_sparse_kernel(const int32_t* __restrict__ sizes, const int32_t* __restrict__ edge_ptr,
+                       const uint8_t* __restrict__ edges, int N, int E1, float* __restrict__ out) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int nb = min(max(sizes[b], 0), N);
+  float* ob = out + (int64_t)b * N * N * E1;
+  const int total = N * N * E1;
+  for (int i = tid; i < total; i += BP_THREADS) {
+    const int ij = i / E1, r = ij / N, c = ij - r * N;
+    ob[i] = r == c ? -0.0f : -1e9f;
+  }
+  __syncthreads();
+  const int e0 = edge_ptr[b], e1 = edge_ptr[b + 1];
+  for (int e = e0 + tid; e < e1; e += BP_THREADS) {
+    const uchar4 ed = reinterpret_cast<const uchar4*>(edges)[e];
+    const int u = ed.x, v = ed.y, c = ed.z;
+    if (u < nb && v < nb && c < E1 - 1) {
+      ob[((int64_t)u * N + v) * E1] = -0.0f;
+      ob[((int64_t)v * N + u) * E1] = -0.0f;
+      ob[((int64_t)u * N + v) * E1 + c + 1] = -0.0f;
+      ob[((int64_t)v * N + u) * E1 + c + 1] = -0.0f;
+    }
+  }
+}
+
 static int launch_sparse(lnb_stream_t stream, SparseBatchParams p, int32_t* tiles, int32_t* rowmap,
                          int32_t* nrows) {
   p.rowmap = rowmap; p.nrows = nrows;
@@ -254,6 +282,21 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
   p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.gext = gext;
   p.node_ids = node_ids; p.mask = mask; p.V = V; p.L = L_dense;
   return launch_sparse(stream, p, tiles, rowmap, nrows);
+}
+
+int lnb_gat_bias_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr, const uint8_t* edges,
+                        int B, int N, int E1, float* bias) {
+  if (!(B >= 0 && N >= 1 && N <= BP_NMAX && E1 >= 2 && E1 <= BP_EMAX)) {
+    lnb::set_err("gat_bias_sparse: B=%d N=%d E1=%d outside 1 <= N <= %d, 2 <= E1 <= %d", B, N, E1, BP_NMAX,
+                 BP_EMAX);
+    return LNB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return LNB_OK;
+  // edges may be NULL when the batch has no bonds: the kernel reads [edge_ptr[b], edge_ptr[b+1]) only
+  LNB_REQUIRE(sizes && edge_ptr && bias, "gat_bias_sparse: null pointer");
+  gat_bias_sparse_kernel<<<B, BP_THREADS, 0, (cudaStream_t)stream>>>(sizes, edge_ptr, edges, N, E1, bias);
+  lnb::count_launch();
+  return lnb::finish_launch("gat_bias_sparse");
 }
 
 }  // extern "C"

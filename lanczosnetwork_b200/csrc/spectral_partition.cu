@@ -16,6 +16,12 @@
 //   4. canonical labels (no edge: -1, the rest numbered by first appearance) and L_cluster / L_cut,
 //      fp32 of the fp64 L4 of the within-cluster and the cut adjacency (every node keeps its self-loop).
 // Every reduction has a fixed order: repeated launches are bit-identical.
+//
+// The sparse entry (lnb_spectral_partition_sparse) differs in step 1 only: it reads the bond lists of
+// lnb_graph_prepare_sparse and forms the fp64 L4 with graph_eigs_sparse's products, (s_i m_ij) s_j with m
+// the bond multiplicity, so padded rows are zero exactly as the dense entry sees them.  The bond pattern
+// stays in a bitmap behind the k-means scratch for step 4, which may write L_cluster / L_cut and writes
+// their ELL rows in lnb_graph_prepare's layout and slot order (diagonal, then ascending column).
 #include "graph_eigs.cuh"
 
 namespace {
@@ -28,10 +34,13 @@ constexpr double SP_TIE = 1e-9;
 
 struct PartParams {
   const float* L; int64_t es;                 // channel 0: L[((b * N + i) * N + j) * es]
+  // sparse entry: the records of lnb_graph_prepare_sparse, bond types < E
+  const int32_t* sizes; const int32_t* edge_ptr; const uint8_t* edges; int E;
   const double* inv_sqrt_deg;                 // [256]
   const double* draws;                        // [1 + (P - 1) * T]
   int B, N, P, T;
-  int32_t* labels; float* L_cluster; float* L_cut; int32_t* status;
+  int32_t* labels; float* L_cluster; float* L_cut; int32_t* status;   // L_cluster / L_cut may be null
+  float* ell_val; uint8_t* ell_idx; int32_t* ell_max; int32_t* gext;  // ELL rows of [L_cluster, L_cut]
 };
 
 // k-means scratch behind the eigensolver's: C, Cn [P][P], cn2, wic [P], dist, xx [N], misc [8],
@@ -40,14 +49,32 @@ __host__ __device__ constexpr size_t km_doubles(int N, int P) {
   return 2 * (size_t)P * P + 2 * (size_t)P + 2 * (size_t)N + 8 + (3 * (size_t)N + 1) / 2;
 }
 
-__host__ __device__ constexpr size_t part_doubles(int N, int W, int P) {
-  return graph_doubles(N, W) + km_doubles(N, P);
+// the sparse entry's bond pattern: N rows of ceil(N / 32) words
+__host__ __device__ constexpr size_t adj_doubles(int N) {
+  return ((size_t)N * ((N + 31) / 32) + 1) / 2;
+}
+
+__host__ __device__ constexpr size_t part_doubles(int N, int W, int P, bool sparse = false) {
+  return graph_doubles(N, W) + km_doubles(N, P) + (sparse ? adj_doubles(N) : 0);
 }
 
 template <int W>
 __device__ __forceinline__ int group_any(int v) {
   if (W == 1) return __any_sync(0xffffffffu, v);
   return __syncthreads_or(v);
+}
+
+template <int W>
+__device__ __forceinline__ int group_max(int v, int* red) {
+  v = __reduce_max_sync(0xffffffffu, v);
+  if (W == 1) return v;
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int m = red[0];
+#pragma unroll
+  for (int w = 1; w < W; ++w) m = max(m, red[w]);
+  return m;
 }
 
 struct Kmeans {
@@ -232,7 +259,7 @@ struct Kmeans {
   }
 };
 
-template <int W>
+template <int W, bool SPARSE>
 __global__ void __launch_bounds__(GE_THREADS)
 spectral_partition_kernel(const PartParams p) {
   extern __shared__ __align__(16) double sp_smem[];
@@ -243,7 +270,7 @@ spectral_partition_kernel(const PartParams p) {
   const int t = wg * 32 + lane;              // row owned by this thread
   const int N = p.N, P = p.P;
   const int b = blockIdx.x * GPC + grp;
-  double* base = sp_smem + (size_t)grp * part_doubles(N, W, P);
+  double* base = sp_smem + (size_t)grp * part_doubles(N, W, P, SPARSE);
   const Work w(base, N, W, wg);
   if (b >= p.B) return;                       // whole groups only: a CTA-wide group has b < B
 
@@ -252,31 +279,77 @@ spectral_partition_kernel(const PartParams p) {
   int* lab = ibase;
   int* canon = ibase + N;                    // lab_old of the k-means, then the canonical labels
   int* linked = ibase + 2 * N;
-  const float* Lb = p.L + (int64_t)b * N * N * p.es;
+  const int NW = (N + 31) >> 5;
+  uint32_t* adj = reinterpret_cast<uint32_t*>(base + graph_doubles(N, W) + km_doubles(N, P));
+  const float* Lb = SPARSE ? nullptr : p.L + (int64_t)b * N * N * p.es;
   auto at = [&](int i, int j) { return __ldg(Lb + ((int64_t)i * N + j) * p.es); };
+  // an off-diagonal entry of the pattern
+  auto edge = [&](int i, int j) {
+    if (SPARSE) return (adj[i * NW + (j >> 5)] >> (j & 31) & 1u) != 0u;
+    return j != i && at(i, j) != 0.f;
+  };
 
   // ---- 1. the operator --------------------------------------------------------------------------
-  if (t < N) {
-    int deg = 1;                                        // the + I of L4
-    for (int j = 0; j < N; ++j) deg += (j != t && at(t, j) != 0.f) ? 1 : 0;
-    linked[t] = deg > 1;
-    w.sc()[t] = at(t, t) != 0.f ? p.inv_sqrt_deg[deg] : 0.0;   // padding: a zero row
-  }
-  gsync<W>();
   int weighted = 0;
-  if (t < N) {
-    const double si = w.sc()[t];
-    for (int j = 0; j < N; ++j) {
-      const float a = at(t, j);
-      // the reference's (s_i * 1) * s_j on the pattern and the diagonal
-      const double v = (j == t || a != 0.f) ? si * w.sc()[j] : 0.0;
-      weighted |= __float_as_uint(__double2float_rn(v)) != __float_as_uint(a);
-      if (j <= t) w.Ap()[tri(t, j)] = v;
+  if (SPARSE) {
+    // graph_eigs_sparse's producer: bond-type bitmask per node pair in Z's storage (free until QL), a
+    // bond listed twice with one type counts once; the pattern bitmap outlives the solver
+    const int n = min(max(p.sizes[b], 0), N);
+    uint32_t* mk = reinterpret_cast<uint32_t*>(w.Z());
+    for (int i = t; i < n * n; i += GT) mk[i] = 0u;
+    for (int i = t; i < N * NW; i += GT) adj[i] = 0u;
+    gsync<W>();
+    const int e0 = p.edge_ptr[b], e1 = p.edge_ptr[b + 1];
+    for (int e = e0 + t; e < e1; e += GT) {
+      const uchar4 ed = reinterpret_cast<const uchar4*>(p.edges)[e];
+      const int u = ed.x, v = ed.y, c = ed.z;
+      if (u < n && v < n && c < p.E) {
+        atomicOr(&mk[u * n + v], 1u << c);
+        atomicOr(&mk[v * n + u], 1u << c);
+        if (u != v) {
+          atomicOr(&adj[u * NW + (v >> 5)], 1u << (v & 31));
+          atomicOr(&adj[v * NW + (u >> 5)], 1u << (u & 31));
+        }
+      }
     }
+    gsync<W>();
+    if (t < N) {
+      int deg = 1, any = 0;                             // the + I of L4
+      for (int j = 0; j < n && t < n; ++j) deg += __popc(mk[t * n + j]);
+      for (int k = 0; k < NW; ++k) any |= adj[t * NW + k] != 0u;
+      linked[t] = any;
+      w.sc()[t] = t < n ? p.inv_sqrt_deg[deg < 255 ? deg : 255] : 0.0;   // padding: a zero row
+    }
+    gsync<W>();
+    if (t < N) {
+      const double si = w.sc()[t];
+      for (int j = 0; j <= t; ++j) {
+        const int m = t < n ? (t == j ? 1 : 0) + __popc(mk[t * n + j]) : 0;
+        w.Ap()[tri(t, j)] = m ? (si * (double)m) * w.sc()[j] : 0.0;
+      }
+    }
+  } else {
+    if (t < N) {
+      int deg = 1;                                        // the + I of L4
+      for (int j = 0; j < N; ++j) deg += (j != t && at(t, j) != 0.f) ? 1 : 0;
+      linked[t] = deg > 1;
+      w.sc()[t] = at(t, t) != 0.f ? p.inv_sqrt_deg[deg] : 0.0;   // padding: a zero row
+    }
+    gsync<W>();
+    if (t < N) {
+      const double si = w.sc()[t];
+      for (int j = 0; j < N; ++j) {
+        const float a = at(t, j);
+        // the reference's (s_i * 1) * s_j on the pattern and the diagonal
+        const double v = (j == t || a != 0.f) ? si * w.sc()[j] : 0.0;
+        weighted |= __float_as_uint(__double2float_rn(v)) != __float_as_uint(a);
+        if (j <= t) w.Ap()[tri(t, j)] = v;
+      }
+    }
+    weighted = group_any<W>(weighted);
+    if (weighted && t < N)
+      for (int j = 0; j <= t; ++j) w.Ap()[tri(t, j)] = (double)at(t, j);
   }
-  weighted = group_any<W>(weighted);
-  if (weighted && t < N)
-    for (int j = 0; j <= t; ++j) w.Ap()[tri(t, j)] = (double)at(t, j);
   gsync<W>();
 
   // ---- 2. eigenvectors: the first P of the reference's order (and the P+1-th eigenvalue) ----------
@@ -311,28 +384,93 @@ spectral_partition_kernel(const PartParams p) {
     p.labels[(int64_t)b * N + t] = canon[t];
     int dc = 1, dt = 1;
     for (int j = 0; j < N; ++j) {
-      if (j == t || at(t, j) == 0.f) continue;
+      if (!edge(t, j)) continue;
       if (lab[j] == lab[t]) ++dc; else ++dt;
     }
     s_cl[t] = p.inv_sqrt_deg[dc];
     s_ct[t] = p.inv_sqrt_deg[dt];
   }
   gsync<W>();
-  float* Oc = p.L_cluster + (int64_t)b * N * N;
-  float* Ot = p.L_cut + (int64_t)b * N * N;
-  for (int idx = t; idx < N * N; idx += GT) {
-    const int r = idx / N, c = idx - r * N;
-    const bool edge = r != c && at(r, c) != 0.f;
-    const bool same = lab[r] == lab[c];
-    Oc[idx] = (r == c || (edge && same)) ? __double2float_rn(s_cl[r] * s_cl[c]) : 0.f;
-    Ot[idx] = (r == c || (edge && !same)) ? __double2float_rn(s_ct[r] * s_ct[c]) : 0.f;
+  if (p.L_cluster) {
+    float* Oc = p.L_cluster + (int64_t)b * N * N;
+    float* Ot = p.L_cut + (int64_t)b * N * N;
+    for (int idx = t; idx < N * N; idx += GT) {
+      const int r = idx / N, c = idx - r * N;
+      const bool e = edge(r, c);
+      const bool same = lab[r] == lab[c];
+      Oc[idx] = (r == c || (e && same)) ? __double2float_rn(s_cl[r] * s_cl[c]) : 0.f;
+      Ot[idx] = (r == c || (e && !same)) ? __double2float_rn(s_ct[r] * s_ct[c]) : 0.f;
+    }
+  }
+  if (SPARSE) {
+    // lnb_graph_prepare of stack([L_cluster, L_cut], 3) with a zero Q: row t of channel ch holds the
+    // diagonal, then its part's edges by ascending column, zero-filled to the channel's longest row.
+    // Every row keeps its self-loop, so the graph's extent is (N, 0).
+    int cnt[2] = {0, 0};
+#pragma unroll
+    for (int ch = 0; ch < 2; ++ch) {
+      const double* sv = ch ? s_ct : s_cl;
+      float* val = p.ell_val + ((int64_t)(b * 2 + ch) * N) * N + t;
+      uint8_t* idx = p.ell_idx + ((int64_t)(b * 2 + ch) * N) * N + t;
+      if (t < N) {
+        val[0] = __double2float_rn(sv[t] * sv[t]);
+        idx[0] = (uint8_t)t;
+        int c = 1;
+        for (int j = 0; j < N; ++j) {
+          if (!edge(t, j) || (lab[j] == lab[t]) != (ch == 0)) continue;
+          val[(int64_t)c * N] = __double2float_rn(sv[t] * sv[j]);
+          idx[(int64_t)c * N] = (uint8_t)j;
+          ++c;
+        }
+        cnt[ch] = c;
+      }
+    }
+    int* red = reinterpret_cast<int*>(w.red());
+    const int m0 = group_max<W>(cnt[0], red);
+    const int m1 = group_max<W>(cnt[1], red + 4);
+#pragma unroll
+    for (int ch = 0; ch < 2; ++ch) {
+      if (t >= N) break;
+      float* val = p.ell_val + ((int64_t)(b * 2 + ch) * N) * N + t;
+      uint8_t* idx = p.ell_idx + ((int64_t)(b * 2 + ch) * N) * N + t;
+      for (int s = cnt[ch]; s < (ch ? m1 : m0); ++s) {
+        val[(int64_t)s * N] = 0.f;
+        idx[(int64_t)s * N] = 0;
+      }
+    }
+    if (t == 0) {
+      p.ell_max[b * 2] = m0;
+      p.ell_max[b * 2 + 1] = m1;
+      p.gext[b * 2] = N;
+      p.gext[b * 2 + 1] = 0;
+    }
   }
 }
 
-static_assert(sizeof(double) * part_doubles(GE_NMAX, 4, SP_PMAX) <= 227 * 1024,
+static_assert(sizeof(double) * part_doubles(GE_NMAX, 4, SP_PMAX, true) <= 227 * 1024,
               "spectral_partition: N = 128, P = 16 must fit one CTA's shared memory");
-static_assert(4 * sizeof(double) * part_doubles(32, 1, SP_PMAX) <= 227 * 1024,
+static_assert(4 * sizeof(double) * part_doubles(32, 1, SP_PMAX, true) <= 227 * 1024,
               "spectral_partition: four N = 32 graphs per CTA");
+
+template <bool SPARSE>
+int launch(lnb_stream_t stream, const PartParams& p, const char* what) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (p.N <= 32) {
+    const size_t shm = 4 * part_doubles(p.N, 1, p.P, SPARSE) * sizeof(double);
+    if (shm > 48 * 1024)
+      cudaFuncSetAttribute(spectral_partition_kernel<1, SPARSE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)shm);
+    spectral_partition_kernel<1, SPARSE><<<lnb::ceil_div(p.B, 4), GE_THREADS, shm, s>>>(p);
+  } else {
+    const size_t shm = part_doubles(p.N, 4, p.P, SPARSE) * sizeof(double);
+    if (shm > 48 * 1024)
+      cudaFuncSetAttribute(spectral_partition_kernel<4, SPARSE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)shm);
+    spectral_partition_kernel<4, SPARSE><<<p.B, GE_THREADS, shm, s>>>(p);
+  }
+  lnb::count_launch();
+  return lnb::finish_launch(what);
+}
 
 }  // namespace
 
@@ -358,20 +496,31 @@ int lnb_spectral_partition(lnb_stream_t stream, const float* L, int64_t elem_str
   p.L = L; p.es = elem_stride; p.inv_sqrt_deg = inv_sqrt_deg; p.draws = draws;
   p.B = B; p.N = N; p.P = P; p.T = 2 + (int)log((double)P);
   p.labels = labels; p.L_cluster = L_cluster; p.L_cut = L_cut; p.status = status;
-  cudaStream_t s = (cudaStream_t)stream;
-  if (N <= 32) {
-    const size_t shm = 4 * part_doubles(N, 1, P) * sizeof(double);
-    if (shm > 48 * 1024)
-      cudaFuncSetAttribute(spectral_partition_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
-    spectral_partition_kernel<1><<<lnb::ceil_div(B, 4), GE_THREADS, shm, s>>>(p);
-  } else {
-    const size_t shm = part_doubles(N, 4, P) * sizeof(double);
-    if (shm > 48 * 1024)
-      cudaFuncSetAttribute(spectral_partition_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
-    spectral_partition_kernel<4><<<B, GE_THREADS, shm, s>>>(p);
+  return launch<false>(stream, p, "spectral_partition");
+}
+
+int lnb_spectral_partition_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr,
+                                  const uint8_t* edges, const double* inv_sqrt_deg, int B, int N, int E, int P,
+                                  const double* draws, int32_t* labels, int32_t* status, float* ell_val,
+                                  uint8_t* ell_idx, int32_t* ell_max, int32_t* gext, float* L_cluster,
+                                  float* L_cut) {
+  if (!(B >= 0 && N >= 1 && N <= GE_NMAX && P >= SP_PMIN && P <= SP_PMAX && P < N && E >= 1 && E <= 32)) {
+    lnb::set_err("spectral_partition_sparse: B=%d N=%d E=%d P=%d outside 1 <= N <= %d, %d <= P <= %d, P < N, "
+                 "1 <= E <= 32", B, N, E, P, GE_NMAX, SP_PMIN, SP_PMAX);
+    return LNB_ERR_UNSUPPORTED;
   }
-  lnb::count_launch();
-  return lnb::finish_launch("spectral_partition");
+  if (B == 0) return LNB_OK;
+  // edges may be NULL when the batch has no bonds: the kernel reads [edge_ptr[b], edge_ptr[b+1]) only
+  LNB_REQUIRE(sizes && edge_ptr && inv_sqrt_deg && draws && labels && status && ell_val && ell_idx && ell_max &&
+                  gext && (L_cluster == nullptr) == (L_cut == nullptr),
+              "spectral_partition_sparse: null pointer");
+  PartParams p = {};
+  p.sizes = sizes; p.edge_ptr = edge_ptr; p.edges = edges; p.E = E;
+  p.inv_sqrt_deg = inv_sqrt_deg; p.draws = draws;
+  p.B = B; p.N = N; p.P = P; p.T = 2 + (int)log((double)P);
+  p.labels = labels; p.L_cluster = L_cluster; p.L_cut = L_cut; p.status = status;
+  p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.gext = gext;
+  return launch<true>(stream, p, "spectral_partition_sparse");
 }
 
 }  // extern "C"

@@ -5,6 +5,7 @@ unchanged (model/lanczos_net.py:15-93, utils/train_helper.py:14-32): ``embedding
 ``filter.{i}.{weight,bias}``, ``spectral_filter.{l}.{0,2,4,6}.{weight,bias}``,
 ``att_func.0.{weight,bias}``.  The forward math lives in CUDA (lanczosnetwork_b200.ops).
 """
+import collections
 import os
 
 import torch
@@ -39,6 +40,10 @@ class Ragged(object):
 
 def _raw(t):
   return t.tensor if isinstance(t, Ragged) else t
+
+
+# the bond-list records of one batch on the device (data.sparse_collate's layout), N = padding target
+SparseRecords = collections.namedtuple('SparseRecords', 'sizes node_ptr node_feat edge_ptr edges N')
 
 
 def _opt(obj, name, default):
@@ -211,6 +216,60 @@ class SpectralNetBase(nn.Module):
     if dtype is not None and t.dtype != dtype:
       t = t.to(dtype)
     return t
+
+  # ------------------------------------------------------------------------------------------
+  # Forward from a sparse batch (data.sparse_collate): the padded inputs are built on the device.
+  SPARSE_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N')
+
+  def forward_sparse(self, batch, label=None):
+    """Forward from a SPARSE batch (data.sparse_collate -> torch tensors, pinned host or device):
+    per-molecule node ids and bond lists; ``D`` / ``V_rows``, when present, are read only by the models
+    that consume eigenpairs.  The padded node ids, mask, ELL rows and whatever else the model reads are
+    built on the device (lnb_graph_prepare_sparse and the model's own producers): the dense
+    B x N x N x (E+1) tensor of the reference's collate never crosses PCIe.  Same scores as ``forward``
+    on the collated batch, bit for bit.  Inference only (raises under autograd).  Returns score or
+    (score, loss)."""
+    if self._check_mode():
+      raise NotImplementedError('forward_sparse is an inference path; train through forward()')
+    dev = self._device()
+    inputs, impl, key = self._sparse_inputs(batch)
+    score = self._graph_forward(impl, inputs, extra_key=key)
+    return self._finish(score, self._to(dev, label))
+
+  def _sparse_inputs(self, batch):
+    """(inputs, impl, extra_key) of _graph_forward for a sparse batch: the bond-list records, whose
+    device batch goes to the model's ``_forward_records`` hook."""
+    if not hasattr(self, '_forward_records'):
+      raise NotImplementedError('%s has no sparse-batch entry; call forward() on the collated batch'
+                                % type(self).__name__)
+    missing = [k for k in self.SPARSE_KEYS if k not in batch]
+    if missing:
+      raise ValueError('forward_sparse: the batch lacks %s (data.sparse_collate records)' % ', '.join(missing))
+    N, B = int(batch['N']), int(batch['sizes'].shape[0])
+    E1 = self.num_edgetype + 1
+    if not (1 <= N <= 128 and 2 <= E1 <= 16):
+      raise ValueError('forward_sparse: N=%d, E+1=%d outside 1 <= N <= 128, 2 <= E+1 <= 16' % (N, E1))
+    for k in ('sizes', 'node_ptr', 'node_feat', 'edge_ptr'):
+      if batch[k].dtype != torch.int32:
+        raise ValueError('forward_sparse: %s must be int32; got %s' % (k, batch[k].dtype))
+    if batch['edges'].dtype != torch.uint8 or batch['edges'].dim() != 2 or batch['edges'].shape[1] != 4:
+      raise ValueError('forward_sparse: edges must be uint8 [E, 4]')
+    self._check_runnable(N, E1)
+    inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
+              Ragged(batch['edges']))
+    return inputs, lambda *a: self._forward_records(SparseRecords(*a, N=N)), ('records', N)
+
+  def _check_runnable(self, N=None, E1=None):
+    """Model-specific checks of a call, run before any launch (N, E1: those of a sparse batch)."""
+
+  def _prepare_records(self, recs, binarize=False, want_dense=False):
+    """lnb_graph_prepare_sparse on the records without Ritz vectors (the zero [rows, 4] block, as the
+    padded path's zero [B, N, 4]): (GraphPrep, node_ids [B,N] int64, mask [B,N] uint8, V = zeros [B,N,4],
+    dense L or None)."""
+    V_rows = torch.zeros((recs.node_feat.shape[0], 4), device=recs.sizes.device, dtype=torch.float32)
+    return ops.graph_prepare_sparse(recs.sizes, recs.node_ptr, recs.node_feat, recs.edge_ptr, recs.edges,
+                                    V_rows, recs.N, self.num_edgetype + 1, binarize=binarize,
+                                    want_dense=want_dense)
 
   # ------------------------------------------------------------------------------------------
   # CUDA-graph replay of the inference forward: the forward is ~15 short kernel launches issued

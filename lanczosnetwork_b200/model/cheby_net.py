@@ -77,3 +77,7 @@ class ChebyNet(SpectralNetBase):
       state = dense(msg.reshape(B * N, CD), self.filter[t].weight, self.filter[t].bias, True,
                     self._wcache, 'filter.%d' % t).reshape(B, N, -1)
     return self._readout(state, mask)
+
+  def _forward_records(self, recs):
+    _, node_ids, mask, _, L = self._prepare_records(recs, want_dense=True)
+    return self._forward_impl(node_ids, L, mask)

@@ -86,3 +86,7 @@ class DCNN(SpectralNetBase):
                                        self._layer_weight(t), self.filter[t].bias, self._wcache,
                                        'filter.%d.perm' % t)
     return self._readout(state, mask)
+
+  def _forward_records(self, recs):
+    _, node_ids, mask, _, L = self._prepare_records(recs, want_dense=True)
+    return self._forward_impl(node_ids, L, mask)

@@ -122,6 +122,11 @@ class GAT(SpectralNetBase):
     head, att = self.output_func[0], self.att_func[0]
     return ops.readout(state, head.weight, head.bias, att.weight.reshape(-1), att.bias, mask)
 
+  def _forward_records(self, recs):
+    _, node_ids, mask, _, _ = self._prepare_records(recs)
+    bias = ops.gat_bias_sparse(recs.sizes, recs.edge_ptr, recs.edges, recs.N, self.num_edgetype + 1)
+    return self._forward_impl(node_ids, bias, mask)
+
 
 class TrainableGAT(GAT):
   """``GAT`` with a training path.  Under ``no_grad`` (or without trainable parameters) the forward is the

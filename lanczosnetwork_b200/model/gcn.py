@@ -46,6 +46,14 @@ class GCN(SpectralNetBase):
     V = torch.zeros((B, N, 4), device=L.device, dtype=torch.float32)
     return self._ritz_conv_stack(None, node_feat.long(), L, None, V, mask)
 
+  def _forward_records(self, recs):
+    # the dense operators only when a layer falls off the stack kernel
+    E1 = self.num_edgetype + 1
+    prep, node_ids, mask, V, L = self._prepare_records(
+        recs, binarize=getattr(self, '_binarize_operators', False),
+        want_dense=not self._sparse_stack_ok(recs.N, E1, 4))
+    return self._ritz_conv_stack(None, node_ids, L, None, V, mask, prep=prep, dims_hint=(recs.N, E1))
+
 
 class GCNFP(GCN):
   """Drop-in for the reference ``model.GCNFP`` (model/gcnfp.py:8-125): GCN on the non-zero pattern

@@ -144,13 +144,17 @@ class GGNN(SpectralNetBase):
       pattern is read; L is not modified); label: B x P; mask: B x N (uint8 / bool / float).
       Returns score (B x P) or (score, loss).
     """
+    self._check_runnable()
+    return self._forward((node_feat, L, mask), label)
+
+  def _check_runnable(self, N=None, E1=None):
+    """The reference's errors of the configs its forward cannot run, before any launch."""
     if self.update_func_name == 'MLP':
       raise TypeError("forward() takes 2 positional arguments but 3 were given: update_func 'MLP' is an "
                       "nn.Sequential, which the reference calls with (messages, state) (model/ggnn.py:168)")
     if self.msg_func is None:
       raise UnboundLocalError("msg_func %r: the reference's propagation reads a message that is never "
                               "assigned (model/ggnn.py:147-154); only 'MLP' runs" % self.config.model.msg_func)
-    return self._forward((node_feat, L, mask), label)
 
   def _train_impl(self, node_feat, L, mask):
     from ..train import ggnn_train
@@ -171,9 +175,20 @@ class GGNN(SpectralNetBase):
     E1 = L.shape[3]
     if not self.fused_supported(N, E1):
       return self._train_impl(node_feat, L, mask)        # RNN update / other shapes: the training formulation
+    return self._propagate(node_feat, ops.graph_prepare(L, binarize=True), mask)
+
+  def _forward_records(self, recs):
+    fused = self.fused_supported(recs.N, self.num_edgetype + 1)
+    prep, node_ids, mask, _, L = self._prepare_records(recs, binarize=True, want_dense=not fused)
+    if not fused:
+      return self._train_impl(node_ids, L, mask)
+    return self._propagate(node_ids, prep, mask)
+
+  def _propagate(self, node_feat, prep, mask):
+    """The fused inference forward from the ELL rows of the 0/1 operators."""
+    B, N = node_feat.shape
     D = self.hidden_dim
     h = embed_input(self, node_feat, self.embedding.weight)
-    prep = ops.graph_prepare(L, binarize=True)            # ELL rows of the 0/1 operators
     params = self._step_params()
     spare = torch.empty_like(h)
     avg = self.aggregate_type == 'avg'

@@ -104,18 +104,26 @@ class GPNN(SpectralNetBase):
       label: B x P; mask: B x N (uint8 / bool / float).
       Returns score (B x P) or (score, loss).
     """
-    if self.update_func_name == 'MLP':
-      raise TypeError("forward() takes 2 positional arguments but 3 were given: update_func 'MLP' is an "
-                      "nn.Sequential, which the reference calls with (messages, state) (model/gpnn.py:210)")
-    if self.msg_func is None:
-      raise UnboundLocalError("msg_func %r: the reference's propagation reads a message that is never "
-                              "assigned (model/gpnn.py:193-200); only 'MLP' runs" % self.config.model.msg_func)
+    self._check_runnable()
     absent = [t is None or t.numel() == 0 for t in (L_cluster, L_cut)]
     if any(absent):
       if not all(absent):
         raise ValueError('GPNN.forward: pass both L_cluster and L_cut, or neither (device partition)')
       L_cluster = L_cut = None
     return self._forward((node_feat, L, L_cluster, L_cut, mask), label)
+
+  def _check_runnable(self, N=None, E1=None):
+    """The reference's errors of the configs its forward cannot run, and (sparse batches, N given) the
+    partition's envelope, before any launch."""
+    if self.update_func_name == 'MLP':
+      raise TypeError("forward() takes 2 positional arguments but 3 were given: update_func 'MLP' is an "
+                      "nn.Sequential, which the reference calls with (messages, state) (model/gpnn.py:210)")
+    if self.msg_func is None:
+      raise UnboundLocalError("msg_func %r: the reference's propagation reads a message that is never "
+                              "assigned (model/gpnn.py:193-200); only 'MLP' runs" % self.config.model.msg_func)
+    if N is not None and not ops.spectral_partition_supported(N, self.num_partition):
+      raise ValueError('GPNN.forward_sparse: N=%d, num_partition=%d outside the device partition\'s envelope'
+                       % (N, self.num_partition))
 
   def _device_partition(self, L):
     """(L_cluster, L_cut) of the collate's spectral clustering, computed on the device."""
@@ -188,13 +196,28 @@ class GPNN(SpectralNetBase):
       return self._train_impl(node_feat, L, L_cluster, L_cut, mask)   # RNN update / other shapes
     if L_cluster is None:
       L_cluster, L_cut = self._device_partition(L)
-    H = self.hidden_dim
-    h = embed_input(self, node_feat, self.embedding.weight)
     # ELL rows of the 0/1 operators and of the valued partition operators; no Ritz vectors, one zero
     # block for both
     zeros = torch.zeros((B, N, 4), device=L.device, dtype=torch.float32)
     prep = ops.graph_prepare(L, zeros, binarize=True)
     pprep = ops.graph_prepare(torch.stack([L_cluster, L_cut], 3), zeros)
+    return self._propagate(node_feat, prep, pprep, mask)
+
+  def _forward_records(self, recs):
+    # the partition's ELL rows come straight from lnb_spectral_partition_sparse
+    fused = self.fused_supported(recs.N, self.num_edgetype + 1)
+    prep, node_ids, mask, _, L = self._prepare_records(recs, binarize=True, want_dense=not fused)
+    if not fused:
+      return self._train_impl(node_ids, L, None, None, mask)
+    _, _, pprep, _, _ = ops.spectral_partition_sparse(recs.sizes, recs.edge_ptr, recs.edges, recs.N,
+                                                      self.num_partition, self.num_edgetype)
+    return self._propagate(node_ids, prep, pprep, mask)
+
+  def _propagate(self, node_feat, prep, pprep, mask):
+    """The fused inference forward from the binarised ELL rows of L and those of [L_cluster, L_cut]."""
+    B, N = node_feat.shape
+    H = self.hidden_dim
+    h = embed_input(self, node_feat, self.embedding.weight)
     step = ggnn_step_params(self._wcache, self.msg_func, self.update_func)
     msg, gates, state = self._partition_params()
     X = torch.empty((B * N, 3 * H), device=h.device, dtype=torch.float32)

@@ -39,41 +39,27 @@ class LanczosNet(SpectralNetBase):
     return self._ritz_conv_stack(None, node_feat.long(), L.float().contiguous(),
                                  D.float().contiguous(), V.float().contiguous(), mask)
 
-  def forward_sparse(self, batch, label=None):
-    """Forward from a SPARSE batch (lanczosnetwork_b200.data.sparse_collate -> torch tensors, pinned
-    host or device): per-molecule node ids, bond lists and the Ritz pairs of the real nodes.  The
-    padded operators, mask, ELL rows and tile table are built on the device
-    (lnb_graph_prepare_sparse); the dense B x N x N x (E+1) tensor of the reference's collate
-    (dataset/qm8.py:220-262) is never materialised and never crosses PCIe.  Same scores as
-    ``forward`` on the collated batch, bit for bit.  A batch without ``V_rows`` and ``D``
-    (``data.sparse_collate(..., eigs=False)``: bond lists and K only) gets the reference's eigenpairs
-    from one lnb_graph_eigs_sparse launch in front of the batch construction, inside the same CUDA
-    graph: no host eigh and no eigenvector bytes on the bus.  Returns score or (score, loss)."""
-    if self._check_mode():
-      raise NotImplementedError('forward_sparse is an inference path; train through forward()')
-    dev = self._device()
+  def _sparse_inputs(self, batch):
+    """A sparse batch here also carries the Ritz pairs of the real nodes (``V_rows``, ``D``), or only K
+    (``data.sparse_collate(..., eigs=False)``): the reference's eigenpairs then come from one
+    lnb_graph_eigs_sparse launch in front of the batch construction, inside the same CUDA graph (no host
+    eigh, no eigenvector bytes on the bus).  A packed batch (data.pack_sparse) crosses PCIe as ONE copy
+    of exactly the bytes present."""
     if 'blob' in batch:
-      # packed batch (data.pack_sparse): ONE H2D copy of exactly the bytes present
       B, N, K = int(batch['B']), int(batch['N']), int(batch['K'])
       cap = data_mod.packed_offsets(B, K)[4] + 16 * 3 + 4 * B * N + 4 * B * N * K + 4 * B * N * 4
       blob = batch['blob']
-      score = self._graph_forward(lambda b_: self._forward_packed_impl(B, N, K, b_),
-                                  (Ragged(blob, max(cap, int(blob.shape[0]))),),
-                                  extra_key=('packed', B, N, K))
-      return self._finish(score, self._to(dev, label))
+      return ((Ragged(blob, max(cap, int(blob.shape[0]))),),
+              lambda b_: self._forward_packed_impl(B, N, K, b_), ('packed', B, N, K))
     N, B = int(batch['N']), int(batch['sizes'].shape[0])
     if 'V_rows' not in batch and 'D' not in batch:
       K = int(batch['K'])
       inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
                 Ragged(batch['edges']))
-      score = self._graph_forward(lambda *a: self._forward_sparse_eigs_impl(N, K, *a), inputs,
-                                  extra_key=('sparse_eigs', N, K))
-      return self._finish(score, self._to(dev, label))
+      return inputs, lambda *a: self._forward_sparse_eigs_impl(N, K, *a), ('sparse_eigs', N, K)
     inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
               Ragged(batch['edges']), Ragged(batch['V_rows'], B * N), batch['D'])
-    score = self._graph_forward(lambda *a: self._forward_sparse_impl(N, *a), inputs,
-                                extra_key=('sparse', N))
-    return self._finish(score, self._to(dev, label))
+    return inputs, lambda *a: self._forward_sparse_impl(N, *a), ('sparse', N)
 
   def _forward_packed_impl(self, B, N, K, blob):
     E1 = self.num_edgetype + 1

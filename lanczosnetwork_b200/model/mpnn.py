@@ -178,9 +178,20 @@ class MPNN(SpectralNetBase):
     E1 = L.shape[3]
     if not self.fused_supported(N, E1):
       return self._train_impl(node_feat, L, mask)        # other shapes: the training formulation
+    return self._propagate(node_feat, ops.graph_prepare(L, binarize=True), mask)
+
+  def _forward_records(self, recs):
+    fused = self.fused_supported(recs.N, self.num_edgetype + 1)
+    prep, node_ids, mask, _, L = self._prepare_records(recs, binarize=True, want_dense=not fused)
+    if not fused:
+      return self._train_impl(node_ids, L, mask)
+    return self._propagate(node_ids, prep, mask)
+
+  def _propagate(self, node_feat, prep, mask):
+    """The fused inference forward from the ELL rows of the 0/1 operators."""
+    B, N = node_feat.shape
     D = self.hidden_dim
     h = embed_input(self, node_feat, self.node_embedding.weight)
-    prep = ops.graph_prepare(L, binarize=True)            # ELL rows of the 0/1 operators
     (m_hi, m_lo, m_b), (g_hi, g_lo, g_b) = self._step_params()
     spare = torch.empty_like(h)
     avg = self.aggregate_type == 'avg'

@@ -14,7 +14,7 @@ from ._lib import GemmDesc, SpectralStack
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'tile_assign', 'spectral_conv_fused',
     'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
-    'spectral_partition', 'partition_draws',
+    'spectral_partition', 'spectral_partition_sparse', 'spectral_partition_supported', 'partition_draws', 'gat_bias_sparse',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
     'sage_operators', 'neighbour_max', 'sage_lstm_step', 'sage_lstm_step_supported', 'sage_lstm_messages',
@@ -438,6 +438,71 @@ def spectral_partition(L, num_partition, seed=1234):
         _stream(A), _ptr(A), int(es), B, N, P, _ptr(_inv_sqrt_deg_table(dev)), _ptr(draws), _ptr(labels),
         _ptr(L_cluster), _ptr(L_cut), _ptr(status)), 'lnb_spectral_partition')
   return labels, L_cluster, L_cut, status
+
+
+def _check_records(who, sizes, edge_ptr, edges):
+  _need_cuda(sizes, edge_ptr, edges)
+  if sizes.dtype != torch.int32 or edge_ptr.dtype != torch.int32 or edge_ptr.shape[0] != sizes.shape[0] + 1:
+    raise ValueError('%s: sizes [B] and edge_ptr [B+1] must be int32' % who)
+  if edges.dtype != torch.uint8 or edges.dim() != 2 or edges.shape[1] != 4 or not edges.is_contiguous():
+    raise ValueError('%s: edges must be a contiguous uint8 [E, 4] tensor' % who)
+
+
+def spectral_partition_supported(N, num_partition):
+  """The envelope of spectral_partition and spectral_partition_sparse: N <= 128, 2 <= P <= 16, P < N - 1."""
+  P, N = int(num_partition), int(N)
+  return PARTITION_P_RANGE[0] <= P <= PARTITION_P_RANGE[1] and 1 <= N <= PARTITION_MAX_N and P < N - 1
+
+
+def spectral_partition_sparse(sizes, edge_ptr, edges, N, num_partition, num_edgetype, seed=1234,
+                              want_dense=False):
+  """spectral_partition from the sparse records of data.sparse_collate (lnb_spectral_partition_sparse):
+  the same partition of every graph padded to N, without the padded operators.  Bond types >=
+  num_edgetype are ignored.  Where no node pair carries two bond types, labels and status equal
+  spectral_partition's on the collated L (status bit 3 is never set).
+  Returns (labels [B,N] int32, status [B] int32, GraphPrep of the two-channel operator
+  [L_cluster, L_cut] -- the ELL rows, ell_max and gext that graph_prepare(stack([L_cluster, L_cut], 3))
+  writes, no tile table --, L_cluster, L_cut [B,N,N] when want_dense, else None)."""
+  P, N, E = int(num_partition), int(N), int(num_edgetype)
+  if not spectral_partition_supported(N, P):
+    raise ValueError('spectral_partition_sparse: N=%d, num_partition=%d outside N <= %d, %d <= num_partition <= %d, '
+                     'num_partition < N - 1' % ((N, P, PARTITION_MAX_N) + PARTITION_P_RANGE))
+  if not 1 <= E <= 32:
+    raise ValueError('spectral_partition_sparse: num_edgetype=%d outside 1..32' % E)
+  _check_records('spectral_partition_sparse', sizes, edge_ptr, edges)
+  dev = sizes.device
+  B = sizes.shape[0]
+  labels = torch.empty((B, N), device=dev, dtype=torch.int32)
+  status = torch.empty((B,), device=dev, dtype=torch.int32)
+  ell_val = torch.empty((B, 2, N, N), device=dev, dtype=torch.float32)
+  ell_idx = torch.empty((B, 2, N, N), device=dev, dtype=torch.uint8)
+  ell_max = torch.empty((B, 2), device=dev, dtype=torch.int32)
+  gext = torch.empty((B, 2), device=dev, dtype=torch.int32)
+  L_cluster = torch.empty((B, N, N), device=dev, dtype=torch.float32) if want_dense else None
+  L_cut = torch.empty((B, N, N), device=dev, dtype=torch.float32) if want_dense else None
+  with torch.cuda.device(dev):
+    draws = _partition_draws_table(dev, N, P, seed)
+    _lib.check(_lib.load().lnb_spectral_partition_sparse(
+        _stream(sizes), _ptr(sizes), _ptr(edge_ptr), _ptr(edges), _ptr(_inv_sqrt_deg_table(dev)), B, N, E, P,
+        _ptr(draws), _ptr(labels), _ptr(status), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(gext),
+        _ptr(L_cluster), _ptr(L_cut)), 'lnb_spectral_partition_sparse')
+  return labels, status, GraphPrep((ell_val, ell_idx, ell_max, gext, None)), L_cluster, L_cut
+
+
+def gat_bias_sparse(sizes, edge_ptr, edges, N, E1):
+  """GAT's additive attention bias [B,N,N,E1] fp32 from the sparse records (lnb_gat_bias_sparse): bit for
+  bit data.gat_bias of the collated operators (-0.0 on the diagonal and on the channel's bonds, -1e9
+  elsewhere)."""
+  N, E1 = int(N), int(E1)
+  if not (1 <= N <= 128 and 2 <= E1 <= 16):
+    raise ValueError('gat_bias_sparse: N=%d, E1=%d outside 1 <= N <= 128, 2 <= E1 <= 16' % (N, E1))
+  _check_records('gat_bias_sparse', sizes, edge_ptr, edges)
+  B = sizes.shape[0]
+  bias = torch.empty((B, N, N, E1), device=sizes.device, dtype=torch.float32)
+  with torch.cuda.device(sizes.device):
+    _lib.check(_lib.load().lnb_gat_bias_sparse(_stream(sizes), _ptr(sizes), _ptr(edge_ptr), _ptr(edges), B, N, E1,
+                                               _ptr(bias)), 'lnb_gat_bias_sparse')
+  return bias
 
 
 def fused_conv_supported(N, Din, K, H, n_short, dense_filter, S=8, E1=7):

@@ -1,0 +1,147 @@
+"""The operator drop-ins from padded batches against forward_sparse from bond-list records.
+
+    python tools/bench_sparse_dropins.py [--B 1024] [--iters 30] [--models GCN GPNN ...]
+
+Per model (seeded weights, data.synthetic_qm8_samples at B, N = 26), one JSON line with:
+  * resident_padded_ms / resident_sparse_ms: the forward from device-resident padded inputs
+    (node_feat, L or GAT's bias, mask) and from device-resident sparse records (CUDA events; both
+    replay the model's captured graph);
+  * e2e_padded_ms / e2e_sparse_ms: from pinned host memory (padded tensors vs sparse records) to the
+    score on the device, the copies included (CUDA events);
+  * collate_padded_ms / collate_sparse_ms: the host collate alone (data.collate (+ data.gat_bias for GAT)
+    vs data.sparse_collate, eigs=False), wall clock;
+  * GPNN only: partition_sparse_ms (lnb_spectral_partition_sparse) against partition_dense_ms
+    (lnb_spectral_partition + graph_prepare of the two operators), each as one captured graph.
+The GPU's name and power limit go into every line.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from lanczosnetwork_b200 import configs, data, ops  # noqa: E402
+from lanczosnetwork_b200 import model as models  # noqa: E402
+
+MODELS = {
+    'GCN': lambda: models.GCN(configs.qm8_gcn()),
+    'GCNFP': lambda: models.GCNFP(configs.qm8_gcn()),
+    'DCNN': lambda: models.DCNN(configs.qm8_dcnn()),
+    'ChebyNet': lambda: models.ChebyNet(configs.qm8_cheby_net()),
+    'GAT': lambda: models.GAT(configs.qm8_gat()),
+    'GGNN': lambda: models.GGNN(configs.qm8_ggnn()),
+    'MPNN': lambda: models.MPNN(configs.qm8_mpnn()),
+    'GPNN': lambda: models.GPNN(configs.qm8_gpnn()),
+}
+
+
+def event_ms(fn, iters):
+  for _ in range(3):
+    fn()
+  torch.cuda.synchronize()
+  a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+  a.record()
+  for _ in range(iters):
+    fn()
+  b.record()
+  torch.cuda.synchronize()
+  return a.elapsed_time(b) / iters
+
+
+def graph_ms(fn, iters):
+  """Mean ms per replay of fn captured as one CUDA graph."""
+  fn()
+  torch.cuda.synchronize()
+  g = torch.cuda.CUDAGraph()
+  s = torch.cuda.Stream()
+  s.wait_stream(torch.cuda.current_stream())
+  with torch.cuda.stream(s):
+    with torch.cuda.graph(g, stream=s):
+      fn()
+  torch.cuda.current_stream().wait_stream(s)
+  return event_ms(g.replay, iters)
+
+
+def wall_ms(fn, reps=3):
+  best = None
+  for _ in range(reps):
+    t0 = time.perf_counter()
+    fn()
+    t = (time.perf_counter() - t0) * 1e3
+    best = t if best is None else min(best, t)
+  return best
+
+
+def gpu_info():
+  try:
+    out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
+                         capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+  except Exception:
+    out = torch.cuda.get_device_name(0)
+  return out
+
+
+def padded_inputs(name, samples, K):
+  c = data.collate(samples, K)
+  L = data.gat_bias(c['L']) if name == 'GAT' else c['L']
+  return c['node_feat'], L, c['node_mask']
+
+
+def main():
+  ap = argparse.ArgumentParser()
+  ap.add_argument('--B', type=int, default=1024)
+  ap.add_argument('--iters', type=int, default=30)
+  ap.add_argument('--models', nargs='+', default=list(MODELS))
+  args = ap.parse_args()
+  if not torch.cuda.is_available():
+    raise SystemExit('bench_sparse_dropins: needs a CUDA device')
+  dev = torch.device('cuda:0')
+  gpu = gpu_info()
+  K = 20
+  samples = data.synthetic_qm8_samples(args.B, seed=5)
+  for name in args.models:
+    torch.manual_seed(0)
+    mod = MODELS[name]().to(dev).eval()
+    nf, L, mask = padded_inputs(name, samples, K)
+    sp = data.sparse_collate(samples, K, eigs=False)
+    host_pad = [torch.from_numpy(a).pin_memory() for a in (nf, L, mask)]
+    dev_pad = [t.to(dev) for t in host_pad]
+    host_sp = {k: (torch.from_numpy(v).pin_memory() if isinstance(v, np.ndarray) else v) for k, v in sp.items()}
+    dev_sp = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in host_sp.items()}
+    row = {'model': name, 'B': args.B, 'N': int(sp['N']), 'gpu': gpu}
+    with torch.no_grad():
+      ref = mod(dev_pad[0], dev_pad[1], mask=dev_pad[2])
+      row['bit_equal'] = bool(torch.equal(mod.forward_sparse(dev_sp), ref))
+      row['resident_padded_ms'] = round(event_ms(lambda: mod(dev_pad[0], dev_pad[1], mask=dev_pad[2]), args.iters), 4)
+      row['resident_sparse_ms'] = round(event_ms(lambda: mod.forward_sparse(dev_sp), args.iters), 4)
+      row['e2e_padded_ms'] = round(event_ms(lambda: mod(host_pad[0], host_pad[1], mask=host_pad[2]), args.iters), 4)
+      row['e2e_sparse_ms'] = round(event_ms(lambda: mod.forward_sparse(host_sp), args.iters), 4)
+    row['h2d_padded_bytes'] = int(sum(t.numel() * t.element_size() for t in host_pad))
+    row['h2d_sparse_bytes'] = int(sum(v.numel() * v.element_size() for v in host_sp.values() if torch.is_tensor(v)))
+    if name == 'GAT':
+      row['collate_padded_ms'] = round(wall_ms(lambda: data.gat_bias(data.collate(samples, K)['L'])), 2)
+    else:
+      row['collate_padded_ms'] = round(wall_ms(lambda: data.collate(samples, K)), 2)
+    row['collate_sparse_ms'] = round(wall_ms(lambda: data.sparse_collate(samples, K, eigs=False)), 2)
+    if name == 'GPNN':
+      P, N = mod.num_partition, int(sp['N'])
+      Ld = dev_pad[1]
+      zeros = torch.zeros((args.B, N, 4), device=dev)
+
+      def dense():
+        _, Lc, Lt, _ = ops.spectral_partition(Ld, P)
+        ops.graph_prepare(torch.stack([Lc, Lt], 3), zeros)
+      row['partition_dense_ms'] = round(graph_ms(dense, args.iters), 4)
+      row['partition_sparse_ms'] = round(graph_ms(lambda: ops.spectral_partition_sparse(
+          dev_sp['sizes'], dev_sp['edge_ptr'], dev_sp['edges'], N, P, mod.num_edgetype), args.iters), 4)
+    print(json.dumps(row), flush=True)
+
+
+if __name__ == '__main__':
+  main()
