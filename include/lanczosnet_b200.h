@@ -448,6 +448,30 @@ int lnb_mpnn_edge_aggregate_backward(lnb_stream_t stream, const float* PQ, const
                                      int avg, float* gPQ);
 
 /* ---------------------------------------------------------------------------------------
+ * Operator products over the ELL rows of lnb_graph_prepare / lnb_graph_prepare_sparse (the training
+ * formulation's L_e X without the dense operators), for the channels c0 <= e < c0 + nc:
+ *   out[b*N+n, col0 + (e-c0)*D + d] = sum_{t < ell_max[b,e]} (val[b,e,t,n] w[b,n,e]) X[b*N + idx[b,e,t,n], d]
+ * and the adjoint over the ELL rows of the TRANSPOSED operators (ellT_*, gextT: lnb_graph_prepare of
+ * L.transpose(1, 2), the contract of lnb_mpnn_edge_aggregate_backward), all channels summed in one thread:
+ *   gX[b*N+m, d] = sum_e sum_t (valT[b,e,t,m] w[b,i,e]) G[b*N + i, (e-c0)*D + d],   i = idxT[b,e,t,m]
+ * w [B,N,E1] is an optional row weight (NULL: 1), folded into every entry's coefficient (one rounding).
+ * X, out, G and gX are row-strided (ldx, ldo, ldg, ldgx in floats, unit column stride) and must not
+ * overlap; every channel writes straight into its column block of out.  Rows at or past gext[b,0] are 0.
+ * Each sum is one fmaf chain in ascending column order (the row's diagonal, slot 0, taken in its place;
+ * the adjoint: one chain per channel, added in channel order): lnb_batched_gemm's order on the dense
+ * operator, so on 0/1 operators, weighted or not, both give the same bits.  One thread per output
+ * element, no atomics: repeated launches are bit-identical.  A 4-wide path runs when D, the strides and
+ * col0 are multiples of 4 and X / out (G / gX) are 16-byte aligned.
+ * Envelope: 1 <= N <= 128, 1 <= E1 <= 16, any D >= 1 (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ * ------------------------------------------------------------------------------------- */
+int lnb_ell_messages(lnb_stream_t stream, const float* X, int64_t ldx, const float* ell_val, const uint8_t* ell_idx,
+                     const int32_t* ell_max, const int32_t* gext, const float* w, int B, int N, int E1, int c0,
+                     int nc, int D, float* out, int64_t ldo, int col0);
+int lnb_ell_messages_adjoint(lnb_stream_t stream, const float* G, int64_t ldg, const float* ellT_val,
+                             const uint8_t* ellT_idx, const int32_t* ellT_max, const int32_t* gextT, const float* w,
+                             int B, int N, int E1, int c0, int nc, int D, float* gX, int64_t ldgx);
+
+/* ---------------------------------------------------------------------------------------
  * Set2Vec readout + output_func of MPNN (model/set2set.py:60-100, model/mpnn.py:198-207), every graph
  * of the batch in one launch.  Per graph, over its set (nodes with mask != 0, or all N when mask is
  * NULL), hidden [2D] = 0, mem [D] = 0, and `steps` times:

@@ -113,6 +113,10 @@ SIGNATURES = {
     'lnb_mpnn_edge_aggregate_backward':
         (c_int, [c_stream, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p, ctypes.c_void_p,
                  ctypes.c_void_p, c_int, c_int, c_int, c_int, c_f32p]),
+    'lnb_ell_messages': (c_int, [c_stream, c_f32p, c_i64] + [ctypes.c_void_p] * 5 + [c_int] * 6 +
+                         [c_f32p, c_i64, c_int]),
+    'lnb_ell_messages_adjoint': (c_int, [c_stream, c_f32p, c_i64] + [ctypes.c_void_p] * 5 + [c_int] * 6 +
+                                 [c_f32p, c_i64]),
     'lnb_set2vec': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
                             c_int, c_int, c_int, c_int, c_int, c_f32p]),
     'lnb_operator_chain': (c_int, [c_stream, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int, c_int,

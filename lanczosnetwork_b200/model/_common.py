@@ -42,8 +42,10 @@ def _raw(t):
   return t.tensor if isinstance(t, Ragged) else t
 
 
-# the bond-list records of one batch on the device (data.sparse_collate's layout), N = padding target
-SparseRecords = collections.namedtuple('SparseRecords', 'sizes node_ptr node_feat edge_ptr edges N')
+# the bond-list records of one batch on the device (data.sparse_collate's layout), N = padding target,
+# K = eigenpairs per graph of a batch without them (sparse_collate(..., eigs=False)), else None
+SparseRecords = collections.namedtuple('SparseRecords', 'sizes node_ptr node_feat edge_ptr edges N K',
+                                       defaults=(None,))
 
 
 def _opt(obj, name, default):
@@ -230,11 +232,31 @@ class SpectralNetBase(nn.Module):
     on the collated batch, bit for bit.  Inference only (raises under autograd).  Returns score or
     (score, loss)."""
     if self._check_mode():
-      raise NotImplementedError('forward_sparse is an inference path; train through forward()')
+      raise NotImplementedError('forward_sparse is an inference path; train through forward() or, from '
+                                'the same records, forward_sparse_train()')
     dev = self._device()
     inputs, impl, key = self._sparse_inputs(batch)
     score = self._graph_forward(impl, inputs, extra_key=key)
     return self._finish(score, self._to(dev, label))
+
+  def forward_sparse_train(self, batch, label=None):
+    """Differentiable forward from the same SPARSE batch as ``forward_sparse`` (data.sparse_collate
+    records, pinned host or device): the training formulation of lanczosnetwork_b200.train with its
+    operator products and adjoints over the ELL rows that lnb_graph_prepare_sparse builds
+    (ops.ell_messages), so neither the padded operators nor their host collate exist.  It runs the
+    training formulation whether or not autograd is on, applies the batch checks of ``forward_sparse``
+    before any device work, and takes no packed batch.  Returns score or (score, loss)."""
+    if not hasattr(self, '_train_records'):
+      raise NotImplementedError('%s has no training entry from sparse batches; train it through forward() '
+                                'on the collated batch' % type(self).__name__)
+    if 'blob' in batch:
+      raise NotImplementedError('%s.forward_sparse_train takes data.sparse_collate records, not packed '
+                                'batches' % type(self).__name__)
+    inputs, _, _ = self._sparse_inputs(batch)
+    dev = self._device()
+    raw = [self._to(dev, _raw(t)) for t in inputs]
+    recs = SparseRecords(*raw[:5], N=int(batch['N']), K=int(batch['K']) if 'K' in batch else None)
+    return self._finish(self._train_records(recs, *raw[5:]), self._to(dev, label))
 
   def _sparse_inputs(self, batch):
     """(inputs, impl, extra_key) of _graph_forward for a sparse batch: the bond-list records, whose

@@ -90,3 +90,8 @@ class DCNN(SpectralNetBase):
   def _forward_records(self, recs):
     _, node_ids, mask, _, L = self._prepare_records(recs, want_dense=True)
     return self._forward_impl(node_ids, L, mask)
+
+  def _train_records(self, recs):
+    from ..train import dcnn_train, ell_operator
+    prep, node_ids, mask, _, _ = self._prepare_records(recs)
+    return dcnn_train(self, node_ids, ell_operator(prep), mask)

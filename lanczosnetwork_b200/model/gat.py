@@ -145,3 +145,12 @@ class TrainableGAT(GAT):
   def _train_impl(self, node_feat, L, mask):
     from ..train import gat_train
     return gat_train(self, node_feat, L, mask)
+
+  def _train_records(self, recs):
+    from ..train import gat_train
+    if self.training and self.dropout > 0.0:
+      raise NotImplementedError('TrainableGAT: dropout %g in training mode is not implemented; train with '
+                                'dropout 0.0' % self.dropout)
+    _, node_ids, mask, _, _ = self._prepare_records(recs)
+    bias = ops.gat_bias_sparse(recs.sizes, recs.edge_ptr, recs.edges, recs.N, self.num_edgetype + 1)
+    return gat_train(self, node_ids, bias, mask)

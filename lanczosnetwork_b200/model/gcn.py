@@ -54,6 +54,11 @@ class GCN(SpectralNetBase):
         want_dense=not self._sparse_stack_ok(recs.N, E1, 4))
     return self._ritz_conv_stack(None, node_ids, L, None, V, mask, prep=prep, dims_hint=(recs.N, E1))
 
+  def _train_records(self, recs):
+    from ..train import ell_operator, ritz_stack_train
+    prep, node_ids, mask, _, _ = self._prepare_records(recs, binarize=getattr(self, '_binarize_operators', False))
+    return ritz_stack_train(self, None, node_ids, ell_operator(prep), None, None, mask)
+
 
 class GCNFP(GCN):
   """Drop-in for the reference ``model.GCNFP`` (model/gcnfp.py:8-125): GCN on the non-zero pattern

@@ -213,6 +213,15 @@ class GPNN(SpectralNetBase):
                                                       self.num_partition, self.num_edgetype)
     return self._propagate(node_ids, prep, pprep, mask)
 
+  def _train_records(self, recs):
+    # the partition operators are constants, as on the padded path: their ELL rows straight from
+    # lnb_spectral_partition_sparse
+    from ..train import ell_operator, gpnn_train
+    prep, node_ids, mask, _, _ = self._prepare_records(recs, binarize=True)
+    _, _, pprep, _, _ = ops.spectral_partition_sparse(recs.sizes, recs.edge_ptr, recs.edges, recs.N,
+                                                      self.num_partition, self.num_edgetype)
+    return gpnn_train(self, node_ids, ell_operator(prep), ell_operator(pprep), None, mask)
+
   def _propagate(self, node_feat, prep, pprep, mask):
     """The fused inference forward from the binarised ELL rows of L and those of [L_cluster, L_cut]."""
     B, N = node_feat.shape

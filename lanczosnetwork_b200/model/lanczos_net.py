@@ -61,6 +61,17 @@ class LanczosNet(SpectralNetBase):
               Ragged(batch['edges']), Ragged(batch['V_rows'], B * N), batch['D'])
     return inputs, lambda *a: self._forward_sparse_impl(N, *a), ('sparse', N)
 
+  def _train_records(self, recs, V_rows=None, D=None):
+    # records without eigenpairs get them from lnb_graph_eigs_sparse, as data (no gradient flows to them)
+    from ..train import ell_operator, ritz_stack_train
+    if V_rows is None:
+      D, V_rows, _ = ops.graph_eigs_sparse(recs.sizes, recs.node_ptr, recs.edge_ptr, recs.edges, recs.N, recs.K,
+                                           num_edgetype=self.num_edgetype, rows=recs.node_feat.shape[0])
+    prep, node_ids, mask, V, _ = ops.graph_prepare_sparse(
+        recs.sizes, recs.node_ptr, recs.node_feat, recs.edge_ptr, recs.edges, V_rows.float().contiguous(), recs.N,
+        self.num_edgetype + 1)
+    return ritz_stack_train(self, None, node_ids, ell_operator(prep), D, V, mask)
+
   def _forward_packed_impl(self, B, N, K, blob):
     E1 = self.num_edgetype + 1
     dense = not self._sparse_stack_ok(N, E1, K)

@@ -187,6 +187,11 @@ class MPNN(SpectralNetBase):
       return self._train_impl(node_ids, L, mask)
     return self._propagate(node_ids, prep, mask)
 
+  def _train_records(self, recs):
+    from ..train import ell_operator, mpnn_train
+    prep, node_ids, mask, _, _ = self._prepare_records(recs, binarize=True)
+    return mpnn_train(self, node_ids, ell_operator(prep), mask)
+
   def _propagate(self, node_feat, prep, mask):
     """The fused inference forward from the ELL rows of the 0/1 operators."""
     B, N = node_feat.shape

@@ -20,7 +20,8 @@ __all__ = [
     'sage_operators', 'neighbour_max', 'sage_lstm_step', 'sage_lstm_step_supported', 'sage_lstm_messages',
     'ggnn_update',
     'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
-    'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'set2vec', 'set2vec_supported',
+    'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'ell_messages', 'ell_messages_adjoint',
+    'set2vec', 'set2vec_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
     'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
@@ -991,6 +992,130 @@ def mpnn_edge_aggregate_backward(PQ, gS, prep, prep_t, avg):
         _stream(PQ), _ptr(PQ), _ptr(gS), _ptr(prep[0]), _ptr(prep[1]), _ptr(prep[2]), _ptr(prep_t[0]),
         _ptr(prep_t[1]), _ptr(prep_t[2]), B, N, E1, int(bool(avg)), _ptr(gPQ)), 'lnb_mpnn_edge_aggregate_backward')
   return gPQ
+
+
+ELL_MAX_N = 128
+ELL_MAX_E1 = 16
+
+
+def _ell_operator(who, prep, c0, nc):
+  """(B, N, E1, nc) of the ELL rows ``prep`` for the channels [c0, c0 + nc), or ValueError."""
+  if len(prep) < 4:
+    raise ValueError('%s: prep must be a GraphPrep (ell_val, ell_idx, ell_max, gext, ...)' % who)
+  val, idx, emax, gext = prep[0], prep[1], prep[2], prep[3]
+  if val.dim() != 4 or val.shape[2] != val.shape[3]:
+    raise ValueError('%s: ell_val must be [B, E1, N, N]; got %s' % (who, tuple(val.shape)))
+  B, E1, N = val.shape[0], val.shape[1], val.shape[2]
+  if not (1 <= N <= ELL_MAX_N and 1 <= E1 <= ELL_MAX_E1):
+    raise ValueError('%s: N=%d, E1=%d outside 1 <= N <= %d, 1 <= E1 <= %d' % (who, N, E1, ELL_MAX_N, ELL_MAX_E1))
+  if (val.dtype != torch.float32 or idx.dtype != torch.uint8 or emax.dtype != torch.int32 or
+      gext.dtype != torch.int32):
+    raise ValueError('%s: ELL rows must be float32 / uint8 / int32 / int32 (ell_val, ell_idx, ell_max, gext)' % who)
+  if (tuple(idx.shape) != tuple(val.shape) or tuple(emax.shape) != (B, E1) or tuple(gext.shape) != (B, 2) or
+      not (val.is_contiguous() and idx.is_contiguous() and emax.is_contiguous() and gext.is_contiguous())):
+    raise ValueError('%s: ell_idx / ell_max / gext do not agree with ell_val %s' % (who, tuple(val.shape)))
+  nc = E1 - c0 if nc is None else int(nc)
+  if not (0 <= c0 and nc >= 1 and c0 + nc <= E1):
+    raise ValueError('%s: channels [%d, %d) outside [0, %d)' % (who, c0, c0 + nc, E1))
+  return B, N, E1, nc
+
+
+def _ell_rows(who, name, t, rows, width, dev):
+  """A row-strided float32 [rows, >= width] view with unit column stride on ``dev``, or ValueError."""
+  if t.dtype != torch.float32 or t.dim() != 2 or t.shape[0] != rows or t.shape[1] < width:
+    raise ValueError('%s: %s must be float32 [%d, >= %d]; got %s %s' % (who, name, rows, width, t.dtype,
+                                                                        tuple(t.shape)))
+  if t.device != dev:
+    raise ValueError('%s: %s is on %s, the operators on %s' % (who, name, t.device, dev))
+  if rows > 1 and t.stride(0) < width or (width > 1 and t.stride(1) != 1):
+    raise ValueError('%s: %s needs unit column stride and a row stride >= %d; got strides %s'
+                     % (who, name, width, t.stride()))
+  return max(int(t.stride(0)), width)
+
+
+def _span(t, width):
+  """[first, last) byte addresses a row-strided float32 view of ``width`` columns reads or writes."""
+  rows = t.shape[0] if t.dim() == 2 else 1
+  if rows == 0 or width == 0:
+    return (t.data_ptr(), t.data_ptr())
+  stride = t.stride(0) if t.dim() == 2 else 0
+  return (t.data_ptr(), t.data_ptr() + 4 * ((rows - 1) * stride + width))
+
+
+def _ell_no_overlap(who, out, out_width, inputs):
+  """ValueError when ``out`` shares storage bytes with any of ``inputs`` ((name, tensor, width) triples):
+  the kernels read their inputs while other threads write ``out``."""
+  o0, o1 = _span(out, out_width)
+  for name, t, width in inputs:
+    if t is None:
+      continue
+    a0, a1 = _span(t, width)
+    if a0 < o1 and o0 < a1:
+      raise ValueError('%s: out overlaps %s' % (who, name))
+
+
+def _ell_weight(who, w, B, N, E1, dev):
+  if w is None:
+    return None
+  if w.dtype != torch.float32 or tuple(w.shape) != (B, N, E1) or not w.is_contiguous() or w.device != dev:
+    raise ValueError('%s: w must be a contiguous float32 [%d, %d, %d] tensor on %s' % (who, B, N, E1, dev))
+  return w
+
+
+def ell_messages(X, prep, c0=0, nc=None, w=None, out=None, col0=0):
+  """L_e X over the ELL rows ``prep`` (graph_prepare / graph_prepare_sparse) for the channels
+  c0 <= e < c0 + nc (default: all from c0), without the dense operators (lnb_ell_messages):
+  out[b*N+n, col0 + (e-c0)*D + d] = w[b,n,e] * sum_t val[b,e,t,n] X[b*N + idx[b,e,t,n], d].
+  X [B*N, D] and ``out`` [B*N, >= col0 + nc*D] are float32 views with unit column stride (any row stride);
+  w [B,N,E1] optional row weights.  Returns out (a new [B*N, nc*D] tensor when not given)."""
+  B, N, E1, nc = _ell_operator('ell_messages', prep, int(c0), nc)
+  dev = prep[0].device
+  D = X.shape[1] if X.dim() == 2 else -1
+  if D < 1:
+    raise ValueError('ell_messages: X must be [B*N, D] with D >= 1; got %s' % (tuple(X.shape),))
+  ldx = _ell_rows('ell_messages', 'X', X, B * N, D, dev)
+  w = _ell_weight('ell_messages', w, B, N, E1, dev)
+  col0 = int(col0)
+  if col0 < 0:
+    raise ValueError('ell_messages: negative column offset %d' % col0)
+  if out is not None:
+    _ell_rows('ell_messages', 'out', out, B * N, col0 + nc * D, dev)
+    _ell_no_overlap('ell_messages', out, col0 + nc * D, (('X', X, D), ('w', w, None if w is None else w.numel())))
+  _need_cuda(*prep[:4], X, w, out)
+  if out is None:
+    out = torch.empty((B * N, col0 + nc * D), device=dev, dtype=torch.float32)
+  ldo = _ell_rows('ell_messages', 'out', out, B * N, col0 + nc * D, dev)
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_ell_messages(
+        _stream(X), _ptr(X), ldx, _ptr(prep[0]), _ptr(prep[1]), _ptr(prep[2]), _ptr(prep[3]), _ptr(w), B, N, E1,
+        int(c0), nc, D, _ptr(out), ldo, col0), 'lnb_ell_messages')
+  return out
+
+
+def ell_messages_adjoint(G, prep_t, D, c0=0, nc=None, w=None, out=None):
+  """The adjoint of ell_messages (lnb_ell_messages_adjoint): gX[b*N+m, d] = sum_e L_e^T (w_e . G_e), read
+  from the ELL rows ``prep_t`` of the TRANSPOSED operators, every channel summed in one thread without
+  atomics.  G [B*N, >= nc*D] (column block e - c0 = G_e) and ``out`` [B*N, >= D] are float32 views with unit
+  column stride; w [B,N,E1] the forward's row weights.  Returns out (a new [B*N, D] tensor when not given)."""
+  B, N, E1, nc = _ell_operator('ell_messages_adjoint', prep_t, int(c0), nc)
+  dev = prep_t[0].device
+  D = int(D)
+  if D < 1:
+    raise ValueError('ell_messages_adjoint: D=%d must be >= 1' % D)
+  ldg = _ell_rows('ell_messages_adjoint', 'G', G, B * N, nc * D, dev)
+  w = _ell_weight('ell_messages_adjoint', w, B, N, E1, dev)
+  if out is not None:
+    _ell_rows('ell_messages_adjoint', 'out', out, B * N, D, dev)
+    _ell_no_overlap('ell_messages_adjoint', out, D, (('G', G, nc * D), ('w', w, None if w is None else w.numel())))
+  _need_cuda(*prep_t[:4], G, w, out)
+  if out is None:
+    out = torch.empty((B * N, D), device=dev, dtype=torch.float32)
+  ldgx = _ell_rows('ell_messages_adjoint', 'out', out, B * N, D, dev)
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_ell_messages_adjoint(
+        _stream(G), _ptr(G), ldg, _ptr(prep_t[0]), _ptr(prep_t[1]), _ptr(prep_t[2]), _ptr(prep_t[3]), _ptr(w),
+        B, N, E1, int(c0), nc, D, _ptr(out), ldgx), 'lnb_ell_messages_adjoint')
+  return out
 
 
 def set2vec_supported(N, D, P):

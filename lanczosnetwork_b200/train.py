@@ -22,11 +22,13 @@ the one-launch fused stack remains the inference path.  Gradients are checked ag
 ``torch.autograd`` over the fp64 CPU oracle in tests/test_gpu_train.py, and function by function
 across the shapes they accept in tests/test_gpu_train_envelope.py.
 """
+import collections
+
 import torch
 
 from . import ops
 
-__all__ = ['dense', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
+__all__ = ['dense', 'EllOperator', 'ell_operator', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
            'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
            'lstm_messages', 'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'gat_attention',
            'gat_train', 'GraphedStep']
@@ -135,8 +137,96 @@ class _OperatorMessages(torch.autograd.Function):
     return None, tmp.sum(dim=1), None, None
 
 
+class EllOperator(collections.namedtuple('EllOperator', 'prep prep_t weight')):
+  """Operators [B,N,N,E1] held as ELL rows instead of a dense tensor: ``prep`` (ops.graph_prepare /
+  graph_prepare_sparse / spectral_partition_sparse), ``prep_t`` the ELL rows of the transposed operators
+  (the adjoint reads them), ``weight`` optional row weights [B,N,E1] (the ``avg`` aggregations) or None.
+  The training functions that take a dense L take this too; their products then run on
+  ops.ell_messages / ell_messages_adjoint."""
+
+  @property
+  def shape(self):
+    B, E1, N = self.prep[0].shape[0], self.prep[0].shape[1], self.prep[0].shape[2]
+    return (B, N, N, E1)
+
+
+def ell_operator(prep, prep_t=None):
+  """EllOperator of ``prep``; ``prep_t`` defaults to ``prep`` itself, right for symmetric operators (the
+  bond-list records: every bond is listed once and both entries of a pair get the same value)."""
+  return EllOperator(prep, prep if prep_t is None else prep_t, None)
+
+
+def _row_sums(op):
+  """sum_j L_e[b, n, j] as [B,N,E1], in ELL slot order: ops.ell_messages of a ones column."""
+  B, N, _, E1 = op.shape
+  ones = torch.ones((B * N, 1), device=op.prep[0].device, dtype=torch.float32)
+  return ops.ell_messages(ones, op.prep).reshape(B, N, E1)
+
+
+def _rows_view(g, width):
+  """g as a view the ELL kernels read in place (unit column stride, row stride >= width), else a copy."""
+  if g.dim() == 2 and (g.shape[1] <= 1 or g.stride(1) == 1) and (g.shape[0] <= 1 or g.stride(0) >= width):
+    return g
+  return g.contiguous()
+
+
+class _EllMessages(torch.autograd.Function):
+  """``_OperatorMessages`` over an EllOperator: X [B*N, D] -> [B*N, nc*D] (lnb_ell_messages); adjoint
+  gX = sum_e L_e^T (w_e . g_e) over the transposed rows (lnb_ell_messages_adjoint).  On 0/1 or unweighted
+  operators both directions give the dense path's bits."""
+
+  @staticmethod
+  def forward(ctx, X, op, c0, nc):
+    ctx.op, ctx.c0, ctx.nc, ctx.D = op, c0, nc, X.shape[1]
+    return ops.ell_messages(_rows_view(X, X.shape[1]), op.prep, c0, nc, w=op.weight)
+
+  @staticmethod
+  def backward(ctx, g):
+    g = _rows_view(g, ctx.nc * ctx.D)
+    op, D, nc = ctx.op, ctx.D, ctx.nc
+    if nc == 1:
+      return ops.ell_messages_adjoint(g, op.prep_t, D, ctx.c0, 1, w=op.weight), None, None, None
+    # one product per channel, summed by the same torch reduction over the same [B, nc, N, D] layout as
+    # _OperatorMessages: the per-channel products are the dense path's bits, so the sum is too
+    B, N = op.shape[0], op.shape[1]
+    tmp = torch.stack([ops.ell_messages_adjoint(g[:, k * D:(k + 1) * D], op.prep_t, D, ctx.c0 + k, 1,
+                                                w=op.weight).view(B, N, D) for k in range(nc)], dim=1)
+    return tmp.sum(dim=1).reshape(B * N, D), None, None, None
+
+
+class _EllChannelMessages(torch.autograd.Function):
+  """[A_e m_e]_e as [B*N, E1*D] over an EllOperator, one message per channel: every channel's product is
+  written straight into its column block (no concatenation); the adjoint reads g's blocks in place."""
+
+  @staticmethod
+  def forward(ctx, op, *msgs):
+    D = msgs[0].shape[1]
+    out = torch.empty((msgs[0].shape[0], len(msgs) * D), device=msgs[0].device, dtype=torch.float32)
+    for e, m in enumerate(msgs):
+      ops.ell_messages(_rows_view(m, D), op.prep, e, 1, w=op.weight, out=out, col0=e * D)
+    ctx.op, ctx.D, ctx.E1 = op, D, len(msgs)
+    return out
+
+  @staticmethod
+  def backward(ctx, g):
+    D = ctx.D
+    g = _rows_view(g, ctx.E1 * D)
+    return (None,) + tuple(ops.ell_messages_adjoint(g[:, e * D:(e + 1) * D], ctx.op.prep_t, D, e, 1, w=ctx.op.weight)
+                           for e in range(ctx.E1))
+
+
+def _operator(L):
+  """The operators as the training functions read them: an EllOperator as is, a dense L as fp32."""
+  return L if isinstance(L, EllOperator) else L.float().contiguous()
+
+
 def operator_messages(L, X, c0=0, nc=None):
-  return _OperatorMessages.apply(L, X, c0, L.shape[3] - c0 if nc is None else nc)
+  """[L_e X]_{c0 <= e < c0 + nc} as [B,N,nc*D] for a dense L [B,N,N,E1] or an EllOperator."""
+  nc = L.shape[3] - c0 if nc is None else nc
+  if isinstance(L, EllOperator):
+    B, N, D = X.shape
+    return _EllMessages.apply(X.reshape(B * N, D), L, c0, nc).reshape(B, N, nc * D)
+  return _OperatorMessages.apply(L, X, c0, nc)
 
 
 class _SpectralMessages(torch.autograd.Function):
@@ -241,13 +331,18 @@ def _input_state(model, node_ids, table):
 
 
 def _row_normalised(A):
-  """A / (rowsum + float32 eps): the ``avg`` aggregation of GGNN, GPNN and MPNN."""
+  """A / (rowsum + float32 eps): the ``avg`` aggregation of GGNN, GPNN and MPNN.  An EllOperator gets
+  the row weights 1 / (rowsum + eps) instead, its row sums in ELL slot order."""
+  if isinstance(A, EllOperator):
+    return A._replace(weight=1.0 / (_row_sums(A) + _EPS))
   return A / (A.sum(dim=2, keepdim=True) + _EPS)
 
 
 def _channel_messages(A, msgs):
   """[A_e m_e]_e as [B*N, E1*D] for the per-channel messages m_e [B*N, D] (an iterable, consumed in
   channel order)."""
+  if isinstance(A, EllOperator):
+    return _EllChannelMessages.apply(A, *list(msgs))
   B, N = A.shape[0], A.shape[1]
   agg = torch.cat([operator_messages(A, m.reshape(B, N, -1), e, 1) for e, m in enumerate(msgs)], dim=2)
   return agg.reshape(B * N, -1)
@@ -255,8 +350,9 @@ def _channel_messages(A, msgs):
 
 def ritz_stack_train(model, state, node_ids, L, D, V, mask):
   """Differentiable convolution stack + readout of LanczosNet / LanczosNetGeneral / GCN
-  (model/lanczos_net.py:125-199): same math, same parameter tensors as the inference path."""
-  L = L.float().contiguous()
+  (model/lanczos_net.py:125-199): same math, same parameter tensors as the inference path.  L: dense
+  [B,N,N,E1] or an EllOperator."""
+  L = _operator(L)
   if node_ids is not None:
     state = embedding(node_ids, model.embedding.weight)
   else:
@@ -301,8 +397,9 @@ def gated_readout(model, state, mask, head=None):
 
 def dcnn_train(model, node_ids, L, mask):
   """Differentiable DCNN (model/dcnn.py:64-124): per layer the edge-type products, then the walk
-  L_0^k X for k in diffusion_dist, concatenated EDGES FIRST (:98), Linear + ReLU."""
-  L = L.float().contiguous()
+  L_0^k X for k in diffusion_dist, concatenated EDGES FIRST (:98), Linear + ReLU.  L: dense or an
+  EllOperator."""
+  L = _operator(L)
   state = embedding(node_ids, model.embedding.weight)
   dist = set(model.diffusion_dist)
   for t in range(model.num_layer):
@@ -313,8 +410,8 @@ def dcnn_train(model, node_ids, L, mask):
 def cheby_train(model, node_ids, L, mask):
   """Differentiable ChebyNet (model/cheby_net.py:64-124): s_0 = L_0 X, s_k = 2 L_0 s_{k-1} - s_{k-2}
   with s_{-1} = X (the reference's index -1 is its LAST slot, :88-93), bond-type products for e >= 1,
-  cat(edges + [s_0 .. s_{order-1}] + [X]) (:99), Linear + ReLU."""
-  L = L.float().contiguous()
+  cat(edges + [s_0 .. s_{order-1}] + [X]) (:99), Linear + ReLU.  L: dense or an EllOperator."""
+  L = _operator(L)
   state = embedding(node_ids, model.embedding.weight)
   E1 = L.shape[3]
   order = model.polynomial_order
@@ -452,7 +549,11 @@ def recurrent_cell(kind, cell, x, h):
 
 
 def _ggnn_operators(L, aggregate_type):
-  """The 0/1 pattern of L, row-normalised by (nnz + float32 eps) for ``avg``: a new tensor."""
+  """The 0/1 pattern of L, row-normalised by (nnz + float32 eps) for ``avg``: a new tensor.  An
+  EllOperator must already hold the pattern (graph_prepare(..., binarize=True)); ``avg`` gives it row
+  weights."""
+  if isinstance(L, EllOperator):
+    return _row_normalised(L) if aggregate_type == 'avg' else L
   A = (L != 0).float()
   if aggregate_type == 'avg':
     A = _row_normalised(A)
@@ -495,12 +596,17 @@ def gpnn_train(model, node_ids, L, L_cluster, L_cut, mask):
   operator, both chains from the same state -> state_func on [state | cluster | cut] -> the GGNN step over
   the 0/1 pattern of L -> dropout] -> gated readout with the head ``output_func``.  P is the valued
   partition operator, row-normalised by (rowsum + float32 eps) for ``avg``; all operators are new tensors
-  (the caller's L, L_cluster and L_cut are not modified)."""
+  (the caller's L, L_cluster and L_cut are not modified).  With an EllOperator L (the 0/1 pattern),
+  ``L_cluster`` is the EllOperator of the two-channel [L_cluster, L_cut] and ``L_cut`` is None."""
   A = _ggnn_operators(L, model.aggregate_type)
-  P = torch.stack([L_cluster, L_cut], 3).float()
+  if isinstance(L_cluster, EllOperator):
+    P = L_cluster
+  else:
+    P = torch.stack([L_cluster, L_cut], 3).float()
   if model.aggregate_type == 'avg':
     P = _row_normalised(P)
-  P = P.contiguous()
+  if not isinstance(P, EllOperator):
+    P = P.contiguous()
   B, N = A.shape[0], A.shape[1]
   h = _input_state(model, node_ids, model.embedding.weight)
   D = h.shape[1]
@@ -577,17 +683,22 @@ def mpnn_train(model, node_ids, L, mask):
   -> GRU cell -> dropout] -> Set2Vec -> output_func.  ``MLP`` messages: PQ = dense(h, [W1a_e ; W1b_e]),
   S = edge_aggregate(PQ), agg_e = S_e W2_e^T + (w nnz_e) b2_e; ``embedding`` messages: A_e (h E_e) as in
   ggnn_train.  A_e is the 0/1 pattern of L_e (row-normalised by nnz + float32 eps for ``avg``); the
-  caller's L is not modified."""
-  A = (L != 0).float()
-  nnz = A.sum(dim=2)                                                           # [B,N,E1]
+  caller's L is not modified.  An EllOperator L must hold the pattern (graph_prepare(..., binarize=True));
+  its ``prep`` / ``prep_t`` then feed edge_aggregate directly."""
+  ell = isinstance(L, EllOperator)
+  A = L if ell else (L != 0).float()
+  nnz = _row_sums(A) if ell else A.sum(dim=2)                                  # [B,N,E1]
   avg = model.aggregate_type == 'avg'
   B, N, E1 = A.shape[0], A.shape[1], A.shape[3]
   h = _input_state(model, node_ids, model.node_embedding.weight)
   D = h.shape[1]
   if model.msg_func_name == 'MLP':
-    zeros = torch.zeros((B, N, 4), device=L.device, dtype=torch.float32)
-    prep = ops.graph_prepare(L, zeros, binarize=True)
-    prep_t = ops.graph_prepare(L.transpose(1, 2), zeros, binarize=True)
+    if ell:
+      prep, prep_t = L.prep, L.prep_t
+    else:
+      zeros = torch.zeros((B, N, 4), device=L.device, dtype=torch.float32)
+      prep = ops.graph_prepare(L, zeros, binarize=True)
+      prep_t = ops.graph_prepare(L.transpose(1, 2), zeros, binarize=True)
     deg = (nnz * (1.0 / (nnz + _EPS)) if avg else nnz).reshape(B * N, E1)     # w_i nnz_e(i)
     first = [seq[0] for seq in model.edge_func]
     second = [seq[2] for seq in model.edge_func]
@@ -597,7 +708,8 @@ def mpnn_train(model, node_ids, L, mask):
   else:
     if avg:
       A = _row_normalised(A)
-    A = A.contiguous()
+    if not ell:
+      A = A.contiguous()
     w_msg = model.edge_embedding.weight.view(E1, D, D).transpose(1, 2).reshape(E1 * D, D)    # stacked E_e^T
   for _ in range(model.num_prop):
     if model.msg_func_name == 'MLP':
@@ -818,18 +930,36 @@ class GraphedStep:
   the object does not advance training.  Not for AdaLanczosNet (its start vector is drawn on the
   host each call)."""
 
-  def __init__(self, model, optimizer, args, kwargs=None, warmup=3):
+  def __init__(self, model, optimizer, args, kwargs=None, warmup=3, sparse=False, edge_capacity=None):
+    """``sparse=True``: ``args`` is ``(batch,)``, the records of data.sparse_collate as torch tensors, and the
+    step is ``model.forward_sparse_train(batch, label=label)``.  ``node_feat`` gets a static buffer of B*N
+    rows, ``edges`` one of ``edge_capacity`` rows (default: the ``Ragged`` bucket of the first batch), and a
+    replay copies only the rows present, so one capture serves every batch with the same B, N and K."""
     kwargs = dict(kwargs or {})
-    if not hasattr(type(model), '_train_impl') or type(model).__name__ == 'AdaLanczosNet':
+    if sparse:
+      if not hasattr(model, '_train_records'):
+        raise TypeError('GraphedStep(sparse=True) needs a drop-in module with forward_sparse_train; %s has none'
+                        % type(model).__name__)
+      if len(args) != 1 or not isinstance(args[0], dict) or 'blob' in args[0]:
+        raise ValueError('GraphedStep(sparse=True) takes one argument: the data.sparse_collate records (batch,)')
+      model._sparse_inputs(args[0])                          # forward_sparse's batch checks
+    elif not hasattr(type(model), '_train_impl') or type(model).__name__ == 'AdaLanczosNet':
       raise TypeError('GraphedStep needs a drop-in module with a host-free training forward')
     if kwargs.get('label') is None:
       raise ValueError('GraphedStep captures the loss: pass label=')
+    if sparse:
+      from .model._common import Ragged
+      edges = args[0]['edges']
+      cap = Ragged(edges, edge_capacity).capacity            # ValueError if the first batch does not fit
     dev = model._device()
     if dev.type != 'cuda':
       raise RuntimeError('GraphedStep needs the module on a CUDA device')
     model.train()
-    self.model, self.optimizer = model, optimizer
-    self._args = [self._static(a, dev) for a in args]
+    self.model, self.optimizer, self.sparse = model, optimizer, bool(sparse)
+    if sparse:
+      self._args = [self._static_records(args[0], dev, cap)]
+    else:
+      self._args = [self._static(a, dev) for a in args]
     self._kwargs = {k: self._static(v, dev) for k, v in kwargs.items()}
     for group in optimizer.param_groups:
       if 'capturable' in group:
@@ -864,10 +994,63 @@ class GraphedStep:
   def _static(x, dev):
     return x.detach().to(dev).clone() if torch.is_tensor(x) else x
 
+  # the ragged record arrays: static buffers of more rows than a batch fills, only the rows present copied
+  _RAGGED = ('node_feat', 'edges', 'V_rows')
+  _RECORD_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N', 'K', 'V_rows', 'D')
+
+  def _static_records(self, batch, dev, cap):
+    B, N = int(batch['sizes'].shape[0]), int(batch['N'])
+    rows = {'node_feat': B * N, 'edges': cap, 'V_rows': B * N}
+    out = {}
+    for k in self._RECORD_KEYS:
+      if k not in batch:
+        continue
+      v = batch[k]
+      if k in self._RAGGED:
+        out[k] = torch.zeros((rows[k],) + tuple(v.shape[1:]), dtype=v.dtype, device=dev)
+        out[k][:v.shape[0]].copy_(v)
+      else:
+        out[k] = self._static(v, dev)
+    return out
+
+  def _copy_records(self, batch, kwargs):
+    """Checks ``batch`` and the tensor ``kwargs`` (the label) against the captured buffers, ValueError before
+    anything is copied; then copies the rows present and the kwargs."""
+    static = self._args[0]
+    for k, dst in self._kwargs.items():
+      if torch.is_tensor(dst):
+        src = kwargs.get(k)
+        if not torch.is_tensor(src) or tuple(src.shape) != tuple(dst.shape):
+          raise ValueError('GraphedStep was captured for %s %s, got %s'
+                           % (k, tuple(dst.shape), tuple(src.shape) if torch.is_tensor(src) else src))
+    if set(k for k in self._RECORD_KEYS if k in batch) != set(static):
+      raise ValueError('GraphedStep was captured for records with %s, got %s'
+                       % (sorted(static), sorted(k for k in self._RECORD_KEYS if k in batch)))
+    for k, dst in static.items():
+      src = batch[k]
+      if not torch.is_tensor(dst):
+        if int(src) != dst:
+          raise ValueError('GraphedStep was captured for %s=%d, got %d' % (k, dst, int(src)))
+      elif k in self._RAGGED:
+        if src.shape[0] > dst.shape[0] or tuple(src.shape[1:]) != tuple(dst.shape[1:]) or src.dtype != dst.dtype:
+          raise ValueError('GraphedStep: %s %s does not fit the captured buffer %s (%s)'
+                           % (k, tuple(src.shape), tuple(dst.shape), dst.dtype))
+      elif tuple(src.shape) != tuple(dst.shape) or src.dtype != dst.dtype:
+        raise ValueError('GraphedStep was captured for %s %s, got %s' % (k, tuple(dst.shape), tuple(src.shape)))
+    for k, dst in static.items():
+      if torch.is_tensor(dst):
+        (dst[:batch[k].shape[0]] if k in self._RAGGED else dst).copy_(batch[k], non_blocking=True)
+    for k, dst in self._kwargs.items():
+      if torch.is_tensor(dst):
+        dst.copy_(kwargs[k], non_blocking=True)
+
   def _body(self, zero=True):
     if zero:
       self.optimizer.zero_grad(set_to_none=True)
-    score, loss = self.model(*self._args, **self._kwargs)
+    if self.sparse:
+      score, loss = self.model.forward_sparse_train(self._args[0], **self._kwargs)
+    else:
+      score, loss = self.model(*self._args, **self._kwargs)
     loss.backward()
     self.optimizer.step()
     return score, loss
@@ -875,6 +1058,11 @@ class GraphedStep:
   def __call__(self, *args, **kwargs):
     """Copy this batch into the captured buffers and replay.  Returns (score, loss): static device
     tensors that the next call overwrites."""
+    if self.sparse:
+      self._copy_records(args[0], kwargs)
+      self.graph.replay()
+      self.replays += 1
+      return self.score, self.loss
     for dst, src in zip(self._args, args):
       if torch.is_tensor(dst):
         if dst.shape != src.shape:
