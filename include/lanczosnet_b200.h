@@ -253,6 +253,42 @@ int lnb_neighbour_max(lnb_stream_t stream, const float* X, const float* ell_val,
                       int32_t* argmax /* [B,N,E1,D] */);
 
 /* ---------------------------------------------------------------------------------------
+ * GraphSAGE's neighbour samples drawn on the device from the SPARSE records of
+ * lnb_graph_prepare_sparse (sizes, node_ptr, node_feat, edge_ptr, edges; same layouts, bond types
+ * >= E1 - 1 ignored), one CTA per graph.  The rule, for graph b, node n < sizes[b] and channel e:
+ *   candidates c[0..L): the non-zero columns of row n of channel e of the padded L4 operator
+ *     (channel 0 the simple graph, e >= 1 bond type e - 1), ascending -- n itself and its bonded
+ *     neighbours;
+ *   x_i = word i % 4 of Philox4x32-10 (Random123's constants) at key (seed lo, seed hi) and counter
+ *     (i / 4, r, ctr lo, ctr hi), r = (b*N + n)*E1 + e, where (seed, ctr) = sample_key[0..1] (int64,
+ *     DEVICE memory: a captured graph draws anew when the caller rewrites the key);
+ *   L >= K: a partial Fisher-Yates, for i < K: j = i + floor(x_i (L - i) / 2^32), swap c[i], c[j],
+ *     sample i = c[i] (a uniform ordered K-subset, numpy's choice(replace=False));
+ *   1 <= L < K: sample i = c[floor(x_i L / 2^32)] (choice(replace=True));
+ *   L = 0 and padded rows: every sample is 0 (the reference collate's zero fill).
+ * nonempty[b, n] = 1 iff some channel has L >= 1, i.e. n < sizes[b].  The multiply-high mapping is
+ * biased by at most L / 2^32 per draw.
+ * Outputs: node_ids [B,N] int64, mask [B,N] uint8 and nonempty [B,N] fp32 always; with
+ *   LNB_SAGE_SAMPLE_NN_IDX nn_idx [B,N,K,E1] int32 (the collate's layout, what lnb_sage_lstm_step reads);
+ *   LNB_SAGE_SAMPLE_ELL the ELL rows, ell_max and gext that lnb_graph_prepare writes for the operator
+ *     of lnb_sage_operators on these samples with a zero Q (same values, same slot order; slots past
+ *     ell_max unwritten; no tile table: lnb_tile_assign builds it from gext);
+ *   LNB_SAGE_SAMPLE_ELL_T (needs LNB_SAGE_SAMPLE_ELL) the same for the transposed operator M_e^T
+ *     (ellT_*, gextT), which the training adjoint reads: M is not symmetric.
+ * Limits: 1 <= N <= 128, 2 <= E1 <= 16, K >= 1, B*N*E1 < 2^31 (LNB_ERR_UNSUPPORTED otherwise,
+ * nothing launched).  edges may be NULL for a batch without bonds.
+ * ------------------------------------------------------------------------------------- */
+#define LNB_SAGE_SAMPLE_NN_IDX 1
+#define LNB_SAGE_SAMPLE_ELL 2
+#define LNB_SAGE_SAMPLE_ELL_T 4
+int lnb_sage_sample_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
+                           const int32_t* node_feat, const int32_t* edge_ptr, const uint8_t* edges,
+                           const int64_t* sample_key, int B, int N, int E1, int K, int flags,
+                           int64_t* node_ids, uint8_t* mask, float* nonempty, int32_t* nn_idx,
+                           float* ell_val, uint8_t* ell_idx, int32_t* ell_max, int32_t* gext,
+                           float* ellT_val, uint8_t* ellT_idx, int32_t* ellT_max, int32_t* gextT);
+
+/* ---------------------------------------------------------------------------------------
  * Embedding rows (model/lanczos_net.py:154): out[r, :] = table[idx[r], :].
  * ------------------------------------------------------------------------------------- */
 int lnb_embedding_rows(lnb_stream_t stream, const int64_t* idx, const float* table,

@@ -85,6 +85,7 @@ SIGNATURES = {
     'lnb_sage_stack_forward': (c_int, [c_stream, ctypes.POINTER(SpectralStack), c_int]),
     'lnb_neighbour_max': (c_int, [c_stream, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_int, c_int,
                                   c_int, c_int, c_f32p, ctypes.c_void_p]),
+    'lnb_sage_sample_sparse': (c_int, [c_stream] + [ctypes.c_void_p] * 6 + [c_int] * 5 + [ctypes.c_void_p] * 12),
     'lnb_ritz_rowmap': (c_int, [c_stream, ctypes.c_void_p, c_int, c_int, ctypes.c_void_p, ctypes.c_void_p]),
     'lnb_ritz_filter_mlp': (c_int, [c_stream, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p, c_f32p,
                                     c_f32p, c_int, c_int, c_int, c_int, c_f32p]),

@@ -25,10 +25,10 @@ nothing (the reference raises an IndexError); under the LSTM aggregator such an 
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, init_cell, init_linears, loss_function
+from ._common import SparseRecords, SpectralNetBase, init_cell, init_linears, loss_function
 from .. import ops
 
-__all__ = ['GraphSAGE', 'LSTMGraphSAGE', 'lstm_gate_matrix', 'lstm_gate_matrix_inverse']
+__all__ = ['GraphSAGE', 'LSTMGraphSAGE', 'SampledGraphSAGE', 'lstm_gate_matrix', 'lstm_gate_matrix_inverse']
 
 SUPPORTED_AGGREGATORS = ('Mean', 'Max')
 EPS = 1.1920928955078125e-07       # np.finfo(np.float32).eps (graph_sage.py:6)
@@ -111,7 +111,11 @@ class GraphSAGE(SpectralNetBase):
       return sage_train(self, node_feat, M, mask)
     # no Ritz vectors: an all-zero block makes lnb_graph_prepare take the extents from M alone
     V = torch.zeros((B, N, 4), device=M.device, dtype=torch.float32)
-    prep = ops.graph_prepare(M, V)
+    return self._stack_score(ops.graph_prepare(M, V), V, node_feat, mask)
+
+  def _stack_score(self, prep, V, node_feat, mask):
+    """The whole model in lnb_sage_stack_forward on the ELL rows ``prep`` of M (V: the zero [B, N, 4])."""
+    E1 = prep[0].shape[1]
     layers = list(range(self.num_layer - 1))
     dims = [self.embedding.weight.shape[1]] + list(self.hidden_dim[:len(layers)])
     H = dims[1]
@@ -198,8 +202,12 @@ class LSTMGraphSAGE(GraphSAGE):
     if not self.lstm_supported(E1):
       from ..train import sage_train                # off the kernel: the training formulation (no_grad)
       return sage_train(self, node_feat, None, mask, samples=(nn_idx, nonempty_mask))
-    idx = nn_idx.to(torch.int32).contiguous()        # converted once per forward
-    ne = nonempty_mask.reshape(B * N).float().contiguous()
+    return self._lstm_score(node_feat, nn_idx.to(torch.int32).contiguous(),   # converted once per forward
+                            nonempty_mask.reshape(B * N).float().contiguous(), mask)
+
+  def _lstm_score(self, node_feat, idx, ne, mask):
+    """LSTM inference on lnb_sage_lstm_step: idx int32 [B, N, K, E1], ne float32 [B*N]."""
+    B, N = node_feat.shape
     state = ops.embedding_rows(node_feat.long().reshape(-1), self.embedding.weight)
     for t in range(self.num_layer - 1):
       g_hi, g_lo, g_b = self._gates(t)
@@ -209,3 +217,72 @@ class LSTMGraphSAGE(GraphSAGE):
       y = ops.linear_tf32x3(msg, w_hi, w_lo, lin.bias, relu=True)
       state = y / (torch.norm(y, 2, dim=1, keepdim=True) + EPS)
     return self._readout(state.view(B, N, -1), mask)
+
+
+class SampledGraphSAGE(LSTMGraphSAGE):
+  """``LSTMGraphSAGE`` (same constructor, parameters, initialisation and ``state_dict``; the same padded
+  ``forward``) that also runs and trains from the bond-list records of data.sparse_collate:
+  ``forward_sparse``, ``forward_sparse_train`` and ``train.GraphedStep(..., sparse=True)``.
+
+  The records carry no neighbour samples: they are drawn on the device (``ops.sage_sample_sparse``) from
+  the distributions of the reference's collate -- K distinct neighbours, or K with replacement when a node
+  has fewer -- with a counter-based generator keyed by ``batch['sample_key']``, an int64 tensor (seed,
+  counter) that the caller changes to get new samples (inside a captured graph too).  numpy's draws are not
+  reproduced, so this class does not make ``forward_sparse``'s usual promise of the collate's scores.  Its
+  contract instead: the scores are, bit for bit, those of ``forward`` on the padded batch built from
+  ``ops.sage_sample_sparse``'s samples (node_ids, nn_idx, nonempty, mask=mask), and the training entry
+  computes ``forward``'s training formulation on the same samples.
+
+  Mean / Max from records: sampler -> tile_assign -> lnb_sage_stack_forward (the count-weighted operator
+  M exists only as ELL rows); off the stack kernel they run ``train.sage_train`` under no_grad on those
+  rows.  LSTM reads the int32 samples directly.  Training: ``train.sage_train`` on the ELL rows of M and
+  M^T (Mean), of M (Max), or on the samples (LSTM)."""
+
+  def _check_runnable(self, N=None, E1=None):
+    if self.agg_func is None:
+      raise TypeError("SampledGraphSAGE: unknown agg_func %r; supported: Mean, Max, LSTM" % (self.agg_func_name,))
+
+  def _sparse_inputs(self, batch):
+    key = batch.get('sample_key') if isinstance(batch, dict) else None
+    if key is None:
+      raise ValueError("SampledGraphSAGE: the batch lacks 'sample_key', the int64 (seed, counter) tensor of "
+                       "the neighbour sampler")
+    if not torch.is_tensor(key) or key.dtype != torch.int64 or tuple(key.shape) != (2,):
+      raise ValueError("SampledGraphSAGE: 'sample_key' must be an int64 tensor of shape (2,); got %r"
+                       % ((key.dtype, tuple(key.shape)) if torch.is_tensor(key) else type(key),))
+    if 'blob' in batch:
+      raise NotImplementedError('SampledGraphSAGE takes data.sparse_collate records, not packed batches')
+    inputs, _, _ = super(SampledGraphSAGE, self)._sparse_inputs(batch)
+    N = int(batch['N'])
+    return (inputs + (key,), lambda *a: self._forward_records(SparseRecords(*a[:5], N=N), a[5]),
+            ('sampled', N))
+
+  def _sample(self, recs, key, **want):
+    return ops.sage_sample_sparse(recs.sizes, recs.node_ptr, recs.node_feat, recs.edge_ptr, recs.edges,
+                                  key.contiguous(), recs.N, self.num_edgetype + 1, self.num_sample_neighbors,
+                                  **want)
+
+  def _forward_records(self, recs, key):
+    from ..train import EllOperator, sage_train
+    E1 = self.num_edgetype + 1
+    if self.agg_func_name == 'LSTM':
+      node_ids, mask, nonempty, nn_idx, _, _ = self._sample(recs, key)
+      if not self.lstm_supported(E1):
+        return sage_train(self, node_ids, None, mask, samples=(nn_idx, nonempty))
+      return self._lstm_score(node_ids, nn_idx, nonempty.view(-1), mask)
+    node_ids, mask, _, _, prep, _ = self._sample(recs, key, want_nn_idx=False, want_ell=True)
+    if not self.stack_supported(recs.N, E1):
+      return sage_train(self, node_ids, EllOperator(prep, None, None), mask, prep=prep)   # no adjoint under no_grad
+    ops.tile_assign(prep, 4)
+    V = torch.zeros((node_ids.shape[0], recs.N, 4), device=node_ids.device, dtype=torch.float32)
+    return self._stack_score(prep, V, node_ids, mask)
+
+  def _train_records(self, recs, key):
+    from ..train import EllOperator, sage_train
+    if self.agg_func_name == 'LSTM':
+      node_ids, mask, nonempty, nn_idx, _, _ = self._sample(recs, key)
+      return sage_train(self, node_ids, None, mask, samples=(nn_idx, nonempty))
+    mean = self.agg_func_name == 'Mean'
+    node_ids, mask, _, _, prep, prep_t = self._sample(recs, key, want_nn_idx=False, want_ell=True, want_ell_t=mean)
+    # Max routes its gradient through the argmax and never reads the transposed rows
+    return sage_train(self, node_ids, EllOperator(prep, prep_t, None), mask, prep=prep)

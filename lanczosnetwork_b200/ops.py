@@ -17,7 +17,7 @@ __all__ = [
     'spectral_partition', 'spectral_partition_sparse', 'spectral_partition_supported', 'partition_draws', 'gat_bias_sparse',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
-    'sage_operators', 'neighbour_max', 'sage_lstm_step', 'sage_lstm_step_supported', 'sage_lstm_messages',
+    'sage_operators', 'sage_sample_sparse', 'neighbour_max', 'sage_lstm_step', 'sage_lstm_step_supported', 'sage_lstm_messages',
     'ggnn_update',
     'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
     'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'ell_messages', 'ell_messages_adjoint',
@@ -574,6 +574,61 @@ def neighbour_max(X, prep):
                                              _ptr(ell_max), B, N, E1, D, _ptr(out), _ptr(arg)),
                'lnb_neighbour_max')
   return out, arg
+
+
+SAGE_SAMPLE_NN_IDX, SAGE_SAMPLE_ELL, SAGE_SAMPLE_ELL_T = 1, 2, 4    # LNB_SAGE_SAMPLE_*
+
+
+def sage_sample_sparse(sizes, node_ptr, node_feat, edge_ptr, edges, sample_key, N, E1, K, want_nn_idx=True,
+                       want_ell=False, want_ell_t=False):
+  """GraphSAGE's neighbour samples drawn on the device from the records of data.sparse_collate
+  (lnb_sage_sample_sparse; the rule is in the C header): K samples per (graph, node, channel) from
+  Philox4x32-10 keyed by ``sample_key``, an int64 [2] CUDA tensor (seed, counter) read on the device.
+  ``want_nn_idx``: the samples [B,N,K,E1] int32.  ``want_ell``: a GraphPrep of the count-weighted operator
+  M = sage_operators(samples, nonempty), the ELL rows, ell_max and gext that graph_prepare(M) writes, its
+  tile table pending (tile_assign(prep, 4)).  ``want_ell_t``: the same for M.transpose(1, 2), no tiles.
+  Returns (node_ids [B,N] int64, mask [B,N] uint8, nonempty [B,N,1] fp32, nn_idx or None, prep or None,
+  prep_t or None)."""
+  N, E1, K = int(N), int(E1), int(K)
+  _check_records('sage_sample_sparse', sizes, edge_ptr, edges)
+  _need_cuda(node_ptr, node_feat, sample_key)
+  if node_ptr.dtype != torch.int32 or node_feat.dtype != torch.int32 or node_ptr.shape[0] != sizes.shape[0] + 1:
+    raise ValueError('sage_sample_sparse: node_ptr [B+1] and node_feat must be int32')
+  if sample_key.dtype != torch.int64 or tuple(sample_key.shape) != (2,) or not sample_key.is_contiguous():
+    raise ValueError('sage_sample_sparse: sample_key must be a contiguous int64 tensor of shape (2,); got %s %s'
+                     % (sample_key.dtype, tuple(sample_key.shape)))
+  B = sizes.shape[0]
+  if not (1 <= N <= 128 and 2 <= E1 <= 16 and K >= 1 and B * N * E1 < 2 ** 31):
+    raise ValueError('sage_sample_sparse: B=%d N=%d E1=%d K=%d outside 1 <= N <= 128, 2 <= E1 <= 16, K >= 1, '
+                     'B*N*E1 < 2^31' % (B, N, E1, K))
+  if want_ell_t and not want_ell:
+    raise ValueError('sage_sample_sparse: want_ell_t needs want_ell')
+  dev = sizes.device
+  node_ids = torch.empty((B, N), device=dev, dtype=torch.int64)
+  mask = torch.empty((B, N), device=dev, dtype=torch.uint8)
+  nonempty = torch.empty((B, N, 1), device=dev, dtype=torch.float32)
+  nn_idx = torch.empty((B, N, K, E1), device=dev, dtype=torch.int32) if want_nn_idx else None
+
+  def ell():
+    return (torch.empty((B, E1, N, N), device=dev, dtype=torch.float32),
+            torch.empty((B, E1, N, N), device=dev, dtype=torch.uint8),
+            torch.empty((B, E1), device=dev, dtype=torch.int32), torch.empty((B, 2), device=dev, dtype=torch.int32))
+  rows = ell() if want_ell else (None,) * 4
+  rows_t = ell() if want_ell_t else (None,) * 4
+  flags = ((SAGE_SAMPLE_NN_IDX if want_nn_idx else 0) | (SAGE_SAMPLE_ELL if want_ell else 0) |
+           (SAGE_SAMPLE_ELL_T if want_ell_t else 0))
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_sage_sample_sparse(
+        _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(node_feat), _ptr(edge_ptr), _ptr(edges),
+        _ptr(sample_key), B, N, E1, K, flags, _ptr(node_ids), _ptr(mask), _ptr(nonempty), _ptr(nn_idx),
+        *[_ptr(t) for t in rows + rows_t]), 'lnb_sage_sample_sparse')
+  prep = prep_t = None
+  if want_ell:
+    prep = GraphPrep(rows + (torch.empty((4 * B + 2,), device=dev, dtype=torch.int32),))
+    prep.tiles_pending = B > 0
+  if want_ell_t:
+    prep_t = GraphPrep(rows_t + (None,))
+  return node_ids, mask, nonempty, nn_idx, prep, prep_t
 
 
 SAGE_MAX = 1        # LNB_SAGE_MAX

@@ -459,10 +459,13 @@ def sage_train(model, node_ids, M, mask, prep=None, samples=None):
   [messages of every channel] -> Linear + ReLU -> row / (||row|| + eps) -> dropout -> gated readout
   with the head filter[num_layer].  Mean messages are M_e X on the count-weighted operators M
   [B,N,N,E1] (ops.sage_operators); Max messages come from ``neighbour_max`` on the ELL lists of M
-  (``prep``, built here when not given).  LSTM messages (``lstm_messages`` with the cell agg_func[t])
-  read ``samples`` = (nn_idx, nonempty_mask) instead; M is then unused."""
+  (``prep``, built here when not given).  M may be an EllOperator instead (its ``prep_t`` the rows of the
+  transposed M, which the Mean adjoint reads; Max takes ``prep`` from it).  LSTM messages (``lstm_messages``
+  with the cell agg_func[t]) read ``samples`` = (nn_idx, nonempty_mask) instead; M is then unused."""
   lstm = model.agg_func_name == 'LSTM'
-  if not lstm:
+  if isinstance(M, EllOperator):
+    prep = M.prep if prep is None else prep
+  elif not lstm:
     M = M.float().contiguous()
   state = embedding(node_ids, model.embedding.weight)
   B, N = state.shape[0], state.shape[1]
@@ -996,7 +999,7 @@ class GraphedStep:
 
   # the ragged record arrays: static buffers of more rows than a batch fills, only the rows present copied
   _RAGGED = ('node_feat', 'edges', 'V_rows')
-  _RECORD_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N', 'K', 'V_rows', 'D')
+  _RECORD_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N', 'K', 'V_rows', 'D', 'sample_key')
 
   def _static_records(self, batch, dev, cap):
     B, N = int(batch['sizes'].shape[0]), int(batch['N'])

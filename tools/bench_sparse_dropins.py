@@ -12,6 +12,11 @@ Per model (seeded weights, data.synthetic_qm8_samples at B, N = 26), one JSON li
     vs data.sparse_collate, eigs=False), wall clock;
   * GPNN only: partition_sparse_ms (lnb_spectral_partition_sparse) against partition_dense_ms
     (lnb_spectral_partition + graph_prepare of the two operators), each as one captured graph.
+  * SampledGraphSAGE (Mean, Max, LSTM, K = 40): the padded side is data.sage_collate (numpy's draws) +
+    forward; the records carry a sample_key and the neighbours are drawn on the device.  bit_equal compares
+    forward_sparse with forward on the padded batch of the device's samples.  sampler_kernel_ms: the
+    sampler kernel (ELL rows of M, as Mean / Max inference runs it) and operators_prepare_kernel_ms: the
+    padded path's lnb_sage_operators + graph_prepare kernels, both per call from torch.profiler.
 The GPU's name and power limit go into every line.
 """
 import argparse
@@ -38,7 +43,11 @@ MODELS = {
     'GGNN': lambda: models.GGNN(configs.qm8_ggnn()),
     'MPNN': lambda: models.MPNN(configs.qm8_mpnn()),
     'GPNN': lambda: models.GPNN(configs.qm8_gpnn()),
+    'SampledGraphSAGE-Mean': lambda: models.SampledGraphSAGE(configs.qm8_graphsage(agg_func='Mean')),
+    'SampledGraphSAGE-Max': lambda: models.SampledGraphSAGE(configs.qm8_graphsage(agg_func='Max')),
+    'SampledGraphSAGE-LSTM': lambda: models.SampledGraphSAGE(configs.qm8_graphsage(agg_func='LSTM')),
 }
+SAGE_K = 40
 
 
 def event_ms(fn, iters):
@@ -87,6 +96,56 @@ def gpu_info():
   return out
 
 
+def profiled_kernel_ms(fn, iters, names):
+  """Mean CUDA time per call of the kernels whose names contain one of ``names`` (torch.profiler)."""
+  from torch.profiler import ProfilerActivity, profile
+  fn()
+  torch.cuda.synchronize()
+  with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    for _ in range(iters):
+      fn()
+    torch.cuda.synchronize()
+  total = sum(e.device_time_total for e in prof.key_averages() if any(n in e.key for n in names))
+  return total / 1e3 / iters
+
+
+def sage_row(name, mod, samples, row, iters, dev):
+  """The SampledGraphSAGE measurements: data.sage_collate + forward against the records."""
+  c = data.sage_collate(samples, SAGE_K, np.random.RandomState(0))
+  host_pad = [torch.from_numpy(c[k]).pin_memory() for k in ('node_feat', 'nn_idx', 'nonempty_mask', 'node_mask')]
+  dev_pad = [t.to(dev) for t in host_pad]
+  sp = data.sparse_collate(samples, 20, eigs=False)
+  sp['sample_key'] = np.array([1234, 0], np.int64)
+  host_sp = {k: (torch.from_numpy(v).pin_memory() if isinstance(v, np.ndarray) else v) for k, v in sp.items()}
+  dev_sp = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in host_sp.items()}
+  E1 = mod.num_edgetype + 1
+  rec = [dev_sp[k] for k in ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'sample_key')]
+  with torch.no_grad():
+    node_ids, mask, ne, nn_idx, _, _ = ops.sage_sample_sparse(*rec, sp['N'], E1, SAGE_K)
+    ref = mod(node_ids, nn_idx.long(), ne, mask=mask)
+    row['bit_equal'] = bool(torch.equal(mod.forward_sparse(dev_sp), ref))
+    row['resident_padded_ms'] = round(event_ms(lambda: mod(dev_pad[0], dev_pad[1], dev_pad[2], mask=dev_pad[3]),
+                                               iters), 4)
+    row['resident_sparse_ms'] = round(event_ms(lambda: mod.forward_sparse(dev_sp), iters), 4)
+    row['e2e_padded_ms'] = round(event_ms(lambda: mod(host_pad[0], host_pad[1], host_pad[2], mask=host_pad[3]),
+                                          iters), 4)
+    row['e2e_sparse_ms'] = round(event_ms(lambda: mod.forward_sparse(host_sp), iters), 4)
+    if name.endswith('Mean'):
+      row['sampler_kernel_ms'] = round(profiled_kernel_ms(
+          lambda: ops.sage_sample_sparse(*rec, sp['N'], E1, SAGE_K, want_nn_idx=False, want_ell=True), iters,
+          ['sage_sample_kernel']), 4)
+      row['sampler_ell_t_kernel_ms'] = round(profiled_kernel_ms(
+          lambda: ops.sage_sample_sparse(*rec, sp['N'], E1, SAGE_K, want_nn_idx=False, want_ell=True,
+                                         want_ell_t=True), iters, ['sage_sample_kernel']), 4)
+      row['operators_prepare_kernel_ms'] = round(profiled_kernel_ms(
+          lambda: ops.graph_prepare(ops.sage_operators(dev_pad[1], dev_pad[2]), defer_tiles=True), iters,
+          ['sage_operator_kernel', 'graph_prepare_kernel']), 4)
+  row['h2d_padded_bytes'] = int(sum(t.numel() * t.element_size() for t in host_pad))
+  row['h2d_sparse_bytes'] = int(sum(v.numel() * v.element_size() for v in host_sp.values() if torch.is_tensor(v)))
+  row['collate_padded_ms'] = round(wall_ms(lambda: data.sage_collate(samples, SAGE_K, np.random.RandomState(0))), 2)
+  row['collate_sparse_ms'] = round(wall_ms(lambda: data.sparse_collate(samples, 20, eigs=False)), 2)
+
+
 def padded_inputs(name, samples, K):
   c = data.collate(samples, K)
   L = data.gat_bias(c['L']) if name == 'GAT' else c['L']
@@ -108,6 +167,11 @@ def main():
   for name in args.models:
     torch.manual_seed(0)
     mod = MODELS[name]().to(dev).eval()
+    if name.startswith('SampledGraphSAGE'):
+      row = {'model': name, 'B': args.B, 'N': int(max(s['L_simple_4'].shape[0] for s in samples)), 'gpu': gpu}
+      sage_row(name, mod, samples, row, args.iters, dev)
+      print(json.dumps(row), flush=True)
+      continue
     nf, L, mask = padded_inputs(name, samples, K)
     sp = data.sparse_collate(samples, K, eigs=False)
     host_pad = [torch.from_numpy(a).pin_memory() for a in (nf, L, mask)]

@@ -12,6 +12,8 @@ Per model and batch size (seeded weights, data.synthetic_qm8_samples, N = 26, Ad
     vs data.sparse_collate), wall clock;
   * h2d_padded_bytes / h2d_sparse_bytes: bytes copied to the device per step (label included).
 LanczosNet runs with the collate's eigenpairs on both sides, GPNN partitions on the device on both sides.
+SampledGraphSAGE (K = 40) trains from data.sage_collate (numpy's draws) on the padded side and from records
+with a sample_key (draws on the device) on the other.
 The GPU's name and power limit go into every line.
 """
 import argparse
@@ -37,12 +39,23 @@ MODELS = {
     'GGNN': lambda: models.GGNN(configs.qm8_ggnn()),
     'MPNN': lambda: models.MPNN(configs.qm8_mpnn()),
     'GPNN': lambda: models.GPNN(configs.qm8_gpnn()),
+    'SampledGraphSAGE-Mean': lambda: models.SampledGraphSAGE(configs.qm8_graphsage(agg_func='Mean')),
+    'SampledGraphSAGE-Max': lambda: models.SampledGraphSAGE(configs.qm8_graphsage(agg_func='Max')),
+    'SampledGraphSAGE-LSTM': lambda: models.SampledGraphSAGE(configs.qm8_graphsage(agg_func='LSTM')),
 }
 K = 20
+SAGE_K = 40
+
+
+def sage_collate(samples):
+  return data.sage_collate(samples, SAGE_K, np.random.RandomState(0))
 
 
 def padded_batch(name, samples, N):
   """(args, kwargs) of the padded forward as numpy arrays, and the label."""
+  if name.startswith('SampledGraphSAGE'):
+    c = sage_collate(samples)
+    return [c['node_feat'], c['nn_idx'], c['nonempty_mask']], {'mask': c['node_mask']}
   c = data.collate(samples, K, num_nodes=N)
   L = data.gat_bias(c['L']) if name == 'TrainableGAT' else c['L']
   args = [c['node_feat'], L] + ([c['D'], c['V']] if name == 'LanczosNet' else [])
@@ -51,6 +64,8 @@ def padded_batch(name, samples, N):
 
 def records(name, samples):
   sp = data.sparse_collate(samples, K, eigs=(name == 'LanczosNet'))
+  if name.startswith('SampledGraphSAGE'):
+    sp['sample_key'] = np.array([1234, 0], np.int64)
   return {k: v for k, v in sp.items() if k not in ('label', 'num_edgetype')}
 
 
@@ -106,7 +121,9 @@ def run(name, B, iters, dev, gpu):
 
   row['h2d_padded_bytes'] = nbytes(args_h + list(kw_h.values()) + [label_h])
   row['h2d_sparse_bytes'] = nbytes(list(rec_h.values()) + [label_h])
-  if name == 'TrainableGAT':
+  if name.startswith('SampledGraphSAGE'):
+    row['collate_padded_ms'] = round(wall_ms(lambda: sage_collate(samples)), 2)
+  elif name == 'TrainableGAT':
     row['collate_padded_ms'] = round(wall_ms(lambda: data.gat_bias(data.collate(samples, K, num_nodes=N)['L'])), 2)
   else:
     row['collate_padded_ms'] = round(wall_ms(lambda: data.collate(samples, K, num_nodes=N)), 2)
