@@ -702,6 +702,52 @@ int lnb_lanczos_ritz(lnb_stream_t stream, const float* A, const uint8_t* mask, c
 int lnb_tridiag_powers(lnb_stream_t stream, const float* T, int B, int K, const int* powers, int S,
                        float* out /* [B,K,S,K] */);
 
+/* ---------------------------------------------------------------------------------------
+ * AdaLanczosNet's Lanczos layer for training (the formulation of train._lanczos_train): the K-step
+ * recurrence with the reference's rules (cumulative validity from beta >= 1e-4, idx = min(#valid, #real
+ * nodes), columns and node rows masked, zero padding to K when N < K) and two classical block Gram-Schmidt
+ * passes with the 1/(q_j.q_j + EPS) scaling, in fp32 with a fixed reduction order.  One CTA per graph.
+ * lnb_lanczos_tridiag_train writes T [B,K,K], Q [B,N,K], alpha, beta [B,K] and idx [B] (each may be NULL).
+ * lnb_lanczos_tridiag_backward recomputes that forward with the same code (T, Q: its recomputed outputs,
+ * optional, bit-equal to the training entry's) and writes gA [B,N,N] = d<gT,T> + <gQ,Q> / dA, the exact
+ * adjoint of the recurrence with acceptance, idx and masks as data; no atomics (deterministic).
+ * mask may be NULL (every node real).  Limits: 1 <= N <= 128, 1 <= K <= 64 (LNB_ERR_UNSUPPORTED
+ * otherwise, nothing launched).
+ * ------------------------------------------------------------------------------------- */
+int lnb_lanczos_tridiag_train(lnb_stream_t stream, const float* A /* [B,N,N] */, const uint8_t* mask,
+                              const float* q1 /* [B,N] */, int B, int N, int K, float* T, float* Q,
+                              float* alpha, float* beta, int32_t* idx);
+int lnb_lanczos_tridiag_backward(lnb_stream_t stream, const float* A, const uint8_t* mask, const float* q1,
+                                 int B, int N, int K, const float* gT /* [B,K,K] */,
+                                 const float* gQ /* [B,N,K] */, float* gA /* [B,N,N] */, float* T,
+                                 float* Q);
+
+/* ---------------------------------------------------------------------------------------
+ * Adjoint of lnb_tridiag_powers: gT[b] = d<gOut[b], out[b]>/dT[b] for the function the forward computes,
+ * P_1 = T and P_{p+1} = P_p Tri(T) with Tri(T) the three diagonals of T (the forward reads only those).
+ * One CTA per graph recomputes P_1 .. P_{pmax-1} in shared memory and runs the reverse sweep, no atomics
+ * (deterministic).  Limit: (6 K + (powers[S-1] + 1) K^2) floats within 227 KB of shared memory
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched); S <= 32.
+ * ------------------------------------------------------------------------------------- */
+int lnb_tridiag_powers_backward(lnb_stream_t stream, const float* T /* [B,K,K] */,
+                                const float* gOut /* [B,K,S,K] */, int B, int K, const int* powers, int S,
+                                float* gT /* [B,K,K] */);
+
+/* ---------------------------------------------------------------------------------------
+ * AdaLanczosNet's Lanczos start vector drawn on the device (the reference draws torch.randn(B, N, 1)
+ * on the CPU generator, model/ada_lanczos_net.py:161).  For graph b < B and node n < N (padded nodes
+ * included; masking and normalisation stay in the Lanczos kernel):
+ *   (x0, x1, x2, x3) = Philox4x32-10 (Random123's constants) at key (seed lo, seed hi) and counter
+ *     (n >> 1, b, ctr lo, ctr hi), where (seed, ctr) = start_key[0..1] (int64, DEVICE memory: a captured
+ *     graph draws anew when the key changes);
+ *   u1 = (fp32(x0) + 1) * 2^-32 and u2 = fp32(x1) * 2^-32 in fp32 (round-to-nearest conversions), so
+ *     u1 is in (0, 1];
+ *   q1[b, n] = sqrtf(-2 logf(u1)) * (n even ? cos : sin)(2 pi u2), the sine and cosine from
+ *     sincospif(2 u2); accurate logf / sincospif, not the fast-math intrinsics.
+ * A standard normal per entry (Box-Muller); words x2, x3 are unused.
+ * ------------------------------------------------------------------------------------- */
+int lnb_ada_start_vector(lnb_stream_t stream, const int64_t* start_key, int B, int N, float* q1 /* [B,N] */);
+
 /* Symmetrised filter blocks (model/ada_lanczos_net.py:275-278):
  *   G[b,s,r,c] = 0.5 * (Y[b, r*K*S + c*S + s] + Y[b, c*K*S + r*S + s])                     */
 int lnb_symmetrize_filters(lnb_stream_t stream, const float* Y, int B, int K, int S,

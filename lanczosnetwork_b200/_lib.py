@@ -142,6 +142,13 @@ SIGNATURES = {
     'lnb_gat_bias_sparse': (c_int, [c_stream] + [ctypes.c_void_p] * 3 + [c_int] * 3 + [ctypes.c_void_p]),
     'lnb_tridiag_powers':(c_int, [c_stream, c_f32p, c_int, c_int, ctypes.POINTER(c_int), c_int,
                                    c_f32p]),
+    'lnb_lanczos_tridiag_train': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_int, c_int, c_int,
+                                          c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_void_p]),
+    'lnb_lanczos_tridiag_backward': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_int, c_int, c_int,
+                                             c_f32p, c_f32p, c_f32p, c_f32p, c_f32p]),
+    'lnb_tridiag_powers_backward': (c_int, [c_stream, c_f32p, c_f32p, c_int, c_int, ctypes.POINTER(c_int), c_int,
+                                            c_f32p]),
+    'lnb_ada_start_vector': (c_int, [c_stream, ctypes.c_void_p, c_int, c_int, c_f32p]),
     'lnb_symmetrize_filters': (c_int, [c_stream, c_f32p, c_int, c_int, c_int, c_f32p]),
 }
 

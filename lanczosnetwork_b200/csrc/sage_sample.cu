@@ -14,6 +14,7 @@
 // (float)count / (float)K as lnb_sage_operators rounds them), and optionally those of M_e^T, which the
 // training adjoint reads.  The dense [B, N, N, E1] operator never exists.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace {
 
@@ -32,17 +33,7 @@ struct SampleParams {
   float* ellT_val; uint8_t* ellT_idx; int32_t* ellT_max; int32_t* gextT;
 };
 
-// Philox4x32-10 (Salmon et al., SC'11), the constants of Random123
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-  }
-  return c;
-}
+using lnb::philox4x32_10;
 
 __device__ __forceinline__ uint32_t word(const uint4& x, int i) {
   return i == 0 ? x.x : i == 1 ? x.y : i == 2 ? x.z : x.w;

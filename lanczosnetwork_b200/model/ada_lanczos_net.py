@@ -13,9 +13,9 @@ import torch.nn as nn
 
 from .. import ops
 from ..spectral_conv import GraphContext, dense, graph_conv_layer
-from ._common import SpectralNetBase
+from ._common import SparseRecords, SpectralNetBase
 
-__all__ = ['AdaLanczosNet']
+__all__ = ['AdaLanczosNet', 'KeyedAdaLanczosNet']
 
 
 class AdaLanczosNet(SpectralNetBase):
@@ -97,3 +97,87 @@ class AdaLanczosNet(SpectralNetBase):
                                self.filter[tt].weight, self.filter[tt].bias, self._wcache,
                                'filter.%d' % tt)
     return self._readout(state, mask)
+
+
+class KeyedAdaLanczosNet(AdaLanczosNet):
+  """``AdaLanczosNet`` (same constructor, parameters, initialisation and ``state_dict``; construction
+  consumes the same CPU random numbers) whose Lanczos start vector is drawn on the device from a key, so
+  that it can be captured in a CUDA graph (``train.GraphedStep``, padded or ``sparse=True``) and run or
+  trained from the bond-list records of data.sparse_collate (``forward_sparse``, ``forward_sparse_train``).
+
+  The key is an int64 tensor (seed, counter) of shape (2,); ``ops.ada_start_vector(key, B, N)`` draws q1
+  [B, N], one standard normal per (graph, padded node), from Philox4x32-10 (the rule is in the C header).
+  ``forward(..., start_key=None)`` reads the module's own key, the non-persistent buffer ``start_key``
+  initialised to (config.seed or 0, 0), and advances its counter on the device after each draw: eager
+  calls, replays of a captured inference graph and ``GraphedStep`` replays each draw a new vector.  An
+  explicit ``start_key`` is used as given and nothing is advanced.  The records entries take the key as
+  ``batch['start_key']`` (required).  Under ``nn.DataParallel`` the replicas share the module's key, so each
+  replica draws the same vectors for its own slice of the batch: pass distinct keys per replica if that
+  matters.
+
+  Contract: the scores of ``forward_sparse`` equal, bit for bit, those of the padded ``_forward_impl`` on
+  data.collate(..., num_nodes=N) with q1 = ops.ada_start_vector(start_key, B, N), and
+  ``forward_sparse_train`` computes this class's padded training formulation on the same q1.  The
+  reference's torch.randn draws are not reproduced; the distribution is the same.  The training
+  formulation is AdaLanczosNet's, except that the Lanczos recurrence runs on lnb_lanczos_tridiag_train and its
+  adjoint lnb_lanczos_tridiag_backward (N <= 128, K <= 64), and the powers of T on lnb_tridiag_powers and its
+  adjoint (when K and the powers fit that kernel), one launch each, instead of chains of GEMMs; outside those
+  envelopes the GEMM chains of AdaLanczosNet run."""
+
+  def __init__(self, config):
+    super(KeyedAdaLanczosNet, self).__init__(config)
+    seed = int(getattr(config, 'seed', 0) or 0)
+    self.register_buffer('start_key', torch.tensor([seed, 0], dtype=torch.int64), persistent=False)
+
+  def forward(self, node_feat, L, label=None, mask=None, start_key=None):
+    """node_feat: long B x N; L: float B x N x N x (E+1); label: B x P; mask: B x N; start_key: int64 (2,)
+    (seed, counter), default the module's own key (advanced after the draw)."""
+    own = start_key is None
+    key = self.start_key if own else start_key
+    ops.check_start_key('KeyedAdaLanczosNet', key)
+    dev = self._device()
+    if self._check_mode():
+      q1 = ops.ada_start_vector(self._to(dev, key), node_feat.shape[0], node_feat.shape[1])
+      score = self._train_impl(self._to(dev, node_feat), self._to(dev, L), self._to(dev, mask), q1)
+    else:
+      score = self._graph_forward(self._keyed_impl, (node_feat, L, mask, key))
+    if own:
+      with torch.no_grad():
+        self.start_key[1:].add_(1)
+    return self._finish(score, self._to(dev, label))
+
+  def _keyed_impl(self, node_feat, L, mask, key):
+    q1 = ops.ada_start_vector(key, node_feat.shape[0], node_feat.shape[1])
+    return self._forward_impl(node_feat, L, mask, q1)
+
+  def _train_impl(self, node_feat, L, mask, q1):
+    from ..train import ada_train, lanczos_tridiag, tridiag_powers
+    K = self.num_eig_vec
+    fits = ops.tridiag_powers_backward_supported(K, self.long_diffusion_dist or [1])
+    return ada_train(self, node_feat, L, mask, q1, powers_fn=tridiag_powers if fits else None,
+                     lanczos_fn=lanczos_tridiag if ops.lanczos_tridiag_train_supported(L.shape[1], K) else None)
+
+  def _sparse_inputs(self, batch):
+    key = batch.get('start_key') if isinstance(batch, dict) else None
+    if key is None:
+      raise ValueError("KeyedAdaLanczosNet: the batch lacks 'start_key', the int64 (seed, counter) tensor of "
+                       "the Lanczos start vector")
+    ops.check_start_key('KeyedAdaLanczosNet', key)
+    if 'blob' in batch:
+      raise NotImplementedError('KeyedAdaLanczosNet takes data.sparse_collate records, not packed batches')
+    inputs, _, _ = super(KeyedAdaLanczosNet, self)._sparse_inputs(batch)
+    N = int(batch['N'])
+    return (inputs + (key,), lambda *a: self._forward_records(SparseRecords(*a[:5], N=N), a[5]),
+            ('keyed', N))
+
+  def _records_inputs(self, recs, key):
+    """node ids, dense operators and mask of the records (lnb_graph_prepare_sparse: the unfused conv
+    layers read the dense L) and the start vector of ``key``."""
+    _, node_ids, mask, _, L = self._prepare_records(recs, want_dense=True)
+    return node_ids, L, mask, ops.ada_start_vector(key, node_ids.shape[0], recs.N)
+
+  def _forward_records(self, recs, key):
+    return self._forward_impl(*self._records_inputs(recs, key))
+
+  def _train_records(self, recs, key):
+    return self._train_impl(*self._records_inputs(recs, key))

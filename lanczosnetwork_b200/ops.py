@@ -23,7 +23,8 @@ __all__ = [
     'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'ell_messages', 'ell_messages_adjoint',
     'set2vec', 'set2vec_supported',
     'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
-    'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
+    'tridiag_powers_backward', 'tridiag_powers_backward_supported', 'ada_start_vector', 'check_start_key',
+    'lanczos_tridiag_train', 'lanczos_tridiag_backward', 'lanczos_tridiag_train_supported', 'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
 
 
@@ -1348,6 +1349,113 @@ def tridiag_powers(T, powers):
     _lib.check(_lib.load().lnb_tridiag_powers(_stream(T), _ptr(T), B, K, _ints(powers), S,
                                               _ptr(out)), 'lnb_tridiag_powers')
   return out
+
+
+def tridiag_powers_backward_supported(K, powers):
+  """True when lnb_tridiag_powers_backward takes K and these powers: at most 32, positive and strictly
+  increasing, (6 K + (max power + 1) K^2) floats within 227 KB of shared memory."""
+  powers = [int(p) for p in powers]
+  return (1 <= len(powers) <= 32 and K >= 1 and powers[0] >= 1 and
+          all(a < b for a, b in zip(powers, powers[1:])) and
+          (6 * K + (powers[-1] + 1) * K * K) * 4 <= 227 * 1024)
+
+
+def tridiag_powers_backward(T, gOut, powers):
+  """Adjoint of ``tridiag_powers``: gT [B,K,K] for gOut [B,K,S,K] (lnb_tridiag_powers_backward).  Raises
+  ValueError before any launch outside ``tridiag_powers_backward_supported``."""
+  B, K = T.shape[0], T.shape[1]
+  S = len(powers)
+  if not tridiag_powers_backward_supported(K, powers):
+    raise ValueError('tridiag_powers_backward: K=%d with powers up to %d outside the shared-memory envelope '
+                     '((6 K + (max power + 1) K^2) * 4 bytes <= 227 KB, at most 32 powers)'
+                     % (K, max(powers) if powers else 0))
+  if tuple(gOut.shape) != (B, K, S, K):
+    raise ValueError('tridiag_powers_backward: gOut must be [B,K,S,K] = %s; got %s'
+                     % ((B, K, S, K), tuple(gOut.shape)))
+  _need_cuda(T, gOut)
+  T, gOut = _f32c(T), _f32c(gOut)
+  gT = torch.empty((B, K, K), device=T.device, dtype=torch.float32)
+  with torch.cuda.device(T.device):
+    _lib.check(_lib.load().lnb_tridiag_powers_backward(_stream(T), _ptr(T), _ptr(gOut), B, K, _ints(powers),
+                                                       S, _ptr(gT)), 'lnb_tridiag_powers_backward')
+  return gT
+
+
+def lanczos_tridiag_train_supported(N, K):
+  """True when lnb_lanczos_tridiag_train / _backward take N and K: 1 <= N <= 128, 1 <= K <= 64."""
+  return 1 <= int(N) <= 128 and 1 <= int(K) <= 64
+
+
+def _lanczos_train_args(who, A, mask, q1, K):
+  B, N = A.shape[0], A.shape[1]
+  if not lanczos_tridiag_train_supported(N, K):
+    raise ValueError('%s: N=%d K=%d outside 1 <= N <= 128, 1 <= K <= 64' % (who, N, K))
+  _need_cuda(A, mask, q1)
+  A = _f32c(A)
+  q1 = _f32c(q1).reshape(B, N)
+  if mask is not None:
+    mask = (mask != 0).to(torch.uint8).contiguous()
+  return A, mask, q1, B, N
+
+
+def lanczos_tridiag_train(A, mask, q1, K):
+  """The Lanczos layer of the training path (lnb_lanczos_tridiag_train): returns dict(T [B,K,K], Q [B,N,K],
+  alpha, beta [B,K], idx [B] int32).  ValueError before any launch outside lanczos_tridiag_train_supported."""
+  A, mask, q1, B, N = _lanczos_train_args('lanczos_tridiag_train', A, mask, q1, K)
+  dev = A.device
+  out = {'T': torch.empty((B, K, K), device=dev, dtype=torch.float32),
+         'Q': torch.empty((B, N, K), device=dev, dtype=torch.float32),
+         'alpha': torch.empty((B, K), device=dev, dtype=torch.float32),
+         'beta': torch.empty((B, K), device=dev, dtype=torch.float32),
+         'idx': torch.empty((B,), device=dev, dtype=torch.int32)}
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_lanczos_tridiag_train(
+        _stream(A), _ptr(A), _ptr(mask), _ptr(q1), B, N, int(K), _ptr(out['T']), _ptr(out['Q']),
+        _ptr(out['alpha']), _ptr(out['beta']), _ptr(out['idx'])), 'lnb_lanczos_tridiag_train')
+  return out
+
+
+def lanczos_tridiag_backward(A, mask, q1, K, gT, gQ, want_tape=False):
+  """gA [B,N,N], the adjoint of lanczos_tridiag_train for the gradients gT [B,K,K] and gQ [B,N,K]
+  (lnb_lanczos_tridiag_backward).  ``want_tape``: also the (T, Q) its recompute produced.  ValueError before
+  any launch outside lanczos_tridiag_train_supported."""
+  A, mask, q1, B, N = _lanczos_train_args('lanczos_tridiag_backward', A, mask, q1, K)
+  gT, gQ = _f32c(gT), _f32c(gQ)
+  if tuple(gT.shape) != (B, K, K) or tuple(gQ.shape) != (B, N, K):
+    raise ValueError('lanczos_tridiag_backward: gT must be %s and gQ %s; got %s, %s'
+                     % ((B, K, K), (B, N, K), tuple(gT.shape), tuple(gQ.shape)))
+  dev = A.device
+  gA = torch.empty((B, N, N), device=dev, dtype=torch.float32)
+  T = torch.empty((B, K, K), device=dev, dtype=torch.float32) if want_tape else None
+  Q = torch.empty((B, N, K), device=dev, dtype=torch.float32) if want_tape else None
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_lanczos_tridiag_backward(
+        _stream(A), _ptr(A), _ptr(mask), _ptr(q1), B, N, int(K), _ptr(gT), _ptr(gQ), _ptr(gA), _ptr(T),
+        _ptr(Q)), 'lnb_lanczos_tridiag_backward')
+  return (gA, T, Q) if want_tape else gA
+
+
+def check_start_key(who, key):
+  if not torch.is_tensor(key) or key.dtype != torch.int64 or tuple(key.shape) != (2,):
+    raise ValueError("%s: 'start_key' must be an int64 tensor of shape (2,) (seed, counter); got %r"
+                     % (who, (key.dtype, tuple(key.shape)) if torch.is_tensor(key) else type(key)))
+
+
+def ada_start_vector(start_key, B, N):
+  """AdaLanczosNet's Lanczos start vector q1 [B,N] fp32 drawn on the device (lnb_ada_start_vector; the
+  rule is in the C header): one standard normal per (graph, padded node) from Philox4x32-10 keyed by
+  ``start_key``, an int64 [2] CUDA tensor (seed, counter) read on the device."""
+  check_start_key('ada_start_vector', start_key)
+  _need_cuda(start_key)
+  B, N = int(B), int(N)
+  if B < 0 or N < 1:
+    raise ValueError('ada_start_vector: bad dims B=%d N=%d' % (B, N))
+  key = start_key.contiguous()
+  q1 = torch.empty((B, N), device=key.device, dtype=torch.float32)
+  with torch.cuda.device(key.device):
+    _lib.check(_lib.load().lnb_ada_start_vector(_stream(key), _ptr(key), B, N, _ptr(q1)),
+               'lnb_ada_start_vector')
+  return q1
 
 
 def symmetrize_filters(Y, K, S):

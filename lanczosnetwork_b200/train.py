@@ -29,7 +29,7 @@ import torch
 from . import ops
 
 __all__ = ['dense', 'EllOperator', 'ell_operator', 'operator_messages', 'spectral_messages', 'embedding', 'ritz_stack_train',
-           'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'ada_train', 'neighbour_max', 'sage_train',
+           'dcnn_train', 'cheby_train', 'gated_readout', 'bmm', 'lanczos_tridiag', 'tridiag_powers', 'ada_train', 'neighbour_max', 'sage_train',
            'lstm_messages', 'ggnn_train', 'gpnn_train', 'recurrent_cell', 'edge_aggregate', 'set2vec_train', 'mpnn_train', 'gat_attention',
            'gat_train', 'GraphedStep']
 
@@ -879,10 +879,78 @@ def _lanczos_train(A, mask, q1, K):
   return T, Q
 
 
-def ada_train(model, node_ids, L, mask, q1):
+class _TridiagPowers(torch.autograd.Function):
+  """out[b, r, s, c] = (T_b ** powers[s])[r, c] on lnb_tridiag_powers (one launch), its adjoint on
+  lnb_tridiag_powers_backward (one launch)."""
+
+  @staticmethod
+  def forward(ctx, T, powers):
+    T = T.contiguous()
+    ctx.save_for_backward(T)
+    ctx.powers = powers
+    return ops.tridiag_powers(T, powers)
+
+  @staticmethod
+  def backward(ctx, g):
+    T, = ctx.saved_tensors
+    return ops.tridiag_powers_backward(T, g.contiguous(), ctx.powers), None
+
+
+def tridiag_powers(T, powers):
+  """Differentiable powers of the tridiagonal T [B,K,K] -> [B,K,S,K] (the layout of ops.tridiag_powers).
+  The forward reads the three diagonals of T for every product after the first, as the kernel does.
+  ValueError outside ops.tridiag_powers_backward_supported."""
+  powers = [int(p) for p in powers]
+  if not ops.tridiag_powers_backward_supported(T.shape[1], powers):
+    raise ValueError('tridiag_powers: K=%d with powers up to %d is outside lnb_tridiag_powers_backward'
+                     % (T.shape[1], max(powers)))
+  return _TridiagPowers.apply(T.float(), powers)
+
+
+class _LanczosTridiag(torch.autograd.Function):
+  """(T, Q) of the K-step Lanczos recurrence on lnb_lanczos_tridiag_train, its adjoint on
+  lnb_lanczos_tridiag_backward (one launch each): the backward recomputes the forward with the same code, so
+  it differentiates the tape the forward returned.  Gradients flow to A only."""
+
+  @staticmethod
+  def forward(ctx, A, mask, q1, K):
+    A = A.contiguous()
+    out = ops.lanczos_tridiag_train(A, mask, q1, K)
+    ctx.save_for_backward(A, mask, q1)
+    ctx.K = K
+    return out['T'], out['Q']
+
+  @staticmethod
+  def backward(ctx, gT, gQ):
+    A, mask, q1 = ctx.saved_tensors
+    K = ctx.K
+    if gT is None:
+      gT = torch.zeros((A.shape[0], K, K), device=A.device, dtype=torch.float32)
+    if gQ is None:
+      gQ = torch.zeros((A.shape[0], A.shape[1], K), device=A.device, dtype=torch.float32)
+    return ops.lanczos_tridiag_backward(A, mask, q1, ctx.K, gT, gQ), None, None, None
+
+
+def lanczos_tridiag(A, mask, q1, K):
+  """Differentiable Lanczos layer of the training path: the formulation of ``_lanczos_train`` (same rules,
+  two block Gram-Schmidt passes) in one forward and one backward launch.  A [B,N,N], mask [B,N] or None,
+  q1 [B,N] or [B,N,1] -> (T [B,K,K], Q [B,N,K]).  ValueError outside ops.lanczos_tridiag_train_supported."""
+  B, N = A.shape[0], A.shape[1]
+  if not ops.lanczos_tridiag_train_supported(N, K):
+    raise ValueError('lanczos_tridiag: N=%d K=%d outside 1 <= N <= 128, 1 <= K <= 64' % (N, K))
+  q1 = q1.reshape(B, N).float().contiguous()
+  if mask is not None:
+    mask = (mask != 0).to(torch.uint8).contiguous()
+  return _LanczosTridiag.apply(A.float(), mask, q1, int(K))
+
+
+def ada_train(model, node_ids, L, mask, q1, powers_fn=None, lanczos_fn=None):
   """Differentiable AdaLanczosNet (model/ada_lanczos_net.py:288-368): embedding -> learned Gaussian
   Laplacian -> Lanczos -> learned filter on the powers of T (the 4096-wide MLP on the wgmma dense
-  kernel) -> graph convolutions with [short walk | Q G_s Q^T X | L_e X] messages -> gated readout."""
+  kernel) -> graph convolutions with [short walk | Q G_s Q^T X | L_e X] messages -> gated readout.
+  ``powers_fn(T, dist)`` -> [B,K,S,K], when given, replaces the chain of ``bmm`` products that forms the
+  powers of T, and ``lanczos_fn(A, mask, q1, K)`` -> (T, Q) replaces ``_lanczos_train`` (the defaults are
+  AdaLanczosNet's own formulation)."""
   L = L.float().contiguous()
   state = embedding(node_ids, model.embedding.weight)
   B, N = state.shape[0], state.shape[1]
@@ -891,14 +959,19 @@ def ada_train(model, node_ids, L, mask, q1):
   if S > 0:
     adj = (L[:, :, :, 0] != 0).to(torch.float32)                    # ada_lanczos_net.py:310-311
     Le = _gaussian_laplacian_train(state, adj)
-    T, Q = _lanczos_train(Le, mask, q1.to(L.device), K)
-    plist, cur = [], T
-    for p in range(1, max(model.long_diffusion_dist) + 1):          # T^p by repeated products (:262-270)
-      if p in model.long_diffusion_dist:
-        plist.append(cur)
-      if p < max(model.long_diffusion_dist):
-        cur = bmm(cur, T)
-    powers = torch.cat(plist, dim=2)                                # [B,K,S*K]: index r, s*K + c (:274)
+    T, Q = (lanczos_fn or _lanczos_train)(Le, mask, q1.to(L.device), K)
+    if powers_fn is not None:
+      P4 = powers_fn(T, model.long_diffusion_dist)                  # [B,K,S,K]
+      powers = P4.reshape(B, K, S * K)
+      plist = P4.unbind(dim=2)
+    else:
+      plist, cur = [], T
+      for p in range(1, max(model.long_diffusion_dist) + 1):        # T^p by repeated products (:262-270)
+        if p in model.long_diffusion_dist:
+          plist.append(cur)
+        if p < max(model.long_diffusion_dist):
+          cur = bmm(cur, T)
+      powers = torch.cat(plist, dim=2)                              # [B,K,S*K]: index r, s*K + c (:274)
   for t in range(model.num_layer):
     msgs = _short_walk(L, state, model.short_diffusion_dist)
     if S > 0:
@@ -931,7 +1004,7 @@ class GraphedStep:
   ``AdamW`` get ``capturable=True`` here; plain SGD needs nothing).  The warm-up iterations torch needs
   before capture are rolled back (parameters and optimizer state restored in place), so constructing
   the object does not advance training.  Not for AdaLanczosNet (its start vector is drawn on the
-  host each call)."""
+  host each call); KeyedAdaLanczosNet draws it on the device and is captured like the others."""
 
   def __init__(self, model, optimizer, args, kwargs=None, warmup=3, sparse=False, edge_capacity=None):
     """``sparse=True``: ``args`` is ``(batch,)``, the records of data.sparse_collate as torch tensors, and the
@@ -999,7 +1072,7 @@ class GraphedStep:
 
   # the ragged record arrays: static buffers of more rows than a batch fills, only the rows present copied
   _RAGGED = ('node_feat', 'edges', 'V_rows')
-  _RECORD_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N', 'K', 'V_rows', 'D', 'sample_key')
+  _RECORD_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N', 'K', 'V_rows', 'D', 'sample_key', 'start_key')
 
   def _static_records(self, batch, dev, cap):
     B, N = int(batch['sizes'].shape[0]), int(batch['N'])
