@@ -197,6 +197,22 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
                                     int32_t* rowmap, int32_t* nrows, int64_t* node_ids, uint8_t* mask,
                                     float* V, float* L_dense);
 
+/* Float-feature variant (LanczosNetGeneral's GraphData records, node features instead of atom ids): the
+ * same records and outputs as lnb_graph_prepare_sparse, except that node_x [node_ptr[B], F] fp32 holds the
+ * feature rows of the real nodes in place of node_feat, and X [B,N,F] receives the padded feature tensor in
+ * place of node_ids: real rows copied bit for bit, padded rows 0 (the reference's GraphData collate followed
+ * by .float()).  The copy takes 16-byte vectors when F % 4 == 0 and node_x and X are 16-byte aligned, scalar
+ * loads otherwise; the bits are the same either way.  Same kernel as lnb_graph_prepare_sparse (a
+ * compile-time variant), one launch plus the tile assignment unless LNB_PREP_DEFER_TILES.
+ * Limits: 1 <= N <= 128, 2 <= E1 <= 16, K >= 1, 1 <= F <= 4096 (LNB_ERR_UNSUPPORTED otherwise, nothing
+ * launched), degrees < 255. */
+int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
+                                      const float* node_x, const int32_t* edge_ptr, const uint8_t* edges,
+                                      const float* V_rows, const double* inv_sqrt_deg, int B, int N, int E1,
+                                      int K, int F, int flags, float* ell_val, uint8_t* ell_idx,
+                                      int32_t* ell_max, int32_t* gext, int32_t* tiles, int32_t* rowmap,
+                                      int32_t* nrows, float* X, uint8_t* mask, float* V, float* L_dense);
+
 /* ---------------------------------------------------------------------------------------
  * The whole convolution stack (and optionally the embedding gather in front and the readout
  * behind it) in ONE persistent kernel: every CTA keeps its packed tile's state in shared memory

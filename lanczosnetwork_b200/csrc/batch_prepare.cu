@@ -36,6 +36,10 @@ struct SparseBatchParams {
   int64_t* node_ids; uint8_t* mask; float* V;     // padded [B,N], [B,N], [B,N,K]
   float* L;                                        // optional dense [B,N,N,E1]
   int32_t* rowmap; int32_t* nrows;                 // written here when the packed batch carries krow_ptr
+  // feature variant (lnb_graph_prepare_sparse_features): float rows instead of atom ids
+  const float* node_x;                             // [node_ptr[B], F] features of the real nodes
+  float* X;                                        // padded [B,N,F]
+  int F;
 };
 
 // multiplicity of entry (i, j) of channel ch (0 = simple graph = sum over bond types)
@@ -51,6 +55,24 @@ __device__ __forceinline__ int entry_mult(const uint32_t* rowmask, int E, int ch
   return m;
 }
 
+// Graph b's padded feature rows X[b] [N,F]: the real rows copied bit for bit, the padded rows zero.
+// 16-byte copies when F and both pointers allow (every row then starts 16-byte aligned), else scalar.
+__device__ __forceinline__ void copy_feature_rows(const float* __restrict__ src, float* __restrict__ dst,
+                                                  int nb, int N, int F, int tid) {
+  const int real = nb * F, total = N * F;
+  if ((F & 3) == 0 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0) {
+    const float4* s4 = reinterpret_cast<const float4*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (int i = tid; i < total / 4; i += BP_THREADS)
+      d4[i] = i < real / 4 ? __ldg(s4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+  } else {
+    for (int i = tid; i < total; i += BP_THREADS) dst[i] = i < real ? __ldg(src + i) : 0.f;
+  }
+}
+
+// kFeat = false: atom ids -> node_ids (lnb_graph_prepare_sparse / _packed); kFeat = true: float feature rows
+// -> X (lnb_graph_prepare_sparse_features, never packed).  Everything else is the same code.
+template <bool kFeat>
 __global__ void __launch_bounds__(BP_THREADS)
 batch_prepare_sparse_kernel(const SparseBatchParams P) {
   extern __shared__ __align__(16) unsigned char bp_smem[];
@@ -60,7 +82,7 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
   const int N = P.N, E1 = P.E1, E = E1 - 1, K = P.K;
   const int32_t* sizes = P.sizes; const int32_t* node_ptr = P.node_ptr; const int32_t* node_feat = P.node_feat;
   const int32_t* edge_ptr = P.edge_ptr; const uint8_t* edges = P.edges; const float* V_rows = P.V_rows;
-  if (P.blob) {                                  // header: byte offsets of the segments (see the C header)
+  if (!kFeat && P.blob) {                        // header: byte offsets of the segments (see the C header)
     const int32_t* hdr = reinterpret_cast<const int32_t*>(P.blob);
     sizes = reinterpret_cast<const int32_t*>(P.blob + hdr[3]);
     node_ptr = reinterpret_cast<const int32_t*>(P.blob + hdr[4]);
@@ -153,9 +175,10 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
   // ---- padded node ids, mask, Ritz vectors; k_eff ---------------------------------------------------
   const int r0 = node_ptr[b];
   for (int n = tid; n < N; n += BP_THREADS) {
-    P.node_ids[(int64_t)b * N + n] = (n < nb) ? (int64_t)node_feat[r0 + n] : 0;
+    if (!kFeat) P.node_ids[(int64_t)b * N + n] = (n < nb) ? (int64_t)node_feat[r0 + n] : 0;
     P.mask[(int64_t)b * N + n] = (n < nb) ? 1 : 0;
   }
+  if (kFeat) copy_feature_rows(P.node_x + (int64_t)r0 * P.F, P.X + (int64_t)b * N * P.F, nb, N, P.F, tid);
   int ke = 0;
   for (int i = tid; i < N * K; i += BP_THREADS) {
     const int n = i / K, k = i - n * K;
@@ -221,14 +244,15 @@ gat_bias_sparse_kernel(const int32_t* __restrict__ sizes, const int32_t* __restr
   }
 }
 
+template <bool kFeat>
 static int launch_sparse(lnb_stream_t stream, SparseBatchParams p, int32_t* tiles, int32_t* rowmap,
                          int32_t* nrows) {
   p.rowmap = rowmap; p.nrows = nrows;
   const size_t smem = (size_t)(p.E1 - 1) * BP_NMAX * BP_NW * 4 + (size_t)p.E1 * BP_NMAX * 8 + (size_t)p.N * p.E1 + 16;
   cudaStream_t s = (cudaStream_t)stream;
   if (smem > 48 * 1024)
-    cudaFuncSetAttribute(batch_prepare_sparse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  batch_prepare_sparse_kernel<<<p.B, BP_THREADS, smem, s>>>(p);
+    cudaFuncSetAttribute(batch_prepare_sparse_kernel<kFeat>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  batch_prepare_sparse_kernel<kFeat><<<p.B, BP_THREADS, smem, s>>>(p);
   lnb::count_launch(1);
   if (p.blob && (p.flags & 2))                     // tile table + row-list offsets came with the batch
     return lnb::finish_launch("graph_prepare_sparse");
@@ -260,7 +284,8 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
   p.B = B; p.N = N; p.E1 = E1; p.K = K; p.flags = flags;
   p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.gext = gext;
   p.node_ids = node_ids; p.mask = mask; p.V = V; p.L = L_dense;
-  return launch_sparse(stream, p, tiles, rowmap, nrows);
+  p.node_x = nullptr; p.X = nullptr; p.F = 0;
+  return launch_sparse<false>(stream, p, tiles, rowmap, nrows);
 }
 
 int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, const double* inv_sqrt_deg,
@@ -281,7 +306,35 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
   p.B = B; p.N = N; p.E1 = E1; p.K = K; p.flags = flags;
   p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.gext = gext;
   p.node_ids = node_ids; p.mask = mask; p.V = V; p.L = L_dense;
-  return launch_sparse(stream, p, tiles, rowmap, nrows);
+  p.node_x = nullptr; p.X = nullptr; p.F = 0;
+  return launch_sparse<false>(stream, p, tiles, rowmap, nrows);
+}
+
+int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
+                                      const float* node_x, const int32_t* edge_ptr, const uint8_t* edges,
+                                      const float* V_rows, const double* inv_sqrt_deg, int B, int N, int E1,
+                                      int K, int F, int flags, float* ell_val, uint8_t* ell_idx,
+                                      int32_t* ell_max, int32_t* gext, int32_t* tiles, int32_t* rowmap,
+                                      int32_t* nrows, float* X, uint8_t* mask, float* V, float* L_dense) {
+  if (!(B >= 0 && N >= 1 && N <= BP_NMAX && E1 >= 2 && E1 <= BP_EMAX && K >= 1 && F >= 1 && F <= 4096)) {
+    lnb::set_err("graph_prepare_sparse_features: B=%d N=%d E1=%d K=%d F=%d outside 1 <= N <= %d, "
+                 "2 <= E1 <= %d, K >= 1, 1 <= F <= 4096", B, N, E1, K, F, BP_NMAX, BP_EMAX);
+    return LNB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return LNB_OK;
+  LNB_REQUIRE(sizes && node_ptr && node_x && edge_ptr && edges && V_rows && inv_sqrt_deg && ell_val &&
+                  ell_idx && ell_max && gext && tiles && X && mask && V,
+              "graph_prepare_sparse_features: null pointer");
+  LNB_REQUIRE((rowmap == nullptr) == (nrows == nullptr),
+              "graph_prepare_sparse_features: rowmap and nrows go together");
+  SparseBatchParams p;
+  p.sizes = sizes; p.node_ptr = node_ptr; p.node_feat = nullptr; p.edge_ptr = edge_ptr;
+  p.edges = edges; p.V_rows = V_rows; p.inv_sqrt_deg = inv_sqrt_deg; p.blob = nullptr;
+  p.B = B; p.N = N; p.E1 = E1; p.K = K; p.flags = flags & ~LNB_PACKED_HOST_TILES;
+  p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.gext = gext;
+  p.node_ids = nullptr; p.mask = mask; p.V = V; p.L = L_dense;
+  p.node_x = node_x; p.X = X; p.F = F;
+  return launch_sparse<true>(stream, p, tiles, rowmap, nrows);
 }
 
 int lnb_gat_bias_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr, const uint8_t* edges,

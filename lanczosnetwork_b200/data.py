@@ -219,8 +219,9 @@ def sparse_collate(samples, num_eigs, eigs=True):
   (ops.graph_prepare_sparse / LanczosNet.forward_sparse): nothing is padded on the host and the
   dense operators are not shipped at all.
 
-  Returns numpy arrays: sizes [B] int32, node_ptr [B+1] int32 (prefix sums), node_feat [sum n] int32,
-  edge_ptr [B+1] int32, edges [sum E, 4] uint8 = {u, v, bond type, 0}, D [B,K] float32 (truncated /
+  Returns numpy arrays: sizes [B] int32, node_ptr [B+1] int32 (prefix sums), node_feat [sum n] int32
+  atom ids, or [sum n, F] float32 feature rows when the records' node_feat is 2-D (the bits of collate's
+  node_feat[b, :n]; SparseLanczosNetGeneral and ops.graph_prepare_sparse_features read them), edge_ptr [B+1] int32, edges [sum E, 4] uint8 = {u, v, bond type, 0}, D [B,K] float32 (truncated /
   zero padded like dataset/qm8.py:268-287), V_rows [sum n, K] float32 (rows of real nodes only),
   N = batch-max node count (the reference's padding target), num_edgetype, label if present.
   ``eigs=False`` (records of ``prepare_graph(..., eigs=False)`` do): no D and no V_rows, only K = num_eigs;
@@ -231,7 +232,11 @@ def sparse_collate(samples, num_eigs, eigs=True):
   node_ptr[1:] = np.cumsum(sizes)
   edge_ptr = np.zeros(B + 1, np.int32)
   edge_ptr[1:] = np.cumsum([len(s['edges']) for s in samples])
-  node_feat = np.concatenate([np.asarray(s['node_feat']).astype(np.int32) for s in samples])
+  feats = [np.asarray(s['node_feat']) for s in samples]
+  if feats[0].ndim == 2:               # float features: each fp64 value rounded once, as collate's float32 rows
+    node_feat = np.concatenate([f.astype(np.float32) for f in feats]).reshape(-1, feats[0].shape[1])
+  else:
+    node_feat = np.concatenate([f.astype(np.int32) for f in feats])
   edges = np.zeros((int(edge_ptr[-1]), 4), np.uint8)
   for b, s in enumerate(samples):
     edges[edge_ptr[b]:edge_ptr[b + 1], :3] = s['edges']

@@ -12,6 +12,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib, ops
+from .. import data as data_mod
 from ..data import check_dist
 from ..spectral_conv import (GraphContext, WeightCache, graph_conv_layer,
                              ritz_filter_coefficients)
@@ -264,6 +265,16 @@ class SpectralNetBase(nn.Module):
     if not hasattr(self, '_forward_records'):
       raise NotImplementedError('%s has no sparse-batch entry; call forward() on the collated batch'
                                 % type(self).__name__)
+    N, B, E1 = self._check_sparse_batch(batch)
+    self._check_runnable(N, E1)
+    inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
+              Ragged(batch['edges']))
+    return inputs, lambda *a: self._forward_records(SparseRecords(*a, N=N)), ('records', N)
+
+  def _check_sparse_batch(self, batch, feature_dim=None):
+    """forward_sparse's checks of a records batch, before any device work: the keys, N and E+1 within the
+    prepare kernel's limits, int32 pointers, uint8 [E, 4] bonds, and int32 atom ids -- or, with
+    ``feature_dim``, float32 [rows, feature_dim] feature rows.  Returns (N, B, E1)."""
     missing = [k for k in self.SPARSE_KEYS if k not in batch]
     if missing:
       raise ValueError('forward_sparse: the batch lacks %s (data.sparse_collate records)' % ', '.join(missing))
@@ -272,14 +283,16 @@ class SpectralNetBase(nn.Module):
     if not (1 <= N <= 128 and 2 <= E1 <= 16):
       raise ValueError('forward_sparse: N=%d, E+1=%d outside 1 <= N <= 128, 2 <= E+1 <= 16' % (N, E1))
     for k in ('sizes', 'node_ptr', 'node_feat', 'edge_ptr'):
-      if batch[k].dtype != torch.int32:
+      if k == 'node_feat' and feature_dim is not None:
+        nf = batch[k]
+        if nf.dtype != torch.float32 or nf.dim() != 2 or nf.shape[1] != feature_dim:
+          raise ValueError('forward_sparse: node_feat must be float32 feature rows [rows, %d]; got %s %s'
+                           % (feature_dim, nf.dtype, tuple(nf.shape)))
+      elif batch[k].dtype != torch.int32:
         raise ValueError('forward_sparse: %s must be int32; got %s' % (k, batch[k].dtype))
     if batch['edges'].dtype != torch.uint8 or batch['edges'].dim() != 2 or batch['edges'].shape[1] != 4:
       raise ValueError('forward_sparse: edges must be uint8 [E, 4]')
-    self._check_runnable(N, E1)
-    inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
-              Ragged(batch['edges']))
-    return inputs, lambda *a: self._forward_records(SparseRecords(*a, N=N)), ('records', N)
+    return N, B, E1
 
   def _check_runnable(self, N=None, E1=None):
     """Model-specific checks of a call, run before any launch (N, E1: those of a sparse batch)."""
@@ -528,11 +541,12 @@ class SpectralNetBase(nn.Module):
         readout=(head.weight, head.bias, att.weight.reshape(-1), att.bias), mask=mask)
     return score
 
-  def _sparse_stack_ok(self, N, E1, K):
+  def _sparse_stack_ok(self, N, E1, K, din0=None):
     """True when every layer of this model runs inside the one-launch stack kernel, so a sparse
-    batch never needs the dense operator tensor."""
+    batch never needs the dense operator tensor.  ``din0``: the input width (default: the embedding's)."""
     S = self.num_scale_long
-    din0 = self.embedding.weight.shape[1]
+    if din0 is None:
+      din0 = self.embedding.weight.shape[1]
     dims = [din0] + list(self.hidden_dim)
     ok = all(ops.fused_conv_supported(N, dims[t], K, dims[t + 1], len(self.short_diffusion_dist), False, S, E1)
              for t in range(self.num_layer))
@@ -547,3 +561,91 @@ class SpectralNetBase(nn.Module):
     if label is not None:
       return score, self.loss_func(score, label)
     return score
+
+
+class RitzRecords(object):
+  """The entries from bond-list records of the Ritz-pair models, mixed in front of SpectralNetBase:
+  ``forward_sparse`` / ``forward_sparse_train`` / ``GraphedStep(sparse=True)`` over records that carry the
+  eigenpairs of the real nodes (``V_rows``, ``D``) or only K (``data.sparse_collate(..., eigs=False)``: one
+  lnb_graph_eigs_sparse launch in front of the batch construction, inside the same CUDA graph -- no host
+  eigh, no eigenvector bytes on the bus).  ``_feature_records`` is the one difference between the users:
+  False, ``node_feat`` holds atom ids and the stack gathers the embedding (LanczosNet); True, it holds float
+  feature rows [rows, input_dim] that the prepare kernel pads into X (SparseLanczosNetGeneral)."""
+
+  _feature_records = False
+
+  def _sparse_inputs(self, batch):
+    feat = self._feature_records
+    if 'blob' in batch:
+      if feat:
+        raise NotImplementedError('%s takes data.sparse_collate records, not packed batches'
+                                  % type(self).__name__)
+      # a packed batch (data.pack_sparse) crosses PCIe as ONE copy of exactly the bytes present
+      B, N, K = int(batch['B']), int(batch['N']), int(batch['K'])
+      cap = data_mod.packed_offsets(B, K)[4] + 16 * 3 + 4 * B * N + 4 * B * N * K + 4 * B * N * 4
+      blob = batch['blob']
+      return ((Ragged(blob, max(cap, int(blob.shape[0]))),),
+              lambda b_: self._forward_packed_impl(B, N, K, b_), ('packed', B, N, K))
+    if feat:
+      self._check_ritz_records(batch)
+    N, B = int(batch['N']), int(batch['sizes'].shape[0])
+    if 'V_rows' not in batch and 'D' not in batch:
+      K = int(batch['K'])
+      inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
+                Ragged(batch['edges']))
+      return inputs, lambda *a: self._forward_sparse_eigs_impl(N, K, *a), ('sparse_eigs', N, K)
+    inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
+              Ragged(batch['edges']), Ragged(batch['V_rows'], B * N), batch['D'])
+    return inputs, lambda *a: self._forward_sparse_impl(N, *a), ('sparse', N)
+
+  def _check_ritz_records(self, batch):
+    """The batch checks of feature records: those of every drop-in with float32 [rows, input_dim] feature
+    rows, then either K alone or both eigenpair arrays."""
+    _, B, _ = self._check_sparse_batch(batch, feature_dim=self.input_dim)
+    if ('V_rows' in batch) != ('D' in batch):
+      raise ValueError('forward_sparse: records carry both V_rows and D, or neither (then K)')
+    if 'V_rows' not in batch:
+      if 'K' not in batch:
+        raise ValueError('forward_sparse: records without eigenpairs need K (data.sparse_collate(..., eigs=False))')
+      return
+    V_rows, D = batch['V_rows'], batch['D']
+    if (V_rows.dtype != torch.float32 or V_rows.dim() != 2 or D.dtype != torch.float32 or
+        tuple(D.shape) != (B, V_rows.shape[1])):
+      raise ValueError('forward_sparse: V_rows must be float32 [rows, K] and D float32 [B, K]; got %s %s and %s %s'
+                       % (V_rows.dtype, tuple(V_rows.shape), D.dtype, tuple(D.shape)))
+
+  def _prepare_ritz_records(self, sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N, **kw):
+    """(GraphPrep, node ids or padded features X, mask, V, L or None) of the records."""
+    prepare = ops.graph_prepare_sparse_features if self._feature_records else ops.graph_prepare_sparse
+    return prepare(sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N, self.num_edgetype + 1, **kw)
+
+  def _ritz_inputs(self, x):
+    """(state, node_ids) of _ritz_conv_stack / ritz_stack_train for the prepare kernel's node output."""
+    return (x, None) if self._feature_records else (None, x)
+
+  def _forward_sparse_impl(self, N, sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, D):
+    E1 = self.num_edgetype + 1
+    K = V_rows.shape[1]
+    dense = not self._sparse_stack_ok(N, E1, K, node_feat.shape[1] if self._feature_records else None)
+    prep, x, mask, V, L = self._prepare_ritz_records(
+        sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N,
+        binarize=getattr(self, '_binarize_operators', False), want_dense=dense, defer_tiles=True)
+    return self._ritz_conv_stack(*self._ritz_inputs(x), L, D.float().contiguous(), V, mask, prep=prep,
+                                 dims_hint=(N, E1))
+
+  def _forward_sparse_eigs_impl(self, N, K, sizes, node_ptr, node_feat, edge_ptr, edges):
+    # V_rows has node_feat's rows (the static capacity under graph replay); rows past node_ptr[B] are
+    # written by nobody and read by nobody
+    D, V_rows, _ = ops.graph_eigs_sparse(sizes, node_ptr, edge_ptr, edges, N, K,
+                                         num_edgetype=self.num_edgetype, rows=node_feat.shape[0])
+    return self._forward_sparse_impl(N, sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, D)
+
+  def _train_records(self, recs, V_rows=None, D=None):
+    # records without eigenpairs get them from lnb_graph_eigs_sparse, as data (no gradient flows to them)
+    from ..train import ell_operator, ritz_stack_train
+    if V_rows is None:
+      D, V_rows, _ = ops.graph_eigs_sparse(recs.sizes, recs.node_ptr, recs.edge_ptr, recs.edges, recs.N, recs.K,
+                                           num_edgetype=self.num_edgetype, rows=recs.node_feat.shape[0])
+    prep, x, mask, V, _ = self._prepare_ritz_records(
+        recs.sizes, recs.node_ptr, recs.node_feat, recs.edge_ptr, recs.edges, V_rows.float().contiguous(), recs.N)
+    return ritz_stack_train(self, *self._ritz_inputs(x), ell_operator(prep), D, V, mask)

@@ -1,10 +1,11 @@
 """Drop-in for the reference ``model.LanczosNetGeneral`` (model/lanczos_net_general.py:13-201):
 LanczosNet with float node features instead of an atom embedding (:156) and the edge-type
-count taken from ``config.dataset.num_edge_type`` (:24)."""
+count taken from ``config.dataset.num_edge_type`` (:24).  ``SparseLanczosNetGeneral`` adds the entries
+from bond-list records with float feature rows."""
 
-from ._common import SpectralNetBase
+from ._common import RitzRecords, SpectralNetBase
 
-__all__ = ['LanczosNetGeneral']
+__all__ = ['LanczosNetGeneral', 'SparseLanczosNetGeneral']
 
 
 class LanczosNetGeneral(SpectralNetBase):
@@ -36,3 +37,19 @@ class LanczosNetGeneral(SpectralNetBase):
   def _forward_impl(self, node_feat, L, D, V, mask):
     return self._ritz_conv_stack(node_feat.float().contiguous(), None, L.float().contiguous(),
                                  D.float().contiguous(), V.float().contiguous(), mask)
+
+
+class SparseLanczosNetGeneral(RitzRecords, LanczosNetGeneral):
+  """LanczosNetGeneral that also runs and trains from bond-list records (``data.sparse_collate`` of
+  ``prepare_graph`` records with float features: ``node_feat`` float32 [sum n, input_dim]).  Same
+  constructor, parameters, initial weights and ``state_dict`` as LanczosNetGeneral, and the same
+  ``forward``; it adds ``forward_sparse``, ``forward_sparse_train`` and ``GraphedStep(sparse=True)``.
+
+  lnb_graph_prepare_sparse_features pads the feature rows into X and builds the ELL rows, mask and V on the
+  device; records without eigenpairs (``eigs=False``, only K) get them from one lnb_graph_eigs_sparse launch
+  in front of it.  Layer 0 (input width 10 in the config) is not a fused-stack shape, so the prepare kernel
+  also writes the dense operators on the device for it, as ``forward`` reads them; they never cross PCIe.
+  Scores from records with eigenpairs equal ``forward`` on ``data.collate`` of the same samples, bit for
+  bit.  Packed batches are not taken."""
+
+  _feature_records = True

@@ -13,7 +13,7 @@ from ._lib import GemmDesc, SpectralStack
 
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'tile_assign', 'spectral_conv_fused',
-    'graph_prepare_sparse', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
+    'graph_prepare_sparse', 'graph_prepare_sparse_features', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
     'spectral_partition', 'spectral_partition_sparse', 'spectral_partition_supported', 'partition_draws', 'gat_bias_sparse',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
@@ -289,6 +289,53 @@ def graph_prepare_sparse(sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N,
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows, prep.tiles_pending = rowmap, nrows, bool(defer_tiles) and B > 0
   return prep, node_ids, mask, V, L
+
+
+def graph_prepare_sparse_features(sizes, node_ptr, node_x, edge_ptr, edges, V_rows, N, E1, binarize=False,
+                                  want_dense=False, defer_tiles=False):
+  """graph_prepare_sparse for records with float node features (lnb_graph_prepare_sparse_features):
+  node_x [>= node_ptr[B], F] float32 holds the feature rows of the real nodes instead of atom ids, and the
+  padded features X [B,N,F] (real rows bit for bit, padded rows 0) come back instead of node ids.
+  1 <= F <= 4096.  Returns (GraphPrep, X [B,N,F], mask [B,N] uint8, V [B,N,K], L [B,N,N,E1] or None)."""
+  for name, t in (('sizes', sizes), ('node_ptr', node_ptr), ('edge_ptr', edge_ptr)):
+    if t.dtype != torch.int32:
+      raise ValueError('graph_prepare_sparse_features: %s must be int32; got %s' % (name, t.dtype))
+  if node_x.dtype != torch.float32 or node_x.dim() != 2 or not node_x.is_contiguous():
+    raise ValueError('graph_prepare_sparse_features: node_x must be a contiguous float32 [rows, F] tensor; got '
+                     '%s %s' % (node_x.dtype, tuple(node_x.shape)))
+  if edges.dtype != torch.uint8 or edges.dim() != 2 or edges.shape[1] != 4 or not edges.is_contiguous():
+    raise ValueError('graph_prepare_sparse_features: edges must be contiguous uint8 [E, 4]')
+  if V_rows.dtype != torch.float32 or V_rows.dim() != 2 or not V_rows.is_contiguous():
+    raise ValueError('graph_prepare_sparse_features: V_rows must be a contiguous float32 [rows, K] tensor')
+  F = int(node_x.shape[1])
+  if not (1 <= int(N) <= 128 and 2 <= int(E1) <= 16 and 1 <= F <= 4096):
+    raise ValueError('graph_prepare_sparse_features: N=%d, E1=%d, F=%d outside 1 <= N <= 128, 2 <= E1 <= 16, '
+                     '1 <= F <= 4096' % (int(N), int(E1), F))
+  _need_cuda(sizes, node_ptr, node_x, edge_ptr, edges, V_rows)
+  dev = sizes.device
+  B = sizes.shape[0]
+  K = V_rows.shape[1]
+  ell_val = torch.empty((B, E1, N, N), device=dev, dtype=torch.float32)
+  ell_idx = torch.empty((B, E1, N, N), device=dev, dtype=torch.uint8)
+  ell_max = torch.empty((B, E1), device=dev, dtype=torch.int32)
+  gext = torch.empty((B, 2), device=dev, dtype=torch.int32)
+  tiles = torch.empty((4 * B + 2,), device=dev, dtype=torch.int32)
+  rowmap = torch.empty((B * K,), device=dev, dtype=torch.int32)
+  nrows = torch.empty((1,), device=dev, dtype=torch.int32)
+  X = torch.empty((B, N, F), device=dev, dtype=torch.float32)
+  mask = torch.empty((B, N), device=dev, dtype=torch.uint8)
+  V = torch.empty((B, N, K), device=dev, dtype=torch.float32)
+  L = torch.empty((B, N, N, E1), device=dev, dtype=torch.float32) if want_dense else None
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_graph_prepare_sparse_features(
+        _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(node_x), _ptr(edge_ptr), _ptr(edges),
+        _ptr(V_rows), _ptr(_inv_sqrt_deg_table(dev)), B, int(N), int(E1), int(K), F,
+        (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0), _ptr(ell_val), _ptr(ell_idx),
+        _ptr(ell_max), _ptr(gext), _ptr(tiles), _ptr(rowmap), _ptr(nrows), _ptr(X), _ptr(mask), _ptr(V), _ptr(L)),
+               'lnb_graph_prepare_sparse_features')
+  prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
+  prep.rowmap, prep.nrows, prep.tiles_pending = rowmap, nrows, bool(defer_tiles) and B > 0
+  return prep, X, mask, V, L
 
 
 def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=False, host_tiles=True):
