@@ -149,6 +149,13 @@ int lnb_spectral_conv_fused(lnb_stream_t stream, const float* X, const float* Q,
                             const float* W_lo, const float* bias, int B, int N, int Din, int E1,
                             int K, int S, int H, int relu, int write_pad, float* out);
 
+/* Length of the fp64 table inv_sqrt_deg that the normalising sparse producers take (lnb_graph_prepare_sparse
+ * and its variants, lnb_graph_eigs_sparse, lnb_spectral_partition(_sparse)): entry d is numpy's
+ * np.power(d, -0.5), entry 0 is 0.  It covers every simple-graph degree of their envelope, deg = 1 + the
+ * multiplicities summed over bond types, at most 1 + 32 * 128 (32 bond types, self-loops included, on 128
+ * nodes). */
+#define LNB_INV_SQRT_DEG_LEN 4098
+
 /* ---------------------------------------------------------------------------------------
  * GPU-side batch construction from SPARSE per-molecule records (replaces, on the device, the host
  * pipeline utils/data_helper.py:92-116,155-156 (L4 = D^-1/2 (A + I) D^-1/2 of every bond channel and
@@ -157,15 +164,15 @@ int lnb_spectral_conv_fused(lnb_stream_t stream, const float* X, const float* Q,
  *   sizes [B] real nodes per graph; node_ptr [B+1] their prefix sums; node_feat [node_ptr[B]] atom
  *   ids of the real nodes; edge_ptr [B+1]; edges [edge_ptr[B]][4] bytes {u, v, bond type, 0}
  *   (undirected bonds listed once, local node indices); V_rows [node_ptr[B], K] Ritz vectors of the
- *   real nodes; inv_sqrt_deg [256] fp64 table of deg^-1/2 (entry 0 = 0) from the host's numpy, so
- *   the fp64 products (scale_i * m_ij) * scale_j and their single rounding to fp32 are bit-identical
- *   to the reference's preprocessing.
+ *   real nodes; inv_sqrt_deg [LNB_INV_SQRT_DEG_LEN] fp64 table of deg^-1/2 (entry 0 = 0) from the
+ *   host's numpy, so the fp64 products (scale_i * m_ij) * scale_j and their single rounding to fp32 are
+ *   bit-identical to the reference's preprocessing.
  * Outputs: everything lnb_graph_prepare emits (same layouts, same bits: ell_val / ell_idx / ell_max /
  * gext / tiles / rowmap / nrows), the padded node_ids [B,N] int64, mask [B,N] uint8 and
  * V [B,N,K] that lnb_spectral_stack_forward reads, and -- only when L_dense != NULL -- the padded dense
  * operators [B,N,N,E1] exactly as the reference's collate builds them.  flags as lnb_graph_prepare
  * (LNB_PREP_DEFER_TILES included).
- * Limits: N <= 128, 2 <= E1 <= 16, degrees < 255.
+ * Limits: N <= 128, 2 <= E1 <= 16.
  * ------------------------------------------------------------------------------------- */
 int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
                              const int32_t* node_feat, const int32_t* edge_ptr, const uint8_t* edges,
@@ -205,7 +212,7 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
  * loads otherwise; the bits are the same either way.  Same kernel as lnb_graph_prepare_sparse (a
  * compile-time variant), one launch plus the tile assignment unless LNB_PREP_DEFER_TILES.
  * Limits: 1 <= N <= 128, 2 <= E1 <= 16, K >= 1, 1 <= F <= 4096 (LNB_ERR_UNSUPPORTED otherwise, nothing
- * launched), degrees < 255. */
+ * launched). */
 int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
                                       const float* node_x, const int32_t* edge_ptr, const uint8_t* edges,
                                       const float* V_rows, const double* inv_sqrt_deg, int B, int N, int E1,
@@ -639,9 +646,9 @@ int lnb_sym_eigs(lnb_stream_t stream, const float* A, int64_t elem_stride, const
  * GPNN's graph partition (utils/spectral_graph_partition.py:10-50 as the GPNN collate calls it per
  * padded graph, dataset/qm8.py:123-136) in one launch.  Per graph b:
  *   1. the operator: channel 0 of L read in place, L[((b*N + i)*N + j) * elem_stride].  The fp64 L4
- *      s_i s_j of its off-diagonal non-zero pattern is rebuilt with inv_sqrt_deg [256] (deg = 1 + the
- *      row's count; a node with a zero diagonal is padding and keeps a zero row); if its fp32 rounding
- *      is channel 0 bit for bit that fp64 matrix is decomposed (the matrix the reference hands eigsh),
+ *      s_i s_j of its off-diagonal non-zero pattern is rebuilt with inv_sqrt_deg [LNB_INV_SQRT_DEG_LEN]
+ *      (deg = 1 + the row's count; a node with a zero diagonal is padding and keeps a zero row); if its
+ *      fp32 rounding is channel 0 bit for bit that fp64 matrix is decomposed (the matrix the reference hands eigsh),
  *      otherwise the widened fp32 values are and status bit 3 is set;
  *   2. the P eigenvectors of largest |lambda| of the whole padded N x N (the solver of lnb_sym_eigs);
  *      bit 1 when |lambda_P| and |lambda_P+1| are within 1e-9 (the reference's choice is then open);
@@ -659,7 +666,7 @@ int lnb_sym_eigs(lnb_stream_t stream, const float* A, int64_t elem_stride, const
  * ------------------------------------------------------------------------------------- */
 int lnb_spectral_partition_draws(int P);
 int lnb_spectral_partition(lnb_stream_t stream, const float* L, int64_t elem_stride, int B, int N, int P,
-                           const double* inv_sqrt_deg /* [256] */, const double* draws, int32_t* labels /* [B,N] */,
+                           const double* inv_sqrt_deg /* [LNB_INV_SQRT_DEG_LEN] */, const double* draws, int32_t* labels /* [B,N] */,
                            float* L_cluster /* [B,N,N] */, float* L_cut /* [B,N,N] */, int32_t* status /* [B] */);
 
 /* GPNN's graph partition from the sparse records of lnb_graph_prepare_sparse (sizes, edge_ptr, edges;

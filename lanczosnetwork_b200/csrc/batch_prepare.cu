@@ -8,9 +8,10 @@
 // PCIe.
 //
 // Bit-exactness: the reference normalises in fp64 -- scale = deg^-1/2, value = (scale_i * m_ij) *
-// scale_j -- and casts to fp32 at collate (dataset/qm8.py:262).  Degrees are small integers, so the
-// host passes a 256-entry fp64 table of numpy's deg^-1/2; the kernel forms the same two fp64
-// products in the same order and rounds once (__double2float_rn): identical bits by construction.
+// scale_j -- and casts to fp32 at collate (dataset/qm8.py:262).  Degrees are integers, so the host
+// passes an fp64 table of numpy's deg^-1/2 covering every degree of the envelope (LNB_INV_SQRT_DEG_LEN);
+// the kernel forms the same two fp64 products in the same order and rounds once (__double2float_rn):
+// identical bits by construction.
 // Masks, ids, ELL indices and extents are integer logic.
 #include "common.cuh"
 
@@ -28,7 +29,7 @@ struct SparseBatchParams {
   const int32_t* edge_ptr;     // [B+1]
   const uint8_t* edges;        // [edge_ptr[B]][4] = {u, v, bond type, 0}, undirected, listed once
   const float* V_rows;         // [node_ptr[B], K] Ritz vectors, rows of real nodes only
-  const double* inv_sqrt_deg;  // [256] deg^-1/2 in fp64 (entry 0 = 0)
+  const double* inv_sqrt_deg;  // [LNB_INV_SQRT_DEG_LEN] deg^-1/2 in fp64 (entry 0 = 0)
   const uint8_t* blob;         // packed batch (lnb_graph_prepare_sparse_packed): the pointers above are derived
                                // from its header on the device, so ONE H2D copy ships a whole batch
   int B, N, E1, K, flags;
@@ -131,7 +132,7 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
       } else {
         for (int w = 0; w < BP_NW; ++w) deg += __popc(rowmask[((ch - 1) * BP_NMAX + i) * BP_NW + w]);
       }
-      sc = P.inv_sqrt_deg[deg < 255 ? deg : 255];
+      sc = P.inv_sqrt_deg[min(deg, LNB_INV_SQRT_DEG_LEN - 1)];
     }
     scale[ch * BP_NMAX + i] = sc;
   }
@@ -274,7 +275,8 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
               "graph_prepare_sparse: bad dims B=%d N=%d E1=%d K=%d (N <= %d, 2 <= E1 <= %d)", B, N, E1,
               K, BP_NMAX, BP_EMAX);
   if (B == 0) return LNB_OK;
-  LNB_REQUIRE(sizes && node_ptr && node_feat && edge_ptr && edges && V_rows && inv_sqrt_deg &&
+  // edges may be NULL when the batch has no bonds: the kernel reads [edge_ptr[b], edge_ptr[b+1]) only
+  LNB_REQUIRE(sizes && node_ptr && node_feat && edge_ptr && V_rows && inv_sqrt_deg &&
                   ell_val && ell_idx && ell_max && gext && tiles && node_ids && mask && V,
               "graph_prepare_sparse: null pointer");
   LNB_REQUIRE((rowmap == nullptr) == (nrows == nullptr), "graph_prepare_sparse: rowmap and nrows go together");
@@ -322,7 +324,8 @@ int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes,
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;
-  LNB_REQUIRE(sizes && node_ptr && node_x && edge_ptr && edges && V_rows && inv_sqrt_deg && ell_val &&
+  // edges may be NULL when the batch has no bonds, as in lnb_graph_prepare_sparse
+  LNB_REQUIRE(sizes && node_ptr && node_x && edge_ptr && V_rows && inv_sqrt_deg && ell_val &&
                   ell_idx && ell_max && gext && tiles && X && mask && V,
               "graph_prepare_sparse_features: null pointer");
   LNB_REQUIRE((rowmap == nullptr) == (nrows == nullptr),

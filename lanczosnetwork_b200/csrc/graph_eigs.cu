@@ -69,7 +69,7 @@ graph_eigs_kernel(const EigParams P) {
     if (t < n) {
       int deg = 1;                                        // the + I of L4
       for (int j = 0; j < n; ++j) deg += __popc(mk[t * n + j]);
-      sc[t] = P.inv_sqrt_deg[deg < 255 ? deg : 255];
+      sc[t] = P.inv_sqrt_deg[min(deg, LNB_INV_SQRT_DEG_LEN - 1)];
     }
     gsync<W>();
     if (t < n) {

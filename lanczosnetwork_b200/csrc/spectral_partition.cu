@@ -36,7 +36,7 @@ struct PartParams {
   const float* L; int64_t es;                 // channel 0: L[((b * N + i) * N + j) * es]
   // sparse entry: the records of lnb_graph_prepare_sparse, bond types < E
   const int32_t* sizes; const int32_t* edge_ptr; const uint8_t* edges; int E;
-  const double* inv_sqrt_deg;                 // [256]
+  const double* inv_sqrt_deg;                 // [LNB_INV_SQRT_DEG_LEN]
   const double* draws;                        // [1 + (P - 1) * T]
   int B, N, P, T;
   int32_t* labels; float* L_cluster; float* L_cut; int32_t* status;   // L_cluster / L_cut may be null
@@ -318,7 +318,7 @@ spectral_partition_kernel(const PartParams p) {
       for (int j = 0; j < n && t < n; ++j) deg += __popc(mk[t * n + j]);
       for (int k = 0; k < NW; ++k) any |= adj[t * NW + k] != 0u;
       linked[t] = any;
-      w.sc()[t] = t < n ? p.inv_sqrt_deg[deg < 255 ? deg : 255] : 0.0;   // padding: a zero row
+      w.sc()[t] = t < n ? p.inv_sqrt_deg[min(deg, LNB_INV_SQRT_DEG_LEN - 1)] : 0.0;   // padding: a zero row
     }
     gsync<W>();
     if (t < N) {

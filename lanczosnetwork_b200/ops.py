@@ -237,15 +237,17 @@ def graph_prepare(L, Q=None, binarize=False, defer_tiles=False):
 
 
 _INV_SQRT_DEG = {}
+# LNB_INV_SQRT_DEG_LEN: every simple-graph degree of the sparse producers' envelope, up to 1 + 32 * 128
+INV_SQRT_DEG_LEN = 4098
 
 
 def _inv_sqrt_deg_table(device):
-  """deg^-1/2 in fp64 for deg = 0..255 exactly as the reference's host code computes it
+  """deg^-1/2 in fp64 for deg = 0 .. INV_SQRT_DEG_LEN - 1 exactly as the reference's host code computes it
   (np.power(deg, -0.5) with inf -> 0, utils/data_helper.py:104-107), cached per device."""
   key = device.index if device.index is not None else torch.cuda.current_device()
   if key not in _INV_SQRT_DEG:
     import numpy as np
-    deg = np.arange(256, dtype=np.float64)
+    deg = np.arange(INV_SQRT_DEG_LEN, dtype=np.float64)
     with np.errstate(divide='ignore'):
       t = np.power(deg, -0.5)
     t[np.isinf(t)] = 0.0
