@@ -77,7 +77,9 @@ class AdaLanczosNet(SpectralNetBase):
       # fused kernel, tridiagonalisation only (no QL / Ritz vectors for the learned filter)
       lz = ops.lanczos_ritz(Le, mask, q1, K, want_ritz=False)
       Q = lz['Q']
-      powers = ops.tridiag_powers(lz['T'], self.long_diffusion_dist)     # [B,K,S,K], once
+      # ascending powers, the order of the reference's T_list (ada_lanczos_net.py:266-268) whatever
+      # the order of the config list
+      powers = ops.tridiag_powers(lz['T'], sorted(self.long_diffusion_dist))   # [B,K,S,K], once
       self.last_lanczos = lz
 
     ctx = GraphContext(L, Q)
@@ -153,7 +155,7 @@ class KeyedAdaLanczosNet(AdaLanczosNet):
   def _train_impl(self, node_feat, L, mask, q1):
     from ..train import ada_train, lanczos_tridiag, tridiag_powers
     K = self.num_eig_vec
-    fits = ops.tridiag_powers_backward_supported(K, self.long_diffusion_dist or [1])
+    fits = ops.tridiag_powers_backward_supported(K, sorted(self.long_diffusion_dist) or [1])
     return ada_train(self, node_feat, L, mask, q1, powers_fn=tridiag_powers if fits else None,
                      lanczos_fn=lanczos_tridiag if ops.lanczos_tridiag_train_supported(L.shape[1], K) else None)
 

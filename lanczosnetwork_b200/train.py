@@ -948,7 +948,7 @@ def ada_train(model, node_ids, L, mask, q1, powers_fn=None, lanczos_fn=None):
   """Differentiable AdaLanczosNet (model/ada_lanczos_net.py:288-368): embedding -> learned Gaussian
   Laplacian -> Lanczos -> learned filter on the powers of T (the 4096-wide MLP on the wgmma dense
   kernel) -> graph convolutions with [short walk | Q G_s Q^T X | L_e X] messages -> gated readout.
-  ``powers_fn(T, dist)`` -> [B,K,S,K], when given, replaces the chain of ``bmm`` products that forms the
+  ``powers_fn(T, dist)`` -> [B,K,S,K] (dist ascending), when given, replaces the chain of ``bmm`` products that forms the
   powers of T, and ``lanczos_fn(A, mask, q1, K)`` -> (T, Q) replaces ``_lanczos_train`` (the defaults are
   AdaLanczosNet's own formulation)."""
   L = L.float().contiguous()
@@ -961,7 +961,7 @@ def ada_train(model, node_ids, L, mask, q1, powers_fn=None, lanczos_fn=None):
     Le = _gaussian_laplacian_train(state, adj)
     T, Q = (lanczos_fn or _lanczos_train)(Le, mask, q1.to(L.device), K)
     if powers_fn is not None:
-      P4 = powers_fn(T, model.long_diffusion_dist)                  # [B,K,S,K]
+      P4 = powers_fn(T, sorted(model.long_diffusion_dist))          # [B,K,S,K], ascending like the chain below
       powers = P4.reshape(B, K, S * K)
       plist = P4.unbind(dim=2)
     else:
