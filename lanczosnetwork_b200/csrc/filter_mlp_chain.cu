@@ -125,11 +125,11 @@ struct ChainPolicy {
     // S <= 8, W1 and W3 (hi + lo) and b3.  The consumers read the previous layer's biases for the
     // last time before the drain these producers have read by now.
     if (layer != cur_layer) {
-      tcg::producers_sync();
+      tcg::producers_sync<ChainPolicy>();
       const int row0 = w_row0(p, layer, 0), row3 = w_row0(p, layer, 3);
       if (!mma0(p)) {
 #pragma unroll 4
-        for (int e = tid; e < p.Hd * S0MAX; e += tcg::PRODUCER_THREADS) {
+        for (int e = tid; e < p.Hd * S0MAX; e += tcg::producer_threads<ChainPolicy>) {
           const int c = e / S0MAX, k = e - c * S0MAX;
           const int64_t o1 = (int64_t)(row0 + c) * p.Hd + k;
           W1s[e] = (k < p.S) ? __ldg(p.W_hi + o1) + __ldg(p.W_lo + o1) : 0.f;
@@ -138,11 +138,11 @@ struct ChainPolicy {
         }
         if (tid < S0MAX) b3s[tid] = tid < p.S ? __ldg(p.bias_all + row3 + tid) : 0.f;
       }
-      for (int e = tid; e < 3 * tcg::BN; e += tcg::PRODUCER_THREADS) {
+      for (int e = tid; e < 3 * tcg::BN; e += tcg::producer_threads<ChainPolicy>) {
         const int st = e / tcg::BN, c = e - st * tcg::BN;
         bs[e] = c < p.Hd ? __ldg(p.bias_all + row0 + st * p.Hd + c) : 0.f;
       }
-      tcg::producers_sync();
+      tcg::producers_sync<ChainPolicy>();
       cur_layer = layer;
       tm.lap(1);
     }

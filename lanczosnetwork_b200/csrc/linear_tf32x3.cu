@@ -95,7 +95,7 @@ struct RowLoadPolicy {
   __device__ __forceinline__ void produce(int, int kb, float (&v)[32]) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = cur[j];
-    load(kb + tcg::NGROUPS, cur);   // this group's next k-block (zeros past K)
+    load(kb + tcg::ProducerGroups<RowLoadPolicy>::value, cur);   // this group's next k-block (zeros past K)
   }
   __device__ __forceinline__ void pre_epilogue(int) {}
   __device__ __forceinline__ void store(int sub, int col, const float (&x)[tcg::EW]) {
@@ -117,13 +117,13 @@ struct RowLoadPolicy {
     if (p.splits == 1) return;
     const int tid = grp * 128 + r;
     __threadfence();                       // this thread's partials are visible device-wide
-    tcg::producers_sync();
+    tcg::producers_sync<RowLoadPolicy>();
     if (tid == 0) {
       const int old = atomicAdd(p.counters + tile, 1);
       *flag = (old == p.splits - 1);
       if (old == p.splits - 1) p.counters[tile] = 0;      // ready for the next launch
     }
-    tcg::producers_sync();
+    tcg::producers_sync<RowLoadPolicy>();
     if (*flag) {
       __threadfence();
       const int ns = sub % n_tiles(p);
@@ -132,7 +132,7 @@ struct RowLoadPolicy {
       const int ncols = left < tcg::BN ? left : tcg::BN;
       const int w0 = w_row0(p, sub);
       const float* base = p.ws + (int64_t)tile * p.splits * tcg::BM * tcg::BN;
-      for (int e = tid; e < tcg::BM * tcg::BN / 4; e += tcg::PRODUCER_THREADS) {
+      for (int e = tid; e < tcg::BM * tcg::BN / 4; e += tcg::producer_threads<RowLoadPolicy>) {
         const int rr = e / (tcg::BN / 4), c4 = (e - rr * (tcg::BN / 4)) * 4;
         if (m0 + rr >= p.M || c4 >= ncols) continue;
         float4 acc = __ldcg(reinterpret_cast<const float4*>(base + rr * tcg::BN + c4));
@@ -152,7 +152,7 @@ struct RowLoadPolicy {
         }
       }
     }
-    tcg::producers_sync();                 // `flag` is rewritten by the next item
+    tcg::producers_sync<RowLoadPolicy>();  // `flag` is rewritten by the next item
   }
 };
 

@@ -129,7 +129,7 @@ struct SageLstmPolicy {
 };
 
 // The skeleton's body under a name of its own, so profiles and SASS dumps name the LSTM step
-__global__ void __launch_bounds__(tcg::THREADS, 1)
+__global__ void __launch_bounds__(tcg::cta_threads<SageLstmPolicy>, 1)
 sage_lstm_step_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                       const SageLstmParams p) {
   tcg::tc_gemm_body<SageLstmPolicy, 0>(map_hi, map_lo, p);
@@ -154,7 +154,7 @@ int launch_step(lnb_stream_t stream, const float* W_hi, const float* W_lo, int D
   const size_t smem = SageLstmPolicy::SMEM_BYTES;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   const int grid = items < tcg::sm_count() ? items : tcg::sm_count();
-  kern<<<grid, tcg::THREADS, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
+  kern<<<grid, tcg::cta_threads<SageLstmPolicy>, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
   lnb::count_launch();
   return lnb::finish_launch(who);
 }

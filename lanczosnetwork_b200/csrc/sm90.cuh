@@ -142,6 +142,15 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// Per-thread register budget of the calling warpgroup (a multiple of 8 in [24, 256]); every warp of
+// the warpgroup executes it.  inc blocks until other warpgroups have released enough with dec.
+template <int kRegs> __device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
+}
+template <int kRegs> __device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
+}
+
 __device__ __forceinline__ uint32_t tf32_rna_bits(float v) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));

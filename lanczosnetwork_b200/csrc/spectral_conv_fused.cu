@@ -29,7 +29,6 @@ constexpr int KMAX = 32;        // max Ritz pairs
 constexpr int GMAX = 32;        // max graphs per tile
 constexpr int RMAX = 128;       // rows per tile
 constexpr int EMAX = 16;        // max operator channels
-constexpr int FR = 8;           // filter coefficients held in registers per row
 
 // --------------------------------------------------------------------------------------------
 // Per-forward operator compression and extents.
@@ -501,6 +500,9 @@ struct SpectralPolicyT {
   static constexpr int kStagesB = 2;      // k-block i + 1 is produced and its W tile loaded during MMA i
   static constexpr int kStagesA = 2;      // 64 KB: also holds Z (Ztot <= 128 rows x H <= 128) in one pass
   static constexpr int LMAX = 8;          // layers run by one launch
+  // Two producer warpgroups take alternate k-blocks: producing a k-block (an ELL gather or U, then
+  // the hi / lo split) takes one group about as long as the MMAs that consume it
+  static constexpr int kProducerGroups = 2;
   struct Params {
     const float* X;         // [B, N, Din0] input state, or nullptr with node_ids/emb (embedding)
     const int64_t* node_ids;// [B, N]
@@ -586,8 +588,7 @@ struct SpectralPolicyT {
   float* Qs;                // [RMAX][K]
   float* Ev;                // [LB][RMAX] staged ELL values
   uint8_t* Ei;              // [LB][RMAX] staged ELL columns as tile-local row indices
-  float fr[FR];             // this (graph, k) row's filter coefficients f[k, 0..S)
-  float u[tcg::BK];         // step 0: this (graph, k) row's U columns of the current d-block
+  const float* frow;        // this (graph, k) row's filter coefficients f[k, 0..S) of the layer
   float* ring;              // the skeleton's A ring: the fused readout's scratch
   tcg::PhaseTimer* ptm = nullptr;   // profiling aid: the current step's timer
 
@@ -678,17 +679,17 @@ struct SpectralPolicyT {
   }
 
   __device__ void step_begin(int m_tile, int sub, int /*kb_first*/, tcg::PhaseTimer& tm) {
-    tcg::producers_sync();              // previous step's smem readers / writers are done
+    tcg::producers_sync<SpectralPolicyT>();              // previous step's smem readers / writers are done
     const int layer = sub >> 1, step = sub & 1;
     if (step == 1 && S > 0) return;     // tile state was staged by step 0 of this layer
     Din = p.Din[layer];
     const int warp = tid >> 5, lane = tid & 31;
-    constexpr int NW = tcg::PRODUCER_THREADS / 32;
+    constexpr int NW = tcg::producer_threads<SpectralPolicyT> / 32;
     const int dv = Din / 4;
     ptm = &tm;
     if (layer == 0) {
     if (warp == 0) build_tables(m_tile);
-    tcg::producers_sync();
+    tcg::producers_sync<SpectralPolicyT>();
     tm.lap(16);
     const int Rtot = tb->Rtot;
     // ---- phase A: asynchronous copies of the real rows of X and Q (one warp per row) --------
@@ -751,67 +752,59 @@ struct SpectralPolicyT {
     tm.lap(18);
     }  // layer == 0: tile state staged once, reused by every layer
     const int Ztot = tb->Ztot;
-    // this thread's (graph, k) row: filter coefficients of this layer into registers
-#pragma unroll
-    for (int i = 0; i < FR; ++i) fr[i] = 0.f;
-    if (S > 0 && r < Ztot) {
-      const float* f = p.coeff + layer * p.coeff_stride + ((int64_t)tb->gid[tb->z_g[r]] * K + tb->z_k[r]) * S;
-#pragma unroll
-      for (int i = 0; i < FR; ++i)
-        if (i < S) fr[i] = __ldg(f + i);
-    }
+    // this thread's (graph, k) row of this layer's filter coefficients (read once per k-block, from L1)
+    frow = p.coeff;                     // a valid address for the rows past Ztot as well
+    if (S > 0 && r < Ztot)
+      frow = p.coeff + layer * p.coeff_stride + ((int64_t)tb->gid[tb->z_g[r]] * K + tb->z_k[r]) * S;
     tm.lap(0);
     sm90::cp_async_wait_all();
-    tcg::producers_sync();
+    tcg::producers_sync<SpectralPolicyT>();
     tm.lap(1);
   }
 
-  __device__ __forceinline__ void produce(int sub, int kb, float (&v)[32]) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = 0.f;
+  // The A row of k-block kb is scale * v (the skeleton multiplies while it splits), so that step 0
+  // keeps only U in registers across the k-blocks of a d-block
+  __device__ __forceinline__ float produce(int sub, int kb, float (&v)[32]) {
     if (kLongScales && (sub & 1) == 0) {
-      // row = (graph, Ritz index): f[k, s] * U[row, d0:d0+32], kb = dblk * S + s
-      if (r >= tb->Ztot) return;
+      // row = (graph, Ritz index): f[k, s] * U[row, d0:d0+32], kb = dblk * S + s; v holds U (zero
+      // for the rows past Ztot, whose scale is 0)
       const int s = kb % S;
-      if (s == 0) {
+      const float f = __ldg(frow + s);             // issued before U is summed
+      if (s < kProducerGroups) {
         // U[(g, k), d0:d0+32] = sum_n Q_g[n, k] X_g[n, d0:d0+32]: every thread of graph g reads the
-        // same X row (a broadcast), consecutive Q entries
-        const int g = tb->z_g[r], n_g = tb->gn[g], nb = tb->nbase[g];
-        const float* xs = Xs + (size_t)nb * XP + (kb / S) * tcg::BK;
-        const float* qs = Qs + (size_t)nb * K + tb->z_k[r];
+        // same X row (a broadcast), consecutive Q entries.  The groups take alternate k-blocks, so
+        // each one's first k-block of the d-block is s = 0 or s = 1: each computes U for itself.
 #pragma unroll
-        for (int j = 0; j < tcg::BK; ++j) u[j] = 0.f;
+        for (int j = 0; j < tcg::BK; ++j) v[j] = 0.f;
+        if (r < tb->Ztot) {
+          const int g = tb->z_g[r], n_g = tb->gn[g], nb = tb->nbase[g];
+          const float* xs = Xs + (size_t)nb * XP + (kb / S) * tcg::BK;
+          const float* qs = Qs + (size_t)nb * K + tb->z_k[r];
 #pragma unroll 2
-        for (int n = 0; n < n_g; ++n) {
-          const float q = qs[(size_t)n * K];
-          const float4* x4 = reinterpret_cast<const float4*>(xs + (size_t)n * XP);
+          for (int n = 0; n < n_g; ++n) {
+            const float q = qs[(size_t)n * K];
+            const float4* x4 = reinterpret_cast<const float4*>(xs + (size_t)n * XP);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 t = x4[j];
-            u[4 * j + 0] = fmaf(q, t.x, u[4 * j + 0]); u[4 * j + 1] = fmaf(q, t.y, u[4 * j + 1]);
-            u[4 * j + 2] = fmaf(q, t.z, u[4 * j + 2]); u[4 * j + 3] = fmaf(q, t.w, u[4 * j + 3]);
+            for (int j = 0; j < 8; ++j) {
+              const float4 t = x4[j];
+              v[4 * j + 0] = fmaf(q, t.x, v[4 * j + 0]); v[4 * j + 1] = fmaf(q, t.y, v[4 * j + 1]);
+              v[4 * j + 2] = fmaf(q, t.z, v[4 * j + 2]); v[4 * j + 3] = fmaf(q, t.w, v[4 * j + 3]);
+            }
           }
         }
       }
-      float f = 0.f;
-      if (S <= FR) {
-#pragma unroll
-        for (int i = 0; i < FR; ++i) f = (i == s) ? fr[i] : f;
-      } else {
-        f = __ldg(p.coeff + (sub >> 1) * p.coeff_stride + ((int64_t)tb->gid[tb->z_g[r]] * K + tb->z_k[r]) * S + s);
-      }
-#pragma unroll
-      for (int j = 0; j < tcg::BK; ++j) v[j] = f * u[j];
-      return;
+      return r < tb->Ztot ? f : 0.f;
     }
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] = 0.f;
     const int j0 = kb * tcg::BK;
     const int c = j0 / Din, d0 = j0 - c * Din;
     // edge type e = c: sparse row of L_e (ELL) times X[:, d0:d0+32]; row = (graph, node)
-    if (r >= tb->Rtot) return;
+    if (r >= tb->Rtot) return 1.f;
     const int e = c;
     if constexpr (kMaxAgg) {
       produce_max(e, d0, v);
-      return;
+      return 1.f;
     }
     const float* xs = Xs + d0;
     const int ts = tb->cnt_e[e], tmax = tb->tmax_e[e];
@@ -855,6 +848,7 @@ struct SpectralPolicyT {
         }
       }
     }
+    return 1.f;
   }
 
   // Max aggregator (STACK_SAGE_MAX): v = elementwise max over X[i, d0:d0+32] for the entries i of
@@ -937,7 +931,7 @@ struct SpectralPolicyT {
   // The edge step's store() overwrites rows of X that other producers may still be reading.
   __device__ void pre_epilogue(int sub) {
     if ((sub & 1) == 0) return;
-    tcg::producers_sync();              // every producer is done reading X
+    tcg::producers_sync<SpectralPolicyT>();              // every producer is done reading X
     if (ptm) ptm->lap(22);              // (profiling) wait for the slowest producer group
   }
 
@@ -1000,15 +994,16 @@ struct SpectralPolicyT {
   // requested) and / or the fused readout.  Between layers the state never leaves the SM.
   __device__ void post_epilogue(int sub) {
     if constexpr (kNormRows) {
-      // thread r stored every chunk of row r itself; the next reader of other rows (next layer's
-      // producers, the write-back and readout below) is behind a producers_sync()
-      if ((sub & 1) != 0 && r < tb->Rtot) normalize_row(Xs + (size_t)r * XP);
+      // every chunk of every row is stored (the skeleton's producers_sync); thread r of the first
+      // group normalises row r, and the next reader of other rows (next layer's producers, the
+      // write-back and readout below) is behind another producers_sync()
+      if ((sub & 1) != 0 && tid < tcg::BM && r < tb->Rtot) normalize_row(Xs + (size_t)r * XP);
     }
     if ((sub & 1) == 0 || (sub >> 1) != p.L - 1) return;
-    tcg::producers_sync();              // every chunk of every row is in shared memory
+    tcg::producers_sync<SpectralPolicyT>();              // every chunk of every row is in shared memory
     if (ptm) ptm->lap(19);
     const int warp = tid >> 5, lane = tid & 31;
-    constexpr int NW = tcg::PRODUCER_THREADS / 32;
+    constexpr int NW = tcg::producer_threads<SpectralPolicyT> / 32;
     const int hv = H / 4, Rtot = tb->Rtot;
     const float* bias = p.bias ? p.bias + (p.L - 1) * H : nullptr;
     if (p.out) {
@@ -1051,31 +1046,31 @@ struct SpectralPolicyT {
     float* Wr = ring;                                // [4 PQ][HP]  W_out rows, w_att, zero rows (the ring is idle)
     float* Yr = Wr + (size_t)4 * PQ * HP;            // [RMAX + 1][P1]  per-row outputs; last = pad row
     float* cx = Yr + (size_t)(RMAX + 1) * P1 + ((4 - ((RMAX + 1) * P1 & 3)) & 3);   // [H], 16 B aligned
-    for (int e = tid; e < 4 * PQ * H; e += tcg::PRODUCER_THREADS) {
+    for (int e = tid; e < 4 * PQ * H; e += tcg::producer_threads<SpectralPolicyT>) {
       const int o = e / H, h = e - o * H;
       Wr[o * HP + h] = (o < P) ? __ldg(p.W_out + o * H + h) : (o == P ? __ldg(p.w_att + h) : 0.f);
     }
     [[maybe_unused]] float den = 1.f;
     if constexpr (kNormRows) den = pad_den(bias_last);
-    for (int h = tid; h < H; h += tcg::PRODUCER_THREADS) {
+    for (int h = tid; h < H; h += tcg::producer_threads<SpectralPolicyT>) {
       float t = bias_last ? __ldg(bias_last + h) : 0.f;
       cx[h] = (p.relu != 0) ? fmaxf(t, 0.f) : t;
       if constexpr (kNormRows) cx[h] = cx[h] / den;
     }
     uint8_t* mk = reinterpret_cast<uint8_t*>(cx + H);   // [ng][N] node masks of the tile's graphs
-    for (int e = tid; e < tb->ng * N; e += tcg::PRODUCER_THREADS) {
+    for (int e = tid; e < tb->ng * N; e += tcg::producer_threads<SpectralPolicyT>) {
       const int g = e / N;
       mk[e] = p.mask ? __ldg(p.mask + (int64_t)tb->gid[g] * N + (e - g * N)) : (uint8_t)1;
     }
-    tcg::producers_sync();
+    tcg::producers_sync<SpectralPolicyT>();
     if (ptm) ptm->lap(20);
     const int Rtot = tb->Rtot;
-    // warp <-> (block of 32 rows, third of the outputs): lane = row, so the row loads are
+    // warp <-> (block of 32 rows, half of the outputs): lane = row, so the row loads are
     // conflict-free and every weight load is one broadcast wavefront
     {
       const int warp = tid >> 5, lane = tid & 31;
       const int rb = warp & 3, og = warp >> 2;
-      const int per = (P1 + tcg::NGROUPS - 1) / tcg::NGROUPS;
+      const int per = (P1 + kProducerGroups - 1) / kProducerGroups;
       const int o_end = min(P1, (og + 1) * per);
       const int row = rb * 32 + lane;
       const float4* x4 = reinterpret_cast<const float4*>(Xs + (size_t)(row < Rtot ? row : 0) * XP);
@@ -1106,7 +1101,7 @@ struct SpectralPolicyT {
         }
       }
       // the constant padded-node row: one warp per output, lanes stride the H features
-      for (int o = warp; o < P1; o += tcg::PRODUCER_THREADS / 32) {
+      for (int o = warp; o < P1; o += tcg::producer_threads<SpectralPolicyT> / 32) {
         float acc = 0.f;
         for (int h = lane; h < H; h += 32) acc = fmaf(cx[h], Wr[o * HP + h], acc);
 #pragma unroll
@@ -1117,9 +1112,9 @@ struct SpectralPolicyT {
         }
       }
     }
-    tcg::producers_sync();
+    tcg::producers_sync<SpectralPolicyT>();
     if (ptm) ptm->lap(21);
-    for (int e = tid; e < tb->ng * P; e += tcg::PRODUCER_THREADS) {
+    for (int e = tid; e < tb->ng * P; e += tcg::producer_threads<SpectralPolicyT>) {
       const int g = e / P, o = e - g * P;
       const int nb = tb->nbase[g], n_g = tb->gn[g];
       const uint8_t* m = mk + g * N;

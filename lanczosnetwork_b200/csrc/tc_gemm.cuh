@@ -19,6 +19,9 @@
 //                   Every consumer warp runs the W cursor and its waits; the elected lane of warp 4
 //                   issues the W tile loads (TMA, predicated inside the asm), kStagesB k-blocks ahead.
 //                   Policies without acc_init keep one MMA group queued (wgmma.wait_group 1).
+// A policy with kProducerGroups = 2 runs 16 warps: two producer warpgroups (warps 0-7) that take
+// alternate k-blocks and split the epilogue's columns, and the consumers in warps 8-15.  512 threads
+// start at 128 registers; setmaxnreg takes the producers down to 88 and the consumers up to 168.
 // The accumulators reach the epilogue through shared memory: once a step's last k-block is
 // multiplied the A ring is dead, and the consumers drain [D_main + D_corr] into it in column
 // passes that the producer threads read back row by row.  A policy may instead have the consumers
@@ -28,21 +31,31 @@
 #include "sm90.cuh"
 #include <stdlib.h>
 #include <type_traits>
+#include <utility>
 
 namespace tcg {
 
 constexpr int BM = 128, BN = 128, BK = 32;
-constexpr int NGROUPS = 1;                         // producer groups (k-block kb -> group kb % NGROUPS)
 constexpr int TILE_B_BYTES = BN * BK * 4;          // 16 KB per hi or lo tile
 constexpr int STAGE_B_BYTES = 2 * TILE_B_BYTES;    // [W_hi tile | W_lo tile] = 256 rows x 128 B
 constexpr int TILE_A_BYTES = BM * BK * 4;          // 16 KB per hi or lo A block
 constexpr int STAGE_A_BYTES = 2 * TILE_A_BYTES;    // [A_hi | A_lo]
 constexpr int EW = 16;                             // epilogue unit: 16 accumulator columns
-constexpr int PRODUCER_THREADS = 128 * NGROUPS;
-constexpr int CONSUMER_WARP0 = PRODUCER_THREADS / 32;
 constexpr int CONSUMER_THREADS = 256;
-constexpr int THREADS = PRODUCER_THREADS + CONSUMER_THREADS;
+constexpr int CONSUMER_REGS = 168;                 // registers per consumer thread with two producer groups
 constexpr int MAX_B_STAGES = 6, MAX_A_STAGES = 4;
+
+// Producer groups of a policy: Policy::kProducerGroups (1 or 2), 1 without it.  Group g is warps
+// [4 g, 4 g + 4) and produces the k-blocks whose running count (over all steps) is g modulo the
+// group count; thread r of every group owns tile row r.
+template <class P, class = void> struct ProducerGroups : std::integral_constant<int, 1> {};
+template <class P>
+struct ProducerGroups<P, std::void_t<decltype(P::kProducerGroups)>> : std::integral_constant<int, P::kProducerGroups> {};
+template <class P> constexpr int producer_threads = 128 * ProducerGroups<P>::value;
+template <class P> constexpr int cta_threads = producer_threads<P> + CONSUMER_THREADS;
+// With two groups the 512 threads start at 128 registers each: the producers give theirs down to
+// this and the consumers take CONSUMER_REGS (2 x 128 x 88 + 2 x 128 x 168 = 65,536)
+template <class P> constexpr int producer_regs = (65536 - CONSUMER_THREADS * CONSUMER_REGS) / producer_threads<P> / 8 * 8;
 // shared memory of the skeleton: W ring + A ring (Policy::kStagesB / kStagesA stages) + barriers
 __host__ __device__ constexpr int core_smem(int stages_b, int stages_a) {
   return stages_b * STAGE_B_BYTES + stages_a * STAGE_A_BYTES + 256;
@@ -108,8 +121,9 @@ struct PhaseTimer {          // thread 0 of the CTA only; no-op unless a buffer 
   }
 };
 
-__device__ __forceinline__ void producers_sync() {   // named barrier 1: all producer threads
-  asm volatile("bar.sync 1, %0;" ::"n"(PRODUCER_THREADS) : "memory");
+template <class Policy>
+__device__ __forceinline__ void producers_sync() {   // named barrier 1: all producer threads (every group)
+  asm volatile("bar.sync 1, %0;" ::"n"(producer_threads<Policy>) : "memory");
 }
 __device__ __forceinline__ void consumers_sync() {   // named barrier 2: both consumer warpgroups
   asm volatile("bar.sync 2, %0;" ::"n"(CONSUMER_THREADS) : "memory");
@@ -130,14 +144,20 @@ __device__ __forceinline__ int stg_index(int row, int col, int pw) {
 //   static void decode(const Params&, int cta, int ncta, int it, int& m_tile, int& sub)
 //   static int  num_kblocks(const Params&, int sub)
 //   static void w_coords(const Params&, int sub, int kb, int& col0, int& row0)   TMA coords of W
-//   Policy(const Params&, uint8_t* policy_smem, int tid)  constructed by producer threads only
+//   static constexpr int kProducerGroups                  optional, 1 (default) or 2: see ProducerGroups
+//   Policy(const Params&, uint8_t* policy_smem, int tid)  constructed by producer threads only (tid <
+//                                                         producer_threads<Policy>)
 //   void step_begin(int m_tile, int sub, int kb_first, PhaseTimer&)   may call producers_sync(); kb_first =
-//                                                         this thread's first k-block of the step
-//   void produce(int sub, int kb, float (&v)[32])         the 32 A values of this thread's row
+//                                                         this thread's group's first k-block of the step
+//   void produce(int sub, int kb, float (&v)[32])         the 32 A values of this thread's row; called
+//                                                         for this thread's group's k-blocks only
 //   void pre_epilogue(int sub)                            after the step's last produce()
-//   void post_epilogue(int sub)                           after the step's last store()
+//   void post_epilogue(int sub)                           after the step's last store(), behind
+//                                                         producers_sync()
 //   void store(int sub, int col, float (&x)[EW])          accumulator columns [col, col+EW) of
-//                                                         this thread's row (main + corr summed)
+//                                                         this thread's row (main + corr summed); with
+//                                                         two groups, group g stores the 16-column
+//                                                         units col / EW = g (mod 2)
 // Optional pair (a policy whose step starts from the previous step's result; without it every
 // accumulator starts at zero):
 //   static bool drain_kept(const Params&, int sub)        the step's drain ([D_main + D_corr], one pass)
@@ -170,10 +190,19 @@ __device__ __forceinline__ int stg_index(int row, int col, int pw) {
 //   producer thread reads its row, then producers_sync), and the consumers write that drain only
 //   after all of the step's MMAs have retired.  (Consecutive operand_from_acc steps are fine: the
 //   drain is then that of the last of them; a CTA's last step is always drained.)
+// Optional form of produce (a policy that reuses a row across several of its k-blocks):
+//   float produce(int sub, int kb, float (&v)[32])        returns a scale: the A values are
+//                                                         __fmul_rn(scale, v[j]).  v is kept from the
+//                                                         thread's previous produce() call of the step
+//                                                         (undefined at its first), so the policy may
+//                                                         leave it as it was.
 template <class P, class = void> struct HasAccInit : std::false_type {};
 template <class P> struct HasAccInit<P, std::void_t<decltype(&P::acc_init)>> : std::true_type {};
 template <class P, class = void> struct HasOperandFromAcc : std::false_type {};
 template <class P> struct HasOperandFromAcc<P, std::void_t<decltype(&P::operand_from_acc)>> : std::true_type {};
+template <class P>
+constexpr bool kScaledProduce =
+    std::is_same_v<decltype(std::declval<P&>().produce(0, 0, std::declval<float (&)[32]>())), float>;
 
 // Whether step it + 1 takes its operand from step it's accumulators (operand_from_acc policies only)
 template <class Policy>
@@ -213,12 +242,16 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
   // fences below; those policies wait for every group, as before.
   constexpr bool kQueue = !kAccInit;
   static_assert(!kOpAcc || SA * BK >= BN, "an operand written from the accumulators needs one A stage per k-block");
+  constexpr int NG = ProducerGroups<Policy>::value, PT = producer_threads<Policy>;
+  constexpr bool kScaled = kScaledProduce<Policy>;
+  static_assert(NG == 1 || (NG == 2 && !kOpAcc && PW % (2 * EW) == 0), "two producer groups: no operand_from_acc");
   Core c = carve(base, SB, SA);
   uint8_t* policy_smem = base + core_smem(SB, SA);
   float* stg = reinterpret_cast<float*>(c.Ast);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // 0: producers, 1 / 2: consumer warpgroups; broadcast from lane 0, so ptxas sees a warp-uniform value
+  // 0 .. NG - 1: producer groups, NG / NG + 1: consumer warpgroups; broadcast from lane 0, so ptxas
+  // sees a warp-uniform value
   const int role = __shfl_sync(0xffffffffu, tid / 128, 0);
   const int cta = blockIdx.x, ncta = gridDim.x;
   // num_steps may read memory (the stack's schedule): broadcast, so every count the consumers' loops
@@ -231,7 +264,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
     prof_c0 = clock64();
   }
 
-  if (warp == CONSUMER_WARP0 && lane == 0) {
+  if (warp == PT / 32 && lane == 0) {
     sm90::tma_prefetch_desc(&map_hi);
     sm90::tma_prefetch_desc(&map_lo);
     for (int s = 0; s < SB; ++s) {
@@ -239,19 +272,21 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
       sm90::mbar_init(&c.b_empty[s], CONSUMER_THREADS / 32);
     }
     for (int s = 0; s < SA; ++s) {
-      sm90::mbar_init(&c.a_full[s], PRODUCER_THREADS);
+      sm90::mbar_init(&c.a_full[s], PT / NG);        // one group produces a k-block
       sm90::mbar_init(&c.a_empty[s], CONSUMER_THREADS / 32);
     }
     sm90::mbar_init(c.stg_full, CONSUMER_THREADS);
-    sm90::mbar_init(c.stg_empty, PRODUCER_THREADS);
+    sm90::mbar_init(c.stg_empty, PT);
     sm90::mbar_init(c.kept_read, CONSUMER_THREADS / 32);
     sm90::fence_barrier_init();
   }
   __syncthreads();
 
-  if (role == 0) {
+  if (NG == 1 ? role == 0 : role < NG) {
     // ================================ producers + epilogue ================================
+    if constexpr (NG > 1) sm90::setmaxnreg_dec<producer_regs<Policy>>();
     const int r = tid & 127;                         // tile row of this thread
+    const int grp = NG == 1 ? 0 : role;              // producer group
     Policy pol(p, policy_smem, tid);
     uint32_t cnt = 0;                                // k-blocks produced so far
     uint32_t npass = 0;                              // drain passes read so far
@@ -270,20 +305,34 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
       }
       PhaseTimer tm;
       tm.start(cta, tid);
-      pol.step_begin(m_tile, sub, 0, tm);
+      pol.step_begin(m_tile, sub, NG == 1 ? 0 : (int)((grp + NG - cnt % NG) % NG), tm);
+      [[maybe_unused]] float v_kept[32];             // kScaled: the row kept across this thread's k-blocks
       for (int kb = 0; kb < nkb; ++kb, ++cnt) {
+        if constexpr (NG > 1) {
+          if (cnt % NG != (uint32_t)grp) continue;   // another group's k-block
+        }
         float v[32];
-        if (!(p.dbg & 8)) pol.produce(sub, kb, v);
+        [[maybe_unused]] float scale = 1.f;
+        if (!(p.dbg & 8)) {
+          if constexpr (kScaled) scale = pol.produce(sub, kb, v_kept);
+          else pol.produce(sub, kb, v);
+        }
         const uint32_t sa = cnt % SA;
-        if (kAccInit && kb == 0 && after_kept) {     // the consumers have read the kept drain
+        // this group's first k-block of the step: the consumers have read the kept drain, which
+        // fills the whole A ring
+        if (kAccInit && (NG == 1 ? kb == 0 : kb < NG) && after_kept) {
           sm90::mbar_wait(c.kept_read, nkept & 1u);
-          ++nkept;
+          if constexpr (NG == 1) ++nkept;
         }
         sm90::mbar_wait(&c.a_empty[sa], ((cnt / SA) & 1u) ^ 1u);
         if (!(p.dbg & 1)) {
           uint8_t* hi = c.Ast + sa * STAGE_A_BYTES + r * 128;
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
+            if constexpr (kScaled) {
+#pragma unroll
+              for (int i = 4 * j; i < 4 * j + 4; ++i) v[i] = __fmul_rn(scale, v_kept[i]);
+            }
             uint4 h, l;
             h.x = sm90::tf32_rna_bits(v[4 * j + 0]); h.y = sm90::tf32_rna_bits(v[4 * j + 1]);
             h.z = sm90::tf32_rna_bits(v[4 * j + 2]); h.w = sm90::tf32_rna_bits(v[4 * j + 3]);
@@ -299,16 +348,20 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
         sm90::fence_proxy_async();                   // visible to the tensor core's operand reads
         sm90::mbar_arrive(&c.a_full[sa]);
       }
+      if constexpr (NG > 1) {
+        if (kAccInit && after_kept) ++nkept;         // also when the group had no k-block to wait for
+      }
       tm.lap((sub & 1) ? 8 : 3);
       pol.pre_epilogue(sub);
       tm.lap(4);
-      // ---- epilogue: the consumers drain the accumulators in passes of PW columns ----
+      // ---- epilogue: the consumers drain the accumulators in passes of PW columns; group g takes
+      // the 16-column units g, g + NG, ... of its row ----
 #pragma unroll 1
       for (int q = 0; q < (kept || to_acc ? 0 : NPASS); ++q, ++npass) {
         sm90::mbar_wait(c.stg_full, npass & 1u);
         if (q == 0) tm.lap((sub & 1) ? 9 : 5);
 #pragma unroll 1
-        for (int col = q * PW; col < (q + 1) * PW; col += EW) {
+        for (int col = q * PW + grp * EW; col < (q + 1) * PW; col += NG * EW) {
           float x[EW];
 #pragma unroll
           for (int j = 0; j < EW; j += 4) {
@@ -320,14 +373,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
         sm90::mbar_arrive(c.stg_empty);
       }
       tm.lap(7);
-      producers_sync();                              // every row is read before the A ring is rewritten
+      producers_sync<Policy>();                      // every row is read before the A ring is rewritten
       pol.post_epilogue(sub);
       tm.lap(10);
       after_kept = kept;
     }
   } else {
     // ================================ MMA consumers ========================================
-    const int wg = role - 1;                         // rows [64 wg, 64 wg + 64) of the tile
+    if constexpr (NG > 1) sm90::setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = role - NG;                        // rows [64 wg, 64 wg + 64) of the tile
     const int wq = warp & 3;
     float d[128];                                    // [D_main (64 x 128) | D_corr (64 x 128)]
     uint32_t cnt = 0, npass = 0;
@@ -336,9 +390,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
     const int row0 = wg * 64 + wq * 16 + (lane >> 2), cl = 2 * (lane & 3);
     // W loads: the cursor walks the k-blocks of all steps in order; the load of k-block i waits until
     // every consumer warp has released k-block i - kStagesB.  Every consumer warp runs the cursor and
-    // the wait, and the elected lane of warp CONSUMER_WARP0 issues the load under a predicate inside
+    // the wait, and the elected lane of the first consumer warp issues the load under a predicate inside
     // the asm: between two MMA groups no consumer warp takes a path another one does not.
-    const bool w_issuer = warp == CONSUMER_WARP0;
+    const bool w_issuer = warp == PT / 32;
     int l_it = 0, l_kb = 0, l_nkb = -1, l_sub = 0;
     uint32_t l_cnt = 0;
     auto load_next = [&]() {
@@ -438,7 +492,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
         release((cnt - 1) % SB, !from_acc, from_acc ? (uint32_t)(nkb - 1) : (cnt - nacc - 1) % SA);
       if (from_acc) nacc += nkb;
       PhaseTimer ctm;
-      if (to_acc) ctm.start_if(cta, tid == PRODUCER_THREADS);
+      if (to_acc) ctm.start_if(cta, tid == PT);
       consumers_sync();                              // both warpgroups are done reading the A ring
       if (to_acc) {
         // The next step's operand: k-block kb = A stage kb holds columns [32 kb, 32 kb + 32) of
@@ -496,7 +550,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_hi, const CU
 }
 
 template <class Policy>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(cta_threads<Policy>, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
                const __grid_constant__ CUtensorMap map_lo, const typename Policy::Params p) {
   tc_gemm_body<Policy, 0>(map_hi, map_lo, p);
@@ -504,7 +558,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_hi,
 
 // The skeleton with pipeline parts switched off (kSkip: SKIP_MMA | SKIP_TMA), for LNB_DBG experiments
 template <class Policy, int kSkip>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(cta_threads<Policy>, 1)
 tc_gemm_probe_kernel(const __grid_constant__ CUtensorMap map_hi,
                      const __grid_constant__ CUtensorMap map_lo, const typename Policy::Params p) {
   tc_gemm_body<Policy, kSkip>(map_hi, map_lo, p);
@@ -625,7 +679,7 @@ static int launch(lnb_stream_t stream, const float* W_hi, const float* W_lo, int
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   int grid = items < sm_count() ? items : sm_count();
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  kern<<<grid, THREADS, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
+  kern<<<grid, cta_threads<Pol>, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
   lnb::count_launch();
   return lnb::finish_launch(who);
 }
