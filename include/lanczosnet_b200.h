@@ -400,6 +400,70 @@ int lnb_gat_attention_backward(lnb_stream_t stream, const float* gout, const flo
                                float* gWh, float* gpar);
 
 /* ---------------------------------------------------------------------------------------
+ * GAT dropout masks (model/gat.py:149-163; the KeyedGAT training forward).  Layer t, channel
+ * c = jj*heads + ii (C channels of F features, layer input width Din, M = B*N node rows) has three
+ * sites sigma, each with its own mask of the same p:
+ *   sigma = 0, input:     the layer input X seen by channel c, element i = (b*N + n)*Din + d
+ *   sigma = 1, attention: att[b, i_row, k] (softmax over i_row), element i = (b*N + i_row)*N + k
+ *   sigma = 2, Wh:        Wh_c = the channel's projection, element i = (b*N + n)*F + f
+ * Element i of a site is decided by
+ *   word = word (i & 3), in the order x, y, z, w, of Philox4x32-10 (Random123's constants) at key
+ *     (seed lo, seed hi) and counter (i >> 2, site, ctr lo, ctr hi), where site = (t << 16) | (c << 2) | sigma
+ *     and (seed, ctr) = dropout_key[0..1] (int64, DEVICE memory: a captured graph draws anew whenever the
+ *     key changes);
+ *   kept iff word >= thr, thr = floor(p * 2^32) computed in fp64 and held as a uint64 (p = 1 keeps nothing);
+ *   a kept value is x * s with s = (float)(1 / (1 - p)) (one fp32 multiply), a dropped value is 0.
+ * One training forward uses one key for every layer, channel and site.  Needs t < 2^16, C <= 2^14 and fewer
+ * than 2^34 elements per site (LNB_ERR_UNSUPPORTED otherwise, nothing launched).  The draws are not
+ * torch's: same distribution, different masks.
+ * ------------------------------------------------------------------------------------- */
+
+/* lnb_gat_attention with the reference's attention and Wh dropout of layer t: att' = att * M_att s and
+ * Wh' = Wh_c * M_wh s replace att and Wh_c in h_c = att' Wh' + state_bias_c; the scores s1, s2 read the
+ * undropped Wh.  Same arguments, layouts, envelope and determinism as lnb_gat_attention, plus dropout_key,
+ * p in [0, 1] and t (the mask rule above). */
+int lnb_gat_attention_dropout(lnb_stream_t stream, const float* Wh, const float* bias, const float* a1,
+                              const float* a2, const float* c1, const float* c2, const float* state_bias,
+                              int B, int N, int E1, int heads, int F, int last, const int64_t* dropout_key,
+                              double p, int t, float* out);
+
+/* Adjoint of lnb_gat_attention_dropout, with its masks drawn again (nothing of the forward is saved):
+ *   gWh[b,k,c] = M_wh s * (sum_i att'[i,k] gh[i]) + gs1[k] a1[c] + gs2[k] a2[c]
+ *   gX[i,k] = att[i,k] (gAtt[i,k] - sum_i' att[i',k] gAtt[i',k]) * (s1[i] + s2[k] > 0 ? 1 : 0.2),
+ *     gAtt = M_att s * (gh Wh'^T)
+ * and h (for ELU') = att' Wh' + state_bias; ga1, ga2 read the undropped Wh.  Arguments, outputs (gpar
+ * per graph, summed by the caller), envelope and determinism as lnb_gat_attention_backward. */
+int lnb_gat_attention_dropout_backward(lnb_stream_t stream, const float* gout, const float* Wh, const float* bias,
+                                       const float* a1, const float* a2, const float* c1, const float* c2,
+                                       const float* state_bias, int B, int N, int E1, int heads, int F, int last,
+                                       const int64_t* dropout_key, double p, int t, float* gWh, float* gpar);
+
+/* The per-channel input dropout and projection of GAT layer t:
+ *   Wh[m, c*F:(c+1)*F] = (X[m,:] * M_c[m,:] s) W_c^T      for every channel c < C and row m < M
+ * X [M, Din], W [C*F, Din] (channel c's weight = rows c*F .. c*F+F-1), Wh [M, C*F]; M_c the input-site
+ * mask of (t, c) (the rule above).  No masked copy of X exists: each mask word is drawn once per
+ * (row, feature, channel) as the operand tile is loaded.  FFMA in fp32, the sum over d in order.
+ * Envelope: Din % 4 == 0, F % 4 == 0, F <= 128; X, W, Wh 16-byte aligned (LNB_ERR_UNSUPPORTED /
+ * LNB_ERR_ARG otherwise, nothing launched). */
+int lnb_gat_dropout_project(lnb_stream_t stream, const float* X, const float* W, int M, int Din, int C, int F,
+                            const int64_t* dropout_key, double p, int t, float* Wh);
+
+/* Row slabs of lnb_gat_dropout_project_backward's gW partials for a shape (a function of the shape
+ * only); its workspace holds slabs * C*F*Din floats. */
+int lnb_gat_dropout_project_slabs(int M, int Din, int C, int F);
+
+/* Adjoint of lnb_gat_dropout_project, with the masks drawn again:
+ *   gX = s sum_{c = 0..C-1} M_c * (gWh_c W_c)              gX [M, Din]
+ *   gW_c = s gWh_c^T (X * M_c)                             gW [C*F, Din]
+ * One launch walks every (row block, 32-feature block) over the channels in order and draws each mask
+ * word once; it writes gX and one gW partial per row slab into `work` [slabs, C*F, Din]; a second launch
+ * sums the slabs in order.  No atomics: repeated launches are bit-identical.  Envelope and alignment of
+ * lnb_gat_dropout_project, plus gWh, gX, gW, work 16-byte aligned. */
+int lnb_gat_dropout_project_backward(lnb_stream_t stream, const float* X, const float* W, const float* gWh,
+                                     int M, int Din, int C, int F, const int64_t* dropout_key, double p, int t,
+                                     float* gX, float* gW, float* work);
+
+/* ---------------------------------------------------------------------------------------
  * GGNN propagation step after the message MLPs (model/ggnn.py:143-171), one persistent 3xTF32 wgmma
  * launch over all B*N rows:
  *   agg[b,n, e*D:(e+1)*D] = sum over the non-zeros m of row n of channel e of  w * M[b*N+m, e*D:(e+1)*D]

@@ -102,6 +102,17 @@ SIGNATURES = {
                                   c_int, c_int, c_int, c_int, c_int, c_int, c_f32p]),
     'lnb_gat_attention_backward': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
                                            c_f32p, c_int, c_int, c_int, c_int, c_int, c_int, c_f32p, c_f32p]),
+    'lnb_gat_attention_dropout': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
+                                          c_int, c_int, c_int, c_int, c_int, c_int, ctypes.c_void_p,
+                                          ctypes.c_double, c_int, c_f32p]),
+    'lnb_gat_attention_dropout_backward':
+        (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int,
+                 c_int, c_int, c_int, ctypes.c_void_p, ctypes.c_double, c_int, c_f32p, c_f32p]),
+    'lnb_gat_dropout_project': (c_int, [c_stream, c_f32p, c_f32p, c_int, c_int, c_int, c_int, ctypes.c_void_p,
+                                        ctypes.c_double, c_int, c_f32p]),
+    'lnb_gat_dropout_project_slabs': (c_int, [c_int, c_int, c_int, c_int]),
+    'lnb_gat_dropout_project_backward': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int,
+                                                 ctypes.c_void_p, ctypes.c_double, c_int, c_f32p, c_f32p, c_f32p]),
     'lnb_ggnn_update': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p,
                                 c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int, c_f32p]),
     'lnb_sage_lstm_step': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,

@@ -16,6 +16,7 @@
 //
 // The training path's adjoint, gat_attention_backward_kernel, is at the end of this file.
 #include "common.cuh"
+#include "gat_dropout.cuh"
 
 namespace {
 
@@ -87,8 +88,44 @@ __device__ __forceinline__ float gat_weight(float x, float m, float z) { return 
 
 __device__ __forceinline__ float elu(float x) { return x > 0.f ? x : expm1f(x); }
 
-__global__ void __launch_bounds__(GAT_THREADS)
-gat_attention_kernel(GatParams p) {
+// The dropout kernels' masks of one head group, in place in shared memory once the scores are taken:
+// Ws [N][gcnt*F] (Wh of channels c0 .. c0+gcnt-1) becomes Wh' = Wh * M_wh s and As [gcnt][N][N] (att)
+// becomes att' = att * M_att s.  One Philox call per four elements of a site: a Wh quad is four features
+// of one node (F % 4 == 0); the [N, N] block of graph b starts at element b*N*N of its site, so its first
+// and last quads may be shared with the neighbouring graphs.
+__device__ __forceinline__ void gat_drop_group(const lnb::GatDrop& d, int b, int N, int F, int c0, int gcnt,
+                                               float* Ws, float* As, int nthreads) {
+  const lnb::GatDropKey key = lnb::gat_drop_key(d);
+  const int gf = gcnt * F, q4 = F >> 2;
+  for (int e = threadIdx.x; e < N * gcnt * q4; e += nthreads) {
+    const int n = e / (gcnt * q4), rem = e - n * (gcnt * q4);
+    const int g = rem / q4, v = rem - g * q4;
+    const uint64_t q = (((uint64_t)b * N + n) * F + 4 * v) >> 2;
+    const uint4 w = lnb::gat_drop_words(key, q, lnb::gat_site(d.layer, c0 + g, lnb::GAT_SITE_WH));
+    float4* x = reinterpret_cast<float4*>(Ws + n * gf + g * F) + v;
+    *x = lnb::gat_drop4(*x, w, d);
+  }
+  const uint64_t base = (uint64_t)b * N * N;
+  const uint64_t qlo = base >> 2;
+  const int nq = (int)(((base + (uint64_t)N * N - 1) >> 2) - qlo + 1);
+  for (int e = threadIdx.x; e < gcnt * nq; e += nthreads) {
+    const int g = e / nq;
+    const uint64_t q = qlo + (e - g * nq);
+    const uint4 w = lnb::gat_drop_words(key, q, lnb::gat_site(d.layer, c0 + g, lnb::GAT_SITE_ATT));
+    float* A = As + (size_t)g * N * N;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int64_t i = (int64_t)(4 * q + j) - (int64_t)base;
+      if (i >= 0 && i < (int64_t)N * N) A[i] = lnb::gat_drop(A[i], lnb::gat_word(w, j), d);
+    }
+  }
+}
+
+// DROP: the training forward with the reference's dropout (lnb_gat_attention_dropout): after the softmax,
+// att' = att * M_att s and Wh' = Wh * M_wh s replace att and Wh in the aggregation; the scores read Wh.
+// DROP = false is lnb_gat_attention (d unused).
+template <bool DROP>
+__device__ __forceinline__ void gat_attention_body(GatParams p, lnb::GatDrop d) {
   extern __shared__ __align__(16) float smem[];
   const int N = p.N, F = p.F, E1 = p.E1, heads = p.heads, G = p.G;
   const int C = E1 * heads;
@@ -159,6 +196,10 @@ gat_attention_kernel(GatParams p) {
       for (int i = 0; i < N; ++i) A[i * N] = A[i * N] / z;
     }
     __syncthreads();
+    if constexpr (DROP) {
+      gat_drop_group(d, b, N, F, c0, gcnt, Ws, As, GAT_THREADS);
+      __syncthreads();
+    }
     // aggregation h = att Wh + state_bias, four features per thread
     const int q4 = F >> 2;
     if (!p.last) {
@@ -221,6 +262,16 @@ gat_attention_kernel(GatParams p) {
   }
 }
 
+__global__ void __launch_bounds__(GAT_THREADS)
+gat_attention_kernel(GatParams p) {
+  gat_attention_body<false>(p, lnb::GatDrop{});
+}
+
+__global__ void __launch_bounds__(GAT_THREADS)
+gat_attention_dropout_kernel(GatParams p, lnb::GatDrop d) {
+  gat_attention_body<true>(p, d);
+}
+
 size_t gat_smem_floats(int N, int F, int G) {
   return (size_t)N * G * F + (size_t)G * N * N + (size_t)N * N + 2 * (size_t)G * N;
 }
@@ -252,8 +303,11 @@ struct GatBwdParams {
   int N, F, E1, heads, G, ngroups, last;
 };
 
-__global__ void __launch_bounds__(GAT_THREADS)
-gat_attention_backward_kernel(GatBwdParams p) {
+// DROP: the adjoint of the dropout forward (lnb_gat_attention_dropout_backward).  The masks are drawn again:
+// Ws and As hold Wh' and att' from the softmax on, gWh's aggregation term is M_wh s (att'^T gh), the softmax
+// adjoint reads gAtt = M_att s (gh Wh'^T), and the score terms ga1 / ga2 read the undropped Wh from memory.
+template <bool DROP>
+__device__ __forceinline__ void gat_attention_backward_body(const GatBwdParams& p, const lnb::GatDrop& dr) {
   extern __shared__ __align__(16) float smem[];
   const int N = p.N, F = p.F, E1 = p.E1, heads = p.heads, G = p.G;
   const int C = E1 * heads;
@@ -308,6 +362,10 @@ gat_attention_backward_kernel(GatBwdParams p) {
                        [=](int i) { return __ldg(bb + (int64_t)(i * N + k) * E1); }, Mx[e], Zs[e]);
   }
   __syncthreads();
+  if constexpr (DROP) {
+    gat_drop_group(dr, b, N, F, c0, gcnt, Ws, As, GAT_THREADS);
+    __syncthreads();
+  }
   if (!p.last) {
     // h = att Wh + state_bias as the forward's aggregation computes it, then gh = gout * ELU'(h)
     for (int e = tid; e < N * gcnt * q4; e += GAT_THREADS) {
@@ -353,7 +411,13 @@ gat_attention_backward_kernel(GatBwdParams p) {
       az = fma(a, (double)x.z, az);
       aw = fma(a, (double)x.w, aw);
     }
-    reinterpret_cast<float4*>(gWhb + k * row + g * F)[v] = make_float4((float)ax, (float)ay, (float)az, (float)aw);
+    float4 o = make_float4((float)ax, (float)ay, (float)az, (float)aw);
+    if constexpr (DROP) {
+      const uint64_t q = (((uint64_t)b * N + k) * F + 4 * v) >> 2;
+      o = lnb::gat_drop4(o, lnb::gat_drop_words(lnb::gat_drop_key(dr), q,
+                                                lnb::gat_site(dr.layer, c0 + g, lnb::GAT_SITE_WH)), dr);
+    }
+    reinterpret_cast<float4*>(gWhb + k * row + g * F)[v] = o;
   }
   __syncthreads();
   // gAtt[i,k] = gh[i] . Wh[k] over the features, in order
@@ -369,6 +433,12 @@ gat_attention_backward_kernel(GatBwdParams p) {
       d = fmaf(a.y, c.y, d);
       d = fmaf(a.z, c.z, d);
       d = fmaf(a.w, c.w, d);
+    }
+    if constexpr (DROP) {
+      const uint64_t i_el = ((uint64_t)b * N + i) * N + k;
+      const uint4 w = lnb::gat_drop_words(lnb::gat_drop_key(dr), i_el >> 2,
+                                          lnb::gat_site(dr.layer, c0 + g, lnb::GAT_SITE_ATT));
+      d = lnb::gat_drop(d, lnb::gat_word(w, (int)(i_el & 3)), dr);
     }
     As[e] = d;
   }
@@ -428,8 +498,13 @@ gat_attention_backward_kernel(GatBwdParams p) {
     double acc = 0.0;
     if (j < 2 * F) {                                  // ga1, ga2
       const float* r = (j < F ? R1 : R2) + g * N;
-      const float* w = Ws + g * F + (j < F ? j : j - F);
-      for (int k = 0; k < N; ++k) acc = fma((double)r[k], (double)w[k * gf], acc);
+      if constexpr (DROP) {                           // Ws holds Wh': the scores read Wh
+        const float* w = Whb + g * F + (j < F ? j : j - F);
+        for (int k = 0; k < N; ++k) acc = fma((double)r[k], (double)__ldg(w + k * row), acc);
+      } else {
+        const float* w = Ws + g * F + (j < F ? j : j - F);
+        for (int k = 0; k < N; ++k) acc = fma((double)r[k], (double)w[k * gf], acc);
+      }
     } else if (j < 3 * F) {                           // gsb
       const float* h = Gs + g * F + (j - 2 * F);
       for (int i = 0; i < N; ++i) acc += (double)h[i * gf];
@@ -441,12 +516,118 @@ gat_attention_backward_kernel(GatBwdParams p) {
   }
 }
 
+__global__ void __launch_bounds__(GAT_THREADS)
+gat_attention_backward_kernel(GatBwdParams p) {
+  gat_attention_backward_body<false>(p, lnb::GatDrop{});
+}
+
+__global__ void __launch_bounds__(GAT_THREADS)
+gat_attention_dropout_backward_kernel(GatBwdParams p, lnb::GatDrop d) {
+  gat_attention_backward_body<true>(p, d);
+}
+
 size_t gat_bwd_smem_floats(int N, int F, int G) {
   return 2 * (size_t)N * G * F + (size_t)G * N * N + 6 * (size_t)G * N;
 }
 
 bool gat_shape_ok(int N, int F, int E1, int heads) {
   return N <= GAT_NMAX && F % 4 == 0 && F <= GAT_FMAX && E1 <= GAT_E1MAX && heads <= GAT_HEADSMAX;
+}
+
+// the launches of lnb_gat_attention(_backward) and of their dropout forms (drop != nullptr); `who` prefixes
+// the error text
+int launch_gat_attention(cudaStream_t stream, const char* who, const float* Wh, const float* bias,
+                         const float* a1, const float* a2, const float* c1, const float* c2,
+                         const float* state_bias, int B, int N, int E1, int heads, int F, int last, float* out,
+                         const lnb::GatDrop* drop) {
+  LNB_REQUIRE(Wh && bias && a1 && a2 && c1 && c2 && state_bias && out, "%s: null pointer", who);
+  LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && heads >= 1 && F >= 1, "%s: bad dims", who);
+  if (N > GAT_NMAX || F % 4 || F > GAT_FMAX || E1 > GAT_E1MAX || heads > GAT_HEADSMAX) {
+    lnb::set_err("%s: N=%d F=%d E1=%d heads=%d outside the kernel (N <= %d, F %% 4 == 0, "
+                 "F <= %d, E1 <= %d, heads <= %d)", who, N, F, E1, heads, GAT_NMAX, GAT_FMAX, GAT_E1MAX,
+                 GAT_HEADSMAX);
+    return LNB_ERR_UNSUPPORTED;
+  }
+  LNB_REQUIRE(((uintptr_t)Wh | (uintptr_t)state_bias | (uintptr_t)out) % 16 == 0,
+              "%s: Wh, state_bias and out must be 16-byte aligned", who);
+  if (B == 0) return LNB_OK;
+  // heads per group: as many as fit the occupancy target, at least one (fits 227 KB in the envelope)
+  int G = heads;
+  while (G > 1 && gat_smem_floats(N, F, G) * sizeof(float) > GAT_SMEM_TARGET) --G;
+  const size_t shm = gat_smem_floats(N, F, G) * sizeof(float);
+  LNB_REQUIRE(shm <= GAT_SMEM_MAX, "%s: %zu bytes of shared memory", who, shm);
+  const int ngroups = (heads + G - 1) / G;
+  const int64_t grid = last ? (int64_t)B : (int64_t)B * E1 * ngroups;
+  LNB_REQUIRE(grid <= 0x7fffffff, "%s: B=%d too large", who, B);
+  if (shm > 48 * 1024) {
+    if (drop)
+      cudaFuncSetAttribute(gat_attention_dropout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+    else
+      cudaFuncSetAttribute(gat_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+  }
+  GatParams p;
+  p.Wh = Wh; p.bias = bias; p.a1 = a1; p.a2 = a2; p.c1 = c1; p.c2 = c2; p.sb = state_bias; p.out = out;
+  p.N = N; p.F = F; p.E1 = E1; p.heads = heads; p.G = G; p.ngroups = ngroups; p.last = last ? 1 : 0;
+  if (drop)
+    gat_attention_dropout_kernel<<<(unsigned)grid, GAT_THREADS, shm, stream>>>(p, *drop);
+  else
+    gat_attention_kernel<<<(unsigned)grid, GAT_THREADS, shm, stream>>>(p);
+  lnb::count_launch();
+  return lnb::finish_launch(who);
+}
+
+int launch_gat_attention_backward(cudaStream_t stream, const char* who, const float* gout, const float* Wh,
+                                  const float* bias, const float* a1, const float* a2, const float* c1,
+                                  const float* c2, const float* state_bias, int B, int N, int E1, int heads,
+                                  int F, int last, float* gWh, float* gpar, const lnb::GatDrop* drop) {
+  LNB_REQUIRE(gout && Wh && bias && a1 && a2 && c1 && c2 && state_bias && gWh && gpar, "%s: null pointer", who);
+  LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && heads >= 1 && F >= 1, "%s: bad dims", who);
+  if (!gat_shape_ok(N, F, E1, heads)) {
+    lnb::set_err("%s: N=%d F=%d E1=%d heads=%d outside the kernel (N <= %d, F %% 4 == 0, "
+                 "F <= %d, E1 <= %d, heads <= %d)", who, N, F, E1, heads, GAT_NMAX, GAT_FMAX, GAT_E1MAX,
+                 GAT_HEADSMAX);
+    return LNB_ERR_UNSUPPORTED;
+  }
+  LNB_REQUIRE(((uintptr_t)gout | (uintptr_t)Wh | (uintptr_t)a1 | (uintptr_t)a2 | (uintptr_t)state_bias |
+               (uintptr_t)gWh) % 16 == 0,
+              "%s: gout, Wh, a1, a2, state_bias and gWh must be 16-byte aligned", who);
+  if (B == 0) return LNB_OK;
+  int G = heads;
+  while (G > 1 && gat_bwd_smem_floats(N, F, G) * sizeof(float) > GAT_SMEM_TARGET) --G;
+  const size_t shm = gat_bwd_smem_floats(N, F, G) * sizeof(float);
+  LNB_REQUIRE(shm <= GAT_SMEM_MAX, "%s: %zu bytes of shared memory", who, shm);
+  const int ngroups = (heads + G - 1) / G;
+  const int64_t grid = (int64_t)B * E1 * ngroups;
+  LNB_REQUIRE(grid <= 0x7fffffff, "%s: B=%d too large", who, B);
+  if (shm > 48 * 1024) {
+    if (drop)
+      cudaFuncSetAttribute(gat_attention_dropout_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)shm);
+    else
+      cudaFuncSetAttribute(gat_attention_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+  }
+  GatBwdParams p;
+  p.gout = gout; p.sb = state_bias; p.Wh = Wh; p.bias = bias; p.a1 = a1; p.a2 = a2; p.c1 = c1; p.c2 = c2;
+  p.gWh = gWh; p.gpar = gpar;
+  p.N = N; p.F = F; p.E1 = E1; p.heads = heads; p.G = G; p.ngroups = ngroups; p.last = last ? 1 : 0;
+  if (drop)
+    gat_attention_dropout_backward_kernel<<<(unsigned)grid, GAT_THREADS, shm, stream>>>(p, *drop);
+  else
+    gat_attention_backward_kernel<<<(unsigned)grid, GAT_THREADS, shm, stream>>>(p);
+  lnb::count_launch();
+  return lnb::finish_launch(who);
+}
+
+// the dropout forms' own checks: the key, p in [0, 1], and the site words of the rule
+int check_gat_drop(const char* who, const int64_t* key, double p, int t, int C, int64_t elements) {
+  LNB_REQUIRE(key, "%s: null dropout_key", who);
+  LNB_REQUIRE(p >= 0.0 && p <= 1.0, "%s: p=%g outside [0, 1]", who, p);
+  if (t < 0 || t >= (1 << 16) || C > (1 << 14) || elements >= (int64_t(1) << 34)) {
+    lnb::set_err("%s: layer %d, %d channels or %lld elements per site outside the mask rule "
+                 "(t < 2^16, C <= 2^14, < 2^34 elements)", who, t, C, (long long)elements);
+    return LNB_ERR_UNSUPPORTED;
+  }
+  return LNB_OK;
 }
 
 }  // namespace
@@ -456,68 +637,42 @@ extern "C" {
 int lnb_gat_attention(lnb_stream_t stream, const float* Wh, const float* bias, const float* a1,
                       const float* a2, const float* c1, const float* c2, const float* state_bias,
                       int B, int N, int E1, int heads, int F, int last, float* out) {
-  LNB_REQUIRE(Wh && bias && a1 && a2 && c1 && c2 && state_bias && out, "gat_attention: null pointer");
-  LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && heads >= 1 && F >= 1, "gat_attention: bad dims");
-  if (N > GAT_NMAX || F % 4 || F > GAT_FMAX || E1 > GAT_E1MAX || heads > GAT_HEADSMAX) {
-    lnb::set_err("gat_attention: N=%d F=%d E1=%d heads=%d outside the kernel (N <= %d, F %% 4 == 0, "
-                 "F <= %d, E1 <= %d, heads <= %d)", N, F, E1, heads, GAT_NMAX, GAT_FMAX, GAT_E1MAX,
-                 GAT_HEADSMAX);
-    return LNB_ERR_UNSUPPORTED;
-  }
-  LNB_REQUIRE(((uintptr_t)Wh | (uintptr_t)state_bias | (uintptr_t)out) % 16 == 0,
-              "gat_attention: Wh, state_bias and out must be 16-byte aligned");
-  if (B == 0) return LNB_OK;
-  // heads per group: as many as fit the occupancy target, at least one (fits 227 KB in the envelope)
-  int G = heads;
-  while (G > 1 && gat_smem_floats(N, F, G) * sizeof(float) > GAT_SMEM_TARGET) --G;
-  const size_t shm = gat_smem_floats(N, F, G) * sizeof(float);
-  LNB_REQUIRE(shm <= GAT_SMEM_MAX, "gat_attention: %zu bytes of shared memory", shm);
-  const int ngroups = (heads + G - 1) / G;
-  const int64_t grid = last ? (int64_t)B : (int64_t)B * E1 * ngroups;
-  LNB_REQUIRE(grid <= 0x7fffffff, "gat_attention: B=%d too large", B);
-  if (shm > 48 * 1024)
-    cudaFuncSetAttribute(gat_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
-  GatParams p;
-  p.Wh = Wh; p.bias = bias; p.a1 = a1; p.a2 = a2; p.c1 = c1; p.c2 = c2; p.sb = state_bias; p.out = out;
-  p.N = N; p.F = F; p.E1 = E1; p.heads = heads; p.G = G; p.ngroups = ngroups; p.last = last ? 1 : 0;
-  gat_attention_kernel<<<(unsigned)grid, GAT_THREADS, shm, (cudaStream_t)stream>>>(p);
-  lnb::count_launch();
-  return lnb::finish_launch("gat_attention");
+  return launch_gat_attention((cudaStream_t)stream, "gat_attention", Wh, bias, a1, a2, c1, c2, state_bias, B, N,
+                              E1, heads, F, last, out, nullptr);
 }
 
 int lnb_gat_attention_backward(lnb_stream_t stream, const float* gout, const float* Wh, const float* bias,
                                const float* a1, const float* a2, const float* c1, const float* c2,
                                const float* state_bias, int B, int N, int E1, int heads, int F, int last,
                                float* gWh, float* gpar) {
-  LNB_REQUIRE(gout && Wh && bias && a1 && a2 && c1 && c2 && state_bias && gWh && gpar,
-              "gat_attention_backward: null pointer");
-  LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && heads >= 1 && F >= 1, "gat_attention_backward: bad dims");
-  if (!gat_shape_ok(N, F, E1, heads)) {
-    lnb::set_err("gat_attention_backward: N=%d F=%d E1=%d heads=%d outside the kernel (N <= %d, F %% 4 == 0, "
-                 "F <= %d, E1 <= %d, heads <= %d)", N, F, E1, heads, GAT_NMAX, GAT_FMAX, GAT_E1MAX,
-                 GAT_HEADSMAX);
-    return LNB_ERR_UNSUPPORTED;
-  }
-  LNB_REQUIRE(((uintptr_t)gout | (uintptr_t)Wh | (uintptr_t)a1 | (uintptr_t)a2 | (uintptr_t)state_bias |
-               (uintptr_t)gWh) % 16 == 0,
-              "gat_attention_backward: gout, Wh, a1, a2, state_bias and gWh must be 16-byte aligned");
-  if (B == 0) return LNB_OK;
-  int G = heads;
-  while (G > 1 && gat_bwd_smem_floats(N, F, G) * sizeof(float) > GAT_SMEM_TARGET) --G;
-  const size_t shm = gat_bwd_smem_floats(N, F, G) * sizeof(float);
-  LNB_REQUIRE(shm <= GAT_SMEM_MAX, "gat_attention_backward: %zu bytes of shared memory", shm);
-  const int ngroups = (heads + G - 1) / G;
-  const int64_t grid = (int64_t)B * E1 * ngroups;
-  LNB_REQUIRE(grid <= 0x7fffffff, "gat_attention_backward: B=%d too large", B);
-  if (shm > 48 * 1024)
-    cudaFuncSetAttribute(gat_attention_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
-  GatBwdParams p;
-  p.gout = gout; p.sb = state_bias; p.Wh = Wh; p.bias = bias; p.a1 = a1; p.a2 = a2; p.c1 = c1; p.c2 = c2;
-  p.gWh = gWh; p.gpar = gpar;
-  p.N = N; p.F = F; p.E1 = E1; p.heads = heads; p.G = G; p.ngroups = ngroups; p.last = last ? 1 : 0;
-  gat_attention_backward_kernel<<<(unsigned)grid, GAT_THREADS, shm, (cudaStream_t)stream>>>(p);
-  lnb::count_launch();
-  return lnb::finish_launch("gat_attention_backward");
+  return launch_gat_attention_backward((cudaStream_t)stream, "gat_attention_backward", gout, Wh, bias, a1, a2, c1,
+                                       c2, state_bias, B, N, E1, heads, F, last, gWh, gpar, nullptr);
+}
+
+int lnb_gat_attention_dropout(lnb_stream_t stream, const float* Wh, const float* bias, const float* a1,
+                              const float* a2, const float* c1, const float* c2, const float* state_bias,
+                              int B, int N, int E1, int heads, int F, int last, const int64_t* dropout_key,
+                              double p, int t, float* out) {
+  const char* who = "gat_attention_dropout";
+  const int64_t per_site = (int64_t)B * N * (N > F ? N : F);
+  const int rc = check_gat_drop(who, dropout_key, p, t, E1 * heads, per_site);
+  if (rc != LNB_OK) return rc;
+  const lnb::GatDrop d = gat_drop_params(dropout_key, p, t);
+  return launch_gat_attention((cudaStream_t)stream, who, Wh, bias, a1, a2, c1, c2, state_bias, B, N, E1, heads,
+                              F, last, out, &d);
+}
+
+int lnb_gat_attention_dropout_backward(lnb_stream_t stream, const float* gout, const float* Wh, const float* bias,
+                                       const float* a1, const float* a2, const float* c1, const float* c2,
+                                       const float* state_bias, int B, int N, int E1, int heads, int F, int last,
+                                       const int64_t* dropout_key, double p, int t, float* gWh, float* gpar) {
+  const char* who = "gat_attention_dropout_backward";
+  const int64_t per_site = (int64_t)B * N * (N > F ? N : F);
+  const int rc = check_gat_drop(who, dropout_key, p, t, E1 * heads, per_site);
+  if (rc != LNB_OK) return rc;
+  const lnb::GatDrop d = gat_drop_params(dropout_key, p, t);
+  return launch_gat_attention_backward((cudaStream_t)stream, who, gout, Wh, bias, a1, a2, c1, c2, state_bias, B, N,
+                                       E1, heads, F, last, gWh, gpar, &d);
 }
 
 }  // extern "C"

@@ -13,13 +13,14 @@ What it does (see INTEGRATION.md):
      ``OPT_IN_CLASSES`` named with ``--opt-in NAME`` (repeatable; e.g. ``--opt-in MPNN``); ``--opt-in GAT``
      (``TRAINING_OPT_IN_CLASSES``) binds ``TrainableGAT`` under the name ``GAT``, and ``--opt-in GraphSAGE``
      (``LSTM_OPT_IN_CLASSES``) binds ``LSTMGraphSAGE`` (which takes ``agg_func: LSTM``) under the name
-     ``GraphSAGE``, for training and test runs;
+     ``GraphSAGE``, for training and test runs; ``--keyed-dropout`` with ``--opt-in GAT`` binds ``KeyedGAT``
+     instead of ``TrainableGAT``, which trains with the config's ``dropout > 0`` (masks drawn on the device);
   3. with ``--device-partition`` (``install(..., device_partition=True)``), rebinds ``spectral_clustering``
      and ``get_L_cluster_cut`` in the dataset modules' globals (``DATASET_MODULES``) to stand-ins, so the GPNN
      collate never runs scikit-learn and ships empty [B,0,0] partition operators; the GPNN drop-in then
      partitions every batch on the device (``ops.spectral_partition``);
-  4. runs the reference ``run_exp.main()`` unchanged (``--opt-in`` and ``--device-partition`` are removed
-     from its argv).
+  4. runs the reference ``run_exp.main()`` unchanged (``--opt-in``, ``--keyed-dropout`` and
+     ``--device-partition`` are removed from its argv).
 """
 import importlib
 import os
@@ -62,15 +63,23 @@ def _check_opt_in(opt_in):
   return tuple(opt_in)
 
 
-def patch_namespace(module, training=False, opt_in=()):
+def _check_keyed_dropout(opt_in, keyed_dropout):
+  if keyed_dropout and 'GAT' not in opt_in:
+    raise ValueError("dropin: keyed_dropout (--keyed-dropout) binds KeyedGAT under the name GAT and needs "
+                     "opt_in=('GAT',) (--opt-in GAT)")
+
+
+def patch_namespace(module, training=False, opt_in=(), keyed_dropout=False):
   """Rebind the class names in ``module``'s globals to the H100 drop-ins: those of ``DROPIN_CLASSES``
   and those of ``opt_in`` (names from ``OPT_IN_CLASSES`` or ``TRAINING_OPT_IN_CLASSES``; any other name
   is a ValueError).  ``training=True`` (a run without ``-t``) rebinds only the classes that have a
   differentiable training path (every class but ``GAT``, which is inference only); a class without one
   keeps the reference's trainable class instead of failing on the first ``loss.backward()``.  A name of
   ``TRAINING_OPT_IN_CLASSES`` in ``opt_in`` is bound to ``Trainable<name>``, one of ``LSTM_OPT_IN_CLASSES`` to
-  ``LSTM<name>``, in training and test runs."""
+  ``LSTM<name>``, in training and test runs.  ``keyed_dropout=True`` (only with ``GAT`` in ``opt_in``, else a
+  ValueError) binds ``KeyedGAT`` under the name ``GAT`` instead of ``TrainableGAT``."""
   opt_in = _check_opt_in(opt_in)
+  _check_keyed_dropout(opt_in, keyed_dropout)
   for name in DROPIN_CLASSES + tuple(n for n in opt_in if n in OPT_IN_CLASSES):
     if hasattr(module, name):
       cls = getattr(_models, name)
@@ -79,7 +88,8 @@ def patch_namespace(module, training=False, opt_in=()):
       setattr(module, name, cls)
   for name in opt_in:
     if name in TRAINING_OPT_IN_CLASSES and hasattr(module, name):
-      setattr(module, name, getattr(_models, 'Trainable' + name))
+      keyed = keyed_dropout and name == 'GAT'
+      setattr(module, name, getattr(_models, ('Keyed' if keyed else 'Trainable') + name))
     if name in LSTM_OPT_IN_CLASSES and hasattr(module, name):
       setattr(module, name, getattr(_models, 'LSTM' + name))
   return module
@@ -104,15 +114,16 @@ def patch_partition(module):
 
 
 def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.graph_runner'),
-            compat=False, training=False, opt_in=(), device_partition=False):
+            compat=False, training=False, opt_in=(), device_partition=False, keyed_dropout=False):
   """Returns the list of patched modules.  ``reference_root`` is put on sys.path if given.
   ``compat=True`` first installs the shims of ``lanczosnetwork_b200.compat`` (missing easydict /
   tensorboardX, PyYAML >= 6, numpy >= 2) so the 2019 checkout imports under a current stack.
   Raises ImportError when NO runner module could be imported and patched: the runners resolve
   the model class by name in their own namespace, so a silent miss would run the reference's
-  classes while claiming the drop-in.  ``opt_in``: see patch_namespace.  ``device_partition``: see patch_partition (the GPNN collate ships
+  classes while claiming the drop-in.  ``opt_in``, ``keyed_dropout``: see patch_namespace.  ``device_partition``: see patch_partition (the GPNN collate ships
   [B,0,0] operators and the GPNN drop-in partitions on the device)."""
   opt_in = _check_opt_in(opt_in)
+  _check_keyed_dropout(opt_in, keyed_dropout)
   if compat:
     from . import compat as _compat
     _compat.install()
@@ -123,7 +134,7 @@ def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.gr
   register_native_op()
   patched = []
   ref_model = importlib.import_module('model')
-  patched.append(patch_namespace(ref_model, training, opt_in))
+  patched.append(patch_namespace(ref_model, training, opt_in, keyed_dropout))
   errors = []
   for name in runner_modules:
     try:
@@ -131,7 +142,7 @@ def install(reference_root=None, runner_modules=('runner.qm8_runner', 'runner.gr
     except ImportError as exc:      # e.g. tensorboardX absent: that runner cannot be used anyway
       errors.append('%s: %s' % (name, exc))
       continue
-    patched.append(patch_namespace(mod, training, opt_in))
+    patched.append(patch_namespace(mod, training, opt_in, keyed_dropout))
   if runner_modules and len(patched) == 1:
     raise ImportError('dropin.install: no runner module could be imported, nothing would call the '
                       'H100 classes (%s); pass compat=True for the shims of '
@@ -156,9 +167,10 @@ def main(argv=None):
     opt_in.append(argv[i + 1])
     del argv[i:i + 2]
   device_partition = '--device-partition' in argv
-  argv = [a for a in argv if a != '--device-partition']
+  keyed_dropout = '--keyed-dropout' in argv
+  argv = [a for a in argv if a not in ('--device-partition', '--keyed-dropout')]
   install(root, compat=True, training=('-t' not in argv and '--test' not in argv), opt_in=opt_in,
-          device_partition=device_partition)
+          device_partition=device_partition, keyed_dropout=keyed_dropout)
   os.chdir(root)
   sys.argv = ['run_exp.py'] + argv
   run_exp = importlib.import_module('run_exp')

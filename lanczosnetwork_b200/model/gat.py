@@ -18,14 +18,15 @@ autograd with trainable parameters the forward raises, and ``dropin.patch_namesp
 keeps the reference class for training runs.  ``TrainableGAT`` (same constructor, parameters and
 checkpoints) adds one: under autograd its forward is ``train.gat_train``, whose attention adjoint is
 ``lnb_gat_attention_backward``; the drop-in binds it under the name ``GAT`` by opt-in only
-(``dropin.TRAINING_OPT_IN_CLASSES``, ``--opt-in GAT``)."""
+(``dropin.TRAINING_OPT_IN_CLASSES``, ``--opt-in GAT``).  ``KeyedGAT`` (same again) also trains with
+``dropout > 0``, its masks drawn on the device from a key (``--opt-in GAT --keyed-dropout``)."""
 import torch
 import torch.nn as nn
 
-from ._common import SpectralNetBase, init_linears, loss_function
+from ._common import SparseRecords, SpectralNetBase, init_linears, loss_function
 from .. import ops
 
-__all__ = ['GAT', 'TrainableGAT']
+__all__ = ['GAT', 'TrainableGAT', 'KeyedGAT']
 
 
 def _linear_grid(num_layer, num_channel, num_heads, make):
@@ -154,3 +155,69 @@ class TrainableGAT(GAT):
     _, node_ids, mask, _, _ = self._prepare_records(recs)
     bias = ops.gat_bias_sparse(recs.sizes, recs.edge_ptr, recs.edges, recs.N, self.num_edgetype + 1)
     return gat_train(self, node_ids, bias, mask)
+
+
+class KeyedGAT(TrainableGAT):
+  """``TrainableGAT`` (same constructor, parameters, initialisation, ``state_dict`` and checkpoints) that
+  also trains with ``dropout > 0``, as the reference does: at every channel of every layer the input, the
+  attention weights and Wh are dropped with p = ``dropout`` (model/gat.py:149-163).  The masks are drawn on
+  the device from a key, so the step can be captured in a CUDA graph (``train.GraphedStep``, padded or
+  ``sparse=True``): each channel's input mask inside the projection (``lnb_gat_dropout_project``, no masked
+  copy of the input exists) and the other two inside the attention kernels (``lnb_gat_attention_dropout``);
+  the adjoints draw them again.
+
+  The key is an int64 tensor (seed, counter) of shape (2,); the rule is in the C header.  In training mode
+  with dropout > 0, ``forward(..., dropout_key=None)`` reads the module's own key, the non-persistent buffer
+  ``dropout_key`` initialised to (config.seed or 0, 0), and advances its counter on the device after the
+  forward: eager calls and ``GraphedStep`` replays each draw new masks.  An explicit ``dropout_key`` is used
+  as given and nothing is advanced.  The records entries take ``batch['dropout_key']`` when present, otherwise
+  the module's key.  That forward is the dropout formulation with or without autograd (the reference's
+  training-mode semantics).  In eval mode, or with dropout 0, this is ``TrainableGAT``: same code, same bits.
+  Under ``nn.DataParallel`` the replicas share the module's key, so each replica draws the same masks for
+  its own slice of the batch: pass distinct keys per replica if that matters.  The reference's torch
+  dropout draws are not reproduced; the distribution is the same."""
+
+  def __init__(self, config):
+    super(KeyedGAT, self).__init__(config)
+    seed = int(getattr(config, 'seed', 0) or 0)
+    self.register_buffer('dropout_key', torch.tensor([seed, 0], dtype=torch.int64), persistent=False)
+
+  def _drops(self):
+    return self.training and self.dropout > 0.0
+
+  def forward(self, node_feat, L, label=None, mask=None, dropout_key=None):
+    """node_feat: long B x N; L: float B x N x N x (E+1) (data.gat_bias); label: B x P; mask: B x N;
+    dropout_key: int64 (2,) (seed, counter), default the module's own key (advanced after the forward)."""
+    if dropout_key is not None:
+      ops.check_dropout_key('KeyedGAT', dropout_key)
+    if not self._drops():
+      return super(KeyedGAT, self).forward(node_feat, L, label, mask)
+    dev = self._device()
+    score = self._dropout_train(self._to(dev, node_feat), self._to(dev, L), self._to(dev, mask), dropout_key)
+    return self._finish(score, self._to(dev, label))
+
+  def _dropout_train(self, node_ids, bias, mask, dropout_key):
+    from ..train import gat_train
+    own = dropout_key is None
+    key = self._to(node_ids.device, self.dropout_key if own else dropout_key)
+    score = gat_train(self, node_ids, bias, mask, dropout_key=key)
+    if own:
+      with torch.no_grad():
+        self.dropout_key[1:].add_(1)
+    return score
+
+  def _sparse_inputs(self, batch):
+    inputs, impl, key = super(KeyedGAT, self)._sparse_inputs(batch)
+    dk = batch.get('dropout_key')
+    if dk is None:
+      return inputs, impl, key
+    ops.check_dropout_key('KeyedGAT', dk)
+    N = int(batch['N'])
+    return inputs + (dk,), lambda *a: self._forward_records(SparseRecords(*a[:5], N=N)), key
+
+  def _train_records(self, recs, dropout_key=None):
+    if not self._drops():
+      return super(KeyedGAT, self)._train_records(recs)
+    _, node_ids, mask, _, _ = self._prepare_records(recs)
+    bias = ops.gat_bias_sparse(recs.sizes, recs.edge_ptr, recs.edges, recs.N, self.num_edgetype + 1)
+    return self._dropout_train(node_ids, bias, mask, dropout_key)

@@ -17,6 +17,8 @@ __all__ = [
     'spectral_partition', 'spectral_partition_sparse', 'spectral_partition_supported', 'partition_draws', 'gat_bias_sparse',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
+    'check_dropout_key', 'gat_attention_dropout', 'gat_attention_dropout_backward', 'gat_dropout_project',
+    'gat_dropout_project_backward', 'gat_dropout_project_supported',
     'sage_operators', 'sage_sample_sparse', 'neighbour_max', 'sage_lstm_step', 'sage_lstm_step_supported', 'sage_lstm_messages',
     'ggnn_update',
     'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
@@ -881,6 +883,125 @@ def gat_attention_backward(gout, Wh, bias, a1, a2, c1, c2, state_bias, out=None,
   g = gpar.sum(dim=0)
   return (gWh, g[:, :F].contiguous(), g[:, F:2 * F].contiguous(), g[:, 3 * F].contiguous(),
           g[:, 3 * F + 1].contiguous(), g[:, 2 * F:3 * F].contiguous())
+
+
+def check_dropout_key(who, key):
+  """``dropout_key``: an int64 tensor of shape (2,), (seed, counter), as ``check_start_key`` asks of a start key."""
+  if not torch.is_tensor(key) or key.dtype != torch.int64 or tuple(key.shape) != (2,):
+    raise ValueError("%s: 'dropout_key' must be an int64 tensor of shape (2,) (seed, counter); got %r"
+                     % (who, (key.dtype, tuple(key.shape)) if torch.is_tensor(key) else type(key)))
+
+
+def _dropout_args(who, key, p, t):
+  check_dropout_key(who, key)
+  _need_cuda(key)
+  p, t = float(p), int(t)
+  if not 0.0 <= p <= 1.0:
+    raise ValueError('%s: p=%g outside [0, 1]' % (who, p))
+  if not 0 <= t < 1 << 16:
+    raise ValueError('%s: layer %d outside 0 <= t < 2^16' % (who, t))
+  return key.contiguous(), p, t
+
+
+def gat_attention_dropout(Wh, bias, a1, a2, c1, c2, state_bias, dropout_key, p, t, last=False):
+  """``gat_attention`` with the reference's attention and Wh dropout of layer ``t`` (lnb_gat_attention_dropout;
+  the mask rule is in the C header): masks drawn on the device from ``dropout_key``, an int64 [2] CUDA
+  tensor (seed, counter) read on the device."""
+  key, p, t = _dropout_args('gat_attention_dropout', dropout_key, p, t)
+  _need_cuda(Wh, bias, a1, a2, c1, c2, state_bias)
+  Wh, bias = _f32c(Wh), _f32c(bias)
+  a1, a2, c1, c2, state_bias = [_f32c(x) for x in (a1, a2, c1, c2, state_bias)]
+  B, N, _, E1 = bias.shape
+  C, F = a1.shape
+  heads = C // E1
+  if heads * E1 != C or tuple(Wh.shape) != (B, N, C * F) or tuple(state_bias.shape) != (C, F):
+    raise ValueError('gat_attention_dropout: Wh %s, bias %s, a1 %s, state_bias %s do not agree'
+                     % (tuple(Wh.shape), tuple(bias.shape), tuple(a1.shape), tuple(state_bias.shape)))
+  out = torch.empty((B, N, F if last else C * F), device=Wh.device, dtype=torch.float32)
+  with torch.cuda.device(Wh.device):
+    _lib.check(_lib.load().lnb_gat_attention_dropout(
+        _stream(Wh), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
+        B, N, E1, heads, F, int(bool(last)), _ptr(key), p, t, _ptr(out)), 'lnb_gat_attention_dropout')
+  return out
+
+
+def gat_attention_dropout_backward(gout, Wh, bias, a1, a2, c1, c2, state_bias, dropout_key, p, t, last=False):
+  """Adjoint of ``gat_attention_dropout`` with the same key, p and t (lnb_gat_attention_dropout_backward): the
+  masks are drawn again.  Returns (gWh, ga1, ga2, gc1, gc2, gsb) as ``gat_attention_backward``."""
+  key, p, t = _dropout_args('gat_attention_dropout_backward', dropout_key, p, t)
+  _need_cuda(gout, Wh, bias, a1, a2, c1, c2, state_bias)
+  Wh, bias, gout = _f32c(Wh), _f32c(bias), _f32c(gout)
+  a1, a2, c1, c2, state_bias = [_f32c(x) for x in (a1, a2, c1, c2, state_bias)]
+  B, N, _, E1 = bias.shape
+  C, F = a1.shape
+  heads = C // E1
+  if (heads * E1 != C or tuple(Wh.shape) != (B, N, C * F) or tuple(state_bias.shape) != (C, F) or
+      tuple(gout.shape) != (B, N, F if last else C * F)):
+    raise ValueError('gat_attention_dropout_backward: gout %s, Wh %s, bias %s, a1 %s, state_bias %s do not agree'
+                     % (tuple(gout.shape), tuple(Wh.shape), tuple(bias.shape), tuple(a1.shape),
+                        tuple(state_bias.shape)))
+  gWh = torch.empty((B, N, C * F), device=Wh.device, dtype=torch.float32)
+  if B == 0:
+    z = torch.zeros((C, F), device=Wh.device, dtype=torch.float32)
+    return gWh, z, z.clone(), z[:, 0].clone(), z[:, 0].clone(), z.clone()
+  gpar = torch.empty((B, C, 3 * F + 2), device=Wh.device, dtype=torch.float32)
+  with torch.cuda.device(Wh.device):
+    _lib.check(_lib.load().lnb_gat_attention_dropout_backward(
+        _stream(Wh), _ptr(gout), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
+        B, N, E1, heads, F, int(bool(last)), _ptr(key), p, t, _ptr(gWh), _ptr(gpar)),
+        'lnb_gat_attention_dropout_backward')
+  g = gpar.sum(dim=0)
+  return (gWh, g[:, :F].contiguous(), g[:, F:2 * F].contiguous(), g[:, 3 * F].contiguous(),
+          g[:, 3 * F + 1].contiguous(), g[:, 2 * F:3 * F].contiguous())
+
+
+def gat_dropout_project_supported(Din, F):
+  """Shapes lnb_gat_dropout_project(_backward) accept (mirrors their checks)."""
+  return Din % 4 == 0 and F % 4 == 0 and F <= 128
+
+
+def _project_dims(who, X, W, C):
+  M, Din = X.shape
+  if C < 1 or W.dim() != 2 or W.shape[1] != Din or W.shape[0] % C:
+    raise ValueError('%s: X %s, W %s do not agree with C=%d channels' % (who, tuple(X.shape), tuple(W.shape), C))
+  return M, Din, W.shape[0] // C
+
+
+def gat_dropout_project(X, W, C, dropout_key, p, t):
+  """GAT's per-channel input dropout and projection of layer ``t`` (lnb_gat_dropout_project):
+  Wh[:, c*F:(c+1)*F] = (X * M_c s) W_c^T for X [M, Din] and W [C*F, Din] (channel c's weight in rows
+  c*F .. c*F+F-1).  Returns Wh [M, C*F]."""
+  key, p, t = _dropout_args('gat_dropout_project', dropout_key, p, t)
+  _need_cuda(X, W)
+  X, W = _f32c(X), _f32c(W)
+  M, Din, F = _project_dims('gat_dropout_project', X, W, int(C))
+  Wh = torch.empty((M, W.shape[0]), device=X.device, dtype=torch.float32)
+  with torch.cuda.device(X.device):
+    _lib.check(_lib.load().lnb_gat_dropout_project(_stream(X), _ptr(X), _ptr(W), M, Din, int(C), F, _ptr(key), p,
+                                                   t, _ptr(Wh)), 'lnb_gat_dropout_project')
+  return Wh
+
+
+def gat_dropout_project_backward(X, W, gWh, C, dropout_key, p, t):
+  """Adjoint of ``gat_dropout_project`` with the same key, p and t (lnb_gat_dropout_project_backward; the masks
+  are drawn again).  Returns (gX [M, Din], gW [C*F, Din])."""
+  key, p, t = _dropout_args('gat_dropout_project_backward', dropout_key, p, t)
+  _need_cuda(X, W, gWh)
+  X, W, gWh = _f32c(X), _f32c(W), _f32c(gWh)
+  C = int(C)
+  M, Din, F = _project_dims('gat_dropout_project_backward', X, W, C)
+  if tuple(gWh.shape) != (M, C * F):
+    raise ValueError('gat_dropout_project_backward: gWh %s, expected %s' % (tuple(gWh.shape), (M, C * F)))
+  lib = _lib.load()
+  slabs = max(int(lib.lnb_gat_dropout_project_slabs(M, Din, C, F)), 1)
+  gX = torch.empty_like(X)
+  gW = torch.empty_like(W)
+  work = torch.empty((slabs, C * F, Din), device=X.device, dtype=torch.float32)
+  with torch.cuda.device(X.device):
+    _lib.check(lib.lnb_gat_dropout_project_backward(_stream(X), _ptr(X), _ptr(W), _ptr(gWh), M, Din, C, F, _ptr(key),
+                                                    p, t, _ptr(gX), _ptr(gW), _ptr(work)),
+               'lnb_gat_dropout_project_backward')
+  return gX, gW
 
 
 def ggnn_update_supported(N, D, E1):

@@ -754,28 +754,86 @@ def gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=False):
                              sb.float().contiguous(), bool(last))
 
 
-def gat_train(model, node_ids, bias, mask):
-  """Differentiable GAT (model/gat.py:125-201) without dropout: embedding -> per layer the head weights
+class _GatAttentionDropout(torch.autograd.Function):
+  """``_GatAttention`` with the attention and Wh dropout of layer t (lnb_gat_attention_dropout and its
+  adjoint).  The backward draws the masks again from the saved device copy of the key the forward drew with
+  (the module advances its own key after the forward)."""
+
+  @staticmethod
+  def forward(ctx, Wh, bias, a1, a2, c1, c2, sb, key, p, t, last):
+    Wh = Wh.contiguous()
+    out = ops.gat_attention_dropout(Wh, bias, a1, a2, c1, c2, sb, key, p, t, last=last)
+    ctx.save_for_backward(Wh, bias, a1, a2, c1, c2, sb, key)
+    ctx.p, ctx.t, ctx.last = p, t, last
+    return out
+
+  @staticmethod
+  def backward(ctx, gout):
+    Wh, bias, a1, a2, c1, c2, sb, key = ctx.saved_tensors
+    gWh, ga1, ga2, gc1, gc2, gsb = ops.gat_attention_dropout_backward(gout.contiguous(), Wh, bias, a1, a2, c1, c2,
+                                                                      sb, key, ctx.p, ctx.t, last=ctx.last)
+    return gWh, None, ga1, ga2, gc1, gc2, gsb, None, None, None, None
+
+
+class _GatDropoutProject(torch.autograd.Function):
+  """Wh = per-channel (X * M_c s) W_c^T of layer t (lnb_gat_dropout_project) and its adjoint
+  (lnb_gat_dropout_project_backward), which draws the input masks again from the saved key copy."""
+
+  @staticmethod
+  def forward(ctx, X, W, C, key, p, t):
+    X, W = X.contiguous(), W.contiguous()
+    ctx.save_for_backward(X, W, key)
+    ctx.C, ctx.p, ctx.t = C, p, t
+    return ops.gat_dropout_project(X, W, C, key, p, t)
+
+  @staticmethod
+  def backward(ctx, gWh):
+    X, W, key = ctx.saved_tensors
+    gX, gW = ops.gat_dropout_project_backward(X, W, gWh.contiguous(), ctx.C, key, ctx.p, ctx.t)
+    return gX, gW, None, None, None, None
+
+
+def gat_train(model, node_ids, bias, mask, dropout_key=None):
+  """Differentiable GAT (model/gat.py:125-201): embedding -> per layer the head weights
   of all (E+1) * heads channels stacked in concat order c = jj * heads + ii on the tape, ONE ``dense``
   projection, a1 / a2 / c1 / c2 stacked likewise, ``gat_attention`` -> gated readout with the head
   ``output_func``.  Every channel reads ``bias_{ii}_{E}_{t}`` (the reference's shared state_bias list),
   so that parameter's gradient sums over all E+1 channels and the other ``bias_{ii}_{jj}_{t}`` get
   none (``grad`` stays None, as in the reference).  ``bias`` is the collate's attention bias
-  [B,N,N,E+1] (data.gat_bias)."""
+  [B,N,N,E+1] (data.gat_bias).
+
+  ``dropout_key`` (int64 [2] CUDA tensor, (seed, counter)): the reference's three dropout sites with
+  p = model.dropout, masks drawn on the device by the rule of the C header -- the projection becomes
+  ``_GatDropoutProject`` (each channel's own input mask) and the attention ``_GatAttentionDropout``.  The
+  Functions keep a copy of the key, so the caller may advance it once the forward is issued.  Without a key
+  there is no dropout."""
   bias = bias.float().contiguous()
+  if dropout_key is not None:
+    dropout_key = dropout_key.detach().clone()
+    p = float(model.dropout)
   state = embedding(node_ids, model.embedding.weight)
   B, N = state.shape[0], state.shape[1]
   E = model.num_edgetype
   for t in range(model.num_layer):
     mods = [(jj, ii) for jj in range(E + 1) for ii in range(model.num_heads[t])]
     w = torch.cat([model.filter[t][jj][ii].weight for jj, ii in mods], dim=0)          # [C*F, Din]
-    Wh = dense(state.reshape(B * N, -1), w, None, False).reshape(B, N, -1)
+    if dropout_key is not None:
+      x = state.reshape(B * N, -1).float()
+      Wh = _GatDropoutProject.apply(x, w.float(), len(mods), dropout_key, p, t).reshape(B, N, -1)
+    else:
+      Wh = dense(state.reshape(B * N, -1), w, None, False).reshape(B, N, -1)
     a1 = torch.cat([model.att_net_1[t][jj][ii].weight for jj, ii in mods], dim=0)       # [C, F]
     a2 = torch.cat([model.att_net_2[t][jj][ii].weight for jj, ii in mods], dim=0)
     c1 = torch.cat([model.att_net_1[t][jj][ii].bias for jj, ii in mods], dim=0)         # [C]
     c2 = torch.cat([model.att_net_2[t][jj][ii].bias for jj, ii in mods], dim=0)
     sb = torch.stack([getattr(model, 'bias_%d_%d_%d' % (ii, E, t)) for _, ii in mods], dim=0)
-    state = gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=(t == model.num_layer - 1))
+    last = t == model.num_layer - 1
+    if dropout_key is not None:
+      state = _GatAttentionDropout.apply(Wh.float(), bias, a1.float().contiguous(), a2.float().contiguous(),
+                                         c1.float().contiguous(), c2.float().contiguous(), sb.float().contiguous(),
+                                         dropout_key, p, t, last)
+    else:
+      state = gat_attention(Wh, bias, a1, a2, c1, c2, sb, last=last)
   return gated_readout(model, state, mask, head=model.output_func[0])
 
 
@@ -1072,7 +1130,8 @@ class GraphedStep:
 
   # the ragged record arrays: static buffers of more rows than a batch fills, only the rows present copied
   _RAGGED = ('node_feat', 'edges', 'V_rows')
-  _RECORD_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N', 'K', 'V_rows', 'D', 'sample_key', 'start_key')
+  _RECORD_KEYS = ('sizes', 'node_ptr', 'node_feat', 'edge_ptr', 'edges', 'N', 'K', 'V_rows', 'D', 'sample_key', 'start_key',
+                  'dropout_key')
 
   def _static_records(self, batch, dev, cap):
     B, N = int(batch['sizes'].shape[0]), int(batch['N'])
