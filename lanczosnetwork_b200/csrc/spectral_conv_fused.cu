@@ -13,8 +13,9 @@
 // Dropping exact zeros is exact, so the result equals the dense reference for arbitrary inputs.
 //
 // Two accumulator lifetimes ("steps") per tile:
-//   step 0  Z = sum_s (f_s . U) W_s^T      rows = (graph, Ritz index), k-blocks d-block-major: at
-//           the first k-block of a d-block the producer thread of row (g, k) computes its 32
+//   step 0  Z = sum_s (f_s . U) W_s^T      rows = (graph, Ritz index), k-blocks by pairs of d-blocks
+//           (s0_kblock: each producer group takes all k-blocks of one d-block of a pair): at the
+//           group's first k-block of a d-block the producer thread of row (g, k) computes its 32
 //           columns of U_g = V_g^T X_g into registers, then scales them by f_s for every s; Z is
 //           drained into the A ring and stays there;
 //   step 1  E = sum_e (L_e X) W_e^T        rows = (graph, node): sparse ELL rows of the operators
@@ -553,10 +554,36 @@ struct SpectralPolicyT {
   static __device__ __forceinline__ int num_kblocks(const Params& p, int sub) {
     return ((sub & 1) == 0 ? p.S : p.E1) * p.Din[sub >> 1] / tcg::BK;
   }
-  // step 0 runs its k-blocks d-block-major (kb = dblk * S + s), so one U block serves S k-blocks
+  // Step 0's k-block kb is (d-block dblk, scale s), W columns s * Din + 32 dblk.  The d-blocks run in
+  // pairs, the k-blocks of a pair alternating between its two d-blocks (kb = 2 (pair S + s) + dblk % 2).
+  // The producer groups take alternate k-blocks, so each group takes every k-block of one d-block of
+  // the pair and computes that d-block's U once, at s = 0 (d-block-major order, kb = dblk S + s, has both
+  // groups compute every U).  An odd last d-block runs on its own (kb = pairs 2 S + s), alternating
+  // between the groups, each computing U at its first k-block of it (s < 2).  first: this k-block is
+  // where the group that takes it computes U.
+  static __device__ __forceinline__ void s0_kblock(int Din, int S, int kb, int& dblk, int& s, bool& first) {
+    const int paired = (Din / tcg::BK) & ~1;       // d-blocks that run in pairs
+    if (kb < paired * S) {
+      const int pr = kb / (2 * S), r = kb - pr * 2 * S;
+      s = r >> 1;
+      dblk = 2 * pr + (r & 1);
+      first = s == 0;
+    } else {
+      s = kb - paired * S;
+      dblk = paired;
+      first = s < kProducerGroups;
+    }
+  }
   static __device__ __forceinline__ void w_coords(const Params& p, int sub, int kb, int& col0, int& row0) {
     const int Din = p.Din[sub >> 1];
-    col0 = (sub & 1) == 0 ? (kb % p.S) * Din + (kb / p.S) * tcg::BK : p.S * Din + kb * tcg::BK;
+    if (kLongScales && (sub & 1) == 0) {          // (the GraphSAGE variants run S = 0: no step 0)
+      int dblk, s;
+      bool first;
+      s0_kblock(Din, p.S, kb, dblk, s, first);
+      col0 = s * Din + dblk * tcg::BK;
+    } else {
+      col0 = p.S * Din + kb * tcg::BK;
+    }
     row0 = (sub >> 1) * p.H;
   }
   // Z of step 0 stays in the A ring for the edge step's acc_init()
@@ -766,19 +793,21 @@ struct SpectralPolicyT {
   // keeps only U in registers across the k-blocks of a d-block
   __device__ __forceinline__ float produce(int sub, int kb, float (&v)[32]) {
     if (kLongScales && (sub & 1) == 0) {
-      // row = (graph, Ritz index): f[k, s] * U[row, d0:d0+32], kb = dblk * S + s; v holds U (zero
-      // for the rows past Ztot, whose scale is 0)
-      const int s = kb % S;
+      // row = (graph, Ritz index): f[k, s] * U[row, d0:d0+32], (dblk, s) from s0_kblock; v holds U
+      // (zero for the rows past Ztot, whose scale is 0)
+      int dblk, s;
+      bool first;
+      s0_kblock(Din, S, kb, dblk, s, first);
       const float f = __ldg(frow + s);             // issued before U is summed
-      if (s < kProducerGroups) {
+      if (first) {
         // U[(g, k), d0:d0+32] = sum_n Q_g[n, k] X_g[n, d0:d0+32]: every thread of graph g reads the
-        // same X row (a broadcast), consecutive Q entries.  The groups take alternate k-blocks, so
-        // each one's first k-block of the d-block is s = 0 or s = 1: each computes U for itself.
+        // same X row (a broadcast), consecutive Q entries.  Computed once per d-block of a pair (by
+        // the group that takes it), twice for an odd last d-block (each group for itself).
 #pragma unroll
         for (int j = 0; j < tcg::BK; ++j) v[j] = 0.f;
         if (r < tb->Ztot) {
           const int g = tb->z_g[r], n_g = tb->gn[g], nb = tb->nbase[g];
-          const float* xs = Xs + (size_t)nb * XP + (kb / S) * tcg::BK;
+          const float* xs = Xs + (size_t)nb * XP + dblk * tcg::BK;
           const float* qs = Qs + (size_t)nb * K + tb->z_k[r];
 #pragma unroll 2
           for (int n = 0; n < n_g; ++n) {
