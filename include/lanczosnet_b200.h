@@ -844,6 +844,14 @@ int lnb_symmetrize_filters(lnb_stream_t stream, const float* Y, int B, int K, in
  * the wgmma kernels fill with per-CTA clock64 totals per phase; NULL disables. */
 int lnb_debug_set_prof(unsigned long long* buf);
 
+/* Testing aid (not used by the product path): n > 0 caps the grid of every persistent wgmma launch
+ * (the dense layers, the GRU and LSTM steps, the filter-MLP chain and the convolution stacks) at n
+ * CTAs, so that each CTA runs several work items; 0 (the default) removes the cap; n < 0 is
+ * LNB_ERR_ARG.  An item's arithmetic does not depend on the CTA that runs it, so the outputs are
+ * the same bits under any cap.  Read at launch: a captured graph keeps the grid it was captured
+ * with. */
+int lnb_debug_set_max_ctas(int n);
+
 #ifdef __cplusplus
 }
 #endif

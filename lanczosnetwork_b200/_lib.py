@@ -94,6 +94,7 @@ SIGNATURES = {
     'lnb_ritz_filter_mlp_ctas': (c_int, [c_stream, c_f32p, ctypes.c_void_p, ctypes.c_void_p, c_f32p, c_f32p,
                                          c_f32p, c_int, c_int, c_int, c_int, c_f32p, c_int]),
     'lnb_debug_set_prof': (c_int, [ctypes.c_void_p]),
+    'lnb_debug_set_max_ctas': (c_int, [c_int]),
     'lnb_embedding_rows': (c_int, [c_stream, ctypes.c_void_p, c_f32p, c_i64, c_int, c_int, c_f32p]),
     'lnb_ritz_power_table': (c_int, [c_stream, c_f32p, c_i64, ctypes.POINTER(c_int), c_int, c_f32p]),
     'lnb_readout': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_void_p,

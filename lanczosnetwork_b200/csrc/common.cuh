@@ -15,6 +15,7 @@ void set_err(const char* fmt, ...);
 void count_launch(int n = 1);
 unsigned long long* prof_buffer();          // profiling aid (lnb_debug_set_prof), nullptr = off
 void set_prof_buffer(unsigned long long* p);
+int debug_max_ctas();                       // testing aid (lnb_debug_set_max_ctas), 0 = no cap
 
 void launch_tile_assign(cudaStream_t s, const int32_t* gext, int B, int K, int32_t* tiles,
                         int32_t* rowmap, int32_t* nrows);   // spectral_conv_fused.cu

@@ -21,6 +21,9 @@ static unsigned long long* g_prof_buf = nullptr;
 unsigned long long* prof_buffer() { return g_prof_buf; }
 void set_prof_buffer(unsigned long long* p) { g_prof_buf = p; }
 
+static int g_max_ctas = 0;
+int debug_max_ctas() { return g_max_ctas; }
+
 }  // namespace lnb
 
 extern "C" {
@@ -37,6 +40,14 @@ int64_t lnb_launch_count(void) { return lnb::g_launches; }
 // not be inside a stream capture, and until it runs, replays of captured graphs see the old buffer.
 int lnb_debug_set_prof(unsigned long long* buf) {
   lnb::set_prof_buffer(buf);
+  return LNB_OK;
+}
+
+// Testing aid: cap the grid of every persistent wgmma launch (tcg::persistent_grid) at n > 0 CTAs;
+// 0 removes the cap.
+int lnb_debug_set_max_ctas(int n) {
+  LNB_REQUIRE(n >= 0, "debug_set_max_ctas: n=%d must be >= 0", n);
+  lnb::g_max_ctas = n;
   return LNB_OK;
 }
 

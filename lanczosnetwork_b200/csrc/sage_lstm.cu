@@ -153,7 +153,7 @@ int launch_step(lnb_stream_t stream, const float* W_hi, const float* W_lo, int D
                                          : tcg::tc_gemm_probe_kernel<SageLstmPolicy, tcg::SKIP_MMA | tcg::SKIP_TMA>;
   const size_t smem = SageLstmPolicy::SMEM_BYTES;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  const int grid = items < tcg::sm_count() ? items : tcg::sm_count();
+  const int grid = tcg::persistent_grid(items);
   kern<<<grid, tcg::cta_threads<SageLstmPolicy>, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
   lnb::count_launch();
   return lnb::finish_launch(who);

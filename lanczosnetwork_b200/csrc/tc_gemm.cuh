@@ -644,6 +644,16 @@ inline int sm_count() {
   return n > 0 ? n : 132;
 }
 
+// CTAs of a persistent launch over `items` work items: min(items, SMs), and at most each positive
+// bound of max_ctas and the testing cap of lnb_debug_set_max_ctas
+inline int persistent_grid(int items, int max_ctas = 0) {
+  int grid = items < sm_count() ? items : sm_count();
+  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
+  const int cap = lnb::debug_max_ctas();
+  if (cap > 0 && grid > cap) grid = cap;
+  return grid;
+}
+
 // g_prof is defined in this header, so every translation unit has its own copy.  Each points its
 // copy at the buffer registered with lnb_debug_set_prof when that has changed since its last launch
 // (a synchronous copy; with no buffer ever registered nothing is copied).
@@ -658,7 +668,7 @@ static int sync_prof_buffer(const char* who) {
   return LNB_OK;
 }
 
-// Launches tc_gemm_kernel<Pol> on min(items, SMs, max_ctas if > 0) persistent CTAs with `smem` bytes of
+// Launches tc_gemm_kernel<Pol> on persistent_grid(items, max_ctas) persistent CTAs with `smem` bytes of
 // dynamic shared memory; W_hi / W_lo are the split row-major [w_rows, w_cols] weights the TMA streams.
 template <class Pol>
 static int launch(lnb_stream_t stream, const float* W_hi, const float* W_lo, int w_rows, int w_cols,
@@ -677,9 +687,7 @@ static int launch(lnb_stream_t stream, const float* W_hi, const float* W_lo, int
               : skip == SKIP_TMA           ? tc_gemm_probe_kernel<Pol, SKIP_TMA>
                                            : tc_gemm_probe_kernel<Pol, SKIP_MMA | SKIP_TMA>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  int grid = items < sm_count() ? items : sm_count();
-  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  kern<<<grid, cta_threads<Pol>, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
+  kern<<<persistent_grid(items, max_ctas), cta_threads<Pol>, smem, (cudaStream_t)stream>>>(map_hi, map_lo, p);
   lnb::count_launch();
   return lnb::finish_launch(who);
 }
