@@ -192,6 +192,10 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
  *   hdr[12] = off(krow_ptr [B+1] i32) (both 0 when absent); hdr[3..6], hdr[11], hdr[12] depend on (B, K)
  *   only, so D and the tiles sit at fixed addresses of a reused buffer (lnb_ritz_power_table and
  *   lnb_spectral_stack_forward read them there).
+ *   hdr[6] and hdr[8] are 0 when the batch carries no eigenpairs (data.pack_sparse of
+ *   data.sparse_collate(..., eigs=False) records, data.PackedMolecules(..., eigs=False)): D and V_rows
+ *   are absent, and so are the tiles and krow_ptr (without the Ritz rows the host cannot know k_eff).
+ *   Such a batch is read through lnb_records_unpack, never by this kernel.
  * The kernel derives its input pointers from the header on the device.  flags bit 1
  * (LNB_PACKED_HOST_TILES): the host knows every graph's extents, so it ships the tiles (the same
  * next-fit table and first-fit-decreasing schedule as lnb_graph_prepare, in the same layout) and the
@@ -203,6 +207,25 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
                                     uint8_t* ell_idx, int32_t* ell_max, int32_t* gext, int32_t* tiles,
                                     int32_t* rowmap, int32_t* nrows, int64_t* node_ids, uint8_t* mask,
                                     float* V, float* L_dense);
+
+/* A packed batch (layout above, with or without eigenpairs) split back into the records of
+ * lnb_graph_prepare_sparse, in ONE launch: the header is read on the device and every segment present is
+ * copied into fixed-capacity buffers -- sizes [B], node_ptr [B+1], edge_ptr [B+1], node_feat [cap_rows],
+ * edges [cap_edges][4], and, when not NULL, D [B,K] and V_rows [cap_rows, K].  Offsets change from batch to
+ * batch, so one captured launch serves every batch of the same (B, K) that fits the capacities.  Copies
+ * are 16-byte vectors (then up to three 4-byte words per segment), grid-stride; the grid depends on the
+ * capacities only.  Nothing past hdr[10] is read, nothing past a capacity is written; rows past
+ * node_ptr[B] / edge_ptr[B] keep their old contents.
+ * blob_bytes: the allocation behind blob (>= 64); every buffer is 16-byte aligned.
+ * status [1]: 0 = copied; otherwise nothing but sizes, node_ptr and edge_ptr is written, all three zero
+ * (every graph empty, so the producers behind read no row), and status is a bit set: 1 = bad magic,
+ * 2 = B or K differs from the header, 4 = a segment outside [64, hdr[10]), unaligned or hdr[10] >
+ * blob_bytes, 8 = node_ptr[B] > cap_rows, 16 = edge_ptr[B] > cap_edges, 32 = D or V_rows requested from a
+ * batch without eigenpairs. */
+int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
+                       int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
+                       int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
+                       int32_t* status);
 
 /* Float-feature variant (LanczosNetGeneral's GraphData records, node features instead of atom ids): the
  * same records and outputs as lnb_graph_prepare_sparse, except that node_x [node_ptr[B], F] fp32 holds the

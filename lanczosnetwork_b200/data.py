@@ -401,27 +401,36 @@ def pack_sparse(sp):
   """A ``sparse_collate`` batch as ONE contiguous uint8 buffer (layout: include/lanczosnet_b200.h,
   lnb_graph_prepare_sparse_packed): a 16-int header with the byte offsets of the segments, the
   fixed-size segments (sizes, node_ptr, edge_ptr, D), then node ids, Ritz rows and the bond list.
-  One H2D copy per step ships the whole batch.  Returns dict(blob, B, N, K, num_edgetype[, label])."""
-  B, K = sp['D'].shape
+  One H2D copy per step ships the whole batch.  Records without eigenpairs (``sparse_collate(...,
+  eigs=False)``) give a blob without D, Ritz rows, tiles and Ritz-row offsets (their header offsets are 0):
+  the node ids start where D would.  Returns dict(blob, B, N, K, num_edgetype, eigs[, label])."""
+  eigs = 'D' in sp
+  B, K = sp['D'].shape if eigs else (len(sp['sizes']), int(sp['K']))
   off_sizes, off_node_ptr, off_edge_ptr, off_D, off, off_tiles, off_krow = packed_offsets(B, K)
-  # extents the device would measure: k_eff = last non-zero column of the graph's Ritz rows + 1
-  k_eff = ritz_extents(sp['V_rows'], sp['node_ptr'])
-  tiles = host_tile_segment(sp['sizes'], k_eff)
-  krow = np.zeros(B + 1, np.int32)
-  krow[1:] = np.cumsum(np.minimum(k_eff, K))
-  off_nf = off
-  off_v = off_nf + _align16(sp['node_feat'].nbytes)
-  off_e = off_v + _align16(sp['V_rows'].nbytes)
+  segs = [(off_sizes, sp['sizes']), (off_node_ptr, sp['node_ptr']), (off_edge_ptr, sp['edge_ptr'])]
+  if eigs:
+    # extents the device would measure: k_eff = last non-zero column of the graph's Ritz rows + 1
+    k_eff = ritz_extents(sp['V_rows'], sp['node_ptr'])
+    krow = np.zeros(B + 1, np.int32)
+    krow[1:] = np.cumsum(np.minimum(k_eff, K))
+    segs += [(off_tiles, host_tile_segment(sp['sizes'], k_eff)), (off_krow, krow), (off_D, sp['D'])]
+    off_nf = off
+    off_v = off_nf + _align16(sp['node_feat'].nbytes)
+    off_e = off_v + _align16(sp['V_rows'].nbytes)
+    segs.append((off_v, sp['V_rows']))
+  else:
+    off_nf, off_D, off_v, off_tiles, off_krow = off_D, 0, 0, 0, 0
+    off_e = off_nf + _align16(sp['node_feat'].nbytes)
   total = off_e + _align16(sp['edges'].nbytes)
   blob = np.zeros(total, np.uint8)
   hdr = blob[:64].view(np.int32)
   hdr[:13] = [PACK_MAGIC, B, K, off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_v, off_e, total,
               off_tiles, off_krow]
-  for off_, arr in ((off_tiles, tiles), (off_krow, krow), (off_sizes, sp['sizes']), (off_node_ptr, sp['node_ptr']), (off_edge_ptr, sp['edge_ptr']),
-                    (off_D, sp['D']), (off_nf, sp['node_feat']), (off_v, sp['V_rows']), (off_e, sp['edges'])):
+  for off_, arr in segs + [(off_nf, sp['node_feat']), (off_e, sp['edges'])]:
     raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
     blob[off_:off_ + raw.size] = raw
-  out = {'blob': blob, 'B': int(B), 'N': int(sp['N']), 'K': int(K), 'num_edgetype': int(sp['num_edgetype'])}
+  out = {'blob': blob, 'B': int(B), 'N': int(sp['N']), 'K': int(K), 'num_edgetype': int(sp['num_edgetype']),
+         'eigs': eigs}
   if 'label' in sp:
     out['label'] = sp['label']
   return out
@@ -434,15 +443,20 @@ class PackedMolecules(object):
   byte -- instead of a Python loop over molecules per step (the reference pads and stacks per batch in
   DataLoader workers, dataset/qm8.py:220-291).  At 1024 molecules: ~1 ms per batch against 9 ms for
   sparse_collate + pack_sparse and 33 ms for the padded collate, i.e. one loader thread keeps up with
-  a GPU step of 0.5 ms only with this path."""
+  a GPU step of 0.5 ms only with this path.
 
-  def __init__(self, samples, num_eigs):
-    sp = sparse_collate(samples, num_eigs)
+  ``eigs=False`` takes ``prepare_graph(..., eigs=False)`` samples (or ignores the eigenpairs of any
+  others): the blobs are those of ``pack_sparse(sparse_collate(..., eigs=False))``, 4 bytes per node instead
+  of 4 (K + 1), and the device computes the eigenpairs where a model reads them."""
+
+  def __init__(self, samples, num_eigs, eigs=True):
+    sp = sparse_collate(samples, num_eigs, eigs=eigs)
     self.K = int(num_eigs)
+    self.eigs = bool(eigs)
     self.num_edgetype = sp['num_edgetype']
     self.sizes, self.node_ptr, self.edge_ptr = sp['sizes'], sp['node_ptr'].astype(np.int64), sp['edge_ptr'].astype(np.int64)
-    self.node_feat, self.edges, self.V_rows, self.D = sp['node_feat'], sp['edges'], sp['V_rows'], sp['D']
-    self.k_eff = ritz_extents(self.V_rows, self.node_ptr)
+    self.node_feat, self.edges, self.V_rows, self.D = sp['node_feat'], sp['edges'], sp.get('V_rows'), sp.get('D')
+    self.k_eff = ritz_extents(self.V_rows, self.node_ptr) if eigs else None
     self.label = sp.get('label')
 
   def __len__(self):
@@ -462,6 +476,8 @@ class PackedMolecules(object):
     buffer): an index list may repeat the largest molecule B times."""
     n = B * int(self.sizes.max())
     e = B * int(np.diff(self.edge_ptr).max())
+    if not self.eigs:
+      return packed_offsets(B, self.K)[3] + _align16(4 * n) + _align16(4 * e)
     return packed_offsets(B, self.K)[4] + _align16(4 * n) + _align16(4 * n * self.K) + _align16(4 * e)
 
   def batch(self, idx, out=None):
@@ -478,12 +494,13 @@ class PackedMolecules(object):
     edge_ptr[1:] = np.cumsum(e_len)
     rows = self._ranges(self.node_ptr[idx], n_len)
     erow = self._ranges(self.edge_ptr[idx], e_len)
-    k_eff = self.k_eff[idx]
-    krow = np.zeros(B + 1, np.int32)
-    krow[1:] = np.cumsum(np.minimum(k_eff, K))
     off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_tiles, off_krow = packed_offsets(B, K)
-    off_v = off_nf + _align16(4 * len(rows))
-    off_e = off_v + _align16(4 * len(rows) * K)
+    if self.eigs:
+      off_v = off_nf + _align16(4 * len(rows))
+      off_e = off_v + _align16(4 * len(rows) * K)
+    else:                                            # pack_sparse's layout without eigenpairs
+      off_nf, off_D, off_v, off_tiles, off_krow = off_D, 0, 0, 0, 0
+      off_e = off_nf + _align16(4 * len(rows))
     total = off_e + _align16(4 * len(erow))
     if out is None:
       blob = np.zeros(total, np.uint8)
@@ -492,7 +509,9 @@ class PackedMolecules(object):
         raise ValueError('PackedMolecules.batch: out must be a flat uint8 buffer of >= %d bytes' % total)
       blob = out[:total]
       blob[:off_nf] = 0                              # header + fixed segments (alignment gaps stay zero)
-      for a, b in ((off_nf + 4 * len(rows), off_v), (off_v + 4 * len(rows) * K, off_e), (off_e + 4 * len(erow), total)):
+      gaps = ((off_nf + 4 * len(rows), off_v), (off_v + 4 * len(rows) * K, off_e)) if self.eigs else \
+          ((off_nf + 4 * len(rows), off_e),)
+      for a, b in gaps + ((off_e + 4 * len(erow), total),):
         blob[a:b] = 0
     blob[:64].view(np.int32)[:13] = [PACK_MAGIC, B, K, off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_v,
                                      off_e, total, off_tiles, off_krow]
@@ -501,16 +520,21 @@ class PackedMolecules(object):
       raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
       blob[off:off + raw.size] = raw
 
-    put(off_tiles, host_tile_segment(sizes, k_eff))
-    put(off_krow, krow)
+    if self.eigs:
+      k_eff = self.k_eff[idx]
+      krow = np.zeros(B + 1, np.int32)
+      krow[1:] = np.cumsum(np.minimum(k_eff, K))
+      put(off_tiles, host_tile_segment(sizes, k_eff))
+      put(off_krow, krow)
+      put(off_D, self.D[idx])
+      np.take(self.V_rows, rows, axis=0, out=blob[off_v:off_v + 4 * len(rows) * K].view(np.float32).reshape(len(rows), K))
     put(off_sizes, sizes)
     put(off_node_ptr, node_ptr)
     put(off_edge_ptr, edge_ptr)
-    put(off_D, self.D[idx])
     np.take(self.node_feat, rows, out=blob[off_nf:off_nf + 4 * len(rows)].view(np.int32))
-    np.take(self.V_rows, rows, axis=0, out=blob[off_v:off_v + 4 * len(rows) * K].view(np.float32).reshape(len(rows), K))
     np.take(self.edges, erow, axis=0, out=blob[off_e:off_e + 4 * len(erow)].reshape(len(erow), 4))
-    res = {'blob': blob, 'B': int(B), 'N': int(sizes.max()) if B else 0, 'K': K, 'num_edgetype': self.num_edgetype}
+    res = {'blob': blob, 'B': int(B), 'N': int(sizes.max()) if B else 0, 'K': K, 'num_edgetype': self.num_edgetype,
+           'eigs': self.eigs}
     if self.label is not None:
       res['label'] = self.label[idx]
     return res

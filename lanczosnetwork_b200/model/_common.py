@@ -43,6 +43,14 @@ def _raw(t):
   return t.tensor if isinstance(t, Ragged) else t
 
 
+def packed_capacity(B, N, K, eigs, nbytes):
+  """Static size of a packed batch's blob under graph replay: the blob of any B molecules of at most N
+  nodes and 4 N bonds each (alignment gaps included), or the blob's own ``nbytes`` when that is larger."""
+  off = data_mod.packed_offsets(B, K)
+  body = off[4] + 4 * B * N * K if eigs else off[3]
+  return max(body + 16 * 3 + 4 * B * N + 4 * B * N * 4, int(nbytes))
+
+
 # the bond-list records of one batch on the device (data.sparse_collate's layout), N = padding target,
 # K = eigenpairs per graph of a batch without them (sparse_collate(..., eigs=False)), else None
 SparseRecords = collections.namedtuple('SparseRecords', 'sizes node_ptr node_feat edge_ptr edges N K',
@@ -231,7 +239,11 @@ class SpectralNetBase(nn.Module):
     built on the device (lnb_graph_prepare_sparse and the model's own producers): the dense
     B x N x N x (E+1) tensor of the reference's collate never crosses PCIe.  Same scores as ``forward``
     on the collated batch, bit for bit.  Inference only (raises under autograd).  Returns score or
-    (score, loss)."""
+    (score, loss).
+
+    A packed batch (data.pack_sparse / data.PackedMolecules.batch: one uint8 blob, with or without
+    eigenpairs) is taken too: one copy of the blob, then lnb_records_unpack splits it into the records on
+    the device, inside the same captured graph, and the model runs exactly as on those records."""
     if self._check_mode():
       raise NotImplementedError('forward_sparse is an inference path; train through forward() or, from '
                                 'the same records, forward_sparse_train()')
@@ -265,6 +277,9 @@ class SpectralNetBase(nn.Module):
     if not hasattr(self, '_forward_records'):
       raise NotImplementedError('%s has no sparse-batch entry; call forward() on the collated batch'
                                 % type(self).__name__)
+    if 'blob' in batch:
+      blob, unpack, key = self._packed_records(batch)
+      return (blob,), lambda b_: self._forward_records(unpack(b_)), key
     N, B, E1 = self._check_sparse_batch(batch)
     self._check_runnable(N, E1)
     inputs = (batch['sizes'], batch['node_ptr'], Ragged(batch['node_feat'], B * N), batch['edge_ptr'],
@@ -293,6 +308,77 @@ class SpectralNetBase(nn.Module):
     if batch['edges'].dtype != torch.uint8 or batch['edges'].dim() != 2 or batch['edges'].shape[1] != 4:
       raise ValueError('forward_sparse: edges must be uint8 [E, 4]')
     return N, B, E1
+
+  PACKED_KEYS = ('blob', 'B', 'N', 'K')
+
+  def _check_packed_batch(self, batch):
+    """forward_sparse's checks of a packed batch (data.pack_sparse / data.PackedMolecules.batch), before any
+    device work: the keys, a flat uint8 blob, N and E+1 within the prepare kernel's limits, and the blob's
+    header -- magic, B and K against the batch's, the total size, node_ptr[B] <= B * N -- which also says
+    whether the blob carries eigenpairs.  A host blob is read in place.  A device blob is read with two
+    small synchronous copies unless the batch says ``eigs`` (pack_sparse and PackedMolecules.batch do):
+    then nothing is read on the host, ``eigs`` is trusted -- LanczosNet runs an eigenpair blob through
+    lnb_graph_prepare_sparse_packed, which reads the Ritz rows, so it must be right -- and the header is
+    checked by lnb_records_unpack on the device only; a batch that fails there gives the scores of empty
+    graphs.  Returns (B, N, K, eigs)."""
+    missing = [k for k in self.PACKED_KEYS if k not in batch]
+    if missing:
+      raise ValueError('forward_sparse: the packed batch lacks %s (data.pack_sparse)' % ', '.join(missing))
+    blob = batch['blob']
+    if not torch.is_tensor(blob) or blob.dtype != torch.uint8 or blob.dim() != 1 or blob.numel() < 64:
+      raise ValueError('forward_sparse: blob must be a flat uint8 tensor of at least 64 bytes')
+    B, N, K = int(batch['B']), int(batch['N']), int(batch['K'])
+    E1 = self.num_edgetype + 1
+    if not (1 <= N <= 128 and 2 <= E1 <= 16):
+      raise ValueError('forward_sparse: N=%d, E+1=%d outside 1 <= N <= 128, 2 <= E+1 <= 16' % (N, E1))
+    if B < 1 or K < 1:
+      raise ValueError('forward_sparse: packed batch with B=%d, K=%d' % (B, K))
+    eigs = batch.get('eigs')
+    if blob.is_cuda and eigs is not None:
+      return B, N, K, bool(eigs)
+    if blob.is_cuda and torch.cuda.is_current_stream_capturing():
+      raise ValueError("forward_sparse: a device blob under stream capture needs batch['eigs'] (its header "
+                       "cannot be read on the host there)")
+
+    def ints(lo, n):                         # a device blob: one small synchronous copy
+      return blob[lo:lo + 4 * n].cpu().view(torch.int32).tolist()
+
+    hdr = ints(0, 16)
+    if hdr[0] != data_mod.PACK_MAGIC:
+      raise ValueError('forward_sparse: blob magic %#x is not %#x (data.pack_sparse)' % (hdr[0] & 0xffffffff,
+                                                                                         data_mod.PACK_MAGIC))
+    if (hdr[1], hdr[2]) != (B, K):
+      raise ValueError('forward_sparse: blob header has B=%d, K=%d; the batch says B=%d, K=%d'
+                       % (hdr[1], hdr[2], B, K))
+    if not 64 <= hdr[10] <= blob.numel():
+      raise ValueError('forward_sparse: blob header total %d bytes outside [64, %d]' % (hdr[10], blob.numel()))
+    if not (64 <= hdr[4] and hdr[4] % 16 == 0 and hdr[4] + 4 * (B + 1) <= hdr[10]):
+      raise ValueError('forward_sparse: blob node_ptr offset %d outside the blob' % hdr[4])
+    rows = ints(hdr[4] + 4 * B, 1)[0]
+    if not 0 <= rows <= B * N:
+      raise ValueError('forward_sparse: node_ptr[B]=%d node rows outside [0, B*N = %d]' % (rows, B * N))
+    has = hdr[6] != 0 or hdr[8] != 0
+    if eigs is not None and bool(eigs) != has:
+      raise ValueError("forward_sparse: batch['eigs'] is %s, the blob %s eigenpairs"
+                       % (bool(eigs), 'carries' if has else 'has no'))
+    return B, N, K, has
+
+  def _packed_records(self, batch):
+    """(blob input, unpack, graph-cache key) of a packed batch for a model with a records entry: the blob
+    as ONE Ragged input whose capacity depends on (B, N, K) only, and ``unpack(device_blob)``, the
+    SparseRecords that lnb_records_unpack writes from it into fixed-capacity buffers (node rows B * N, the
+    bonds the blob's capacity can hold), so one captured graph serves every batch of the same shape."""
+    B, N, K, eigs = self._check_packed_batch(batch)
+    self._check_runnable(N, self.num_edgetype + 1)
+    blob = batch['blob']
+    return (Ragged(blob, packed_capacity(B, N, K, eigs, blob.shape[0])),
+            lambda b_: self._unpack_records(b_, B, N, K), ('packed_records', B, N, K))
+
+  def _unpack_records(self, blob, B, N, K):
+    """SparseRecords of a device blob (lnb_records_unpack; the eigenpairs, if any, stay in the blob).  The
+    bonds lie behind the offset where D starts, with or without eigenpairs: they fit in the bytes past it."""
+    cap_edges = (blob.shape[0] - data_mod.packed_offsets(B, K)[3]) // 4
+    return SparseRecords(*ops.records_unpack(blob, B, K, B * N, cap_edges)[:5], N=N)
 
   def _check_runnable(self, N=None, E1=None):
     """Model-specific checks of a call, run before any launch (N, E1: those of a sparse batch)."""
@@ -342,10 +428,13 @@ class SpectralNetBase(nn.Module):
     # Inputs already resident on this device: a graph bound to their addresses needs no copy at
     # all.  Such a graph is captured the second time the same buffers show up (data loaders /
     # serving loops that recycle a few device buffers); any live tensor found at a captured
-    # address with the captured shape and dtype is read correctly, so no reference is kept.
+    # address with the captured shape and dtype is read correctly, so no reference is kept.  The key
+    # holds a Ragged input's own row count too: the captured forward reads the tensor it was given,
+    # so a slice of another length at the same address is another graph.
     raw = [_raw(t) for t in inputs]
     if all(t is None or (t.is_cuda and t.device == dev and t.is_contiguous()) for t in raw):
-      pkey = key + tuple(None if t is None else t.data_ptr() for t in raw)
+      pkey = key + tuple(None if t is None else t.data_ptr() for t in raw) + tuple(
+          t.rows for t in inputs if isinstance(t, Ragged))
       zc = self.__dict__.setdefault('_graphs_resident', {})
       hit = zc.get(pkey)
       if hit is not None and hit['sig'] == sig:
@@ -581,10 +670,14 @@ class RitzRecords(object):
         raise NotImplementedError('%s takes data.sparse_collate records, not packed batches'
                                   % type(self).__name__)
       # a packed batch (data.pack_sparse) crosses PCIe as ONE copy of exactly the bytes present
-      B, N, K = int(batch['B']), int(batch['N']), int(batch['K'])
-      cap = data_mod.packed_offsets(B, K)[4] + 16 * 3 + 4 * B * N + 4 * B * N * K + 4 * B * N * 4
+      B, N, K, eigs = self._check_packed_batch(batch)
       blob = batch['blob']
-      return ((Ragged(blob, max(cap, int(blob.shape[0]))),),
+      if not eigs:
+        # without eigenpairs: records_unpack, then the path of records without them
+        return ((Ragged(blob, packed_capacity(B, N, K, False, blob.shape[0])),),
+                lambda b_: self._forward_sparse_eigs_impl(N, K, *self._unpack_records(b_, B, N, K)[:5]),
+                ('packed_eigs', B, N, K))
+      return ((Ragged(blob, packed_capacity(B, N, K, True, blob.shape[0])),),
               lambda b_: self._forward_packed_impl(B, N, K, b_), ('packed', B, N, K))
     if feat:
       self._check_ritz_records(batch)

@@ -23,7 +23,7 @@ checkpoints) adds one: under autograd its forward is ``train.gat_train``, whose 
 import torch
 import torch.nn as nn
 
-from ._common import SparseRecords, SpectralNetBase, init_linears, loss_function
+from ._common import SpectralNetBase, init_linears, loss_function
 from .. import ops
 
 __all__ = ['GAT', 'TrainableGAT', 'KeyedGAT']
@@ -212,8 +212,7 @@ class KeyedGAT(TrainableGAT):
     if dk is None:
       return inputs, impl, key
     ops.check_dropout_key('KeyedGAT', dk)
-    N = int(batch['N'])
-    return inputs + (dk,), lambda *a: self._forward_records(SparseRecords(*a[:5], N=N)), key
+    return inputs + (dk,), lambda *a: impl(*a[:-1]), key        # inference draws no mask: the key rides along
 
   def _train_records(self, recs, dropout_key=None):
     if not self._drops():

@@ -222,7 +222,9 @@ class LSTMGraphSAGE(GraphSAGE):
 class SampledGraphSAGE(LSTMGraphSAGE):
   """``LSTMGraphSAGE`` (same constructor, parameters, initialisation and ``state_dict``; the same padded
   ``forward``) that also runs and trains from the bond-list records of data.sparse_collate:
-  ``forward_sparse``, ``forward_sparse_train`` and ``train.GraphedStep(..., sparse=True)``.
+  ``forward_sparse``, ``forward_sparse_train`` and ``train.GraphedStep(..., sparse=True)``.  ``forward_sparse``
+  also takes packed batches (data.pack_sparse / data.PackedMolecules, with the same ``sample_key``): the same
+  scores as the records they pack.
 
   The records carry no neighbour samples: they are drawn on the device (``ops.sage_sample_sparse``) from
   the distributions of the reference's collate -- K distinct neighbours, or K with replacement when a node
@@ -251,7 +253,8 @@ class SampledGraphSAGE(LSTMGraphSAGE):
       raise ValueError("SampledGraphSAGE: 'sample_key' must be an int64 tensor of shape (2,); got %r"
                        % ((key.dtype, tuple(key.shape)) if torch.is_tensor(key) else type(key),))
     if 'blob' in batch:
-      raise NotImplementedError('SampledGraphSAGE takes data.sparse_collate records, not packed batches')
+      blob, unpack, pkey = self._packed_records(batch)
+      return (blob, key), lambda b_, k_: self._forward_records(unpack(b_), k_), pkey
     inputs, _, _ = super(SampledGraphSAGE, self)._sparse_inputs(batch)
     N = int(batch['N'])
     return (inputs + (key,), lambda *a: self._forward_records(SparseRecords(*a[:5], N=N), a[5]),

@@ -13,7 +13,8 @@ from ._lib import GemmDesc, SpectralStack
 
 __all__ = [
     'bgemm', 'split_tf32', 'linear_tf32x3', 'linear_tf32x3_grouped', 'graph_prepare', 'tile_assign', 'spectral_conv_fused',
-    'graph_prepare_sparse', 'graph_prepare_sparse_features', 'graph_prepare_sparse_packed', 'graph_eigs_sparse', 'sym_eigs',
+    'graph_prepare_sparse', 'graph_prepare_sparse_features', 'graph_prepare_sparse_packed', 'records_unpack',
+    'graph_eigs_sparse', 'sym_eigs',
     'spectral_partition', 'spectral_partition_sparse', 'spectral_partition_supported', 'partition_draws', 'gat_bias_sparse',
     'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
@@ -376,6 +377,37 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows = rowmap, nrows
   return prep, node_ids, mask, V, L
+
+
+def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False):
+  """A packed batch (data.pack_sparse / data.PackedMolecules: a 16-byte aligned uint8 CUDA buffer) split
+  into the records of data.sparse_collate by lnb_records_unpack, one launch whose segment offsets come from
+  the header on the device.  cap_rows / cap_edges: rows of node_feat / edges (at least node_ptr[B] /
+  edge_ptr[B]; rows past those stay unwritten).  eigs: also unpack D and V_rows (the batch must carry them).
+  A malformed header or an overflow is reported in ``status`` (see the C header), with every graph empty.
+  Returns (sizes [B], node_ptr [B+1], node_feat [cap_rows], edge_ptr [B+1], edges [cap_edges, 4], D [B, K]
+  or None, V_rows [cap_rows, K] or None, status [1] int32)."""
+  _need_cuda(blob)
+  if blob.dtype != torch.uint8 or blob.dim() != 1 or not blob.is_contiguous() or blob.numel() < 64:
+    raise ValueError('records_unpack: blob must be a contiguous 1-D uint8 tensor of >= 64 bytes')
+  if blob.data_ptr() % 16:
+    raise ValueError('records_unpack: blob must be 16-byte aligned')
+  B, K, cap_rows, cap_edges = int(B), int(K), int(cap_rows), int(cap_edges)
+  if B < 1 or K < 1 or cap_rows < 0 or cap_edges < 0:
+    raise ValueError('records_unpack: B=%d, K=%d, cap_rows=%d, cap_edges=%d' % (B, K, cap_rows, cap_edges))
+  dev = blob.device
+  i32 = dict(device=dev, dtype=torch.int32)
+  sizes, node_ptr, edge_ptr = torch.empty((B,), **i32), torch.empty((B + 1,), **i32), torch.empty((B + 1,), **i32)
+  node_feat = torch.empty((cap_rows,), **i32)
+  edges = torch.empty((cap_edges, 4), device=dev, dtype=torch.uint8)
+  D = torch.empty((B, K), device=dev, dtype=torch.float32) if eigs else None
+  V_rows = torch.empty((cap_rows, K), device=dev, dtype=torch.float32) if eigs else None
+  status = torch.empty((1,), **i32)
+  with torch.cuda.device(dev):
+    _lib.check(_lib.load().lnb_records_unpack(
+        _stream(blob), _ptr(blob), blob.numel(), B, K, cap_rows, cap_edges, _ptr(sizes), _ptr(node_ptr),
+        _ptr(node_feat), _ptr(edge_ptr), _ptr(edges), _ptr(D), _ptr(V_rows), _ptr(status)), 'lnb_records_unpack')
+  return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, status
 
 
 def graph_eigs_sparse(sizes, node_ptr, edge_ptr, edges, N, K, num_edgetype=32, rows=None):
