@@ -196,6 +196,10 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
  *   data.sparse_collate(..., eigs=False) records, data.PackedMolecules(..., eigs=False)): D and V_rows
  *   are absent, and so are the tiles and krow_ptr (without the Ritz rows the host cannot know k_eff).
  *   Such a batch is read through lnb_records_unpack, never by this kernel.
+ *   hdr[13] = off(label [B, P] f32), hdr[14] = P: the labels of a training batch (data.pack_sparse(...,
+ *   label=True), data.PackedMolecules(..., labels=True)), the last segment, behind the bonds; every other
+ *   offset is that of the same batch without labels, and hdr[10] counts the segment.  Both are 0 when the
+ *   batch carries no labels.  Only lnb_records_unpack_labels reads the segment.
  * The kernel derives its input pointers from the header on the device.  flags bit 1
  * (LNB_PACKED_HOST_TILES): the host knows every graph's extents, so it ships the tiles (the same
  * next-fit table and first-fit-decreasing schedule as lnb_graph_prepare, in the same layout) and the
@@ -226,6 +230,15 @@ int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_by
                        int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
                        int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
                        int32_t* status);
+
+/* lnb_records_unpack that also copies the label segment (hdr[13], hdr[14]) into label [B, P] (16-byte
+ * aligned), in the same launch.  A batch without the segment, with another P or with the segment outside
+ * [64, hdr[10]) adds status bit 64, with every graph empty and nothing copied, as the other failures do.
+ * lnb_records_unpack ignores a label segment. */
+int lnb_records_unpack_labels(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
+                              int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
+                              int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
+                              int32_t* status, int P, float* label);
 
 /* Float-feature variant (LanczosNetGeneral's GraphData records, node features instead of atom ids): the
  * same records and outputs as lnb_graph_prepare_sparse, except that node_x [node_ptr[B], F] fp32 holds the

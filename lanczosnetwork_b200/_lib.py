@@ -78,6 +78,8 @@ SIGNATURES = {
                                         [ctypes.c_void_p] * 11),
     'lnb_records_unpack': (c_int, [c_stream, ctypes.c_void_p, c_i64, c_int, c_int, c_i64, c_i64] +
                            [ctypes.c_void_p] * 8),
+    'lnb_records_unpack_labels': (c_int, [c_stream, ctypes.c_void_p, c_i64, c_int, c_int, c_i64, c_i64] +
+                                  [ctypes.c_void_p] * 8 + [c_int, ctypes.c_void_p]),
     'lnb_graph_prepare_sparse_features': (c_int, [c_stream] + [ctypes.c_void_p] * 7 + [c_int] * 6 +
                                           [ctypes.c_void_p] * 11),
     'lnb_spectral_conv_fused':

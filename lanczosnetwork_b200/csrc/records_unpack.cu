@@ -2,7 +2,8 @@
 // data.sparse_collate, on the device, in one launch (lnb_records_unpack).  The records producers
 // (lnb_graph_prepare_sparse, lnb_gat_bias_sparse, lnb_spectral_partition_sparse, lnb_sage_sample_sparse,
 // lnb_graph_eigs_sparse) then run unchanged behind it, so every drop-in with a records entry takes the
-// one-H2D-copy format at the cost of one D2D copy of the blob's bytes.
+// one-H2D-copy format at the cost of one D2D copy of the blob's bytes.  lnb_records_unpack_labels also
+// copies the label segment [B, P] of a training batch (the same launch, an eighth segment).
 //
 // The segment offsets change from batch to batch, so they are read here, on the device: one captured
 // graph serves every batch of a (B, N, K) whose rows fit the capacities.  Every block validates the
@@ -15,7 +16,7 @@
 namespace {
 
 constexpr int RU_THREADS = 256;
-constexpr int RU_SEGS = 7;          // sizes, node_ptr, edge_ptr, node_feat, edges, D, V_rows
+constexpr int RU_SEGS = 8;          // sizes, node_ptr, edge_ptr, node_feat, edges, D, V_rows, label
 constexpr int32_t RU_MAGIC = 0x4c4e4231;
 
 struct UnpackParams {
@@ -25,6 +26,7 @@ struct UnpackParams {
   int64_t cap_rows, cap_edges;
   int32_t* sizes; int32_t* node_ptr; int32_t* node_feat; int32_t* edge_ptr; uint8_t* edges;
   float* D; float* V_rows;
+  int P; float* label;                 // label [B, P] of lnb_records_unpack_labels, else 0 / NULL
   int32_t* status;
 };
 
@@ -66,14 +68,18 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
     if (!st && rows > P.cap_rows) st |= 8;
     if (!st && nedge > P.cap_edges) st |= 16;
     if (!st && !eigs && (P.D || P.V_rows)) st |= 32;
+    if (!st && P.label && (hdr[14] != P.P || !seg_ok(hdr[13], 4 * B * P.P, total))) st |= 64;
     s_status = st;
     if (!st) {
-      const int64_t src[RU_SEGS] = {hdr[3], hdr[4], hdr[5], hdr[7], hdr[9], hdr[6], hdr[8]};
+      // a label segment is read only when asked for: lnb_records_unpack ignores it
+      const int64_t src[RU_SEGS] = {hdr[3], hdr[4], hdr[5], hdr[7], hdr[9], hdr[6], hdr[8], P.label ? hdr[13] : 0};
       const int64_t bytes[RU_SEGS] = {4 * B, 4 * (B + 1), 4 * (B + 1), 4 * rows, 4 * nedge,
-                                      P.D ? 4 * B * K : 0, P.V_rows ? 4 * rows * K : 0};
+                                      P.D ? 4 * B * K : 0, P.V_rows ? 4 * rows * K : 0,
+                                      P.label ? 4 * B * P.P : 0};
       uint8_t* dst[RU_SEGS] = {reinterpret_cast<uint8_t*>(P.sizes), reinterpret_cast<uint8_t*>(P.node_ptr),
                                reinterpret_cast<uint8_t*>(P.edge_ptr), reinterpret_cast<uint8_t*>(P.node_feat),
-                               P.edges, reinterpret_cast<uint8_t*>(P.D), reinterpret_cast<uint8_t*>(P.V_rows)};
+                               P.edges, reinterpret_cast<uint8_t*>(P.D), reinterpret_cast<uint8_t*>(P.V_rows),
+                               reinterpret_cast<uint8_t*>(P.label)};
       // every segment is a whole number of 4-byte words: 16-byte vectors, then up to three words
       s_units[0] = 0;
       for (int s = 0; s < RU_SEGS; ++s) {
@@ -112,30 +118,26 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
   }
 }
 
-}  // namespace
-
-extern "C" {
-
-int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
-                       int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
-                       int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
-                       int32_t* status) {
+int launch_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K, int64_t cap_rows,
+                  int64_t cap_edges, int32_t* sizes, int32_t* node_ptr, int32_t* node_feat, int32_t* edge_ptr,
+                  uint8_t* edges, float* D, float* V_rows, int P, float* label, int32_t* status) {
   LNB_REQUIRE(B >= 1 && K >= 1 && cap_rows >= 0 && cap_edges >= 0 && blob_bytes >= 64,
               "records_unpack: bad dims B=%d K=%d cap_rows=%lld cap_edges=%lld blob_bytes=%lld", B, K,
               (long long)cap_rows, (long long)cap_edges, (long long)blob_bytes);
   LNB_REQUIRE(blob && sizes && node_ptr && edge_ptr && status && (node_feat || cap_rows == 0) &&
                   (edges || cap_edges == 0),
               "records_unpack: null pointer");
-  const void* ptrs[] = {blob, sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows};
+  const void* ptrs[] = {blob, sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, label};
   for (const void* p : ptrs)
     LNB_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, "records_unpack: buffers must be 16-byte aligned");
   UnpackParams p;
   p.blob = blob; p.blob_bytes = blob_bytes; p.B = B; p.K = K; p.cap_rows = cap_rows; p.cap_edges = cap_edges;
   p.sizes = sizes; p.node_ptr = node_ptr; p.node_feat = node_feat; p.edge_ptr = edge_ptr; p.edges = edges;
-  p.D = D; p.V_rows = V_rows; p.status = status;
+  p.D = D; p.V_rows = V_rows; p.P = P; p.label = label; p.status = status;
   // the grid depends on the capacities only (a captured launch serves every batch that fits them)
   const int64_t max_bytes = 12 * (int64_t)B + 8 + 4 * cap_rows + 4 * cap_edges +
-                            (D ? 4 * (int64_t)B * K : 0) + (V_rows ? 4 * cap_rows * K : 0);
+                            (D ? 4 * (int64_t)B * K : 0) + (V_rows ? 4 * cap_rows * K : 0) +
+                            (label ? 4 * (int64_t)B * P : 0);
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -144,6 +146,27 @@ int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_by
   records_unpack_kernel<<<grid, RU_THREADS, 0, (cudaStream_t)stream>>>(p);
   lnb::count_launch();
   return lnb::finish_launch("records_unpack");
+}
+
+}  // namespace
+
+extern "C" {
+
+int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
+                       int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
+                       int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
+                       int32_t* status) {
+  return launch_unpack(stream, blob, blob_bytes, B, K, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr,
+                       edges, D, V_rows, 0, nullptr, status);
+}
+
+int lnb_records_unpack_labels(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
+                              int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
+                              int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
+                              int32_t* status, int P, float* label) {
+  LNB_REQUIRE(P >= 1 && label, "records_unpack_labels: P=%d, label %p", P, (const void*)label);
+  return launch_unpack(stream, blob, blob_bytes, B, K, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr,
+                       edges, D, V_rows, P, label, status);
 }
 
 }  // extern "C"

@@ -397,14 +397,18 @@ def ritz_extents(V_rows, node_ptr):
   return np.where(any_col.any(axis=1), last, 0).astype(np.int64)
 
 
-def pack_sparse(sp):
+def pack_sparse(sp, label=False):
   """A ``sparse_collate`` batch as ONE contiguous uint8 buffer (layout: include/lanczosnet_b200.h,
   lnb_graph_prepare_sparse_packed): a 16-int header with the byte offsets of the segments, the
   fixed-size segments (sizes, node_ptr, edge_ptr, D), then node ids, Ritz rows and the bond list.
   One H2D copy per step ships the whole batch.  Records without eigenpairs (``sparse_collate(...,
   eigs=False)``) give a blob without D, Ritz rows, tiles and Ritz-row offsets (their header offsets are 0):
-  the node ids start where D would.  Returns dict(blob, B, N, K, num_edgetype, eigs[, label])."""
+  the node ids start where D would.  ``label=True``: the records' labels [B, P] float32 follow the bonds as
+  one more segment (hdr[13], hdr[14]), for training from the blob (train.GraphedStep(..., packed=True));
+  every other byte is that of the blob without them.  Returns dict(blob, B, N, K, num_edgetype, eigs[, label])."""
   eigs = 'D' in sp
+  if label and 'label' not in sp:
+    raise ValueError('pack_sparse: label=True needs records with labels (samples with a label)')
   B, K = sp['D'].shape if eigs else (len(sp['sizes']), int(sp['K']))
   off_sizes, off_node_ptr, off_edge_ptr, off_D, off, off_tiles, off_krow = packed_offsets(B, K)
   segs = [(off_sizes, sp['sizes']), (off_node_ptr, sp['node_ptr']), (off_edge_ptr, sp['edge_ptr'])]
@@ -422,10 +426,17 @@ def pack_sparse(sp):
     off_nf, off_D, off_v, off_tiles, off_krow = off_D, 0, 0, 0, 0
     off_e = off_nf + _align16(sp['node_feat'].nbytes)
   total = off_e + _align16(sp['edges'].nbytes)
+  if label:
+    lab = np.ascontiguousarray(sp['label'], np.float32).reshape(B, -1)
+    off_l, P = total, lab.shape[1]
+    total = off_l + _align16(lab.nbytes)
+    segs.append((off_l, lab))
   blob = np.zeros(total, np.uint8)
   hdr = blob[:64].view(np.int32)
   hdr[:13] = [PACK_MAGIC, B, K, off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_v, off_e, total,
               off_tiles, off_krow]
+  if label:
+    hdr[13:15] = [off_l, P]
   for off_, arr in segs + [(off_nf, sp['node_feat']), (off_e, sp['edges'])]:
     raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
     blob[off_:off_ + raw.size] = raw
@@ -447,12 +458,18 @@ class PackedMolecules(object):
 
   ``eigs=False`` takes ``prepare_graph(..., eigs=False)`` samples (or ignores the eigenpairs of any
   others): the blobs are those of ``pack_sparse(sparse_collate(..., eigs=False))``, 4 bytes per node instead
-  of 4 (K + 1), and the device computes the eigenpairs where a model reads them."""
+  of 4 (K + 1), and the device computes the eigenpairs where a model reads them.
 
-  def __init__(self, samples, num_eigs, eigs=True):
+  ``labels=True`` writes each batch's labels into the blob, as ``pack_sparse(..., label=True)`` does: the
+  batches train.GraphedStep(..., packed=True) trains from."""
+
+  def __init__(self, samples, num_eigs, eigs=True, labels=False):
     sp = sparse_collate(samples, num_eigs, eigs=eigs)
+    if labels and 'label' not in sp:
+      raise ValueError('PackedMolecules: labels=True needs samples with a label')
     self.K = int(num_eigs)
     self.eigs = bool(eigs)
+    self.labels = bool(labels)
     self.num_edgetype = sp['num_edgetype']
     self.sizes, self.node_ptr, self.edge_ptr = sp['sizes'], sp['node_ptr'].astype(np.int64), sp['edge_ptr'].astype(np.int64)
     self.node_feat, self.edges, self.V_rows, self.D = sp['node_feat'], sp['edges'], sp.get('V_rows'), sp.get('D')
@@ -476,9 +493,10 @@ class PackedMolecules(object):
     buffer): an index list may repeat the largest molecule B times."""
     n = B * int(self.sizes.max())
     e = B * int(np.diff(self.edge_ptr).max())
+    lab = _align16(4 * B * self.label.shape[1]) if self.labels else 0
     if not self.eigs:
-      return packed_offsets(B, self.K)[3] + _align16(4 * n) + _align16(4 * e)
-    return packed_offsets(B, self.K)[4] + _align16(4 * n) + _align16(4 * n * self.K) + _align16(4 * e)
+      return packed_offsets(B, self.K)[3] + _align16(4 * n) + _align16(4 * e) + lab
+    return packed_offsets(B, self.K)[4] + _align16(4 * n) + _align16(4 * n * self.K) + _align16(4 * e) + lab
 
   def batch(self, idx, out=None):
     """Packed batch of the molecules ``idx`` (order kept).  ``out``: optional uint8 buffer (e.g. the numpy
@@ -501,7 +519,10 @@ class PackedMolecules(object):
     else:                                            # pack_sparse's layout without eigenpairs
       off_nf, off_D, off_v, off_tiles, off_krow = off_D, 0, 0, 0, 0
       off_e = off_nf + _align16(4 * len(rows))
-    total = off_e + _align16(4 * len(erow))
+    off_l = total = off_e + _align16(4 * len(erow))
+    if self.labels:
+      P = self.label.shape[1]
+      total = off_l + _align16(4 * B * P)
     if out is None:
       blob = np.zeros(total, np.uint8)
     else:
@@ -511,10 +532,14 @@ class PackedMolecules(object):
       blob[:off_nf] = 0                              # header + fixed segments (alignment gaps stay zero)
       gaps = ((off_nf + 4 * len(rows), off_v), (off_v + 4 * len(rows) * K, off_e)) if self.eigs else \
           ((off_nf + 4 * len(rows), off_e),)
-      for a, b in gaps + ((off_e + 4 * len(erow), total),):
+      tail = (((off_e + 4 * len(erow), off_l), (off_l + 4 * B * P, total)) if self.labels else
+              ((off_e + 4 * len(erow), total),))
+      for a, b in gaps + tail:
         blob[a:b] = 0
     blob[:64].view(np.int32)[:13] = [PACK_MAGIC, B, K, off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_v,
                                      off_e, total, off_tiles, off_krow]
+    if self.labels:
+      blob[:64].view(np.int32)[13:15] = [off_l, P]
 
     def put(off, arr):
       raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
@@ -533,6 +558,8 @@ class PackedMolecules(object):
     put(off_edge_ptr, edge_ptr)
     np.take(self.node_feat, rows, out=blob[off_nf:off_nf + 4 * len(rows)].view(np.int32))
     np.take(self.edges, erow, axis=0, out=blob[off_e:off_e + 4 * len(erow)].reshape(len(erow), 4))
+    if self.labels:
+      np.take(self.label, idx, axis=0, out=blob[off_l:off_l + 4 * B * P].view(np.float32).reshape(B, P))
     res = {'blob': blob, 'B': int(B), 'N': int(sizes.max()) if B else 0, 'K': K, 'num_edgetype': self.num_edgetype,
            'eigs': self.eigs}
     if self.label is not None:

@@ -43,11 +43,14 @@ def _raw(t):
   return t.tensor if isinstance(t, Ragged) else t
 
 
-def packed_capacity(B, N, K, eigs, nbytes):
+def packed_capacity(B, N, K, eigs, nbytes, label_dim=0):
   """Static size of a packed batch's blob under graph replay: the blob of any B molecules of at most N
-  nodes and 4 N bonds each (alignment gaps included), or the blob's own ``nbytes`` when that is larger."""
+  nodes and 4 N bonds each (alignment gaps included), or the blob's own ``nbytes`` when that is larger.
+  ``label_dim`` = P > 0 counts a label segment [B, P] float32 (data.pack_sparse(..., label=True))."""
   off = data_mod.packed_offsets(B, K)
   body = off[4] + 4 * B * N * K if eigs else off[3]
+  if label_dim:
+    body += data_mod._align16(4 * B * int(label_dim))
   return max(body + 16 * 3 + 4 * B * N + 4 * B * N * 4, int(nbytes))
 
 
@@ -373,6 +376,43 @@ class SpectralNetBase(nn.Module):
     blob = batch['blob']
     return (Ragged(blob, packed_capacity(B, N, K, eigs, blob.shape[0])),
             lambda b_: self._unpack_records(b_, B, N, K), ('packed_records', B, N, K))
+
+  def _takes_packed_training(self):
+    """True when ``train.GraphedStep(..., packed=True)`` trains this model: it has a training entry from records
+    and its ``forward_sparse`` takes packed batches."""
+    return hasattr(self, '_train_records') and hasattr(self, '_forward_records')
+
+  def _check_packed_train(self, batch):
+    """GraphedStep(packed=True)'s checks of a labelled packed batch, before any copy: those of
+    ``forward_sparse`` with the header always read (a device blob with a small synchronous copy, even when the
+    batch says ``eigs``: a training step must never run on a batch the device would refuse), and a label
+    segment inside the blob.  Returns (B, N, K, eigs, P, total bytes)."""
+    B, N, K, eigs = self._check_packed_batch({k: v for k, v in batch.items() if k != 'eigs'})
+    if 'eigs' in batch and bool(batch['eigs']) != eigs:
+      raise ValueError("GraphedStep: batch['eigs'] is %s, the blob %s eigenpairs"
+                       % (bool(batch['eigs']), 'carries' if eigs else 'has no'))
+    hdr = batch['blob'][:64].cpu().view(torch.int32).tolist()
+    total, off, P = hdr[10], hdr[13], hdr[14]
+    if P < 1 or off < 64 or off % 16 or off + 4 * B * P > total:
+      raise ValueError('GraphedStep: the packed batch carries no labels (label offset %d, P=%d): build it with '
+                       'data.pack_sparse(..., label=True) or data.PackedMolecules(..., labels=True)' % (off, P))
+    return B, N, K, eigs, P, total
+
+  def _train_packed(self, batch, P):
+    """The training forward of a device blob with labels (the static batch of GraphedStep(packed=True)):
+    lnb_records_unpack_labels into fixed-capacity records, then ``_train_records`` with whatever key the batch
+    carries after the blob, as ``forward_sparse_train`` passes it.  Returns (score, label [B, P], status)."""
+    inputs, _, _ = self._sparse_inputs(batch)
+    B, N, K = int(batch['B']), int(batch['N']), int(batch['K'])
+    recs, _, _, label, status = self._unpack_labelled(batch['blob'], B, N, K, P)
+    return self._train_records(recs, *[_raw(t) for t in inputs[1:]]), label, status
+
+  def _unpack_labelled(self, blob, B, N, K, P, eigs=False):
+    """lnb_records_unpack_labels of a device blob: (SparseRecords, D, V_rows, label [B, P], status), D and
+    V_rows None without ``eigs``.  Capacities as in ``_unpack_records``."""
+    cap_edges = (blob.shape[0] - data_mod.packed_offsets(B, K)[3]) // 4
+    out = ops.records_unpack(blob, B, K, B * N, cap_edges, eigs=eigs, label_dim=P)
+    return (SparseRecords(*out[:5], N=N, K=K),) + tuple(out[5:])
 
   def _unpack_records(self, blob, B, N, K):
     """SparseRecords of a device blob (lnb_records_unpack; the eigenpairs, if any, stay in the blob).  The
@@ -706,6 +746,16 @@ class RitzRecords(object):
         tuple(D.shape) != (B, V_rows.shape[1])):
       raise ValueError('forward_sparse: V_rows must be float32 [rows, K] and D float32 [B, K]; got %s %s and %s %s'
                        % (V_rows.dtype, tuple(V_rows.shape), D.dtype, tuple(D.shape)))
+
+  def _takes_packed_training(self):
+    return not self._feature_records            # float feature rows have no packed layout
+
+  def _train_packed(self, batch, P):
+    """A labelled blob with eigenpairs trains on its D and V_rows; one without gets them from
+    lnb_graph_eigs_sparse, as records without them do."""
+    recs, D, V_rows, label, status = self._unpack_labelled(batch['blob'], int(batch['B']), int(batch['N']),
+                                                           int(batch['K']), P, eigs=bool(batch['eigs']))
+    return self._train_records(recs, V_rows, D), label, status
 
   def _prepare_ritz_records(self, sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N, **kw):
     """(GraphPrep, node ids or padded features X, mask, V, L or None) of the records."""

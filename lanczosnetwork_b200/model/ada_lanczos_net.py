@@ -172,6 +172,9 @@ class KeyedAdaLanczosNet(AdaLanczosNet):
     return (inputs + (key,), lambda *a: self._forward_records(SparseRecords(*a[:5], N=N), a[5]),
             ('keyed', N))
 
+  def _takes_packed_training(self):
+    return False                                   # packed batches are refused (_sparse_inputs)
+
   def _records_inputs(self, recs, key):
     """node ids, dense operators and mask of the records (lnb_graph_prepare_sparse: the unfused conv
     layers read the dense L) and the start vector of ``key``."""

@@ -379,22 +379,27 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
   return prep, node_ids, mask, V, L
 
 
-def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False):
+def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False, label_dim=0):
   """A packed batch (data.pack_sparse / data.PackedMolecules: a 16-byte aligned uint8 CUDA buffer) split
   into the records of data.sparse_collate by lnb_records_unpack, one launch whose segment offsets come from
   the header on the device.  cap_rows / cap_edges: rows of node_feat / edges (at least node_ptr[B] /
   edge_ptr[B]; rows past those stay unwritten).  eigs: also unpack D and V_rows (the batch must carry them).
   A malformed header or an overflow is reported in ``status`` (see the C header), with every graph empty.
   Returns (sizes [B], node_ptr [B+1], node_feat [cap_rows], edge_ptr [B+1], edges [cap_edges, 4], D [B, K]
-  or None, V_rows [cap_rows, K] or None, status [1] int32)."""
+  or None, V_rows [cap_rows, K] or None, status [1] int32).
+
+  ``label_dim`` = P > 0: also unpack the batch's labels (data.pack_sparse(..., label=True)) through
+  lnb_records_unpack_labels, in the same launch; a batch without them, or with another P, sets status bit 64.
+  Returns (sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, label [B, P] float32, status)."""
   _need_cuda(blob)
   if blob.dtype != torch.uint8 or blob.dim() != 1 or not blob.is_contiguous() or blob.numel() < 64:
     raise ValueError('records_unpack: blob must be a contiguous 1-D uint8 tensor of >= 64 bytes')
   if blob.data_ptr() % 16:
     raise ValueError('records_unpack: blob must be 16-byte aligned')
-  B, K, cap_rows, cap_edges = int(B), int(K), int(cap_rows), int(cap_edges)
-  if B < 1 or K < 1 or cap_rows < 0 or cap_edges < 0:
-    raise ValueError('records_unpack: B=%d, K=%d, cap_rows=%d, cap_edges=%d' % (B, K, cap_rows, cap_edges))
+  B, K, cap_rows, cap_edges, P = int(B), int(K), int(cap_rows), int(cap_edges), int(label_dim)
+  if B < 1 or K < 1 or cap_rows < 0 or cap_edges < 0 or P < 0:
+    raise ValueError('records_unpack: B=%d, K=%d, cap_rows=%d, cap_edges=%d, label_dim=%d'
+                     % (B, K, cap_rows, cap_edges, P))
   dev = blob.device
   i32 = dict(device=dev, dtype=torch.int32)
   sizes, node_ptr, edge_ptr = torch.empty((B,), **i32), torch.empty((B + 1,), **i32), torch.empty((B + 1,), **i32)
@@ -403,11 +408,16 @@ def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False):
   D = torch.empty((B, K), device=dev, dtype=torch.float32) if eigs else None
   V_rows = torch.empty((cap_rows, K), device=dev, dtype=torch.float32) if eigs else None
   status = torch.empty((1,), **i32)
+  args = (_stream(blob), _ptr(blob), blob.numel(), B, K, cap_rows, cap_edges, _ptr(sizes), _ptr(node_ptr),
+          _ptr(node_feat), _ptr(edge_ptr), _ptr(edges), _ptr(D), _ptr(V_rows), _ptr(status))
+  if not P:
+    with torch.cuda.device(dev):
+      _lib.check(_lib.load().lnb_records_unpack(*args), 'lnb_records_unpack')
+    return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, status
+  label = torch.empty((B, P), device=dev, dtype=torch.float32)
   with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_records_unpack(
-        _stream(blob), _ptr(blob), blob.numel(), B, K, cap_rows, cap_edges, _ptr(sizes), _ptr(node_ptr),
-        _ptr(node_feat), _ptr(edge_ptr), _ptr(edges), _ptr(D), _ptr(V_rows), _ptr(status)), 'lnb_records_unpack')
-  return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, status
+    _lib.check(_lib.load().lnb_records_unpack_labels(*args, P, _ptr(label)), 'lnb_records_unpack_labels')
+  return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, label, status
 
 
 def graph_eigs_sparse(sizes, node_ptr, edge_ptr, edges, N, K, num_edgetype=32, rows=None):

@@ -1064,13 +1064,39 @@ class GraphedStep:
   the object does not advance training.  Not for AdaLanczosNet (its start vector is drawn on the
   host each call); KeyedAdaLanczosNet draws it on the device and is captured like the others."""
 
-  def __init__(self, model, optimizer, args, kwargs=None, warmup=3, sparse=False, edge_capacity=None):
+  def __init__(self, model, optimizer, args, kwargs=None, warmup=3, sparse=False, edge_capacity=None,
+               packed=False):
     """``sparse=True``: ``args`` is ``(batch,)``, the records of data.sparse_collate as torch tensors, and the
     step is ``model.forward_sparse_train(batch, label=label)``.  ``node_feat`` gets a static buffer of B*N
     rows, ``edges`` one of ``edge_capacity`` rows (default: the ``Ragged`` bucket of the first batch), and a
-    replay copies only the rows present, so one capture serves every batch with the same B, N and K."""
+    replay copies only the rows present, so one capture serves every batch with the same B, N and K.
+
+    ``packed=True``: ``args`` is ``(batch,)``, a packed batch WITH its labels (data.pack_sparse(...,
+    label=True), data.PackedMolecules(..., labels=True)), and no ``label=`` is passed.  Each call is one copy
+    of the blob's own bytes into a static blob of ``packed_capacity`` bytes, then the replay: the blob is
+    split on the device (lnb_records_unpack_labels) and the model's training entry from records runs on it,
+    with ``model.loss_func`` on the unpacked labels.  One capture serves every batch with the same (B, N, K,
+    P, eigs).  Keys (``sample_key``, ``dropout_key``) travel beside the blob, as in ``sparse=True``.  For GCN,
+    GCNFP, DCNN, ChebyNet, TrainableGAT, KeyedGAT, GGNN, MPNN, GPNN, SampledGraphSAGE and LanczosNet (blobs
+    with or without eigenpairs).  Every call checks the header on the host before copying (a pinned blob in
+    place, a device blob with a small synchronous copy) and raises ValueError, leaving parameters and optimizer
+    state untouched, rather than step on a batch the device would refuse.  ``step.status`` is the unpack's
+    status (device int32 [1], 0 = copied).  ``step.input_consumed`` is a new CUDA event per call, recorded
+    after that call's copy: a loader refills the host buffer it passed only once that event has completed
+    (with two pinned buffers, keep each call's event beside its buffer)."""
     kwargs = dict(kwargs or {})
-    if sparse:
+    if packed:
+      if sparse:
+        raise ValueError('GraphedStep: sparse=True and packed=True exclude each other')
+      takes = getattr(model, '_takes_packed_training', None)
+      if takes is None or not takes():
+        raise TypeError('GraphedStep(packed=True) trains GCN, GCNFP, DCNN, ChebyNet, TrainableGAT, KeyedGAT, GGNN, '
+                        'MPNN, GPNN, SampledGraphSAGE and LanczosNet from packed batches; %s is not among them'
+                        % type(model).__name__)
+      self._check_packed_args(args, kwargs)
+      shape = model._check_packed_train(args[0])
+      model._sparse_inputs(args[0])                          # the model's own checks (its keys)
+    elif sparse:
       if not hasattr(model, '_train_records'):
         raise TypeError('GraphedStep(sparse=True) needs a drop-in module with forward_sparse_train; %s has none'
                         % type(model).__name__)
@@ -1079,7 +1105,7 @@ class GraphedStep:
       model._sparse_inputs(args[0])                          # forward_sparse's batch checks
     elif not hasattr(type(model), '_train_impl') or type(model).__name__ == 'AdaLanczosNet':
       raise TypeError('GraphedStep needs a drop-in module with a host-free training forward')
-    if kwargs.get('label') is None:
+    if not packed and kwargs.get('label') is None:
       raise ValueError('GraphedStep captures the loss: pass label=')
     if sparse:
       from .model._common import Ragged
@@ -1089,8 +1115,11 @@ class GraphedStep:
     if dev.type != 'cuda':
       raise RuntimeError('GraphedStep needs the module on a CUDA device')
     model.train()
-    self.model, self.optimizer, self.sparse = model, optimizer, bool(sparse)
-    if sparse:
+    self.model, self.optimizer, self.sparse, self.packed = model, optimizer, bool(sparse), bool(packed)
+    if packed:
+      self._args = [self._static_packed(args[0], dev, shape)]
+      self.input_consumed = None
+    elif sparse:
       self._args = [self._static_records(args[0], dev, cap)]
     else:
       self._args = [self._static(a, dev) for a in args]
@@ -1179,10 +1208,61 @@ class GraphedStep:
       if torch.is_tensor(dst):
         dst.copy_(kwargs[k], non_blocking=True)
 
+  _PACKED_KEYS = ('sample_key', 'dropout_key')
+
+  @staticmethod
+  def _check_packed_args(args, kwargs):
+    if len(args) != 1 or not isinstance(args[0], dict) or 'blob' not in args[0]:
+      raise ValueError('GraphedStep(packed=True) takes one argument: the packed batch (batch,) of '
+                       'data.pack_sparse(..., label=True) or data.PackedMolecules(..., labels=True)')
+    if kwargs:
+      raise ValueError('GraphedStep(packed=True): the labels travel in the blob; got %s=' % ', '.join(sorted(kwargs)))
+
+  def _static_packed(self, batch, dev, shape):
+    B, N, K, eigs, P, total = shape
+    from .model._common import packed_capacity
+    self._packed_shape = (B, N, K, eigs, P)
+    blob = torch.zeros(packed_capacity(B, N, K, eigs, total, label_dim=P), dtype=torch.uint8, device=dev)
+    blob[:total].copy_(batch['blob'][:total])
+    out = {'blob': blob, 'B': B, 'N': N, 'K': K, 'eigs': eigs}
+    for k in self._PACKED_KEYS:
+      if k in batch:
+        out[k] = self._static(batch[k], dev)
+    return out
+
+  def _copy_packed(self, args, kwargs):
+    """Checks a packed batch on the host against the captured one -- ValueError before anything is copied --
+    then copies the blob's own bytes and the keys, and records ``input_consumed`` behind the copy."""
+    self._check_packed_args(args, kwargs)
+    batch, static = args[0], self._args[0]
+    B, N, K, eigs, P, total = self.model._check_packed_train(batch)
+    if (B, N, K, eigs, P) != self._packed_shape:
+      raise ValueError('GraphedStep was captured for packed batches of (B, N, K, eigs, P) = %s, got %s'
+                       % (self._packed_shape, (B, N, K, eigs, P)))
+    if total > static['blob'].numel():
+      raise ValueError('GraphedStep: a blob of %d bytes exceeds the captured capacity of %d bytes'
+                       % (total, static['blob'].numel()))
+    keys = [k for k in self._PACKED_KEYS if k in batch]
+    if set(keys) != set(k for k in self._PACKED_KEYS if k in static):
+      raise ValueError('GraphedStep was captured for a packed batch with keys %s, got %s'
+                       % (sorted(k for k in self._PACKED_KEYS if k in static), sorted(keys)))
+    for k in keys:
+      src = batch[k]
+      if not torch.is_tensor(src) or tuple(src.shape) != tuple(static[k].shape) or src.dtype != static[k].dtype:
+        raise ValueError('GraphedStep was captured for %s %s %s' % (k, tuple(static[k].shape), static[k].dtype))
+    static['blob'][:total].copy_(batch['blob'][:total], non_blocking=True)
+    for k in keys:
+      static[k].copy_(batch[k], non_blocking=True)
+    self.input_consumed = torch.cuda.Event()               # this call's own: a loader keeps one per buffer
+    self.input_consumed.record()
+
   def _body(self, zero=True):
     if zero:
       self.optimizer.zero_grad(set_to_none=True)
-    if self.sparse:
+    if self.packed:
+      score, label, self.status = self.model._train_packed(self._args[0], self._packed_shape[4])
+      score, loss = self.model._finish(score, label)
+    elif self.sparse:
       score, loss = self.model.forward_sparse_train(self._args[0], **self._kwargs)
     else:
       score, loss = self.model(*self._args, **self._kwargs)
@@ -1193,8 +1273,11 @@ class GraphedStep:
   def __call__(self, *args, **kwargs):
     """Copy this batch into the captured buffers and replay.  Returns (score, loss): static device
     tensors that the next call overwrites."""
-    if self.sparse:
-      self._copy_records(args[0], kwargs)
+    if self.packed or self.sparse:
+      if self.packed:
+        self._copy_packed(args, kwargs)
+      else:
+        self._copy_records(args[0], kwargs)
       self.graph.replay()
       self.replays += 1
       return self.score, self.loss
