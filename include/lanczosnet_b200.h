@@ -183,24 +183,36 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
 
 /* Packed variant: the whole sparse batch in ONE contiguous, 16-byte aligned device buffer, so a step
  * costs a single H2D copy of exactly the bytes present (eight ranks issuing seven small copies each
- * were host-bound).  Layout, all offsets in bytes and multiples of 16, int32 header first:
- *   hdr[0] = 0x4c4e4231 ("LNB1"), hdr[1] = B, hdr[2] = K, hdr[3] = off(sizes [B] i32),
- *   hdr[4] = off(node_ptr [B+1] i32), hdr[5] = off(edge_ptr [B+1] i32), hdr[6] = off(D [B,K] f32),
- *   hdr[7] = off(node_feat [sum n] i32), hdr[8] = off(V_rows [sum n, K] f32),
- *   hdr[9] = off(edges [sum E][4] u8), hdr[10] = total bytes,
- *   hdr[11] = off(tiles [3B+4] i32: the next-fit table [B+2], then the tile schedule [2B+2]),
- *   hdr[12] = off(krow_ptr [B+1] i32) (both 0 when absent); hdr[3..6], hdr[11], hdr[12] depend on (B, K)
- *   only, so D and the tiles sit at fixed addresses of a reused buffer (lnb_ritz_power_table and
- *   lnb_spectral_stack_forward read them there).
- *   hdr[6] and hdr[8] are 0 when the batch carries no eigenpairs (data.pack_sparse of
- *   data.sparse_collate(..., eigs=False) records, data.PackedMolecules(..., eigs=False)): D and V_rows
- *   are absent, and so are the tiles and krow_ptr (without the Ritz rows the host cannot know k_eff).
- *   Such a batch is read through lnb_records_unpack, never by this kernel.
- *   hdr[13] = off(label [B, P] f32), hdr[14] = P: the labels of a training batch (data.pack_sparse(...,
- *   label=True), data.PackedMolecules(..., labels=True)), the last segment, behind the bonds; every other
- *   offset is that of the same batch without labels, and hdr[10] counts the segment.  Both are 0 when the
- *   batch carries no labels.  Only lnb_records_unpack_labels reads the segment.
- * The kernel derives its input pointers from the header on the device.  flags bit 1
+ * were host-bound).  Layout: an int32 header hdr[16] of LNB_PACK_HDR_BYTES, its slots named below (the
+ * rest 0), then the body [LNB_PACK_HDR_BYTES, TOTAL): the segments, at byte offsets that are multiples of
+ * 16.  SIZES, NODE_PTR, EDGE_PTR, D,
+ * TILES and KROW depend on (B, K) only, so D and the tiles sit at fixed addresses of a reused buffer
+ * (lnb_ritz_power_table and lnb_spectral_stack_forward read them there).
+ * D, V_ROWS, TILES and KROW are 0 when the batch carries no eigenpairs (data.pack_sparse of
+ * data.sparse_collate(..., eigs=False) records, data.PackedMolecules(..., eigs=False)): without the Ritz
+ * rows the host cannot know k_eff.  Such a batch is read through lnb_records_unpack, never by this kernel.
+ * LABEL and P: the labels of a training batch (data.pack_sparse(..., label=True),
+ * data.PackedMolecules(..., labels=True)), the last segment, behind the bonds; every other offset is that
+ * of the same batch without labels, and TOTAL counts the segment.  Both are 0 when the batch carries no
+ * labels.  Only lnb_records_unpack_labels reads the segment. */
+#define LNB_PACK_MAGIC 0x4c4e4231   /* "LNB1" */
+#define LNB_PACK_HDR_BYTES 64
+#define LNB_PACK_HDR_MAGIC 0        /* LNB_PACK_MAGIC */
+#define LNB_PACK_HDR_B 1
+#define LNB_PACK_HDR_K 2
+#define LNB_PACK_HDR_SIZES 3        /* offset of sizes [B] i32 */
+#define LNB_PACK_HDR_NODE_PTR 4     /* offset of node_ptr [B+1] i32 */
+#define LNB_PACK_HDR_EDGE_PTR 5     /* offset of edge_ptr [B+1] i32 */
+#define LNB_PACK_HDR_D 6            /* offset of D [B,K] f32 */
+#define LNB_PACK_HDR_NODE_FEAT 7    /* offset of node_feat [sum n] i32 */
+#define LNB_PACK_HDR_V_ROWS 8       /* offset of V_rows [sum n, K] f32 */
+#define LNB_PACK_HDR_EDGES 9        /* offset of edges [sum E][4] u8 */
+#define LNB_PACK_HDR_TOTAL 10       /* total bytes */
+#define LNB_PACK_HDR_TILES 11       /* offset of tiles [3B+4] i32: next-fit table [B+2], tile schedule [2B+2] */
+#define LNB_PACK_HDR_KROW 12        /* offset of krow_ptr [B+1] i32 */
+#define LNB_PACK_HDR_LABEL 13       /* offset of label [B, P] f32 */
+#define LNB_PACK_HDR_P 14
+/* The kernel derives its input pointers from the header on the device.  flags bit 1
  * (LNB_PACKED_HOST_TILES): the host knows every graph's extents, so it ships the tiles (the same
  * next-fit table and first-fit-decreasing schedule as lnb_graph_prepare, in the same layout) and the
  * prefix sums krow_ptr of k_eff; the kernel expands the Ritz row list itself and NO tile-assignment
@@ -218,22 +230,26 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
  * edges [cap_edges][4], and, when not NULL, D [B,K] and V_rows [cap_rows, K].  Offsets change from batch to
  * batch, so one captured launch serves every batch of the same (B, K) that fits the capacities.  Copies
  * are 16-byte vectors (then up to three 4-byte words per segment), grid-stride; the grid depends on the
- * capacities only.  Nothing past hdr[10] is read, nothing past a capacity is written; rows past
+ * capacities only.  Nothing past the header's TOTAL is read, nothing past a capacity is written; rows past
  * node_ptr[B] / edge_ptr[B] keep their old contents.
- * blob_bytes: the allocation behind blob (>= 64); every buffer is 16-byte aligned.
+ * blob_bytes: the allocation behind blob (>= LNB_PACK_HDR_BYTES); every buffer is 16-byte aligned.
  * status [1]: 0 = copied; otherwise nothing but sizes, node_ptr and edge_ptr is written, all three zero
- * (every graph empty, so the producers behind read no row), and status is a bit set: 1 = bad magic,
- * 2 = B or K differs from the header, 4 = a segment outside [64, hdr[10]), unaligned or hdr[10] >
- * blob_bytes, 8 = node_ptr[B] > cap_rows, 16 = edge_ptr[B] > cap_edges, 32 = D or V_rows requested from a
- * batch without eigenpairs. */
+ * (every graph empty, so the producers behind read no row), and status is a set of the bits below. */
+#define LNB_UNPACK_BAD_MAGIC 1
+#define LNB_UNPACK_BAD_SHAPE 2      /* B or K differs from the header */
+#define LNB_UNPACK_BAD_SEGMENT 4    /* a segment unaligned or outside the body, or TOTAL > blob_bytes */
+#define LNB_UNPACK_ROWS_OVER 8      /* node_ptr[B] > cap_rows */
+#define LNB_UNPACK_EDGES_OVER 16    /* edge_ptr[B] > cap_edges */
+#define LNB_UNPACK_NO_EIGS 32       /* D or V_rows requested from a batch without eigenpairs */
+#define LNB_UNPACK_NO_LABELS 64     /* lnb_records_unpack_labels: no label segment of that P in the body */
 int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
                        int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
                        int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
                        int32_t* status);
 
-/* lnb_records_unpack that also copies the label segment (hdr[13], hdr[14]) into label [B, P] (16-byte
+/* lnb_records_unpack that also copies the label segment (LABEL, P) into label [B, P] (16-byte
  * aligned), in the same launch.  A batch without the segment, with another P or with the segment outside
- * [64, hdr[10]) adds status bit 64, with every graph empty and nothing copied, as the other failures do.
+ * the body adds LNB_UNPACK_NO_LABELS, with every graph empty and nothing copied, as the other failures do.
  * lnb_records_unpack ignores a label segment. */
 int lnb_records_unpack_labels(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
                               int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,

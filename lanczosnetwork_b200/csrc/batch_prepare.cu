@@ -84,17 +84,17 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
   const int32_t* sizes = P.sizes; const int32_t* node_ptr = P.node_ptr; const int32_t* node_feat = P.node_feat;
   const int32_t* edge_ptr = P.edge_ptr; const uint8_t* edges = P.edges; const float* V_rows = P.V_rows;
   if (!kFeat && P.blob) {                        // header: byte offsets of the segments (see the C header)
-    const int32_t* hdr = reinterpret_cast<const int32_t*>(P.blob);
-    sizes = reinterpret_cast<const int32_t*>(P.blob + hdr[3]);
-    node_ptr = reinterpret_cast<const int32_t*>(P.blob + hdr[4]);
-    edge_ptr = reinterpret_cast<const int32_t*>(P.blob + hdr[5]);
-    node_feat = reinterpret_cast<const int32_t*>(P.blob + hdr[7]);
-    V_rows = reinterpret_cast<const float*>(P.blob + hdr[8]);
-    edges = P.blob + hdr[9];
-    if ((P.flags & 2) && hdr[12] > 0 && P.rowmap) {
+    const int32_t* header = reinterpret_cast<const int32_t*>(P.blob);
+    sizes = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_SIZES]);
+    node_ptr = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_NODE_PTR]);
+    edge_ptr = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_EDGE_PTR]);
+    node_feat = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_NODE_FEAT]);
+    V_rows = reinterpret_cast<const float*>(P.blob + header[LNB_PACK_HDR_V_ROWS]);
+    edges = P.blob + header[LNB_PACK_HDR_EDGES];
+    if ((P.flags & LNB_PACKED_HOST_TILES) && header[LNB_PACK_HDR_KROW] > 0 && P.rowmap) {
       // compact Ritz row list {b*K + k : k < k_eff(b)} from the host's prefix sums (the host also ships
       // the tile table, so no tile-assignment launch follows)
-      const int32_t* krow = reinterpret_cast<const int32_t*>(P.blob + hdr[12]);
+      const int32_t* krow = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_KROW]);
       const int k0 = krow[b], k1 = krow[b + 1];
       for (int i = threadIdx.x; i < k1 - k0; i += BP_THREADS) P.rowmap[k0 + i] = b * P.K + i;
       if (b == 0 && threadIdx.x == 0) P.nrows[0] = krow[P.B];
@@ -255,7 +255,7 @@ static int launch_sparse(lnb_stream_t stream, SparseBatchParams p, int32_t* tile
     cudaFuncSetAttribute(batch_prepare_sparse_kernel<kFeat>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   batch_prepare_sparse_kernel<kFeat><<<p.B, BP_THREADS, smem, s>>>(p);
   lnb::count_launch(1);
-  if (p.blob && (p.flags & 2))                     // tile table + row-list offsets came with the batch
+  if (p.blob && (p.flags & LNB_PACKED_HOST_TILES))  // tile table + row-list offsets came with the batch
     return lnb::finish_launch("graph_prepare_sparse");
   return lnb::launch_tiles_or_rowmap(s, p.flags, p.gext, p.B, p.K, tiles, rowmap, nrows,
                                      "graph_prepare_sparse");
@@ -298,7 +298,8 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
   LNB_REQUIRE(B >= 0 && N >= 1 && N <= BP_NMAX && E1 >= 2 && E1 <= BP_EMAX && K >= 1,
               "graph_prepare_sparse_packed: bad dims B=%d N=%d E1=%d K=%d", B, N, E1, K);
   if (B == 0) return LNB_OK;
-  LNB_REQUIRE(blob && inv_sqrt_deg && ell_val && ell_idx && ell_max && gext && (tiles || (flags & 2)) && node_ids && mask && V,
+  LNB_REQUIRE(blob && inv_sqrt_deg && ell_val && ell_idx && ell_max && gext &&
+                  (tiles || (flags & LNB_PACKED_HOST_TILES)) && node_ids && mask && V,
               "graph_prepare_sparse_packed: null pointer");
   LNB_REQUIRE((reinterpret_cast<uintptr_t>(blob) & 15) == 0, "graph_prepare_sparse_packed: blob must be 16-byte aligned");
   LNB_REQUIRE((rowmap == nullptr) == (nrows == nullptr), "graph_prepare_sparse_packed: rowmap and nrows go together");

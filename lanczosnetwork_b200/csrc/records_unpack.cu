@@ -17,7 +17,6 @@ namespace {
 
 constexpr int RU_THREADS = 256;
 constexpr int RU_SEGS = 8;          // sizes, node_ptr, edge_ptr, node_feat, edges, D, V_rows, label
-constexpr int32_t RU_MAGIC = 0x4c4e4231;
 
 struct UnpackParams {
   const uint8_t* blob;
@@ -30,9 +29,9 @@ struct UnpackParams {
   int32_t* status;
 };
 
-// [off, off + bytes) inside the body [64, total) of the blob, 16-byte aligned
+// [off, off + bytes) inside the body [LNB_PACK_HDR_BYTES, total) of the blob, 16-byte aligned
 __device__ __forceinline__ bool seg_ok(int64_t off, int64_t bytes, int64_t total) {
-  return off >= 64 && (off & 15) == 0 && bytes >= 0 && off + bytes <= total;
+  return off >= LNB_PACK_HDR_BYTES && (off & 15) == 0 && bytes >= 0 && off + bytes <= total;
 }
 
 __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const UnpackParams P) {
@@ -40,39 +39,46 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
   __shared__ int64_t s_src[RU_SEGS], s_units[RU_SEGS + 1], s_vec[RU_SEGS];
   __shared__ uint8_t* s_dst[RU_SEGS];
   if (threadIdx.x == 0) {
-    const int32_t* hdr = reinterpret_cast<const int32_t*>(P.blob);
+    const int32_t* header = reinterpret_cast<const int32_t*>(P.blob);
     const int64_t B = P.B, K = P.K;
     int st = 0;
-    if (hdr[0] != RU_MAGIC) st |= 1;
-    if (hdr[1] != P.B || hdr[2] != P.K) st |= 2;
-    const int64_t total = hdr[10];
+    if (header[LNB_PACK_HDR_MAGIC] != LNB_PACK_MAGIC) st |= LNB_UNPACK_BAD_MAGIC;
+    if (header[LNB_PACK_HDR_B] != P.B || header[LNB_PACK_HDR_K] != P.K) st |= LNB_UNPACK_BAD_SHAPE;
+    const int64_t total = header[LNB_PACK_HDR_TOTAL];
     int64_t rows = 0, nedge = 0;
-    const bool eigs = hdr[6] != 0 || hdr[8] != 0;
+    const bool eigs = header[LNB_PACK_HDR_D] != 0 || header[LNB_PACK_HDR_V_ROWS] != 0;
     if (!st) {
-      if (total < 64 || total > P.blob_bytes || (total & 15) ||
-          !seg_ok(hdr[3], 4 * B, total) || !seg_ok(hdr[4], 4 * (B + 1), total) ||
-          !seg_ok(hdr[5], 4 * (B + 1), total)) {
-        st |= 4;
+      if (total < LNB_PACK_HDR_BYTES || total > P.blob_bytes || (total & 15) ||
+          !seg_ok(header[LNB_PACK_HDR_SIZES], 4 * B, total) ||
+          !seg_ok(header[LNB_PACK_HDR_NODE_PTR], 4 * (B + 1), total) ||
+          !seg_ok(header[LNB_PACK_HDR_EDGE_PTR], 4 * (B + 1), total)) {
+        st |= LNB_UNPACK_BAD_SEGMENT;
       } else {
-        const int32_t* np_ = reinterpret_cast<const int32_t*>(P.blob + hdr[4]);
-        const int32_t* ep_ = reinterpret_cast<const int32_t*>(P.blob + hdr[5]);
+        const int32_t* np_ = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_NODE_PTR]);
+        const int32_t* ep_ = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_EDGE_PTR]);
         rows = np_[B];
         nedge = ep_[B];
         if (np_[0] != 0 || ep_[0] != 0 || rows < 0 || nedge < 0 ||
-            !seg_ok(hdr[7], 4 * rows, total) || !seg_ok(hdr[9], 4 * nedge, total))
-          st |= 4;
-        else if (eigs && (!seg_ok(hdr[6], 4 * B * K, total) || !seg_ok(hdr[8], 4 * rows * K, total)))
-          st |= 4;                                   // present eigenpairs come as both segments
+            !seg_ok(header[LNB_PACK_HDR_NODE_FEAT], 4 * rows, total) ||
+            !seg_ok(header[LNB_PACK_HDR_EDGES], 4 * nedge, total))
+          st |= LNB_UNPACK_BAD_SEGMENT;
+        else if (eigs && (!seg_ok(header[LNB_PACK_HDR_D], 4 * B * K, total) ||
+                          !seg_ok(header[LNB_PACK_HDR_V_ROWS], 4 * rows * K, total)))
+          st |= LNB_UNPACK_BAD_SEGMENT;              // present eigenpairs come as both segments
       }
     }
-    if (!st && rows > P.cap_rows) st |= 8;
-    if (!st && nedge > P.cap_edges) st |= 16;
-    if (!st && !eigs && (P.D || P.V_rows)) st |= 32;
-    if (!st && P.label && (hdr[14] != P.P || !seg_ok(hdr[13], 4 * B * P.P, total))) st |= 64;
+    if (!st && rows > P.cap_rows) st |= LNB_UNPACK_ROWS_OVER;
+    if (!st && nedge > P.cap_edges) st |= LNB_UNPACK_EDGES_OVER;
+    if (!st && !eigs && (P.D || P.V_rows)) st |= LNB_UNPACK_NO_EIGS;
+    if (!st && P.label && (header[LNB_PACK_HDR_P] != P.P || !seg_ok(header[LNB_PACK_HDR_LABEL], 4 * B * P.P, total)))
+      st |= LNB_UNPACK_NO_LABELS;
     s_status = st;
     if (!st) {
       // a label segment is read only when asked for: lnb_records_unpack ignores it
-      const int64_t src[RU_SEGS] = {hdr[3], hdr[4], hdr[5], hdr[7], hdr[9], hdr[6], hdr[8], P.label ? hdr[13] : 0};
+      const int64_t src[RU_SEGS] = {header[LNB_PACK_HDR_SIZES], header[LNB_PACK_HDR_NODE_PTR],
+                                    header[LNB_PACK_HDR_EDGE_PTR], header[LNB_PACK_HDR_NODE_FEAT],
+                                    header[LNB_PACK_HDR_EDGES], header[LNB_PACK_HDR_D],
+                                    header[LNB_PACK_HDR_V_ROWS], P.label ? header[LNB_PACK_HDR_LABEL] : 0};
       const int64_t bytes[RU_SEGS] = {4 * B, 4 * (B + 1), 4 * (B + 1), 4 * rows, 4 * nedge,
                                       P.D ? 4 * B * K : 0, P.V_rows ? 4 * rows * K : 0,
                                       P.label ? 4 * B * P.P : 0};
@@ -121,7 +127,7 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
 int launch_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K, int64_t cap_rows,
                   int64_t cap_edges, int32_t* sizes, int32_t* node_ptr, int32_t* node_feat, int32_t* edge_ptr,
                   uint8_t* edges, float* D, float* V_rows, int P, float* label, int32_t* status) {
-  LNB_REQUIRE(B >= 1 && K >= 1 && cap_rows >= 0 && cap_edges >= 0 && blob_bytes >= 64,
+  LNB_REQUIRE(B >= 1 && K >= 1 && cap_rows >= 0 && cap_edges >= 0 && blob_bytes >= LNB_PACK_HDR_BYTES,
               "records_unpack: bad dims B=%d K=%d cap_rows=%lld cap_edges=%lld blob_bytes=%lld", B, K,
               (long long)cap_rows, (long long)cap_edges, (long long)blob_bytes);
   LNB_REQUIRE(blob && sizes && node_ptr && edge_ptr && status && (node_feat || cap_rows == 0) &&

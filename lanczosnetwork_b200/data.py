@@ -14,11 +14,13 @@ Mirrors the parts of the reference that *feed* the spectral-convolution forward:
 All arithmetic follows the reference's fp64-then-cast-to-fp32 convention so the padded
 batch tensors are bit-identical to what the reference loader would hand the model.
 """
+import collections
+
 import numpy as np
 
 __all__ = [
     'check_dist', 'get_laplacian', 'get_graph_laplacian_eigs', 'prepare_graph',
-    'collate', 'gat_bias', 'partition_operators', 'random_partition_labels', 'sage_collate', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
+    'collate', 'gat_bias', 'partition_operators', 'random_partition_labels', 'sage_collate', 'sparse_collate', 'pack_sparse', 'packed_offsets', 'packed_layout', 'packed_capacity', 'read_packed_header', 'synthetic_molecule', 'synthetic_qm8_samples', 'synthetic_qm8_batch',
     'synthetic_regression_graphs',
 ]
 
@@ -260,14 +262,19 @@ def sparse_collate(samples, num_eigs, eigs=True):
 
 PACK_MAGIC = 0x4c4e4231          # "LNB1"
 
+# the int32 slots of a packed batch's header in slot order: LNB_PACK_HDR_* of include/lanczosnet_b200.h
+PackHeader = collections.namedtuple('PackHeader', 'magic B K sizes node_ptr edge_ptr D node_feat V_rows edges '
+                                                  'total tiles krow label P')
+PackedOffsets = collections.namedtuple('PackedOffsets', 'sizes node_ptr edge_ptr D var tiles krow')
+
 
 def _align16(x):
   return (int(x) + 15) & ~15
 
 
 def packed_offsets(B, K):
-  """Byte offsets of the fixed-position segments of a packed batch (they depend on B and K only):
-  (off_sizes, off_node_ptr, off_edge_ptr, off_D, off_variable)."""
+  """Byte offsets of the segments of a packed batch that depend on B and K only (a PackedOffsets); ``var``
+  is where the node ids of a batch with eigenpairs start."""
   off_sizes = 64
   off_node_ptr = off_sizes + _align16(4 * B)
   off_edge_ptr = off_node_ptr + _align16(4 * (B + 1))
@@ -275,7 +282,39 @@ def packed_offsets(B, K):
   off_tiles = off_D + _align16(4 * B * K)
   off_krow = off_tiles + _align16(4 * tile_segment_ints(B))
   off_var = off_krow + _align16(4 * (B + 1))
-  return off_sizes, off_node_ptr, off_edge_ptr, off_D, off_var, off_tiles, off_krow
+  return PackedOffsets(off_sizes, off_node_ptr, off_edge_ptr, off_D, off_var, off_tiles, off_krow)
+
+
+def packed_layout(B, K, rows, nedges, eigs, P=0):
+  """The PackHeader of a packed batch of B graphs with ``rows`` nodes and ``nedges`` bonds in all.  Without
+  ``eigs`` there is no D, V_rows, tiles or krow segment, and the node ids start where D would.  P > 0: a label
+  segment [B, P] float32 behind the bonds."""
+  o = packed_offsets(B, K)
+  if eigs:
+    D, node_feat, tiles, krow = o.D, o.var, o.tiles, o.krow
+    V_rows = node_feat + _align16(4 * rows)
+    edges = V_rows + _align16(4 * rows * K)
+  else:
+    D, node_feat, V_rows, tiles, krow = 0, o.D, 0, 0, 0
+    edges = node_feat + _align16(4 * rows)
+  label = edges + _align16(4 * nedges)
+  total = label + _align16(4 * B * P)
+  return PackHeader(PACK_MAGIC, B, K, o.sizes, o.node_ptr, o.edge_ptr, D, node_feat, V_rows, edges, total, tiles,
+                    krow, label if P else 0, P)
+
+
+def packed_capacity(B, N, K, eigs, nbytes, label_dim=0):
+  """Static size of a packed batch's blob under graph replay: the blob of any B molecules of at most N
+  nodes and 4 N bonds each, or the blob's own ``nbytes`` when that is larger.  ``label_dim`` = P > 0 counts a
+  label segment [B, P] float32 (pack_sparse(..., label=True))."""
+  return max(packed_layout(B, K, B * N, 4 * B * N, eigs, int(label_dim)).total, int(nbytes))
+
+
+def read_packed_header(blob):
+  """The PackHeader of a packed batch's blob (numpy array or torch tensor): a host blob is read in place, a
+  device blob with one 64-byte copy."""
+  head = blob[:64].cpu().numpy() if hasattr(blob, 'cpu') else blob[:64]
+  return PackHeader(*head.view(np.int32)[:len(PackHeader._fields)].tolist())
 
 
 def host_tile_table(sizes, k_eff, rows_per_tile=128, graphs_per_tile=32):
@@ -404,42 +443,30 @@ def pack_sparse(sp, label=False):
   One H2D copy per step ships the whole batch.  Records without eigenpairs (``sparse_collate(...,
   eigs=False)``) give a blob without D, Ritz rows, tiles and Ritz-row offsets (their header offsets are 0):
   the node ids start where D would.  ``label=True``: the records' labels [B, P] float32 follow the bonds as
-  one more segment (hdr[13], hdr[14]), for training from the blob (train.GraphedStep(..., packed=True));
+  one more segment (slots label and P), for training from the blob (train.GraphedStep(..., packed=True));
   every other byte is that of the blob without them.  Returns dict(blob, B, N, K, num_edgetype, eigs[, label])."""
   eigs = 'D' in sp
   if label and 'label' not in sp:
     raise ValueError('pack_sparse: label=True needs records with labels (samples with a label)')
   B, K = sp['D'].shape if eigs else (len(sp['sizes']), int(sp['K']))
-  off_sizes, off_node_ptr, off_edge_ptr, off_D, off, off_tiles, off_krow = packed_offsets(B, K)
-  segs = [(off_sizes, sp['sizes']), (off_node_ptr, sp['node_ptr']), (off_edge_ptr, sp['edge_ptr'])]
+  lab = np.ascontiguousarray(sp['label'], np.float32).reshape(B, -1) if label else None
+  h = packed_layout(B, K, len(sp['node_feat']), len(sp['edges']), eigs, lab.shape[1] if label else 0)
+  segs = [(h.sizes, sp['sizes']), (h.node_ptr, sp['node_ptr']), (h.edge_ptr, sp['edge_ptr']),
+          (h.node_feat, sp['node_feat']), (h.edges, sp['edges'])]
   if eigs:
     # extents the device would measure: k_eff = last non-zero column of the graph's Ritz rows + 1
     k_eff = ritz_extents(sp['V_rows'], sp['node_ptr'])
     krow = np.zeros(B + 1, np.int32)
     krow[1:] = np.cumsum(np.minimum(k_eff, K))
-    segs += [(off_tiles, host_tile_segment(sp['sizes'], k_eff)), (off_krow, krow), (off_D, sp['D'])]
-    off_nf = off
-    off_v = off_nf + _align16(sp['node_feat'].nbytes)
-    off_e = off_v + _align16(sp['V_rows'].nbytes)
-    segs.append((off_v, sp['V_rows']))
-  else:
-    off_nf, off_D, off_v, off_tiles, off_krow = off_D, 0, 0, 0, 0
-    off_e = off_nf + _align16(sp['node_feat'].nbytes)
-  total = off_e + _align16(sp['edges'].nbytes)
+    segs += [(h.tiles, host_tile_segment(sp['sizes'], k_eff)), (h.krow, krow), (h.D, sp['D']),
+             (h.V_rows, sp['V_rows'])]
   if label:
-    lab = np.ascontiguousarray(sp['label'], np.float32).reshape(B, -1)
-    off_l, P = total, lab.shape[1]
-    total = off_l + _align16(lab.nbytes)
-    segs.append((off_l, lab))
-  blob = np.zeros(total, np.uint8)
-  hdr = blob[:64].view(np.int32)
-  hdr[:13] = [PACK_MAGIC, B, K, off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_v, off_e, total,
-              off_tiles, off_krow]
-  if label:
-    hdr[13:15] = [off_l, P]
-  for off_, arr in segs + [(off_nf, sp['node_feat']), (off_e, sp['edges'])]:
+    segs.append((h.label, lab))
+  blob = np.zeros(h.total, np.uint8)
+  blob[:64].view(np.int32)[:len(h)] = h
+  for off, arr in segs:
     raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
-    blob[off_:off_ + raw.size] = raw
+    blob[off:off + raw.size] = raw
   out = {'blob': blob, 'B': int(B), 'N': int(sp['N']), 'K': int(K), 'num_edgetype': int(sp['num_edgetype']),
          'eigs': eigs}
   if 'label' in sp:
@@ -491,12 +518,9 @@ class PackedMolecules(object):
   def max_bytes(self, B):
     """Upper bound of the blob of any B molecules, repeats included (for a reusable pinned staging
     buffer): an index list may repeat the largest molecule B times."""
-    n = B * int(self.sizes.max())
-    e = B * int(np.diff(self.edge_ptr).max())
-    lab = _align16(4 * B * self.label.shape[1]) if self.labels else 0
-    if not self.eigs:
-      return packed_offsets(B, self.K)[3] + _align16(4 * n) + _align16(4 * e) + lab
-    return packed_offsets(B, self.K)[4] + _align16(4 * n) + _align16(4 * n * self.K) + _align16(4 * e) + lab
+    P = self.label.shape[1] if self.labels else 0
+    return packed_layout(B, self.K, B * int(self.sizes.max()), B * int(np.diff(self.edge_ptr).max()), self.eigs,
+                         P).total
 
   def batch(self, idx, out=None):
     """Packed batch of the molecules ``idx`` (order kept).  ``out``: optional uint8 buffer (e.g. the numpy
@@ -512,34 +536,20 @@ class PackedMolecules(object):
     edge_ptr[1:] = np.cumsum(e_len)
     rows = self._ranges(self.node_ptr[idx], n_len)
     erow = self._ranges(self.edge_ptr[idx], e_len)
-    off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_tiles, off_krow = packed_offsets(B, K)
-    if self.eigs:
-      off_v = off_nf + _align16(4 * len(rows))
-      off_e = off_v + _align16(4 * len(rows) * K)
-    else:                                            # pack_sparse's layout without eigenpairs
-      off_nf, off_D, off_v, off_tiles, off_krow = off_D, 0, 0, 0, 0
-      off_e = off_nf + _align16(4 * len(rows))
-    off_l = total = off_e + _align16(4 * len(erow))
-    if self.labels:
-      P = self.label.shape[1]
-      total = off_l + _align16(4 * B * P)
+    P = self.label.shape[1] if self.labels else 0
+    h = packed_layout(B, K, len(rows), len(erow), self.eigs, P)
     if out is None:
-      blob = np.zeros(total, np.uint8)
+      blob = np.zeros(h.total, np.uint8)
     else:
-      if out.dtype != np.uint8 or out.ndim != 1 or out.size < total:
-        raise ValueError('PackedMolecules.batch: out must be a flat uint8 buffer of >= %d bytes' % total)
-      blob = out[:total]
-      blob[:off_nf] = 0                              # header + fixed segments (alignment gaps stay zero)
-      gaps = ((off_nf + 4 * len(rows), off_v), (off_v + 4 * len(rows) * K, off_e)) if self.eigs else \
-          ((off_nf + 4 * len(rows), off_e),)
-      tail = (((off_e + 4 * len(erow), off_l), (off_l + 4 * B * P, total)) if self.labels else
-              ((off_e + 4 * len(erow), total),))
-      for a, b in gaps + tail:
-        blob[a:b] = 0
-    blob[:64].view(np.int32)[:13] = [PACK_MAGIC, B, K, off_sizes, off_node_ptr, off_edge_ptr, off_D, off_nf, off_v,
-                                     off_e, total, off_tiles, off_krow]
-    if self.labels:
-      blob[:64].view(np.int32)[13:15] = [off_l, P]
+      if out.dtype != np.uint8 or out.ndim != 1 or out.size < h.total:
+        raise ValueError('PackedMolecules.batch: out must be a flat uint8 buffer of >= %d bytes' % h.total)
+      blob = out[:h.total]
+      blob[:h.node_feat] = 0                         # header + fixed segments (alignment gaps stay zero)
+      body = [(off, n) for off, n in ((h.node_feat, 4 * len(rows)), (h.V_rows, 4 * len(rows) * K),
+                                      (h.edges, 4 * len(erow)), (h.label, 4 * B * P)) if off]
+      for (off, n), end in zip(body, [off for off, _ in body[1:]] + [h.total]):
+        blob[off + n:end] = 0                        # the alignment gap behind each segment
+    blob[:64].view(np.int32)[:len(h)] = h
 
     def put(off, arr):
       raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
@@ -549,17 +559,18 @@ class PackedMolecules(object):
       k_eff = self.k_eff[idx]
       krow = np.zeros(B + 1, np.int32)
       krow[1:] = np.cumsum(np.minimum(k_eff, K))
-      put(off_tiles, host_tile_segment(sizes, k_eff))
-      put(off_krow, krow)
-      put(off_D, self.D[idx])
-      np.take(self.V_rows, rows, axis=0, out=blob[off_v:off_v + 4 * len(rows) * K].view(np.float32).reshape(len(rows), K))
-    put(off_sizes, sizes)
-    put(off_node_ptr, node_ptr)
-    put(off_edge_ptr, edge_ptr)
-    np.take(self.node_feat, rows, out=blob[off_nf:off_nf + 4 * len(rows)].view(np.int32))
-    np.take(self.edges, erow, axis=0, out=blob[off_e:off_e + 4 * len(erow)].reshape(len(erow), 4))
+      put(h.tiles, host_tile_segment(sizes, k_eff))
+      put(h.krow, krow)
+      put(h.D, self.D[idx])
+      np.take(self.V_rows, rows, axis=0,
+              out=blob[h.V_rows:h.V_rows + 4 * len(rows) * K].view(np.float32).reshape(len(rows), K))
+    put(h.sizes, sizes)
+    put(h.node_ptr, node_ptr)
+    put(h.edge_ptr, edge_ptr)
+    np.take(self.node_feat, rows, out=blob[h.node_feat:h.node_feat + 4 * len(rows)].view(np.int32))
+    np.take(self.edges, erow, axis=0, out=blob[h.edges:h.edges + 4 * len(erow)].reshape(len(erow), 4))
     if self.labels:
-      np.take(self.label, idx, axis=0, out=blob[off_l:off_l + 4 * B * P].view(np.float32).reshape(B, P))
+      np.take(self.label, idx, axis=0, out=blob[h.label:h.label + 4 * B * P].view(np.float32).reshape(B, P))
     res = {'blob': blob, 'B': int(B), 'N': int(sizes.max()) if B else 0, 'K': K, 'num_edgetype': self.num_edgetype,
            'eigs': self.eigs}
     if self.label is not None:

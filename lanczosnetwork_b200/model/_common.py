@@ -13,7 +13,7 @@ import torch.nn as nn
 
 from .. import _lib, ops
 from .. import data as data_mod
-from ..data import check_dist
+from ..data import check_dist, packed_capacity
 from ..spectral_conv import (GraphContext, WeightCache, graph_conv_layer,
                              ritz_filter_coefficients)
 
@@ -41,17 +41,6 @@ class Ragged(object):
 
 def _raw(t):
   return t.tensor if isinstance(t, Ragged) else t
-
-
-def packed_capacity(B, N, K, eigs, nbytes, label_dim=0):
-  """Static size of a packed batch's blob under graph replay: the blob of any B molecules of at most N
-  nodes and 4 N bonds each (alignment gaps included), or the blob's own ``nbytes`` when that is larger.
-  ``label_dim`` = P > 0 counts a label segment [B, P] float32 (data.pack_sparse(..., label=True))."""
-  off = data_mod.packed_offsets(B, K)
-  body = off[4] + 4 * B * N * K if eigs else off[3]
-  if label_dim:
-    body += data_mod._align16(4 * B * int(label_dim))
-  return max(body + 16 * 3 + 4 * B * N + 4 * B * N * 4, int(nbytes))
 
 
 # the bond-list records of one batch on the device (data.sparse_collate's layout), N = padding target,
@@ -323,7 +312,7 @@ class SpectralNetBase(nn.Module):
     then nothing is read on the host, ``eigs`` is trusted -- LanczosNet runs an eigenpair blob through
     lnb_graph_prepare_sparse_packed, which reads the Ritz rows, so it must be right -- and the header is
     checked by lnb_records_unpack on the device only; a batch that fails there gives the scores of empty
-    graphs.  Returns (B, N, K, eigs)."""
+    graphs.  Returns (B, N, K, eigs, header): the data.PackHeader read, None when nothing was read."""
     missing = [k for k in self.PACKED_KEYS if k not in batch]
     if missing:
       raise ValueError('forward_sparse: the packed batch lacks %s (data.pack_sparse)' % ', '.join(missing))
@@ -338,44 +327,41 @@ class SpectralNetBase(nn.Module):
       raise ValueError('forward_sparse: packed batch with B=%d, K=%d' % (B, K))
     eigs = batch.get('eigs')
     if blob.is_cuda and eigs is not None:
-      return B, N, K, bool(eigs)
+      return B, N, K, bool(eigs), None
     if blob.is_cuda and torch.cuda.is_current_stream_capturing():
       raise ValueError("forward_sparse: a device blob under stream capture needs batch['eigs'] (its header "
                        "cannot be read on the host there)")
 
-    def ints(lo, n):                         # a device blob: one small synchronous copy
-      return blob[lo:lo + 4 * n].cpu().view(torch.int32).tolist()
-
-    hdr = ints(0, 16)
-    if hdr[0] != data_mod.PACK_MAGIC:
-      raise ValueError('forward_sparse: blob magic %#x is not %#x (data.pack_sparse)' % (hdr[0] & 0xffffffff,
+    hdr = data_mod.read_packed_header(blob)
+    if hdr.magic != data_mod.PACK_MAGIC:
+      raise ValueError('forward_sparse: blob magic %#x is not %#x (data.pack_sparse)' % (hdr.magic & 0xffffffff,
                                                                                          data_mod.PACK_MAGIC))
-    if (hdr[1], hdr[2]) != (B, K):
+    if (hdr.B, hdr.K) != (B, K):
       raise ValueError('forward_sparse: blob header has B=%d, K=%d; the batch says B=%d, K=%d'
-                       % (hdr[1], hdr[2], B, K))
-    if not 64 <= hdr[10] <= blob.numel():
-      raise ValueError('forward_sparse: blob header total %d bytes outside [64, %d]' % (hdr[10], blob.numel()))
-    if not (64 <= hdr[4] and hdr[4] % 16 == 0 and hdr[4] + 4 * (B + 1) <= hdr[10]):
-      raise ValueError('forward_sparse: blob node_ptr offset %d outside the blob' % hdr[4])
-    rows = ints(hdr[4] + 4 * B, 1)[0]
+                       % (hdr.B, hdr.K, B, K))
+    if not 64 <= hdr.total <= blob.numel():
+      raise ValueError('forward_sparse: blob header total %d bytes outside [64, %d]' % (hdr.total, blob.numel()))
+    if not (64 <= hdr.node_ptr and hdr.node_ptr % 16 == 0 and hdr.node_ptr + 4 * (B + 1) <= hdr.total):
+      raise ValueError('forward_sparse: blob node_ptr offset %d outside the blob' % hdr.node_ptr)
+    rows = blob[hdr.node_ptr + 4 * B:][:4].cpu().view(torch.int32).item()     # node_ptr[B], a second read
     if not 0 <= rows <= B * N:
       raise ValueError('forward_sparse: node_ptr[B]=%d node rows outside [0, B*N = %d]' % (rows, B * N))
-    has = hdr[6] != 0 or hdr[8] != 0
+    has = hdr.D != 0 or hdr.V_rows != 0
     if eigs is not None and bool(eigs) != has:
       raise ValueError("forward_sparse: batch['eigs'] is %s, the blob %s eigenpairs"
                        % (bool(eigs), 'carries' if has else 'has no'))
-    return B, N, K, has
+    return B, N, K, has, hdr
 
   def _packed_records(self, batch):
     """(blob input, unpack, graph-cache key) of a packed batch for a model with a records entry: the blob
     as ONE Ragged input whose capacity depends on (B, N, K) only, and ``unpack(device_blob)``, the
     SparseRecords that lnb_records_unpack writes from it into fixed-capacity buffers (node rows B * N, the
     bonds the blob's capacity can hold), so one captured graph serves every batch of the same shape."""
-    B, N, K, eigs = self._check_packed_batch(batch)
+    B, N, K, eigs, _ = self._check_packed_batch(batch)
     self._check_runnable(N, self.num_edgetype + 1)
     blob = batch['blob']
     return (Ragged(blob, packed_capacity(B, N, K, eigs, blob.shape[0])),
-            lambda b_: self._unpack_records(b_, B, N, K), ('packed_records', B, N, K))
+            lambda b_: self._unpack(b_, B, N, K)[0], ('packed_records', B, N, K))
 
   def _takes_packed_training(self):
     """True when ``train.GraphedStep(..., packed=True)`` trains this model: it has a training entry from records
@@ -386,17 +372,16 @@ class SpectralNetBase(nn.Module):
     """GraphedStep(packed=True)'s checks of a labelled packed batch, before any copy: those of
     ``forward_sparse`` with the header always read (a device blob with a small synchronous copy, even when the
     batch says ``eigs``: a training step must never run on a batch the device would refuse), and a label
-    segment inside the blob.  Returns (B, N, K, eigs, P, total bytes)."""
-    B, N, K, eigs = self._check_packed_batch({k: v for k, v in batch.items() if k != 'eigs'})
+    segment inside the blob.  Returns (header, N, eigs), the header a data.PackHeader."""
+    B, N, K, eigs, hdr = self._check_packed_batch({k: v for k, v in batch.items() if k != 'eigs'})
     if 'eigs' in batch and bool(batch['eigs']) != eigs:
       raise ValueError("GraphedStep: batch['eigs'] is %s, the blob %s eigenpairs"
                        % (bool(batch['eigs']), 'carries' if eigs else 'has no'))
-    hdr = batch['blob'][:64].cpu().view(torch.int32).tolist()
-    total, off, P = hdr[10], hdr[13], hdr[14]
-    if P < 1 or off < 64 or off % 16 or off + 4 * B * P > total:
+    if hdr.P < 1 or hdr.label < 64 or hdr.label % 16 or hdr.label + 4 * B * hdr.P > hdr.total:
       raise ValueError('GraphedStep: the packed batch carries no labels (label offset %d, P=%d): build it with '
-                       'data.pack_sparse(..., label=True) or data.PackedMolecules(..., labels=True)' % (off, P))
-    return B, N, K, eigs, P, total
+                       'data.pack_sparse(..., label=True) or data.PackedMolecules(..., labels=True)'
+                       % (hdr.label, hdr.P))
+    return hdr, N, eigs
 
   def _train_packed(self, batch, P):
     """The training forward of a device blob with labels (the static batch of GraphedStep(packed=True)):
@@ -404,21 +389,16 @@ class SpectralNetBase(nn.Module):
     carries after the blob, as ``forward_sparse_train`` passes it.  Returns (score, label [B, P], status)."""
     inputs, _, _ = self._sparse_inputs(batch)
     B, N, K = int(batch['B']), int(batch['N']), int(batch['K'])
-    recs, _, _, label, status = self._unpack_labelled(batch['blob'], B, N, K, P)
+    recs, _, _, label, status = self._unpack(batch['blob'], B, N, K, P)
     return self._train_records(recs, *[_raw(t) for t in inputs[1:]]), label, status
 
-  def _unpack_labelled(self, blob, B, N, K, P, eigs=False):
-    """lnb_records_unpack_labels of a device blob: (SparseRecords, D, V_rows, label [B, P], status), D and
-    V_rows None without ``eigs``.  Capacities as in ``_unpack_records``."""
-    cap_edges = (blob.shape[0] - data_mod.packed_offsets(B, K)[3]) // 4
+  def _unpack(self, blob, B, N, K, P=0, eigs=False):
+    """ops.records_unpack of a device blob into fixed-capacity records: B * N node rows, and as many bonds as
+    the bytes past D's offset hold (the bonds lie behind it, with or without eigenpairs); P > 0 adds the labels.
+    Returns (SparseRecords, D, V_rows[, label [B, P]], status), D and V_rows None without ``eigs``."""
+    cap_edges = (blob.shape[0] - data_mod.packed_offsets(B, K).D) // 4
     out = ops.records_unpack(blob, B, K, B * N, cap_edges, eigs=eigs, label_dim=P)
     return (SparseRecords(*out[:5], N=N, K=K),) + tuple(out[5:])
-
-  def _unpack_records(self, blob, B, N, K):
-    """SparseRecords of a device blob (lnb_records_unpack; the eigenpairs, if any, stay in the blob).  The
-    bonds lie behind the offset where D starts, with or without eigenpairs: they fit in the bytes past it."""
-    cap_edges = (blob.shape[0] - data_mod.packed_offsets(B, K)[3]) // 4
-    return SparseRecords(*ops.records_unpack(blob, B, K, B * N, cap_edges)[:5], N=N)
 
   def _check_runnable(self, N=None, E1=None):
     """Model-specific checks of a call, run before any launch (N, E1: those of a sparse batch)."""
@@ -710,15 +690,13 @@ class RitzRecords(object):
         raise NotImplementedError('%s takes data.sparse_collate records, not packed batches'
                                   % type(self).__name__)
       # a packed batch (data.pack_sparse) crosses PCIe as ONE copy of exactly the bytes present
-      B, N, K, eigs = self._check_packed_batch(batch)
-      blob = batch['blob']
+      B, N, K, eigs, _ = self._check_packed_batch(batch)
+      inputs = (Ragged(batch['blob'], packed_capacity(B, N, K, eigs, batch['blob'].shape[0])),)
       if not eigs:
         # without eigenpairs: records_unpack, then the path of records without them
-        return ((Ragged(blob, packed_capacity(B, N, K, False, blob.shape[0])),),
-                lambda b_: self._forward_sparse_eigs_impl(N, K, *self._unpack_records(b_, B, N, K)[:5]),
+        return (inputs, lambda b_: self._forward_sparse_eigs_impl(N, K, *self._unpack(b_, B, N, K)[0][:5]),
                 ('packed_eigs', B, N, K))
-      return ((Ragged(blob, packed_capacity(B, N, K, True, blob.shape[0])),),
-              lambda b_: self._forward_packed_impl(B, N, K, b_), ('packed', B, N, K))
+      return inputs, lambda b_: self._forward_packed_impl(B, N, K, b_), ('packed', B, N, K)
     if feat:
       self._check_ritz_records(batch)
     N, B = int(batch['N']), int(batch['sizes'].shape[0])
@@ -753,8 +731,8 @@ class RitzRecords(object):
   def _train_packed(self, batch, P):
     """A labelled blob with eigenpairs trains on its D and V_rows; one without gets them from
     lnb_graph_eigs_sparse, as records without them do."""
-    recs, D, V_rows, label, status = self._unpack_labelled(batch['blob'], int(batch['B']), int(batch['N']),
-                                                           int(batch['K']), P, eigs=bool(batch['eigs']))
+    recs, D, V_rows, label, status = self._unpack(batch['blob'], int(batch['B']), int(batch['N']),
+                                                  int(batch['K']), P, eigs=bool(batch['eigs']))
     return self._train_records(recs, V_rows, D), label, status
 
   def _prepare_ritz_records(self, sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N, **kw):

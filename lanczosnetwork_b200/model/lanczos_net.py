@@ -42,7 +42,7 @@ class LanczosNet(RitzRecords, SpectralNetBase):
   def _forward_packed_impl(self, B, N, K, blob):
     E1 = self.num_edgetype + 1
     dense = not self._sparse_stack_ok(N, E1, K)
-    off_D = data_mod.packed_offsets(B, K)[3]
+    off_D = data_mod.packed_offsets(B, K).D
     D = blob[off_D:off_D + 4 * B * K].view(torch.float32).reshape(B, K)     # fixed address in the buffer
     prep, node_ids, mask, V, L = ops.graph_prepare_sparse_packed(
         blob, B, N, E1, K, binarize=getattr(self, '_binarize_operators', False), want_dense=dense)

@@ -206,6 +206,7 @@ def tile_assign(prep, K):
 
 
 PREP_DEFER_TILES = 4    # LNB_PREP_DEFER_TILES
+PACKED_HOST_TILES = 2   # LNB_PACKED_HOST_TILES
 
 
 def graph_prepare(L, Q=None, binarize=False, defer_tiles=False):
@@ -357,7 +358,7 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
   gext = torch.empty((B, 2), device=dev, dtype=torch.int32)
   if host_tiles:
     from .data import packed_offsets, tile_segment_ints
-    off_tiles = packed_offsets(B, K)[5]
+    off_tiles = packed_offsets(B, K).tiles
     # the next-fit table and, behind it, the tile schedule the stack kernel runs
     tiles = blob[off_tiles:off_tiles + 4 * tile_segment_ints(B)].view(torch.int32)
   else:
@@ -371,8 +372,8 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
   with torch.cuda.device(dev):
     _lib.check(_lib.load().lnb_graph_prepare_sparse_packed(
         _stream(blob), _ptr(blob), _ptr(_inv_sqrt_deg_table(dev)), int(B), int(N), int(E1), int(K),
-        (1 if binarize else 0) | (2 if host_tiles else 0), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(gext), _ptr(tiles),
-        _ptr(rowmap), _ptr(nrows), _ptr(node_ids), _ptr(mask), _ptr(V), _ptr(L)),
+        (1 if binarize else 0) | (PACKED_HOST_TILES if host_tiles else 0), _ptr(ell_val), _ptr(ell_idx),
+        _ptr(ell_max), _ptr(gext), _ptr(tiles), _ptr(rowmap), _ptr(nrows), _ptr(node_ids), _ptr(mask), _ptr(V), _ptr(L)),
                'lnb_graph_prepare_sparse_packed')
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows = rowmap, nrows

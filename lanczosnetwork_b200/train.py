@@ -1094,7 +1094,7 @@ class GraphedStep:
                         'MPNN, GPNN, SampledGraphSAGE and LanczosNet from packed batches; %s is not among them'
                         % type(model).__name__)
       self._check_packed_args(args, kwargs)
-      shape = model._check_packed_train(args[0])
+      checked = model._check_packed_train(args[0])
       model._sparse_inputs(args[0])                          # the model's own checks (its keys)
     elif sparse:
       if not hasattr(model, '_train_records'):
@@ -1117,7 +1117,7 @@ class GraphedStep:
     model.train()
     self.model, self.optimizer, self.sparse, self.packed = model, optimizer, bool(sparse), bool(packed)
     if packed:
-      self._args = [self._static_packed(args[0], dev, shape)]
+      self._args = [self._static_packed(args[0], dev, *checked)]
       self.input_consumed = None
     elif sparse:
       self._args = [self._static_records(args[0], dev, cap)]
@@ -1218,13 +1218,13 @@ class GraphedStep:
     if kwargs:
       raise ValueError('GraphedStep(packed=True): the labels travel in the blob; got %s=' % ', '.join(sorted(kwargs)))
 
-  def _static_packed(self, batch, dev, shape):
-    B, N, K, eigs, P, total = shape
-    from .model._common import packed_capacity
-    self._packed_shape = (B, N, K, eigs, P)
-    blob = torch.zeros(packed_capacity(B, N, K, eigs, total, label_dim=P), dtype=torch.uint8, device=dev)
-    blob[:total].copy_(batch['blob'][:total])
-    out = {'blob': blob, 'B': B, 'N': N, 'K': K, 'eigs': eigs}
+  def _static_packed(self, batch, dev, hdr, N, eigs):
+    from .data import packed_capacity
+    self._packed_shape = (hdr.B, N, hdr.K, eigs, hdr.P)
+    blob = torch.zeros(packed_capacity(hdr.B, N, hdr.K, eigs, hdr.total, label_dim=hdr.P), dtype=torch.uint8,
+                       device=dev)
+    blob[:hdr.total].copy_(batch['blob'][:hdr.total])
+    out = {'blob': blob, 'B': hdr.B, 'N': N, 'K': hdr.K, 'eigs': eigs}
     for k in self._PACKED_KEYS:
       if k in batch:
         out[k] = self._static(batch[k], dev)
@@ -1235,13 +1235,13 @@ class GraphedStep:
     then copies the blob's own bytes and the keys, and records ``input_consumed`` behind the copy."""
     self._check_packed_args(args, kwargs)
     batch, static = args[0], self._args[0]
-    B, N, K, eigs, P, total = self.model._check_packed_train(batch)
-    if (B, N, K, eigs, P) != self._packed_shape:
+    hdr, N, eigs = self.model._check_packed_train(batch)
+    if (hdr.B, N, hdr.K, eigs, hdr.P) != self._packed_shape:
       raise ValueError('GraphedStep was captured for packed batches of (B, N, K, eigs, P) = %s, got %s'
-                       % (self._packed_shape, (B, N, K, eigs, P)))
-    if total > static['blob'].numel():
+                       % (self._packed_shape, (hdr.B, N, hdr.K, eigs, hdr.P)))
+    if hdr.total > static['blob'].numel():
       raise ValueError('GraphedStep: a blob of %d bytes exceeds the captured capacity of %d bytes'
-                       % (total, static['blob'].numel()))
+                       % (hdr.total, static['blob'].numel()))
     keys = [k for k in self._PACKED_KEYS if k in batch]
     if set(keys) != set(k for k in self._PACKED_KEYS if k in static):
       raise ValueError('GraphedStep was captured for a packed batch with keys %s, got %s'
@@ -1250,7 +1250,7 @@ class GraphedStep:
       src = batch[k]
       if not torch.is_tensor(src) or tuple(src.shape) != tuple(static[k].shape) or src.dtype != static[k].dtype:
         raise ValueError('GraphedStep was captured for %s %s %s' % (k, tuple(static[k].shape), static[k].dtype))
-    static['blob'][:total].copy_(batch['blob'][:total], non_blocking=True)
+    static['blob'][:hdr.total].copy_(batch['blob'][:hdr.total], non_blocking=True)
     for k in keys:
       static[k].copy_(batch[k], non_blocking=True)
     self.input_consumed = torch.cuda.Event()               # this call's own: a loader keeps one per buffer

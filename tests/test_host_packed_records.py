@@ -9,7 +9,8 @@ from lanczosnetwork_b200 import configs, data
 from lanczosnetwork_b200.model import (DCNN, GAT, GCN, GCNFP, GGNN, GPNN, MPNN, ChebyNet, KeyedAdaLanczosNet,
                                        KeyedGAT, LanczosNet, SampledGraphSAGE, SparseLanczosNetGeneral,
                                        TrainableGAT)
-from lanczosnetwork_b200.model._common import Ragged, packed_capacity
+from lanczosnetwork_b200.data import packed_capacity
+from lanczosnetwork_b200.model._common import Ragged
 
 K = 20
 DROPINS = {

@@ -8,7 +8,7 @@ import torch
 from lanczosnetwork_b200 import configs, data
 from lanczosnetwork_b200.model import (GAT, GCN, GGNN, KeyedAdaLanczosNet, KeyedGAT, LanczosNet, SampledGraphSAGE,
                                        SparseLanczosNetGeneral)
-from lanczosnetwork_b200.model._common import packed_capacity
+from lanczosnetwork_b200.data import packed_capacity
 from lanczosnetwork_b200.train import GraphedStep
 
 K = 20

@@ -167,7 +167,7 @@ def main():
     print(json.dumps(row), flush=True)
   # the unpack kernel alone, profiled after the timed loops (the profiler slows the host)
   blob = torch.from_numpy(pool.batch(idxs[0])['blob']).to(dev)
-  cap = (blob.numel() - data.packed_offsets(B, K)[3]) // 4
+  cap = (blob.numel() - data.packed_offsets(B, K).D) // 4
   print(json.dumps({'kernel': 'lnb_records_unpack', 'B': B, 'gpu': gpu, 'blob_bytes': host['blob_bytes'],
                     'unpack_kernel_ms': round(profiled_kernel_ms(
                         lambda: ops.records_unpack(blob, B, K, B * 26, cap), 50, ['records_unpack_kernel']), 4)}),
