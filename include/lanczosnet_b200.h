@@ -29,6 +29,35 @@ typedef void* lnb_stream_t; /* cudaStream_t */
 #define LNB_ERR_ARG (-1)
 #define LNB_ERR_UNSUPPORTED (-2)
 
+/* Shape limits: an entry point returns LNB_ERR_UNSUPPORTED outside its envelope, which the comments below
+ * state in these names.  Kernels that feed one another share a name. */
+#define LNB_MAX_N 128               /* padded nodes per graph of the records producers, the ELL messages, the
+                                       eigensolver, the partition, the convolution stack, GAT and Set2Vec */
+#define LNB_MAX_N_ELL 255           /* nodes a uint8 ELL column index addresses: lnb_graph_prepare and the
+                                       kernels that read only its ELL rows (GRU updates, neighbour max) */
+#define LNB_MAX_E1 16               /* operator channels E1 = bond types + 1 */
+#define LNB_MAX_WIDTH 128           /* feature width of the tensor-core kernels: one 128-column wgmma tile */
+#define LNB_PREPARE_MAX_F 4096      /* float node features of lnb_graph_prepare_sparse_features */
+#define LNB_CONV_MAX_K 32           /* Ritz pairs of the fused convolution */
+#define LNB_CONV_MAX_LAYERS 8       /* layers of one lnb_spectral_stack_forward (lnb_spectral_stack.Din) */
+#define LNB_FILTER_MLP_MAX_S 32     /* long scales of the Ritz power table and the filter-MLP chain */
+#define LNB_GAT_MAX_WIDTH 128       /* GAT head width F */
+#define LNB_GAT_MAX_HEADS 32
+#define LNB_SET2VEC_MAX_P 128       /* Set2Vec outputs */
+#define LNB_CHAIN_MAX_N 32          /* nodes of the one-launch operator chain and its walk */
+#define LNB_CHAIN_MAX_STEPS 64      /* steps of that chain, and short-walk steps of lnb_graph_messages */
+#define LNB_MESSAGES_MAX_N 32       /* lnb_graph_messages */
+#define LNB_MESSAGES_MAX_K 32
+#define LNB_MESSAGES_MAX_S 8
+#define LNB_LANCZOS_FUSED_MAX_N 1024 /* lnb_lanczos_ritz */
+#define LNB_LANCZOS_MAX_K 64        /* Lanczos steps of the fused kernel and of the training path */
+#define LNB_LANCZOS_TRAIN_MAX_N 128 /* lnb_lanczos_tridiag_train / _backward: one thread per node */
+#define LNB_TRIDIAG_POWERS_MAX_S 32 /* powers of lnb_tridiag_powers and its adjoint */
+#define LNB_EIGS_MAX_K 128          /* eigenpairs of lnb_graph_eigs_sparse / lnb_sym_eigs */
+#define LNB_EIGS_MAX_E 32           /* bond types the sparse eigensolver and partition read (one bit each) */
+#define LNB_PARTITION_MIN_P 2       /* clusters of lnb_spectral_partition(_sparse) */
+#define LNB_PARTITION_MAX_P 16
+
 /* ABI version (bumped on any signature change) and last error text of the calling thread. */
 int lnb_abi_version(void);
 const char* lnb_last_error(void);
@@ -134,9 +163,9 @@ int lnb_linear_tf32x3_grouped(lnb_stream_t stream, const float* A, const float* 
  * above writes them (one CTA).
  * Skipping exact zeros / padded rows is exact.  write_pad != 0 also writes the constant rows
  * act(bias) of padded nodes (needed when the full [B,N,H] tensor is read afterwards).
- * Requirements of the fused kernel: N <= 128, Din % 32 == 0, K % 4 == 0, K <= 32, H % 4 == 0,
- * H <= 128, E1 <= 16; W is [H, (S+E1)*Din].  Returns LNB_ERR_UNSUPPORTED otherwise (callers
- * use the unfused ops).
+ * Requirements of the fused kernel: N <= LNB_MAX_N, Din % 32 == 0, K % 4 == 0, K <= LNB_CONV_MAX_K,
+ * H % 4 == 0, H <= LNB_MAX_WIDTH, E1 <= LNB_MAX_E1; W is [H, (S+E1)*Din].  Returns LNB_ERR_UNSUPPORTED
+ * otherwise (callers use the unfused ops).
  * ------------------------------------------------------------------------------------- */
 int lnb_graph_prepare(lnb_stream_t stream, const float* L, const float* Q, int B, int N, int E1,
                       int K, float* ell_val, uint8_t* ell_idx, int32_t* ell_max, int32_t* gext,
@@ -172,7 +201,7 @@ int lnb_spectral_conv_fused(lnb_stream_t stream, const float* X, const float* Q,
  * V [B,N,K] that lnb_spectral_stack_forward reads, and -- only when L_dense != NULL -- the padded dense
  * operators [B,N,N,E1] exactly as the reference's collate builds them.  flags as lnb_graph_prepare
  * (LNB_PREP_DEFER_TILES included).
- * Limits: N <= 128, 2 <= E1 <= 16.
+ * Limits: N <= LNB_MAX_N, 2 <= E1 <= LNB_MAX_E1.
  * ------------------------------------------------------------------------------------- */
 int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
                              const int32_t* node_feat, const int32_t* edge_ptr, const uint8_t* edges,
@@ -263,8 +292,8 @@ int lnb_records_unpack_labels(lnb_stream_t stream, const uint8_t* blob, int64_t 
  * by .float()).  The copy takes 16-byte vectors when F % 4 == 0 and node_x and X are 16-byte aligned, scalar
  * loads otherwise; the bits are the same either way.  Same kernel as lnb_graph_prepare_sparse (a
  * compile-time variant), one launch plus the tile assignment unless LNB_PREP_DEFER_TILES.
- * Limits: 1 <= N <= 128, 2 <= E1 <= 16, K >= 1, 1 <= F <= 4096 (LNB_ERR_UNSUPPORTED otherwise, nothing
- * launched). */
+ * Limits: 1 <= N <= LNB_MAX_N, 2 <= E1 <= LNB_MAX_E1, K >= 1, 1 <= F <= LNB_PREPARE_MAX_F
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched). */
 int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
                                       const float* node_x, const int32_t* edge_ptr, const uint8_t* edges,
                                       const float* V_rows, const double* inv_sqrt_deg, int B, int N, int E1,
@@ -281,7 +310,7 @@ int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes,
  * emb_table [emb_rows, Din[0]] (model/lanczos_net.py:154).  Outputs: out_state [B,N,H] (may be
  * NULL) and / or score [B,P] from the fused readout (model/lanczos_net.py:185-194; mask may be
  * NULL = mean over all N nodes; P <= 48).  Same shape limits as lnb_spectral_conv_fused, plus
- * Din[l>0] == H, num_layers <= 8 and a 16-byte aligned bias.
+ * Din[l>0] == H, num_layers <= LNB_CONV_MAX_LAYERS and a 16-byte aligned bias.
  * ------------------------------------------------------------------------------------- */
 typedef struct lnb_spectral_stack {
   const float* X; const int64_t* node_ids; const float* emb_table;
@@ -317,7 +346,7 @@ int lnb_spectral_stack_forward(lnb_stream_t stream, const lnb_spectral_stack* de
  * lnb_neighbour_max: the Max messages on their own (the training path),
  *   out[b, n, e*D + f] = max over the ELL entries m of row n of channel e of X[b, m, f]
  *   argmax[b, n, e, f] = that m (ties: lowest m), -1 for a row without entries (out = 0).
- * X [B, N, D]; ell_* from lnb_graph_prepare on the operators above; N <= 255.
+ * X [B, N, D]; ell_* from lnb_graph_prepare on the operators above; N <= LNB_MAX_N_ELL.
  * ------------------------------------------------------------------------------------- */
 #define LNB_SAGE_MAX 1
 int lnb_sage_operators(lnb_stream_t stream, const int64_t* nn_idx, const float* nonempty, int B, int N,
@@ -350,7 +379,7 @@ int lnb_neighbour_max(lnb_stream_t stream, const float* X, const float* ell_val,
  *     ell_max unwritten; no tile table: lnb_tile_assign builds it from gext);
  *   LNB_SAGE_SAMPLE_ELL_T (needs LNB_SAGE_SAMPLE_ELL) the same for the transposed operator M_e^T
  *     (ellT_*, gextT), which the training adjoint reads: M is not symmetric.
- * Limits: 1 <= N <= 128, 2 <= E1 <= 16, K >= 1, B*N*E1 < 2^31 (LNB_ERR_UNSUPPORTED otherwise,
+ * Limits: 1 <= N <= LNB_MAX_N, 2 <= E1 <= LNB_MAX_E1, K >= 1, B*N*E1 < 2^31 (LNB_ERR_UNSUPPORTED otherwise,
  * nothing launched).  edges may be NULL for a batch without bonds.
  * ------------------------------------------------------------------------------------- */
 #define LNB_SAGE_SAMPLE_NN_IDX 1
@@ -374,7 +403,7 @@ int lnb_embedding_rows(lnb_stream_t stream, const int64_t* idx, const float* tab
  * correctly rounded from a double-precision pow.  The per-layer filter MLP
  * (model/lanczos_net.py:109-113) is then four lnb_batched_gemm / lnb_linear_tf32x3 calls over
  * the B*K rows, batched over all layers at once because the input does not depend on the
- * layer state.  powers: host pointer to S ints (S <= 32).
+ * layer state.  powers: host pointer to S ints (S <= LNB_FILTER_MLP_MAX_S).
  * ------------------------------------------------------------------------------------- */
 int lnb_ritz_power_table(lnb_stream_t stream, const float* D, int64_t rows, const int* powers,
                          int S, float* table /* [rows, S] */);
@@ -389,7 +418,8 @@ int lnb_ritz_power_table(lnb_stream_t stream, const float* D, int64_t rows, cons
  * (S rows); bias_all uses the same row indexing.  lnb_ritz_rowmap builds the compact row list
  * {b*K + k : k < k_eff(b)} from the extents of lnb_graph_prepare (rows of zero-padded Ritz pairs
  * multiply zero Ritz vectors downstream and are skipped; their coeff entries stay unwritten).
- * Requirements: S <= 32, hidden % 32 == 0, hidden <= 128 (else LNB_ERR_UNSUPPORTED).
+ * Requirements: S <= LNB_FILTER_MLP_MAX_S, hidden % 32 == 0, hidden <= LNB_MAX_WIDTH (else
+ * LNB_ERR_UNSUPPORTED).
  * lnb_ritz_filter_mlp_ctas: the same with at most `ctas` persistent CTAs (0: one per SM), e.g. one
  * SM fewer while lnb_tile_assign holds an SM beside it, so no CTA waits for that SM.  An item's
  * arithmetic does not depend on the CTA that runs it: coeff is bit-identical for every `ctas`.
@@ -426,8 +456,8 @@ int lnb_readout(lnb_stream_t stream, const float* state, const float* W_out, con
  * reference collate builds, dataset/qm8.py:196-219), a1/a2/state_bias [C,F], c1/c2 [C].  fp32 dots in
  * feature order, max-subtracted softmax with expf, ELU with expm1f; the channel sum runs in a fixed
  * order, so repeated launches are bit-identical.  Wh, state_bias and out 16-byte aligned.
- * Envelope: N <= 128, F % 4 == 0, F <= 128, E1 <= 16, heads <= 32 (LNB_ERR_UNSUPPORTED otherwise,
- * nothing launched).
+ * Envelope: N <= LNB_MAX_N, F % 4 == 0, F <= LNB_GAT_MAX_WIDTH, E1 <= LNB_MAX_E1, heads <= LNB_GAT_MAX_HEADS
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
  * ------------------------------------------------------------------------------------- */
 int lnb_gat_attention(lnb_stream_t stream, const float* Wh, const float* bias, const float* a1,
                       const float* a2, const float* c1, const float* c2, const float* state_bias,
@@ -495,7 +525,7 @@ int lnb_gat_attention_dropout_backward(lnb_stream_t stream, const float* gout, c
  * X [M, Din], W [C*F, Din] (channel c's weight = rows c*F .. c*F+F-1), Wh [M, C*F]; M_c the input-site
  * mask of (t, c) (the rule above).  No masked copy of X exists: each mask word is drawn once per
  * (row, feature, channel) as the operand tile is loaded.  FFMA in fp32, the sum over d in order.
- * Envelope: Din % 4 == 0, F % 4 == 0, F <= 128; X, W, Wh 16-byte aligned (LNB_ERR_UNSUPPORTED /
+ * Envelope: Din % 4 == 0, F % 4 == 0, F <= LNB_GAT_MAX_WIDTH; X, W, Wh 16-byte aligned (LNB_ERR_UNSUPPORTED /
  * LNB_ERR_ARG otherwise, nothing launched). */
 int lnb_gat_dropout_project(lnb_stream_t stream, const float* X, const float* W, int M, int Din, int C, int F,
                             const int64_t* dropout_key, double p, int t, float* Wh);
@@ -530,8 +560,9 @@ int lnb_gat_dropout_project_backward(lnb_stream_t stream, const float* X, const 
  * is gate g of hidden unit u, g = r, z, n_in, n_h:  r = [W_ir | W_hr], z = [W_iz | W_hz],
  * n_in = [W_in | 0], n_h = [0 | W_hn] (weight_ih / weight_hh of torch.nn.GRUCell); bias [4D] in the same
  * order: b_ir + b_hr, b_iz + b_hz, b_in, b_hn.  M, h, out, W 16-byte aligned.
- * Envelope: 1 <= N <= 255, D % 32 == 0, 32 <= D <= 128, 1 <= E1 <= 16 (LNB_ERR_UNSUPPORTED otherwise,
- * nothing launched).  Summation order is fixed: repeated launches are bit-identical.
+ * Envelope: 1 <= N <= LNB_MAX_N_ELL, D % 32 == 0, 32 <= D <= LNB_MAX_WIDTH, 1 <= E1 <= LNB_MAX_E1
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).  Summation order is fixed: repeated launches are
+ * bit-identical.
  * ------------------------------------------------------------------------------------- */
 int lnb_ggnn_update(lnb_stream_t stream, const float* M, const float* h, const float* ell_val,
                     const uint8_t* ell_idx, const int32_t* ell_max, const float* W_hi, const float* W_lo,
@@ -552,7 +583,7 @@ int lnb_ggnn_update(lnb_stream_t stream, const float* M, const float* h, const f
  * W_hi / W_lo: tf32 split of [W_ih | W_hh] [4D, 2D] (torch.nn.LSTMCell) with row (u/4)*16 + g*4 + u%4 =
  * gate g of hidden unit u, g = i, f, g, o; bias [4D] = b_ih + b_hh in the same order.  state, h, c, out
  * and W 16-byte aligned.
- * Envelope: D % 32 == 0, 32 <= D <= 128, 1 <= E1 <= 16, K >= 1, 0 <= t < K (LNB_ERR_UNSUPPORTED for
+ * Envelope: D % 32 == 0, 32 <= D <= LNB_MAX_WIDTH, 1 <= E1 <= LNB_MAX_E1, K >= 1, 0 <= t < K (LNB_ERR_UNSUPPORTED for
  * D / E1 outside it, nothing launched).  Summation order is fixed: repeated launches are bit-identical.
  * ------------------------------------------------------------------------------------- */
 int lnb_sage_lstm_step(lnb_stream_t stream, const float* state, const int32_t* nn_idx, const float* nonempty,
@@ -574,7 +605,7 @@ int lnb_sage_lstm_step(lnb_stream_t stream, const float* state, const int32_t* n
  * state_func, whose blocks 1 and 2 are the outputs).
  * W_hi / W_lo: tf32 split of gru_gate_matrix of the partition GRUCell, [4H, 2H] (layout of
  * lnb_ggnn_update with E1 = 1); bias [4H].
- * Envelope: 1 <= N <= 255, H % 32 == 0, 32 <= H <= 128; pointers 16-byte aligned and ldm, ldh, ldo
+ * Envelope: 1 <= N <= LNB_MAX_N_ELL, H % 32 == 0, 32 <= H <= LNB_MAX_WIDTH; pointers 16-byte aligned and ldm, ldh, ldo
  * multiples of 4, at least H; no output (nor h_copy) may share an element with any h or with each other.
  * Outside it: LNB_ERR_UNSUPPORTED, nothing launched.  Summation order is fixed: repeated launches are
  * bit-identical.
@@ -598,8 +629,9 @@ int lnb_gpnn_partition_update(lnb_stream_t stream, const float* M0, const float*
  * input part is the folded F = [W_ih,e W2_e]_e | [W_ih,e b2_e]_e (zero padded to 64*E1 + 32 columns).
  * ell_*: lnb_graph_prepare of L [B,N,N,E1].  h and out [B*N, D] (out must not alias h).  PQ, h, out, W
  * 16-byte aligned.  S is computed in the producer warps and never written out.
- * Envelope: 1 <= N <= 255, D % 32 == 0, 32 <= D <= 128, 1 <= E1 <= 16 (LNB_ERR_UNSUPPORTED otherwise,
- * nothing launched).  Summation order is fixed: repeated launches are bit-identical.
+ * Envelope: 1 <= N <= LNB_MAX_N_ELL, D % 32 == 0, 32 <= D <= LNB_MAX_WIDTH, 1 <= E1 <= LNB_MAX_E1
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).  Summation order is fixed: repeated launches are
+ * bit-identical.
  * ------------------------------------------------------------------------------------- */
 int lnb_mpnn_update(lnb_stream_t stream, const float* PQ, const float* h, const float* ell_val,
                     const uint8_t* ell_idx, const int32_t* ell_max, const float* W_hi, const float* W_lo,
@@ -612,7 +644,7 @@ int lnb_mpnn_update(lnb_stream_t stream, const float* PQ, const float* h, const 
  *   gP_e[j] = sum_i A_e[i,j] w_i [P_e[j] + Q_e[i] > 0] gS_e[i]
  * written as gPQ [B*N, E1*128] in the layout of PQ.  ellT_* are lnb_graph_prepare of the transposed
  * operators L.transpose(1, 2) (operators need not be symmetric).  One thread per output element, sums
- * in ELL order, no atomics: deterministic.  Envelope: 1 <= N <= 255, 1 <= E1 <= 16
+ * in ELL order, no atomics: deterministic.  Envelope: 1 <= N <= LNB_MAX_N_ELL, 1 <= E1 <= LNB_MAX_E1
  * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
  * ------------------------------------------------------------------------------------- */
 int lnb_mpnn_edge_aggregate(lnb_stream_t stream, const float* PQ, const float* ell_val, const uint8_t* ell_idx,
@@ -637,7 +669,7 @@ int lnb_mpnn_edge_aggregate_backward(lnb_stream_t stream, const float* PQ, const
  * operator, so on 0/1 operators, weighted or not, both give the same bits.  One thread per output
  * element, no atomics: repeated launches are bit-identical.  A 4-wide path runs when D, the strides and
  * col0 are multiples of 4 and X / out (G / gX) are 16-byte aligned.
- * Envelope: 1 <= N <= 128, 1 <= E1 <= 16, any D >= 1 (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ * Envelope: 1 <= N <= LNB_MAX_N, 1 <= E1 <= LNB_MAX_E1, any D >= 1 (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
  * ------------------------------------------------------------------------------------- */
 int lnb_ell_messages(lnb_stream_t stream, const float* X, int64_t ldx, const float* ell_val, const uint8_t* ell_idx,
                      const int32_t* ell_max, const int32_t* gext, const float* w, int B, int N, int E1, int c0,
@@ -658,8 +690,8 @@ int lnb_ell_messages_adjoint(lnb_stream_t stream, const float* G, int64_t ldg, c
  * X [B,N,D]; mask [B,N] uint8 or NULL; WgT [2D, 4D] = the four gate Linear weights stacked [4D, 2D] and
  * transposed; bg [4D]; W1 [D, D] used as [in, out]; W2 [D]; W_out [P, 2D]; b_out [P]; score [B,P].
  * fp32, every sum in a fixed order: repeated launches are bit-identical.
- * Envelope: 1 <= N <= 128, D % 32 == 0, 32 <= D <= 128, 1 <= P <= 128 (LNB_ERR_UNSUPPORTED otherwise,
- * nothing launched).
+ * Envelope: 1 <= N <= LNB_MAX_N, D % 32 == 0, 32 <= D <= LNB_MAX_WIDTH, 1 <= P <= LNB_SET2VEC_MAX_P
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
  * ------------------------------------------------------------------------------------- */
 int lnb_set2vec(lnb_stream_t stream, const float* X, const uint8_t* mask, const float* WgT, const float* bg,
                 const float* W1, const float* W2, const float* W_out, const float* b_out, int B, int N, int D,
@@ -673,7 +705,8 @@ int lnb_set2vec(lnb_stream_t stream, const float* X, const uint8_t* mask, const 
  *                   (model/cheby_net.py:88-93).
  * Result number i (0-based) is written to out[b, n, (out_col0 + block_of_step[i]) * D + d] when
  * block_of_step[i] >= 0 (host array of `steps` ints); out strides in elements.  One launch for
- * the whole chain: operator and walk stay in shared memory / registers.  N <= 32, steps <= 64
+ * the whole chain: operator and walk stay in shared memory / registers.  N <= LNB_CHAIN_MAX_N,
+ * steps <= LNB_CHAIN_MAX_STEPS
  * (LNB_ERR_UNSUPPORTED otherwise: callers use lnb_batched_gemm per step).
  * ------------------------------------------------------------------------------------- */
 int lnb_operator_chain(lnb_stream_t stream, const float* L, const float* X, int B, int N, int E1,
@@ -689,8 +722,9 @@ int lnb_operator_chain(lnb_stream_t stream, const float* L, const float* X, int 
  * step i (1-based) goes to column block block_of_step[i-1] (< 0: not stored; host array of
  * short_steps ints), the long scales to blocks n_short + s, the edge types to n_short + S + e; every
  * block is D columns wide; out strides in elements.  One CTA per graph, thread per feature column,
- * operators and filters in shared memory, every intermediate in registers.  N <= 32, K <= 32,
- * E1 <= 16, S <= 8 (LNB_ERR_UNSUPPORTED otherwise: callers compose lnb_batched_gemm calls).
+ * operators and filters in shared memory, every intermediate in registers.  N <= LNB_MESSAGES_MAX_N,
+ * K <= LNB_MESSAGES_MAX_K, E1 <= LNB_MAX_E1, S <= LNB_MESSAGES_MAX_S, short_steps <= LNB_CHAIN_MAX_STEPS
+ * (LNB_ERR_UNSUPPORTED otherwise: callers compose lnb_batched_gemm calls).
  * ------------------------------------------------------------------------------------- */
 int lnb_graph_messages(lnb_stream_t stream, const float* L, const float* X, const float* Q,
                        const float* filt, int B, int N, int E1, int D, int K, int S, int dense_filter,
@@ -740,12 +774,12 @@ int lnb_tridiag_ritz(lnb_stream_t stream, const float* alpha, const float* beta,
  * is one rounding of an fp64 value.  Eigenvectors are defined up to sign and, for a repeated
  * eigenvalue, up to a rotation inside its eigenspace.  status[b]: bit 0 = QL sweeps exhausted.
  * One warp per graph for N <= 32, one CTA per graph above; repeated launches are bit-identical.
- * Envelope: 1 <= N <= 128, 1 <= K <= 128 (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ * Envelope: 1 <= N <= LNB_MAX_N, 1 <= K <= LNB_EIGS_MAX_K (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
  *
  * lnb_graph_eigs_sparse: the operator is the fp64 L4 = D^-1/2 (A + I) D^-1/2 of the simple graph
  *   (A summed over bond types; a bond listed twice with one type counts once), built from the sparse
  *   records of lnb_graph_prepare_sparse (sizes, node_ptr, edge_ptr, edges with bond types < E,
- *   1 <= E <= 32, inv_sqrt_deg) with the same fp64 products in the same order, so the solver's input
+ *   1 <= E <= LNB_EIGS_MAX_E, inv_sqrt_deg) with the same fp64 products in the same order, so the solver's input
  *   is bit for bit the matrix the reference hands eigh.  V_rows [node_ptr[B], K]: the rows of the real
  *   nodes, the layout lnb_graph_prepare_sparse reads (data.sparse_collate's).
  * lnb_sym_eigs: the operator is the fp32 A[((b*N + i)*N + j) * elem_stride] (elem_stride = E1 reads
@@ -777,8 +811,9 @@ int lnb_sym_eigs(lnb_stream_t stream, const float* A, int64_t elem_stride, const
  *      part of the pattern (every node keeps its unit self-loop), bit for bit data.partition_operators.
  * status [B]: bit 0 = QL sweeps exhausted, bits 1-3 as above.  One warp per graph for N <= 32, one CTA
  * above; repeated launches are bit-identical; no allocation, no synchronisation (capturable).
- * Envelope: 1 <= N <= 128, 2 <= P <= 16, P < N (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
- * lnb_spectral_partition_draws: the draw count for P, 0 outside 2 <= P <= 16.
+ * Envelope: 1 <= N <= LNB_MAX_N, LNB_PARTITION_MIN_P <= P <= LNB_PARTITION_MAX_P, P < N
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
+ * lnb_spectral_partition_draws: the draw count for P, 0 outside LNB_PARTITION_MIN_P..LNB_PARTITION_MAX_P.
  * ------------------------------------------------------------------------------------- */
 int lnb_spectral_partition_draws(int P);
 int lnb_spectral_partition(lnb_stream_t stream, const float* L, int64_t elem_stride, int B, int N, int P,
@@ -786,14 +821,15 @@ int lnb_spectral_partition(lnb_stream_t stream, const float* L, int64_t elem_str
                            float* L_cluster /* [B,N,N] */, float* L_cut /* [B,N,N] */, int32_t* status /* [B] */);
 
 /* GPNN's graph partition from the sparse records of lnb_graph_prepare_sparse (sizes, edge_ptr, edges;
- * bond types >= E are ignored, E <= 32): steps 2-3 of lnb_spectral_partition on the fp64 L4 that
+ * bond types >= E are ignored, E <= LNB_EIGS_MAX_E): steps 2-3 of lnb_spectral_partition on the fp64 L4 that
  * lnb_graph_eigs_sparse builds (padded rows zero, as the dense entry sees the collated channel 0), so
  * labels and status equal lnb_spectral_partition's on the collated L wherever no node pair carries two
  * bond types (status bit 3 is never set).  Outputs: labels, status, and the ELL rows of the two-channel
  * operator [L_cluster, L_cut] (ell_val / ell_idx [B,2,N,N], ell_max [B,2], gext [B,2] = {N, 0}) in the
  * layout and slot order of lnb_graph_prepare over stack([L_cluster, L_cut], 3) with a zero Q, so
  * lnb_gpnn_partition_update reads them as they are; L_cluster / L_cut [B,N,N] when not NULL (both or
- * neither).  Same envelope as lnb_spectral_partition (and 1 <= E <= 32); capturable, no allocation. */
+ * neither).  Same envelope as lnb_spectral_partition (and 1 <= E <= LNB_EIGS_MAX_E); capturable, no
+ * allocation. */
 int lnb_spectral_partition_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr,
                                   const uint8_t* edges, const double* inv_sqrt_deg, int B, int N, int E, int P,
                                   const double* draws, int32_t* labels /* [B,N] */, int32_t* status /* [B] */,
@@ -803,8 +839,8 @@ int lnb_spectral_partition_sparse(lnb_stream_t stream, const int32_t* sizes, con
 /* GAT's additive attention bias [B,N,N,E1] fp32 from the sparse records (sizes, edge_ptr, edges of
  * lnb_graph_prepare_sparse): bit for bit data.gat_bias of the collated operators, i.e. -0.0 (sign
  * included) on the diagonal of every node (padded ones too) and on every bond of the channel (channel 0:
- * any bond type < E1 - 1, channel e: type e - 1), -1e9 elsewhere.  Envelope: 1 <= N <= 128,
- * 2 <= E1 <= 16 (LNB_ERR_UNSUPPORTED otherwise, nothing launched). */
+ * any bond type < E1 - 1, channel e: type e - 1), -1e9 elsewhere.  Envelope: 1 <= N <= LNB_MAX_N,
+ * 2 <= E1 <= LNB_MAX_E1 (LNB_ERR_UNSUPPORTED otherwise, nothing launched). */
 int lnb_gat_bias_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr, const uint8_t* edges,
                         int B, int N, int E1, float* bias /* [B,N,N,E1] */);
 
@@ -824,7 +860,7 @@ int lnb_gat_bias_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t
  * LNB_LANCZOS_PROPER = the textbook Krylov factorisation (m = #valid + 1 vectors, T_m with m alphas
  * and m-1 betas, no row masking; idx[b] = m) whose Ritz values are eigenvalues of A -- the mode of
  * the online (D, V) provider.
- * Limits: N <= 1024, K <= 64 and a basis of K*(N+1) floats within shared memory
+ * Limits: N <= LNB_LANCZOS_FUSED_MAX_N, K <= LNB_LANCZOS_MAX_K and a basis of K*(N+1) floats within shared memory
  * (LNB_ERR_UNSUPPORTED otherwise: use lnb_lanczos_tridiag + lnb_tridiag_ritz).
  * ------------------------------------------------------------------------------------- */
 #define LNB_LANCZOS_PROPER 1
@@ -836,7 +872,7 @@ int lnb_lanczos_ritz(lnb_stream_t stream, const float* A, const uint8_t* mask, c
 /* ---------------------------------------------------------------------------------------
  * Powers of the tridiagonal for the learned filter (model/ada_lanczos_net.py:262-274):
  *   out[b, r, s, c] = (T_b ** powers[s])[r, c]    (the MLP input layout r*S*K + s*K + c)
- * powers: host pointer to S strictly increasing positive ints.
+ * powers: host pointer to S strictly increasing positive ints, S <= LNB_TRIDIAG_POWERS_MAX_S.
  * ------------------------------------------------------------------------------------- */
 int lnb_tridiag_powers(lnb_stream_t stream, const float* T, int B, int K, const int* powers, int S,
                        float* out /* [B,K,S,K] */);
@@ -850,8 +886,8 @@ int lnb_tridiag_powers(lnb_stream_t stream, const float* T, int B, int K, const 
  * lnb_lanczos_tridiag_backward recomputes that forward with the same code (T, Q: its recomputed outputs,
  * optional, bit-equal to the training entry's) and writes gA [B,N,N] = d<gT,T> + <gQ,Q> / dA, the exact
  * adjoint of the recurrence with acceptance, idx and masks as data; no atomics (deterministic).
- * mask may be NULL (every node real).  Limits: 1 <= N <= 128, 1 <= K <= 64 (LNB_ERR_UNSUPPORTED
- * otherwise, nothing launched).
+ * mask may be NULL (every node real).  Limits: 1 <= N <= LNB_LANCZOS_TRAIN_MAX_N, 1 <= K <= LNB_LANCZOS_MAX_K
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
  * ------------------------------------------------------------------------------------- */
 int lnb_lanczos_tridiag_train(lnb_stream_t stream, const float* A /* [B,N,N] */, const uint8_t* mask,
                               const float* q1 /* [B,N] */, int B, int N, int K, float* T, float* Q,
@@ -866,7 +902,7 @@ int lnb_lanczos_tridiag_backward(lnb_stream_t stream, const float* A, const uint
  * P_1 = T and P_{p+1} = P_p Tri(T) with Tri(T) the three diagonals of T (the forward reads only those).
  * One CTA per graph recomputes P_1 .. P_{pmax-1} in shared memory and runs the reverse sweep, no atomics
  * (deterministic).  Limit: (6 K + (powers[S-1] + 1) K^2) floats within 227 KB of shared memory
- * (LNB_ERR_UNSUPPORTED otherwise, nothing launched); S <= 32.
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched); S <= LNB_TRIDIAG_POWERS_MAX_S.
  * ------------------------------------------------------------------------------------- */
 int lnb_tridiag_powers_backward(lnb_stream_t stream, const float* T /* [B,K,K] */,
                                 const float* gOut /* [B,K,S,K] */, int B, int K, const int* powers, int S,

@@ -18,9 +18,7 @@
 namespace {
 
 constexpr int BP_THREADS = 256;
-constexpr int BP_EMAX = 16;      // operator channels (bond types + 1)
-constexpr int BP_NMAX = 128;     // padded nodes per graph (4 x 32-bit adjacency words per row)
-constexpr int BP_NW = BP_NMAX / 32;
+constexpr int BP_NW = LNB_MAX_N / 32;   // 32-bit adjacency words per row
 
 struct SparseBatchParams {
   const int32_t* sizes;        // [B] real nodes per graph
@@ -49,9 +47,9 @@ __device__ __forceinline__ int entry_mult(const uint32_t* rowmask, int E, int ch
   const uint32_t bit = 1u << (j & 31);
   int m = (i == j) ? 1 : 0;                        // the + I of L4
   if (ch == 0) {
-    for (int c = 0; c < E; ++c) m += (rowmask[(c * BP_NMAX + i) * BP_NW + w] & bit) ? 1 : 0;
+    for (int c = 0; c < E; ++c) m += (rowmask[(c * LNB_MAX_N + i) * BP_NW + w] & bit) ? 1 : 0;
   } else {
-    m += (rowmask[((ch - 1) * BP_NMAX + i) * BP_NW + w] & bit) ? 1 : 0;
+    m += (rowmask[((ch - 1) * LNB_MAX_N + i) * BP_NW + w] & bit) ? 1 : 0;
   }
   return m;
 }
@@ -77,7 +75,7 @@ template <bool kFeat>
 __global__ void __launch_bounds__(BP_THREADS)
 batch_prepare_sparse_kernel(const SparseBatchParams P) {
   extern __shared__ __align__(16) unsigned char bp_smem[];
-  __shared__ int s_max[BP_EMAX];
+  __shared__ int s_max[LNB_MAX_E1];
   __shared__ int s_ke;
   const int b = blockIdx.x, tid = threadIdx.x;
   const int N = P.N, E1 = P.E1, E = E1 - 1, K = P.K;
@@ -102,11 +100,11 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
   }
   const int nb = min(max(sizes[b], 0), N);
   uint32_t* rowmask = reinterpret_cast<uint32_t*>(bp_smem);              // [E][NMAX][NW]
-  double* scale = reinterpret_cast<double*>(rowmask + (size_t)E * BP_NMAX * BP_NW);   // [E1][NMAX]
-  uint8_t* cnt_s = reinterpret_cast<uint8_t*>(scale + (size_t)E1 * BP_NMAX);          // [N*E1]
+  double* scale = reinterpret_cast<double*>(rowmask + (size_t)E * LNB_MAX_N * BP_NW);   // [E1][NMAX]
+  uint8_t* cnt_s = reinterpret_cast<uint8_t*>(scale + (size_t)E1 * LNB_MAX_N);          // [N*E1]
 
-  for (int i = tid; i < E * BP_NMAX * BP_NW; i += BP_THREADS) rowmask[i] = 0u;
-  if (tid < BP_EMAX) s_max[tid] = 0;
+  for (int i = tid; i < E * LNB_MAX_N * BP_NW; i += BP_THREADS) rowmask[i] = 0u;
+  if (tid < LNB_MAX_E1) s_max[tid] = 0;
   if (tid == 0) s_ke = 0;
   __syncthreads();
   // ---- adjacency bitmaps from the bond list (idempotent: duplicates do not double count) ----------
@@ -115,8 +113,8 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
     const uchar4 ed = reinterpret_cast<const uchar4*>(edges)[e];
     const int u = ed.x, v = ed.y, c = ed.z;
     if (u < nb && v < nb && c < E) {
-      atomicOr(&rowmask[(c * BP_NMAX + u) * BP_NW + (v >> 5)], 1u << (v & 31));
-      atomicOr(&rowmask[(c * BP_NMAX + v) * BP_NW + (u >> 5)], 1u << (u & 31));
+      atomicOr(&rowmask[(c * LNB_MAX_N + u) * BP_NW + (v >> 5)], 1u << (v & 31));
+      atomicOr(&rowmask[(c * LNB_MAX_N + v) * BP_NW + (u >> 5)], 1u << (u & 31));
     }
   }
   __syncthreads();
@@ -128,13 +126,13 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
       int deg = 1;
       if (ch == 0) {
         for (int c = 0; c < E; ++c)
-          for (int w = 0; w < BP_NW; ++w) deg += __popc(rowmask[(c * BP_NMAX + i) * BP_NW + w]);
+          for (int w = 0; w < BP_NW; ++w) deg += __popc(rowmask[(c * LNB_MAX_N + i) * BP_NW + w]);
       } else {
-        for (int w = 0; w < BP_NW; ++w) deg += __popc(rowmask[((ch - 1) * BP_NMAX + i) * BP_NW + w]);
+        for (int w = 0; w < BP_NW; ++w) deg += __popc(rowmask[((ch - 1) * LNB_MAX_N + i) * BP_NW + w]);
       }
       sc = P.inv_sqrt_deg[min(deg, LNB_INV_SQRT_DEG_LEN - 1)];
     }
-    scale[ch * BP_NMAX + i] = sc;
+    scale[ch * LNB_MAX_N + i] = sc;
   }
   __syncthreads();
   // ---- ELL rows, same order as lnb_graph_prepare: diagonal first, then ascending column ------------
@@ -146,7 +144,7 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
     uint8_t* idx = P.ell_idx + ((int64_t)(b * E1 + ch) * N) * N + n;
     int cnt = 0;
     if (n < nb) {
-      const double sn = scale[ch * BP_NMAX + n];
+      const double sn = scale[ch * LNB_MAX_N + n];
       {
         const int m = entry_mult(rowmask, E, ch, n, n);
         const float v = __double2float_rn((sn * (double)m) * sn);
@@ -154,14 +152,14 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
       }
       for (int w = 0; w < BP_NW; ++w) {
         uint32_t bits = 0u;
-        if (ch == 0) { for (int c = 0; c < E; ++c) bits |= rowmask[(c * BP_NMAX + n) * BP_NW + w]; }
-        else bits = rowmask[((ch - 1) * BP_NMAX + n) * BP_NW + w];
+        if (ch == 0) { for (int c = 0; c < E; ++c) bits |= rowmask[(c * LNB_MAX_N + n) * BP_NW + w]; }
+        else bits = rowmask[((ch - 1) * LNB_MAX_N + n) * BP_NW + w];
         while (bits) {
           const int j = (w << 5) + __ffs(bits) - 1;
           bits &= bits - 1;
           if (j == n) continue;
           const int m = entry_mult(rowmask, E, ch, n, j);
-          const float v = __double2float_rn((sn * (double)m) * scale[ch * BP_NMAX + j]);
+          const float v = __double2float_rn((sn * (double)m) * scale[ch * LNB_MAX_N + j]);
           if (v != 0.f) {
             val[(int64_t)cnt * N] = binarize ? 1.f : v;
             idx[(int64_t)cnt * N] = (uint8_t)j;
@@ -210,7 +208,7 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
       float v = 0.f;
       if (r < nb && c < nb) {
         const int m = entry_mult(rowmask, E, ch, r, c);
-        if (m) v = __double2float_rn((scale[ch * BP_NMAX + r] * (double)m) * scale[ch * BP_NMAX + c]);
+        if (m) v = __double2float_rn((scale[ch * LNB_MAX_N + r] * (double)m) * scale[ch * LNB_MAX_N + c]);
       }
       Lg[i] = v;
     }
@@ -249,7 +247,8 @@ template <bool kFeat>
 static int launch_sparse(lnb_stream_t stream, SparseBatchParams p, int32_t* tiles, int32_t* rowmap,
                          int32_t* nrows) {
   p.rowmap = rowmap; p.nrows = nrows;
-  const size_t smem = (size_t)(p.E1 - 1) * BP_NMAX * BP_NW * 4 + (size_t)p.E1 * BP_NMAX * 8 + (size_t)p.N * p.E1 + 16;
+  const size_t smem = (size_t)(p.E1 - 1) * LNB_MAX_N * BP_NW * 4 + (size_t)p.E1 * LNB_MAX_N * 8 +
+                       (size_t)p.N * p.E1 + 16;
   cudaStream_t s = (cudaStream_t)stream;
   if (smem > 48 * 1024)
     cudaFuncSetAttribute(batch_prepare_sparse_kernel<kFeat>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -271,9 +270,9 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
                              int K, int flags, float* ell_val, uint8_t* ell_idx, int32_t* ell_max,
                              int32_t* gext, int32_t* tiles, int32_t* rowmap, int32_t* nrows,
                              int64_t* node_ids, uint8_t* mask, float* V, float* L_dense) {
-  LNB_REQUIRE(B >= 0 && N >= 1 && N <= BP_NMAX && E1 >= 2 && E1 <= BP_EMAX && K >= 1,
+  LNB_REQUIRE(B >= 0 && N >= 1 && N <= LNB_MAX_N && E1 >= 2 && E1 <= LNB_MAX_E1 && K >= 1,
               "graph_prepare_sparse: bad dims B=%d N=%d E1=%d K=%d (N <= %d, 2 <= E1 <= %d)", B, N, E1,
-              K, BP_NMAX, BP_EMAX);
+              K, LNB_MAX_N, LNB_MAX_E1);
   if (B == 0) return LNB_OK;
   // edges may be NULL when the batch has no bonds: the kernel reads [edge_ptr[b], edge_ptr[b+1]) only
   LNB_REQUIRE(sizes && node_ptr && node_feat && edge_ptr && V_rows && inv_sqrt_deg &&
@@ -295,7 +294,7 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
                                     uint8_t* ell_idx, int32_t* ell_max, int32_t* gext, int32_t* tiles,
                                     int32_t* rowmap, int32_t* nrows, int64_t* node_ids, uint8_t* mask,
                                     float* V, float* L_dense) {
-  LNB_REQUIRE(B >= 0 && N >= 1 && N <= BP_NMAX && E1 >= 2 && E1 <= BP_EMAX && K >= 1,
+  LNB_REQUIRE(B >= 0 && N >= 1 && N <= LNB_MAX_N && E1 >= 2 && E1 <= LNB_MAX_E1 && K >= 1,
               "graph_prepare_sparse_packed: bad dims B=%d N=%d E1=%d K=%d", B, N, E1, K);
   if (B == 0) return LNB_OK;
   LNB_REQUIRE(blob && inv_sqrt_deg && ell_val && ell_idx && ell_max && gext &&
@@ -319,9 +318,10 @@ int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes,
                                       int K, int F, int flags, float* ell_val, uint8_t* ell_idx,
                                       int32_t* ell_max, int32_t* gext, int32_t* tiles, int32_t* rowmap,
                                       int32_t* nrows, float* X, uint8_t* mask, float* V, float* L_dense) {
-  if (!(B >= 0 && N >= 1 && N <= BP_NMAX && E1 >= 2 && E1 <= BP_EMAX && K >= 1 && F >= 1 && F <= 4096)) {
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && E1 >= 2 && E1 <= LNB_MAX_E1 && K >= 1 && F >= 1 &&
+        F <= LNB_PREPARE_MAX_F)) {
     lnb::set_err("graph_prepare_sparse_features: B=%d N=%d E1=%d K=%d F=%d outside 1 <= N <= %d, "
-                 "2 <= E1 <= %d, K >= 1, 1 <= F <= 4096", B, N, E1, K, F, BP_NMAX, BP_EMAX);
+                 "2 <= E1 <= %d, K >= 1, 1 <= F <= 4096", B, N, E1, K, F, LNB_MAX_N, LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;
@@ -343,9 +343,9 @@ int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes,
 
 int lnb_gat_bias_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* edge_ptr, const uint8_t* edges,
                         int B, int N, int E1, float* bias) {
-  if (!(B >= 0 && N >= 1 && N <= BP_NMAX && E1 >= 2 && E1 <= BP_EMAX)) {
-    lnb::set_err("gat_bias_sparse: B=%d N=%d E1=%d outside 1 <= N <= %d, 2 <= E1 <= %d", B, N, E1, BP_NMAX,
-                 BP_EMAX);
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && E1 >= 2 && E1 <= LNB_MAX_E1)) {
+    lnb::set_err("gat_bias_sparse: B=%d N=%d E1=%d outside 1 <= N <= %d, 2 <= E1 <= %d", B, N, E1, LNB_MAX_N,
+                 LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;

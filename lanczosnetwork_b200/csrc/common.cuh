@@ -9,6 +9,9 @@
 
 namespace lnb {
 
+// dynamic shared memory one CTA may opt in to on sm_90a
+constexpr int SMEM_MAX = 227 * 1024;
+
 // thread-local error text + launch counter (no other global mutable state)
 char* err_buf();
 void set_err(const char* fmt, ...);

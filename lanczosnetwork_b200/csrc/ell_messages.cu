@@ -14,8 +14,6 @@
 
 namespace {
 
-constexpr int EM_NMAX = 128;
-constexpr int EM_E1MAX = 16;
 constexpr int EM_THREADS = 256;
 
 struct EllParams {
@@ -131,8 +129,8 @@ int ell_checks(const char* who, const EllParams& p) {
   LNB_REQUIRE(p.val && p.idx && p.ell_max && p.gext && p.in && p.out, "%s: null pointer", who);
   LNB_REQUIRE(p.B >= 0 && p.N >= 1 && p.E1 >= 1 && p.D >= 1, "%s: bad dims B=%d N=%d E1=%d D=%d", who, p.B, p.N,
               p.E1, p.D);
-  if (p.N > EM_NMAX || p.E1 > EM_E1MAX) {
-    lnb::set_err("%s: N=%d E1=%d outside the kernel (N <= %d, E1 <= %d)", who, p.N, p.E1, EM_NMAX, EM_E1MAX);
+  if (p.N > LNB_MAX_N || p.E1 > LNB_MAX_E1) {
+    lnb::set_err("%s: N=%d E1=%d outside the kernel (N <= %d, E1 <= %d)", who, p.N, p.E1, LNB_MAX_N, LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE(p.c0 >= 0 && p.nc >= 1 && p.c0 + p.nc <= p.E1, "%s: channels [%d, %d) outside [0, %d)", who, p.c0,

@@ -285,7 +285,7 @@ int lnb_ritz_filter_mlp_ctas(lnb_stream_t stream, const float* table, const int3
   LNB_REQUIRE(table && W_hi && W_lo && bias_all && coeff, "ritz_filter_mlp: null pointer");
   LNB_REQUIRE((rowmap == nullptr) == (nrows == nullptr), "ritz_filter_mlp: rowmap and nrows go together");
   LNB_REQUIRE(Rall >= 0 && L >= 1 && S >= 1 && Hd >= 1 && ctas >= 0, "ritz_filter_mlp: bad dims");
-  if (S > 32 || Hd % 32 != 0 || Hd > tcg::BN) {
+  if (S > LNB_FILTER_MLP_MAX_S || Hd % 32 != 0 || Hd > LNB_MAX_WIDTH) {
     lnb::set_err("ritz_filter_mlp: unsupported shape S=%d hidden=%d (needs S<=32, hidden%%32==0, hidden<=128)", S, Hd);
     return LNB_ERR_UNSUPPORTED;
   }

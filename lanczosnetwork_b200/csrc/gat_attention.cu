@@ -21,9 +21,7 @@
 namespace {
 
 constexpr int GAT_THREADS = 256;
-constexpr int GAT_NMAX = 128, GAT_FMAX = 128, GAT_E1MAX = 16, GAT_HEADSMAX = 32;
 constexpr size_t GAT_SMEM_TARGET = 48 * 1024;     // head groups are sized to this when possible
-constexpr size_t GAT_SMEM_MAX = 227 * 1024;
 
 struct GatParams {
   const float* Wh;          // [B, N, C*F]
@@ -531,7 +529,7 @@ size_t gat_bwd_smem_floats(int N, int F, int G) {
 }
 
 bool gat_shape_ok(int N, int F, int E1, int heads) {
-  return N <= GAT_NMAX && F % 4 == 0 && F <= GAT_FMAX && E1 <= GAT_E1MAX && heads <= GAT_HEADSMAX;
+  return N <= LNB_MAX_N && F % 4 == 0 && F <= LNB_GAT_MAX_WIDTH && E1 <= LNB_MAX_E1 && heads <= LNB_GAT_MAX_HEADS;
 }
 
 // the launches of lnb_gat_attention(_backward) and of their dropout forms (drop != nullptr); `who` prefixes
@@ -542,10 +540,10 @@ int launch_gat_attention(cudaStream_t stream, const char* who, const float* Wh, 
                          const lnb::GatDrop* drop) {
   LNB_REQUIRE(Wh && bias && a1 && a2 && c1 && c2 && state_bias && out, "%s: null pointer", who);
   LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && heads >= 1 && F >= 1, "%s: bad dims", who);
-  if (N > GAT_NMAX || F % 4 || F > GAT_FMAX || E1 > GAT_E1MAX || heads > GAT_HEADSMAX) {
+  if (!gat_shape_ok(N, F, E1, heads)) {
     lnb::set_err("%s: N=%d F=%d E1=%d heads=%d outside the kernel (N <= %d, F %% 4 == 0, "
-                 "F <= %d, E1 <= %d, heads <= %d)", who, N, F, E1, heads, GAT_NMAX, GAT_FMAX, GAT_E1MAX,
-                 GAT_HEADSMAX);
+                 "F <= %d, E1 <= %d, heads <= %d)", who, N, F, E1, heads, LNB_MAX_N, LNB_GAT_MAX_WIDTH, LNB_MAX_E1,
+                 LNB_GAT_MAX_HEADS);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE(((uintptr_t)Wh | (uintptr_t)state_bias | (uintptr_t)out) % 16 == 0,
@@ -555,7 +553,7 @@ int launch_gat_attention(cudaStream_t stream, const char* who, const float* Wh, 
   int G = heads;
   while (G > 1 && gat_smem_floats(N, F, G) * sizeof(float) > GAT_SMEM_TARGET) --G;
   const size_t shm = gat_smem_floats(N, F, G) * sizeof(float);
-  LNB_REQUIRE(shm <= GAT_SMEM_MAX, "%s: %zu bytes of shared memory", who, shm);
+  LNB_REQUIRE(shm <= lnb::SMEM_MAX, "%s: %zu bytes of shared memory", who, shm);
   const int ngroups = (heads + G - 1) / G;
   const int64_t grid = last ? (int64_t)B : (int64_t)B * E1 * ngroups;
   LNB_REQUIRE(grid <= 0x7fffffff, "%s: B=%d too large", who, B);
@@ -584,8 +582,8 @@ int launch_gat_attention_backward(cudaStream_t stream, const char* who, const fl
   LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && heads >= 1 && F >= 1, "%s: bad dims", who);
   if (!gat_shape_ok(N, F, E1, heads)) {
     lnb::set_err("%s: N=%d F=%d E1=%d heads=%d outside the kernel (N <= %d, F %% 4 == 0, "
-                 "F <= %d, E1 <= %d, heads <= %d)", who, N, F, E1, heads, GAT_NMAX, GAT_FMAX, GAT_E1MAX,
-                 GAT_HEADSMAX);
+                 "F <= %d, E1 <= %d, heads <= %d)", who, N, F, E1, heads, LNB_MAX_N, LNB_GAT_MAX_WIDTH, LNB_MAX_E1,
+                 LNB_GAT_MAX_HEADS);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE(((uintptr_t)gout | (uintptr_t)Wh | (uintptr_t)a1 | (uintptr_t)a2 | (uintptr_t)state_bias |
@@ -595,7 +593,7 @@ int launch_gat_attention_backward(cudaStream_t stream, const char* who, const fl
   int G = heads;
   while (G > 1 && gat_bwd_smem_floats(N, F, G) * sizeof(float) > GAT_SMEM_TARGET) --G;
   const size_t shm = gat_bwd_smem_floats(N, F, G) * sizeof(float);
-  LNB_REQUIRE(shm <= GAT_SMEM_MAX, "%s: %zu bytes of shared memory", who, shm);
+  LNB_REQUIRE(shm <= lnb::SMEM_MAX, "%s: %zu bytes of shared memory", who, shm);
   const int ngroups = (heads + G - 1) / G;
   const int64_t grid = (int64_t)B * E1 * ngroups;
   LNB_REQUIRE(grid <= 0x7fffffff, "%s: B=%d too large", who, B);

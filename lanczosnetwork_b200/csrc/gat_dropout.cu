@@ -18,7 +18,7 @@
 namespace {
 
 constexpr int PJ_THREADS = 256;
-constexpr int PJ_BM = 128, PJ_BK = 32, PJ_FMAX = 128, PJ_RTMAX = 16;
+constexpr int PJ_BM = 128, PJ_BK = 32, PJ_RTMAX = 16;
 constexpr int PB_BM = 64, PB_BD = 32;
 constexpr int64_t PB_WORK_FLOATS = 16 << 20;        // slabs are capped so the partials stay within 64 MB
 
@@ -26,7 +26,7 @@ __global__ void __launch_bounds__(PJ_THREADS)
 gat_dropout_project_kernel(const float* __restrict__ X, const float* __restrict__ W, int M, int Din, int C,
                            int F, lnb::GatDrop d, float* __restrict__ Wh) {
   __shared__ __align__(16) float Xs[PJ_BK][PJ_BM + 4];       // X * M_c s, transposed
-  __shared__ __align__(16) float Ws[PJ_BK][PJ_FMAX];         // W_c^T
+  __shared__ __align__(16) float Ws[PJ_BK][LNB_GAT_MAX_WIDTH];         // W_c^T
   const int tid = threadIdx.x;
   const int c = blockIdx.y;
   const int m0 = blockIdx.x * PJ_BM;
@@ -250,10 +250,10 @@ int check_project(const char* who, const void* X, const void* W, const void* out
   LNB_REQUIRE(X && W && out && key, "%s: null pointer", who);
   LNB_REQUIRE(M >= 0 && Din >= 1 && C >= 1 && F >= 1, "%s: bad dims M=%d Din=%d C=%d F=%d", who, M, Din, C, F);
   LNB_REQUIRE(p >= 0.0 && p <= 1.0, "%s: p=%g outside [0, 1]", who, p);
-  if (Din % 4 || F % 4 || F > PJ_FMAX || t < 0 || t >= (1 << 16) || C > (1 << 14) ||
+  if (Din % 4 || F % 4 || F > LNB_GAT_MAX_WIDTH || t < 0 || t >= (1 << 16) || C > (1 << 14) ||
       (int64_t)M * Din >= (int64_t(1) << 34) || (int64_t)C * F > 0x7fffffff) {
     lnb::set_err("%s: Din=%d F=%d C=%d t=%d M=%d outside the kernel (Din %% 4 == 0, F %% 4 == 0, F <= %d) or the "
-                 "mask rule (t < 2^16, C <= 2^14, M*Din < 2^34)", who, Din, F, C, t, M, PJ_FMAX);
+                 "mask rule (t < 2^16, C <= 2^14, M*Din < 2^34)", who, Din, F, C, t, M, LNB_GAT_MAX_WIDTH);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE(((uintptr_t)X | (uintptr_t)W | (uintptr_t)out) % 16 == 0, "%s: X, W and the output must be 16-byte "

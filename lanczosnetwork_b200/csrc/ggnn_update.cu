@@ -13,7 +13,6 @@
 
 namespace {
 
-constexpr int GG_DMAX = 128, GG_NMAX = 255, GG_E1MAX = 16;
 
 struct GgnnUpdateParams {
   const float* M;          // [rows, E1*D]
@@ -66,9 +65,9 @@ int lnb_ggnn_update(lnb_stream_t stream, const float* M, const float* h, const f
               "ggnn_update: null pointer");
   LNB_REQUIRE(B >= 0 && N >= 1 && D >= 1 && E1 >= 1, "ggnn_update: bad dims B=%d N=%d D=%d E1=%d", B, N, D,
               E1);
-  if (N > GG_NMAX || D % 32 || D > GG_DMAX || E1 > GG_E1MAX) {
+  if (N > LNB_MAX_N_ELL || D % 32 || D > LNB_MAX_WIDTH || E1 > LNB_MAX_E1) {
     lnb::set_err("ggnn_update: N=%d D=%d E1=%d outside the kernel (N <= %d, D %% 32 == 0, D <= %d, "
-                 "E1 <= %d)", N, D, E1, GG_NMAX, GG_DMAX, GG_E1MAX);
+                 "E1 <= %d)", N, D, E1, LNB_MAX_N_ELL, LNB_MAX_WIDTH, LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE(((uintptr_t)M | (uintptr_t)h | (uintptr_t)out | (uintptr_t)W_hi | (uintptr_t)W_lo) % 16 == 0,

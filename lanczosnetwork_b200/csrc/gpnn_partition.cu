@@ -17,7 +17,6 @@
 
 namespace {
 
-constexpr int GP_HMAX = 128, GP_NMAX = 255;
 constexpr int GP_PARTS = 2;                   // cluster, cut
 
 struct GpnnPartitionParams {
@@ -129,9 +128,9 @@ int lnb_gpnn_partition_update(lnb_stream_t stream, const float* M0, const float*
     ++np;
   }
   LNB_REQUIRE(np > 0 || !h_copy, "gpnn_partition_update: h_copy needs an active part");
-  if (N > GP_NMAX || H % 32 || H < 32 || H > GP_HMAX) {
+  if (N > LNB_MAX_N_ELL || H % 32 || H < 32 || H > LNB_MAX_WIDTH) {
     lnb::set_err("gpnn_partition_update: N=%d H=%d outside the kernel (N <= %d, H %% 32 == 0, 32 <= H <= %d)",
-                 N, H, GP_NMAX, GP_HMAX);
+                 N, H, LNB_MAX_N_ELL, LNB_MAX_WIDTH);
     return LNB_ERR_UNSUPPORTED;
   }
   uintptr_t al = (uintptr_t)W_hi | (uintptr_t)W_lo | (uintptr_t)h_copy;

@@ -15,9 +15,6 @@ namespace {
 
 using namespace eigs;
 
-constexpr int GE_KMAX = 128;
-constexpr int GE_EMAX = 32;      // bond types of the sparse producer (one bit each)
-
 struct EigParams {
   // dense producer: A[((b * N + i) * N + j) * es], lower triangle read (eigh's default UPLO='L')
   const float* A; int64_t es;
@@ -132,9 +129,9 @@ int launch(lnb_stream_t stream, const EigParams& p, const char* what) {
   return lnb::finish_launch(what);
 }
 
-static_assert(sizeof(double) * graph_doubles(GE_NMAX, 4) <= 227 * 1024,
+static_assert(sizeof(double) * graph_doubles(LNB_MAX_N, 4) <= lnb::SMEM_MAX,
               "graph_eigs: N = 128 must fit one CTA's shared memory");
-static_assert(4 * sizeof(double) * graph_doubles(32, 1) <= 227 * 1024, "graph_eigs: four N = 32 graphs per CTA");
+static_assert(4 * sizeof(double) * graph_doubles(32, 1) <= lnb::SMEM_MAX, "graph_eigs: four N = 32 graphs per CTA");
 
 }  // namespace
 
@@ -143,9 +140,9 @@ extern "C" {
 int lnb_graph_eigs_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t* node_ptr,
                           const int32_t* edge_ptr, const uint8_t* edges, const double* inv_sqrt_deg, int B,
                           int N, int E, int K, float* D, float* V_rows, int32_t* status) {
-  if (!(B >= 0 && N >= 1 && N <= GE_NMAX && K >= 1 && K <= GE_KMAX && E >= 1 && E <= GE_EMAX)) {
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && K >= 1 && K <= LNB_EIGS_MAX_K && E >= 1 && E <= LNB_EIGS_MAX_E)) {
     lnb::set_err("graph_eigs_sparse: B=%d N=%d E=%d K=%d outside 1 <= N <= %d, 1 <= K <= %d, 1 <= E <= %d",
-                 B, N, E, K, GE_NMAX, GE_KMAX, GE_EMAX);
+                 B, N, E, K, LNB_MAX_N, LNB_EIGS_MAX_K, LNB_EIGS_MAX_E);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;
@@ -160,9 +157,9 @@ int lnb_graph_eigs_sparse(lnb_stream_t stream, const int32_t* sizes, const int32
 
 int lnb_sym_eigs(lnb_stream_t stream, const float* A, int64_t elem_stride, const int32_t* sizes, int B, int N,
                  int K, float* D, float* V, int32_t* status) {
-  if (!(B >= 0 && N >= 1 && N <= GE_NMAX && K >= 1 && K <= GE_KMAX && elem_stride >= 1)) {
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && K >= 1 && K <= LNB_EIGS_MAX_K && elem_stride >= 1)) {
     lnb::set_err("sym_eigs: B=%d N=%d K=%d stride=%lld outside 1 <= N <= %d, 1 <= K <= %d", B, N, K,
-                 (long long)elem_stride, GE_NMAX, GE_KMAX);
+                 (long long)elem_stride, LNB_MAX_N, LNB_EIGS_MAX_K);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;

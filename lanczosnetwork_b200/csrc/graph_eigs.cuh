@@ -20,7 +20,6 @@
 namespace eigs {
 
 constexpr int GE_THREADS = 128;
-constexpr int GE_NMAX = 128;     // same limit as lnb_graph_prepare_sparse
 constexpr int GE_SWEEPS = 60;    // QL sweeps per eigenvalue before status bit 0 is set
 
 // packed lower triangle, row-major: element (i, j), i >= j

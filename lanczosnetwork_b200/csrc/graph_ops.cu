@@ -168,21 +168,20 @@ gaussian_laplacian_kernel(const float* __restrict__ x, const float* __restrict__
 // live in shared memory; a thread keeps its column of the new walk in N <= 32 registers, so one
 // step costs N^2 FMA + N^2/4 broadcast loads per thread.  Selected steps are written straight into
 // their column block of the message matrix (block index = sel[step], < 0: not stored).
-constexpr int CHAIN_NMAX = 32, CHAIN_STEPS_MAX = 64;
-struct ChainSel { int8_t blk[CHAIN_STEPS_MAX]; };
+struct ChainSel { int8_t blk[LNB_CHAIN_MAX_STEPS]; };
 
 __global__ void __launch_bounds__(128)
 operator_chain_kernel(const float* __restrict__ L, const float* __restrict__ X, int N, int E1, int D,
                       int steps, int cheby, ChainSel sel, float* __restrict__ out, int64_t out_sb,
                       int64_t out_sn, int out_col0) {
-  __shared__ __align__(16) float Lt[CHAIN_NMAX][CHAIN_NMAX];   // Lt[i][n] = L_0[n][i]
+  __shared__ __align__(16) float Lt[LNB_CHAIN_MAX_N][LNB_CHAIN_MAX_N];   // Lt[i][n] = L_0[n][i]
   extern __shared__ __align__(16) float walk[];                // [2][N][Dc] ping-pong, Dc = blockDim.x
   const int g = blockIdx.x, d0 = blockIdx.y * blockDim.x, t = threadIdx.x;
   const int Dc = blockDim.x;
   const bool live = d0 + t < D;
   const float* Lg = L + (int64_t)g * N * N * E1;
-  for (int e = t; e < CHAIN_NMAX * CHAIN_NMAX; e += Dc) {
-    const int i = e / CHAIN_NMAX, n = e % CHAIN_NMAX;
+  for (int e = t; e < LNB_CHAIN_MAX_N * LNB_CHAIN_MAX_N; e += Dc) {
+    const int i = e / LNB_CHAIN_MAX_N, n = e % LNB_CHAIN_MAX_N;
     Lt[i][n] = (i < N && n < N) ? __ldg(Lg + ((int64_t)n * N + i) * E1) : 0.f;
   }
   float* w0 = walk;
@@ -191,18 +190,18 @@ operator_chain_kernel(const float* __restrict__ L, const float* __restrict__ X, 
   for (int n = 0; n < N; ++n) w0[n * Dc + t] = live ? __ldg(Xg + (int64_t)n * D + t) : 0.f;
   __syncthreads();
   float* og = out + (int64_t)g * out_sb + d0 + t;
-  float prev2[CHAIN_NMAX];                                     // Chebyshev: s_{k-2} of this column
+  float prev2[LNB_CHAIN_MAX_N];                                     // Chebyshev: s_{k-2} of this column
 #pragma unroll
-  for (int n = 0; n < CHAIN_NMAX; ++n) prev2[n] = (cheby && n < N) ? w0[n * Dc + t] : 0.f;
+  for (int n = 0; n < LNB_CHAIN_MAX_N; ++n) prev2[n] = (cheby && n < N) ? w0[n * Dc + t] : 0.f;
   for (int s = 0; s < steps; ++s) {
-    float acc[CHAIN_NMAX];
+    float acc[LNB_CHAIN_MAX_N];
 #pragma unroll
-    for (int n = 0; n < CHAIN_NMAX; ++n) acc[n] = 0.f;
+    for (int n = 0; n < LNB_CHAIN_MAX_N; ++n) acc[n] = 0.f;
     for (int i = 0; i < N; ++i) {
       const float o = w0[i * Dc + t];
       const float4* l4 = reinterpret_cast<const float4*>(&Lt[i][0]);
 #pragma unroll
-      for (int q = 0; q < CHAIN_NMAX / 4; ++q) {
+      for (int q = 0; q < LNB_CHAIN_MAX_N / 4; ++q) {
         const float4 l = l4[q];
         acc[4 * q + 0] = fmaf(l.x, o, acc[4 * q + 0]); acc[4 * q + 1] = fmaf(l.y, o, acc[4 * q + 1]);
         acc[4 * q + 2] = fmaf(l.z, o, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(l.w, o, acc[4 * q + 3]);
@@ -210,7 +209,7 @@ operator_chain_kernel(const float* __restrict__ L, const float* __restrict__ X, 
     }
     const int blk = sel.blk[s];
 #pragma unroll
-    for (int n = 0; n < CHAIN_NMAX; ++n) {
+    for (int n = 0; n < LNB_CHAIN_MAX_N; ++n) {
       if (n < N) {
         float v = acc[n];
         if (cheby && s > 0) {                                  // s_k = 2 L s_{k-1} - s_{k-2}
@@ -236,7 +235,6 @@ operator_chain_kernel(const float* __restrict__ L, const float* __restrict__ X, 
 // the operators (transposed), Q, Q^T and the filters are staged once in shared memory and read as
 // 16-byte broadcasts.  Replaces five launches of the FFMA batched GEMM per layer (36 us each at
 // B = 256, tiles of 64 x 64 for 26-row operands) by one.
-constexpr int MSG_NMAX = 32, MSG_KMAX = 32;
 
 struct MsgParams {
   const float* L; const float* X; const float* Q; const float* G; const float* coeff;
@@ -246,15 +244,15 @@ struct MsgParams {
 };
 
 __device__ __forceinline__ void msg_matvec(const float* __restrict__ Mt /* [32][32]: Mt[i][n] */,
-                                           const float (&in)[MSG_NMAX], float (&acc)[MSG_NMAX]) {
+                                           const float (&in)[LNB_MESSAGES_MAX_N], float (&acc)[LNB_MESSAGES_MAX_N]) {
 #pragma unroll
-  for (int n = 0; n < MSG_NMAX; ++n) acc[n] = 0.f;
+  for (int n = 0; n < LNB_MESSAGES_MAX_N; ++n) acc[n] = 0.f;
 #pragma unroll
-  for (int i = 0; i < MSG_NMAX; ++i) {
+  for (int i = 0; i < LNB_MESSAGES_MAX_N; ++i) {
     const float o = in[i];
-    const float4* l4 = reinterpret_cast<const float4*>(Mt + i * MSG_NMAX);
+    const float4* l4 = reinterpret_cast<const float4*>(Mt + i * LNB_MESSAGES_MAX_N);
 #pragma unroll
-    for (int q = 0; q < MSG_NMAX / 4; ++q) {
+    for (int q = 0; q < LNB_MESSAGES_MAX_N / 4; ++q) {
       const float4 l = l4[q];
       acc[4 * q + 0] = fmaf(l.x, o, acc[4 * q + 0]); acc[4 * q + 1] = fmaf(l.y, o, acc[4 * q + 1]);
       acc[4 * q + 2] = fmaf(l.z, o, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(l.w, o, acc[4 * q + 3]);
@@ -267,102 +265,103 @@ graph_messages_kernel(const MsgParams P) {
   extern __shared__ __align__(16) float msg_smem[];
   const int N = P.N, E1 = P.E1, D = P.D, K = P.K, S = P.S;
   float* Lt = msg_smem;                                   // [E1][32][32]  Lt[e][i][n] = L[n][i][e]
-  float* Qs = Lt + (size_t)E1 * MSG_NMAX * MSG_NMAX;      // [32 n][32 k]
-  float* Qt = Qs + MSG_NMAX * MSG_KMAX;                   // [32 k][32 n]
-  float* Gs = Qt + MSG_NMAX * MSG_KMAX;                   // [S][32][32] dense blocks, or [S][32] diagonals
+  float* Qs = Lt + (size_t)E1 * LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_N;   // [32 n][32 k]
+  float* Qt = Qs + LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_K;                // [32 k][32 n]
+  float* Gs = Qt + LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_K;                // [S][32][32] dense blocks, or [S][32] diagonals
   const int g = blockIdx.x, d = blockIdx.y * blockDim.x + threadIdx.x, t = threadIdx.x, nt = blockDim.x;
   // blockIdx.z: 0 = edge types + short walk, 1 = long scales (two CTAs per graph halve the serial
   // work of a column; each stages only what it reads)
   const bool do_edges = blockIdx.z == 0, do_long = (gridDim.z == 1 || blockIdx.z == 1) && S > 0;
   const bool live = d < D;
   const float* Lg = P.L + (int64_t)g * N * N * E1;
-  if (do_edges) for (int e = t; e < E1 * MSG_NMAX * MSG_NMAX; e += nt) Lt[e] = 0.f;
-  if (do_long) for (int e = t; e < 2 * MSG_NMAX * MSG_KMAX; e += nt) Qs[e] = 0.f;
+  if (do_edges) for (int e = t; e < E1 * LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_N; e += nt) Lt[e] = 0.f;
+  if (do_long) for (int e = t; e < 2 * LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_K; e += nt) Qs[e] = 0.f;
   __syncthreads();
   if (do_edges) for (int e = t; e < N * N * E1; e += nt) {              // coalesced read, transposed scatter
     const int ch = e % E1, ij = e / E1, r = ij / N, c = ij - r * N;
-    Lt[((size_t)ch * MSG_NMAX + c) * MSG_NMAX + r] = __ldg(Lg + e);
+    Lt[((size_t)ch * LNB_MESSAGES_MAX_N + c) * LNB_MESSAGES_MAX_N + r] = __ldg(Lg + e);
   }
   if (do_long) {
     const float* Qg = P.Q + (int64_t)g * N * K;
     for (int e = t; e < N * K; e += nt) {
       const int n = e / K, k = e - n * K;
       const float v = __ldg(Qg + e);
-      Qs[n * MSG_KMAX + k] = v;
-      Qt[k * MSG_NMAX + n] = v;
+      Qs[n * LNB_MESSAGES_MAX_K + k] = v;
+      Qt[k * LNB_MESSAGES_MAX_N + n] = v;
     }
     if (P.dense_filter) {
       const float* Gg = P.G + (int64_t)g * S * K * K;
-      for (int e = t; e < S * MSG_KMAX * MSG_KMAX; e += nt) {
-        const int s = e / (MSG_KMAX * MSG_KMAX), rc = e - s * MSG_KMAX * MSG_KMAX;
-        const int r = rc / MSG_KMAX, c = rc - r * MSG_KMAX;
+      for (int e = t; e < S * LNB_MESSAGES_MAX_K * LNB_MESSAGES_MAX_K; e += nt) {
+        const int s = e / (LNB_MESSAGES_MAX_K * LNB_MESSAGES_MAX_K);
+        const int rc = e - s * LNB_MESSAGES_MAX_K * LNB_MESSAGES_MAX_K;
+        const int r = rc / LNB_MESSAGES_MAX_K, c = rc - r * LNB_MESSAGES_MAX_K;
         // row r of Gs = column r of G_s (what the unrolled product over the input index reads)
         Gs[e] = (r < K && c < K) ? __ldg(Gg + ((int64_t)s * K + c) * K + r) : 0.f;
       }
     } else {
       const float* fg = P.coeff + (int64_t)g * K * S;       // [K][S]
-      for (int e = t; e < S * MSG_KMAX; e += nt) {
-        const int s = e / MSG_KMAX, k = e - s * MSG_KMAX;
+      for (int e = t; e < S * LNB_MESSAGES_MAX_K; e += nt) {
+        const int s = e / LNB_MESSAGES_MAX_K, k = e - s * LNB_MESSAGES_MAX_K;
         Gs[e] = (k < K) ? __ldg(fg + (int64_t)k * S + s) : 0.f;
       }
     }
   }
-  float x[MSG_NMAX];
+  float x[LNB_MESSAGES_MAX_N];
   const float* Xg = P.X + (int64_t)g * N * D + d;
 #pragma unroll
-  for (int n = 0; n < MSG_NMAX; ++n) x[n] = (live && n < N) ? __ldg(Xg + (int64_t)n * D) : 0.f;
+  for (int n = 0; n < LNB_MESSAGES_MAX_N; ++n) x[n] = (live && n < N) ? __ldg(Xg + (int64_t)n * D) : 0.f;
   __syncthreads();
   float* og = P.out + (int64_t)g * P.out_sb + d;
-  float y[MSG_NMAX];
+  float y[LNB_MESSAGES_MAX_N];
   // ---- edge types (and the first step of the short walk: both are L_0 X) ------------------------
   if (do_edges)
   for (int e = E1 - 1; e >= 0; --e) {                      // channel 0 last: its result seeds the walk
-    msg_matvec(Lt + (size_t)e * MSG_NMAX * MSG_NMAX, x, y);
+    msg_matvec(Lt + (size_t)e * LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_N, x, y);
     if (live) {
 #pragma unroll
-      for (int n = 0; n < MSG_NMAX; ++n)
+      for (int n = 0; n < LNB_MESSAGES_MAX_N; ++n)
         if (n < N) og[(int64_t)n * P.out_sn + (int64_t)(P.n_short + S + e) * D] = y[n];
     }
   }
   // ---- short diffusion walk: w_k = L_0 w_{k-1} (lanczos_net.py:164-169) ---------------------------
   for (int step = 1; do_edges && step <= P.short_steps; ++step) {
     if (step > 1) {
-      float w[MSG_NMAX];
+      float w[LNB_MESSAGES_MAX_N];
 #pragma unroll
-      for (int n = 0; n < MSG_NMAX; ++n) w[n] = y[n];
+      for (int n = 0; n < LNB_MESSAGES_MAX_N; ++n) w[n] = y[n];
       msg_matvec(Lt, w, y);
     }
     const int blk = P.sel.blk[step - 1];
     if (blk >= 0 && live) {
 #pragma unroll
-      for (int n = 0; n < MSG_NMAX; ++n)
+      for (int n = 0; n < LNB_MESSAGES_MAX_N; ++n)
         if (n < N) og[(int64_t)n * P.out_sn + (int64_t)blk * D] = y[n];
     }
   }
   // ---- long scales: Q G_s (Q^T x) -------------------------------------------------------------------
   if (do_long) {
-    float u[MSG_KMAX];
+    float u[LNB_MESSAGES_MAX_K];
 #pragma unroll
-    for (int k = 0; k < MSG_KMAX; ++k) u[k] = 0.f;
+    for (int k = 0; k < LNB_MESSAGES_MAX_K; ++k) u[k] = 0.f;
 #pragma unroll
-    for (int n = 0; n < MSG_NMAX; ++n) {                   // u = Q^T x
+    for (int n = 0; n < LNB_MESSAGES_MAX_N; ++n) {                   // u = Q^T x
       const float o = x[n];
-      const float4* q4 = reinterpret_cast<const float4*>(Qs + n * MSG_KMAX);
+      const float4* q4 = reinterpret_cast<const float4*>(Qs + n * LNB_MESSAGES_MAX_K);
 #pragma unroll
-      for (int q = 0; q < MSG_KMAX / 4; ++q) {
+      for (int q = 0; q < LNB_MESSAGES_MAX_K / 4; ++q) {
         const float4 l = q4[q];
         u[4 * q + 0] = fmaf(l.x, o, u[4 * q + 0]); u[4 * q + 1] = fmaf(l.y, o, u[4 * q + 1]);
         u[4 * q + 2] = fmaf(l.z, o, u[4 * q + 2]); u[4 * q + 3] = fmaf(l.w, o, u[4 * q + 3]);
       }
     }
     for (int s = 0; s < S; ++s) {
-      float w[MSG_KMAX];
+      float w[LNB_MESSAGES_MAX_K];
       if (P.dense_filter) {
-        msg_matvec(Gs + (size_t)s * MSG_KMAX * MSG_KMAX, u, w);        // w = G_s u
+        msg_matvec(Gs + (size_t)s * LNB_MESSAGES_MAX_K * LNB_MESSAGES_MAX_K, u, w);        // w = G_s u
       } else {
-        const float4* f4 = reinterpret_cast<const float4*>(Gs + s * MSG_KMAX);
+        const float4* f4 = reinterpret_cast<const float4*>(Gs + s * LNB_MESSAGES_MAX_K);
 #pragma unroll
-        for (int q = 0; q < MSG_KMAX / 4; ++q) {
+        for (int q = 0; q < LNB_MESSAGES_MAX_K / 4; ++q) {
           const float4 f = f4[q];
           w[4 * q + 0] = f.x * u[4 * q + 0]; w[4 * q + 1] = f.y * u[4 * q + 1];
           w[4 * q + 2] = f.z * u[4 * q + 2]; w[4 * q + 3] = f.w * u[4 * q + 3];
@@ -371,7 +370,7 @@ graph_messages_kernel(const MsgParams P) {
       msg_matvec(Qt, w, y);                                             // y = Q w
       if (live) {
 #pragma unroll
-        for (int n = 0; n < MSG_NMAX; ++n)
+        for (int n = 0; n < LNB_MESSAGES_MAX_N; ++n)
           if (n < N) og[(int64_t)n * P.out_sn + (int64_t)(P.n_short + s) * D] = y[n];
       }
     }
@@ -420,7 +419,7 @@ int lnb_embedding_rows(lnb_stream_t stream, const int64_t* idx, const float* tab
 int lnb_ritz_power_table(lnb_stream_t stream, const float* D, int64_t rows, const int* powers,
                          int S, float* table) {
   LNB_REQUIRE(D && powers && table, "ritz_power_table: null pointer");
-  LNB_REQUIRE(rows >= 0 && S >= 1 && S <= 32, "ritz_power_table: bad dims rows=%lld S=%d",
+  LNB_REQUIRE(rows >= 0 && S >= 1 && S <= LNB_FILTER_MLP_MAX_S, "ritz_power_table: bad dims rows=%lld S=%d",
               (long long)rows, S);
   if (rows == 0) return LNB_OK;
   PowerList pw;
@@ -440,7 +439,7 @@ int lnb_readout(lnb_stream_t stream, const float* state, const float* W_out, con
   const int HP = H | 1;
   size_t shm = ((size_t)(P + 1) * HP + (size_t)RO_NODES * HP + (size_t)RO_NODES * (P + 1)) *
                sizeof(float);
-  LNB_REQUIRE(shm <= 227 * 1024, "readout: H=%d P=%d exceed shared memory", H, P);
+  LNB_REQUIRE(shm <= lnb::SMEM_MAX, "readout: H=%d P=%d exceed shared memory", H, P);
   if (shm > 48 * 1024)
     cudaFuncSetAttribute(readout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
   readout_kernel<<<B, RO_THREADS, shm, (cudaStream_t)stream>>>(state, W_out, b_out, w_att, b_att,
@@ -455,7 +454,7 @@ int lnb_gaussian_laplacian(lnb_stream_t stream, const float* x, const float* L, 
   LNB_REQUIRE(B >= 0 && N >= 1 && Dx >= 1 && E1 >= 1, "gaussian_laplacian: bad dims");
   if (B == 0) return LNB_OK;
   size_t shm = ((size_t)N * (Dx | 1) + N + 32) * sizeof(float);
-  if (shm > 227 * 1024) {
+  if (shm > lnb::SMEM_MAX) {
     lnb::set_err("gaussian_laplacian: N=%d x Dx=%d node features exceed shared memory", N, Dx);
     return LNB_ERR_UNSUPPORTED;
   }
@@ -472,14 +471,14 @@ int lnb_operator_chain(lnb_stream_t stream, const float* L, const float* X, int 
                        int64_t out_batch_stride, int64_t out_row_stride, int out_col0) {
   LNB_REQUIRE(L && X && out && block_of_step, "operator_chain: null pointer");
   LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && D >= 1 && steps >= 1, "operator_chain: bad dims");
-  if (N > CHAIN_NMAX || steps > CHAIN_STEPS_MAX) {
+  if (N > LNB_CHAIN_MAX_N || steps > LNB_CHAIN_MAX_STEPS) {
     lnb::set_err("operator_chain: N=%d steps=%d exceed the register-resident kernel (N <= %d, steps <= %d)",
-                 N, steps, CHAIN_NMAX, CHAIN_STEPS_MAX);
+                 N, steps, LNB_CHAIN_MAX_N, LNB_CHAIN_MAX_STEPS);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;
   ChainSel sel;
-  for (int s = 0; s < CHAIN_STEPS_MAX; ++s) sel.blk[s] = s < steps ? (int8_t)block_of_step[s] : (int8_t)-1;
+  for (int s = 0; s < LNB_CHAIN_MAX_STEPS; ++s) sel.blk[s] = s < steps ? (int8_t)block_of_step[s] : (int8_t)-1;
   const int threads = 128;
   dim3 grid((unsigned)B, (unsigned)lnb::ceil_div(D, threads));
   const size_t shm = (size_t)2 * N * threads * sizeof(float);
@@ -498,7 +497,8 @@ int lnb_graph_messages(lnb_stream_t stream, const float* L, const float* X, cons
   LNB_REQUIRE(short_steps == 0 || block_of_step, "graph_messages: block_of_step missing");
   LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1 && D >= 1 && S >= 0 && short_steps >= 0 && n_short >= 0,
               "graph_messages: bad dims");
-  if (N > MSG_NMAX || (S > 0 && K > MSG_KMAX) || E1 > 16 || S > 8 || short_steps > CHAIN_STEPS_MAX) {
+  if (N > LNB_MESSAGES_MAX_N || (S > 0 && K > LNB_MESSAGES_MAX_K) || E1 > LNB_MAX_E1 || S > LNB_MESSAGES_MAX_S ||
+      short_steps > LNB_CHAIN_MAX_STEPS) {
     lnb::set_err("graph_messages: N=%d K=%d E1=%d S=%d outside the one-launch kernel (N,K <= 32, E1 <= 16, S <= 8)",
                  N, K, E1, S);
     return LNB_ERR_UNSUPPORTED;
@@ -508,11 +508,12 @@ int lnb_graph_messages(lnb_stream_t stream, const float* L, const float* X, cons
   p.L = L; p.X = X; p.Q = Q; p.G = dense_filter ? filt : nullptr; p.coeff = dense_filter ? nullptr : filt;
   p.N = N; p.E1 = E1; p.D = D; p.K = K; p.S = S; p.dense_filter = dense_filter;
   p.short_steps = short_steps; p.n_short = n_short;
-  for (int s = 0; s < CHAIN_STEPS_MAX; ++s) p.sel.blk[s] = s < short_steps ? (int8_t)block_of_step[s] : (int8_t)-1;
+  for (int s = 0; s < LNB_CHAIN_MAX_STEPS; ++s) p.sel.blk[s] = s < short_steps ? (int8_t)block_of_step[s] : (int8_t)-1;
   p.out = out; p.out_sb = out_batch_stride; p.out_sn = out_row_stride;
   const int threads = 128;
-  const size_t shm = ((size_t)E1 * MSG_NMAX * MSG_NMAX + 2 * MSG_NMAX * MSG_KMAX +
-                      (S > 0 ? (dense_filter ? (size_t)S * MSG_KMAX * MSG_KMAX : (size_t)S * MSG_KMAX) : 0)) * sizeof(float);
+  const size_t shm = ((size_t)E1 * LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_N + 2 * LNB_MESSAGES_MAX_N * LNB_MESSAGES_MAX_K +
+                      (S > 0 ? (dense_filter ? (size_t)S * LNB_MESSAGES_MAX_K * LNB_MESSAGES_MAX_K
+                                             : (size_t)S * LNB_MESSAGES_MAX_K) : 0)) * sizeof(float);
   if (shm > 48 * 1024)
     cudaFuncSetAttribute(graph_messages_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
   dim3 grid((unsigned)B, (unsigned)lnb::ceil_div(D, threads), S > 0 ? 2u : 1u);

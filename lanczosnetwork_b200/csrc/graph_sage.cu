@@ -80,7 +80,7 @@ int lnb_sage_operators(lnb_stream_t stream, const int64_t* nn_idx, const float* 
   LNB_REQUIRE(B >= 0 && N >= 1 && K >= 1 && E1 >= 1, "sage_operators: bad dims B=%d N=%d K=%d E1=%d",
               B, N, K, E1);
   const size_t shm = (size_t)N * E1 * sizeof(int);
-  if (shm > 227 * 1024) {
+  if (shm > lnb::SMEM_MAX) {
     lnb::set_err("sage_operators: N=%d, E1=%d need %zu B of shared memory", N, E1, shm);
     return LNB_ERR_UNSUPPORTED;
   }
@@ -97,7 +97,7 @@ int lnb_sage_operators(lnb_stream_t stream, const int64_t* nn_idx, const float* 
 int lnb_neighbour_max(lnb_stream_t stream, const float* X, const float* ell_val, const uint8_t* ell_idx,
                       const int32_t* ell_max, int B, int N, int E1, int D, float* out, int32_t* argmax) {
   LNB_REQUIRE(X && ell_val && ell_idx && ell_max && out && argmax, "neighbour_max: null pointer");
-  LNB_REQUIRE(B >= 0 && N >= 1 && N <= 255 && E1 >= 1 && D >= 1,
+  LNB_REQUIRE(B >= 0 && N >= 1 && N <= LNB_MAX_N_ELL && E1 >= 1 && D >= 1,
               "neighbour_max: bad dims B=%d N=%d E1=%d D=%d", B, N, E1, D);
   const int64_t total = (int64_t)B * N * E1 * D;
   if (total == 0) return LNB_OK;

@@ -381,7 +381,7 @@ int lnb_lanczos_tridiag(lnb_stream_t stream, const float* A, const uint8_t* mask
   if (B == 0) return LNB_OK;
   cudaStream_t s = (cudaStream_t)stream;
   const int iters = N < K ? N : K;
-  if (N <= 1024 && K <= 64) {
+  if (N <= LNB_LANCZOS_FUSED_MAX_N && K <= LNB_LANCZOS_MAX_K) {
     // the fused kernel without its QL stage: operator rows loaded coalesced ONCE and packed on chip,
     // butterfly projections (it replaced the round-1 warp / resident-operator kernels at every size)
     const int rc = lnb_lanczos_ritz(stream, A, mask, q1, B, N, K, 0, T, Q, alpha, beta, idx, nullptr, nullptr, nullptr);
@@ -393,7 +393,7 @@ int lnb_lanczos_tridiag(lnb_stream_t stream, const float* A, const uint8_t* mask
     size_t stage = (size_t)N * (N + 1) * sizeof(float);
     int stage_A = (base + stage <= 220 * 1024) ? 1 : 0;
     size_t shm = base + (stage_A ? stage : 0);
-    LNB_REQUIRE(shm <= 227 * 1024,
+    LNB_REQUIRE(shm <= lnb::SMEM_MAX,
                 "lanczos_tridiag: Krylov basis (N=%d, K=%d) does not fit shared memory", N, K);
     cudaFuncSetAttribute(lanczos_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)shm);
@@ -413,7 +413,7 @@ int lnb_tridiag_ritz(lnb_stream_t stream, const float* alpha, const float* beta,
   const int KP = K | 1;
   if (N <= 32) {
     size_t shm = (size_t)4 * (32 * KP + 8 * K) * sizeof(float);
-    LNB_REQUIRE(shm <= 227 * 1024, "tridiag_ritz: K=%d too large", K);
+    LNB_REQUIRE(shm <= lnb::SMEM_MAX, "tridiag_ritz: K=%d too large", K);
     if (shm > 48 * 1024)
       cudaFuncSetAttribute(tridiag_ritz_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)shm);
@@ -421,7 +421,7 @@ int lnb_tridiag_ritz(lnb_stream_t stream, const float* alpha, const float* beta,
                                                                   ritz_vec, status);
   } else {
     size_t shm = ((size_t)N * KP + 8 * K) * sizeof(float);
-    LNB_REQUIRE(shm <= 227 * 1024, "tridiag_ritz: N=%d K=%d does not fit shared memory", N, K);
+    LNB_REQUIRE(shm <= lnb::SMEM_MAX, "tridiag_ritz: N=%d K=%d does not fit shared memory", N, K);
     cudaFuncSetAttribute(tridiag_ritz_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)shm);
     tridiag_ritz_kernel<4><<<B, 128, shm, s>>>(alpha, beta, Q, B, N, K, theta, ritz_vec, status);
@@ -433,7 +433,7 @@ int lnb_tridiag_ritz(lnb_stream_t stream, const float* alpha, const float* beta,
 int lnb_tridiag_powers(lnb_stream_t stream, const float* T, int B, int K, const int* powers, int S,
                        float* out) {
   LNB_REQUIRE(T && powers && out, "tridiag_powers: null pointer");
-  LNB_REQUIRE(B >= 0 && K >= 1 && S >= 1 && S <= 32, "tridiag_powers: bad dims B=%d K=%d S=%d",
+  LNB_REQUIRE(B >= 0 && K >= 1 && S >= 1 && S <= LNB_TRIDIAG_POWERS_MAX_S, "tridiag_powers: bad dims B=%d K=%d S=%d",
               B, K, S);
   for (int i = 0; i < S; ++i)
     LNB_REQUIRE(powers[i] >= 1 && (i == 0 || powers[i] > powers[i - 1]),
@@ -443,7 +443,7 @@ int lnb_tridiag_powers(lnb_stream_t stream, const float* T, int B, int K, const 
   PowerList pw;
   for (int i = 0; i < S; ++i) pw.v[i] = powers[i];
   size_t shm = ((size_t)2 * K * K + 3 * K) * sizeof(float);
-  LNB_REQUIRE(shm <= 227 * 1024, "tridiag_powers: K=%d too large", K);
+  LNB_REQUIRE(shm <= lnb::SMEM_MAX, "tridiag_powers: K=%d too large", K);
   if (shm > 48 * 1024)
     cudaFuncSetAttribute(tridiag_powers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)shm);

@@ -133,6 +133,7 @@ size_t powers_backward_smem(int K, int pmax) {
 //   dA += zbar q_i^T  in the order of the sweep.  Acceptance, idx and the masks are data (no gradient).
 // ------------------------------------------------------------------------------------------------------
 constexpr int LZ_THREADS = 128;
+static_assert(LNB_LANCZOS_TRAIN_MAX_N <= LZ_THREADS, "thread n owns node n");
 constexpr float kLzEps = 1.1920928955078125e-07f;   // np.finfo(np.float32).eps (ada_lanczos_net.py:8)
 constexpr float kLzBetaLowerBound = 1.0e-4f;        // ada_lanczos_net.py:169
 
@@ -374,8 +375,8 @@ size_t lanczos_train_smem(int N, int K, bool backward) {
 }
 
 int launch_lanczos_train(lnb_stream_t stream, const LzParams& p, int B, const char* who) {
-  if (!(p.N >= 1 && p.N <= LZ_THREADS && p.K >= 1 && p.K <= 64 &&
-        lanczos_train_smem(p.N, p.K, true) <= 227 * 1024)) {
+  if (!(p.N >= 1 && p.N <= LNB_LANCZOS_TRAIN_MAX_N && p.K >= 1 && p.K <= LNB_LANCZOS_MAX_K &&
+        lanczos_train_smem(p.N, p.K, true) <= lnb::SMEM_MAX)) {
     lnb::set_err("%s: N=%d K=%d outside 1 <= N <= 128, 1 <= K <= 64", who, p.N, p.K);
     return LNB_ERR_UNSUPPORTED;
   }
@@ -410,13 +411,14 @@ int lnb_lanczos_tridiag_backward(lnb_stream_t stream, const float* A, const uint
 int lnb_tridiag_powers_backward(lnb_stream_t stream, const float* T, const float* gOut, int B, int K,
                                 const int* powers, int S, float* gT) {
   LNB_REQUIRE(powers, "tridiag_powers_backward: null powers");
-  LNB_REQUIRE(B >= 0 && K >= 1 && S >= 1 && S <= 32, "tridiag_powers_backward: bad dims B=%d K=%d S=%d",
+  LNB_REQUIRE(B >= 0 && K >= 1 && S >= 1 && S <= LNB_TRIDIAG_POWERS_MAX_S,
+              "tridiag_powers_backward: bad dims B=%d K=%d S=%d",
               B, K, S);
   for (int i = 0; i < S; ++i)
     LNB_REQUIRE(powers[i] >= 1 && (i == 0 || powers[i] > powers[i - 1]),
                 "tridiag_powers_backward: powers must be positive and strictly increasing");
   const size_t shm = powers_backward_smem(K, powers[S - 1]);
-  if (shm > 227 * 1024) {
+  if (shm > lnb::SMEM_MAX) {
     lnb::set_err("tridiag_powers_backward: K=%d with powers up to %d needs %zu bytes of shared memory "
                  "(limit 227 KB)", K, powers[S - 1], shm);
     return LNB_ERR_UNSUPPORTED;

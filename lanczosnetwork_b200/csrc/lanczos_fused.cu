@@ -716,7 +716,6 @@ static bool plan_fused(int N, int K, int tpg, int npt, FusedPlan& pl) {
   zw = (zw + 3) & ~3;
   const int fixed = K * NS + NP + zw + 4 * K4 + 4 + 128 + 4;
   const int ql_words = ((K * (K | 1) + 3) & ~3) + K * K4 + K4 + 4 * K + 8;   // Zt, Zr, rank, rotation ring, descriptors
-  const int smem_max = 227 * 1024;
   // target capacity: every entry of a dense operator while that is cheap (N <= 48: <= 13.5 KB),
   // else 12 non-zeros per row
   long want = (long)N * N;
@@ -727,9 +726,9 @@ static bool plan_fused(int N, int K, int tpg, int npt, FusedPlan& pl) {
   int pool_words = pool_words_for(want);
   long per_graph = ((long)fixed + pool_words + 3) & ~3L;
   long cap = want;
-  if (per_graph * gpc * 4 > smem_max) {
+  if (per_graph * gpc * 4 > lnb::SMEM_MAX) {
     // shrink the pool to what fits one CTA per SM (still at least 4 per row), else give up
-    const long room = smem_max / 4 / gpc - fixed - 4;
+    const long room = lnb::SMEM_MAX / 4 / gpc - fixed - 4;
     if (room < ql_words) return false;
     cap = room * 4 / 6;
     if (cap > 65535) cap = 65535;
@@ -740,10 +739,10 @@ static bool plan_fused(int N, int K, int tpg, int npt, FusedPlan& pl) {
   } else {
     // use the slack of the SM share (k CTAs per SM) for a larger pool
     const long bytes = per_graph * gpc * 4;
-    int ctas = (int)(smem_max / (bytes + 1024));
+    int ctas = (int)(lnb::SMEM_MAX / (bytes + 1024));
     if (ctas < 1) ctas = 1;
     if (ctas > 8) ctas = 8;
-    const long share_words = (smem_max / ctas - 1024) / 4 / gpc;
+    const long share_words = (lnb::SMEM_MAX / ctas - 1024) / 4 / gpc;
     const long room = share_words - fixed - 4;
     if (room > pool_words) {
       long c2 = room * 4 / 6;
@@ -757,7 +756,7 @@ static bool plan_fused(int N, int K, int tpg, int npt, FusedPlan& pl) {
   pl.p.cap = (int)cap; pl.p.pool_words = pool_words; pl.p.per_graph = (int)per_graph;
   pl.p.zw = zw;
   pl.smem = (size_t)per_graph * gpc * 4;
-  return pl.smem <= (size_t)smem_max;
+  return pl.smem <= (size_t)lnb::SMEM_MAX;
 }
 
 template <int TPG, int NPT, int KB>
@@ -787,7 +786,7 @@ int lnb_lanczos_ritz(lnb_stream_t stream, const float* A, const uint8_t* mask, c
   LNB_REQUIRE(A && q1 && alpha && beta && idx, "lanczos_ritz: null pointer");
   LNB_REQUIRE((theta == nullptr) == (ritz_vec == nullptr) && (theta == nullptr) == (status == nullptr),
               "lanczos_ritz: theta, ritz_vec and status are given (or omitted) together");
-  if (N > 1024 || K > 64) {
+  if (N > LNB_LANCZOS_FUSED_MAX_N || K > LNB_LANCZOS_MAX_K) {
     lnb::set_err("lanczos_ritz: N=%d K=%d outside the fused kernel (N <= 1024, K <= 64)", N, K);
     return LNB_ERR_UNSUPPORTED;
   }

@@ -21,7 +21,6 @@
 
 namespace {
 
-constexpr int MP_DMAX = 128, MP_NMAX = 255, MP_E1MAX = 16;
 constexpr int MP_H = 64;                  // edge-network hidden width (model/mpnn.py:60)
 constexpr int MP_PQ = 2 * MP_H;           // PQ columns per channel: 64 P, then 64 Q
 
@@ -47,7 +46,7 @@ struct MpnnUpdatePolicy : gru::Step<MpnnUpdatePolicy, MpnnUpdateParams> {
         const int64_t line = ((int64_t)(b * p.E1 + e) * p.N) * p.N + n;
         const int cnt = gru::ell_count(p.ell_val, line, __ldg(p.ell_max + b * p.E1 + e), p.N);
 #pragma unroll
-        for (int j = 0; j < MP_E1MAX; ++j)
+        for (int j = 0; j < LNB_MAX_E1; ++j)
           if (j == e) v[j] = gru::row_weight(cnt, p.avg) * (float)cnt;
       }
       return;
@@ -163,8 +162,8 @@ int edge_aggregate_checks(const char* who, const float* PQ, const float* ell_val
                           const int32_t* ell_max, const float* out, int B, int N, int E1) {
   LNB_REQUIRE(PQ && ell_val && ell_idx && ell_max && out, "%s: null pointer", who);
   LNB_REQUIRE(B >= 0 && N >= 1 && E1 >= 1, "%s: bad dims B=%d N=%d E1=%d", who, B, N, E1);
-  if (N > MP_NMAX || E1 > MP_E1MAX) {
-    lnb::set_err("%s: N=%d E1=%d outside the kernel (N <= %d, E1 <= %d)", who, N, E1, MP_NMAX, MP_E1MAX);
+  if (N > LNB_MAX_N_ELL || E1 > LNB_MAX_E1) {
+    lnb::set_err("%s: N=%d E1=%d outside the kernel (N <= %d, E1 <= %d)", who, N, E1, LNB_MAX_N_ELL, LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE((int64_t)B * N * E1 * MP_PQ <= 0x7fffffff, "%s: B*N too large", who);
@@ -182,9 +181,9 @@ int lnb_mpnn_update(lnb_stream_t stream, const float* PQ, const float* h, const 
               "mpnn_update: null pointer");
   LNB_REQUIRE(B >= 0 && N >= 1 && D >= 1 && E1 >= 1, "mpnn_update: bad dims B=%d N=%d D=%d E1=%d", B, N, D,
               E1);
-  if (N > MP_NMAX || D % 32 || D < 32 || D > MP_DMAX || E1 > MP_E1MAX) {
+  if (N > LNB_MAX_N_ELL || D % 32 || D < 32 || D > LNB_MAX_WIDTH || E1 > LNB_MAX_E1) {
     lnb::set_err("mpnn_update: N=%d D=%d E1=%d outside the kernel (N <= %d, D %% 32 == 0, 32 <= D <= %d, "
-                 "E1 <= %d)", N, D, E1, MP_NMAX, MP_DMAX, MP_E1MAX);
+                 "E1 <= %d)", N, D, E1, LNB_MAX_N_ELL, LNB_MAX_WIDTH, LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE(((uintptr_t)PQ | (uintptr_t)h | (uintptr_t)out | (uintptr_t)W_hi | (uintptr_t)W_lo) % 16 == 0,

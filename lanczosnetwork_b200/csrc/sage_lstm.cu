@@ -21,7 +21,6 @@
 
 namespace {
 
-constexpr int SL_DMAX = 128, SL_E1MAX = 16;
 
 struct SageLstmParams {
   const float* state;      // [B*N, D]  the layer's input
@@ -170,9 +169,9 @@ int lnb_sage_lstm_step(lnb_stream_t stream, const float* state, const int32_t* n
   LNB_REQUIRE(B >= 0 && N >= 1 && K >= 1 && E1 >= 1 && D >= 1, "sage_lstm_step: bad dims B=%d N=%d K=%d E1=%d D=%d",
               B, N, K, E1, D);
   LNB_REQUIRE(t >= 0 && t < K, "sage_lstm_step: step t=%d outside [0, K=%d)", t, K);
-  if (D % 32 || D > SL_DMAX || E1 > SL_E1MAX) {
-    lnb::set_err("sage_lstm_step: D=%d E1=%d outside the kernel (D %% 32 == 0, D <= %d, E1 <= %d)", D, E1, SL_DMAX,
-                 SL_E1MAX);
+  if (D % 32 || D > LNB_MAX_WIDTH || E1 > LNB_MAX_E1) {
+    lnb::set_err("sage_lstm_step: D=%d E1=%d outside the kernel (D %% 32 == 0, D <= %d, E1 <= %d)", D, E1, LNB_MAX_WIDTH,
+                 LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   LNB_REQUIRE(t == 0 || h, "sage_lstm_step: h is null at step t=%d > 0", t);

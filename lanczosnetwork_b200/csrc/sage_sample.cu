@@ -19,9 +19,7 @@
 namespace {
 
 constexpr int SS_THREADS = 256;
-constexpr int SS_NMAX = 128;
-constexpr int SS_NW = SS_NMAX / 32;     // 32-bit words per adjacency row
-constexpr int SS_EMAX = 16;
+constexpr int SS_NW = LNB_MAX_N / 32;     // 32-bit words per adjacency row
 
 struct SampleParams {
   const int32_t* sizes; const int32_t* node_ptr; const int32_t* node_feat;
@@ -72,7 +70,7 @@ __device__ __forceinline__ int select_bit(const uint32_t* m, int j) {
 __global__ void __launch_bounds__(SS_THREADS)
 sage_sample_kernel(const SampleParams P) {
   extern __shared__ __align__(16) unsigned char ss_smem[];
-  __shared__ int s_max[SS_EMAX], s_maxT[SS_EMAX];
+  __shared__ int s_max[LNB_MAX_E1], s_maxT[LNB_MAX_E1];
   __shared__ int s_ne;
   const int b = blockIdx.x, tid = threadIdx.x;
   const int N = P.N, E1 = P.E1, E = E1 - 1, K = P.K;
@@ -85,7 +83,7 @@ sage_sample_kernel(const SampleParams P) {
   uint8_t* cntT_s = cnt_s + N * E1;                                                  // [N*E1]
 
   for (int i = tid; i < E * N * SS_NW; i += SS_THREADS) adj[i] = 0u;
-  if (tid < SS_EMAX) { s_max[tid] = 0; s_maxT[tid] = 0; }
+  if (tid < LNB_MAX_E1) { s_max[tid] = 0; s_maxT[tid] = 0; }
   if (tid == 0) s_ne = 0;
   __syncthreads();
   // ---- adjacency from the bond list, as lnb_graph_prepare_sparse builds it -------------------------
@@ -248,10 +246,10 @@ int lnb_sage_sample_sparse(lnb_stream_t stream, const int32_t* sizes, const int3
                            int64_t* node_ids, uint8_t* mask, float* nonempty, int32_t* nn_idx,
                            float* ell_val, uint8_t* ell_idx, int32_t* ell_max, int32_t* gext,
                            float* ellT_val, uint8_t* ellT_idx, int32_t* ellT_max, int32_t* gextT) {
-  if (!(B >= 0 && N >= 1 && N <= SS_NMAX && E1 >= 2 && E1 <= SS_EMAX && K >= 1 &&
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && E1 >= 2 && E1 <= LNB_MAX_E1 && K >= 1 &&
         (int64_t)B * N * E1 < ((int64_t)1 << 31))) {
     lnb::set_err("sage_sample_sparse: B=%d N=%d E1=%d K=%d outside 1 <= N <= %d, 2 <= E1 <= %d, K >= 1, "
-                 "B*N*E1 < 2^31", B, N, E1, K, SS_NMAX, SS_EMAX);
+                 "B*N*E1 < 2^31", B, N, E1, K, LNB_MAX_N, LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   const int known = LNB_SAGE_SAMPLE_NN_IDX | LNB_SAGE_SAMPLE_ELL | LNB_SAGE_SAMPLE_ELL_T;

@@ -20,7 +20,7 @@
 
 namespace {
 
-constexpr int S2V_NMAX = 128, S2V_DMAX = 128, S2V_PMAX = 128, S2V_GMAX = 8;
+constexpr int S2V_GMAX = 8;
 constexpr int S2V_THREADS = 512;
 constexpr size_t S2V_SMEM_MAX = 200 * 1024;
 
@@ -172,9 +172,9 @@ int lnb_set2vec(lnb_stream_t stream, const float* X, const uint8_t* mask, const 
   LNB_REQUIRE(X && WgT && bg && W1 && W2 && W_out && b_out && score, "set2vec: null pointer");
   LNB_REQUIRE(B >= 0 && N >= 1 && D >= 1 && P >= 1 && steps >= 0, "set2vec: bad dims B=%d N=%d D=%d P=%d steps=%d",
               B, N, D, P, steps);
-  if (N > S2V_NMAX || D % 32 || D > S2V_DMAX || P > S2V_PMAX) {
+  if (N > LNB_MAX_N || D % 32 || D > LNB_MAX_WIDTH || P > LNB_SET2VEC_MAX_P) {
     lnb::set_err("set2vec: N=%d D=%d P=%d outside the kernel (N <= %d, D %% 32 == 0, D <= %d, P <= %d)", N, D,
-                 P, S2V_NMAX, S2V_DMAX, S2V_PMAX);
+                 P, LNB_MAX_N, LNB_MAX_WIDTH, LNB_SET2VEC_MAX_P);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;

@@ -26,10 +26,9 @@
 
 namespace {
 
-constexpr int KMAX = 32;        // max Ritz pairs
 constexpr int GMAX = 32;        // max graphs per tile
 constexpr int RMAX = 128;       // rows per tile
-constexpr int EMAX = 16;        // max operator channels
+static_assert(LNB_MAX_N <= RMAX, "every graph of the envelope fits one tile");
 
 // --------------------------------------------------------------------------------------------
 // Per-forward operator compression and extents.
@@ -45,11 +44,11 @@ graph_prepare_kernel(const float* __restrict__ L, const float* __restrict__ Q, i
                      float* __restrict__ ell_val, uint8_t* __restrict__ ell_idx,
                      int32_t* __restrict__ ell_max, int32_t* __restrict__ gext, int binarize) {
   extern __shared__ __align__(16) float gp_smem[];     // [N*N*E1] this graph's operators (optional)
-  __shared__ int s_max[EMAX];
+  __shared__ int s_max[LNB_MAX_E1];
   __shared__ int s_ext[2];
-  __shared__ uint8_t cnt_s[256 * EMAX];                // non-zeros per (row, channel); N <= 255
+  __shared__ uint8_t cnt_s[(LNB_MAX_N_ELL + 1) * LNB_MAX_E1];  // non-zeros per (row, channel)
   const int b = blockIdx.x, tid = threadIdx.x;
-  if (tid < EMAX) s_max[tid] = 0;
+  if (tid < LNB_MAX_E1) s_max[tid] = 0;
   if (tid < 2) s_ext[tid] = 0;
   const int64_t per = (int64_t)N * N * E1;
   const float* Lg = L + b * per;
@@ -123,8 +122,8 @@ graph_prepare_kernel(const float* __restrict__ L, const float* __restrict__ Q, i
   if (tid < 2) gext[b * 2 + tid] = s_ext[tid];
 }
 
-// (n_eff, k_eff) classes of the schedule's counting sort: n_eff <= RMAX, k_eff <= KMAX
-constexpr int SCH_KC = KMAX + 1;
+// (n_eff, k_eff) classes of the schedule's counting sort: n_eff <= RMAX, k_eff <= LNB_CONV_MAX_K
+constexpr int SCH_KC = LNB_CONV_MAX_K + 1;
 constexpr int SCH_NCLS = (RMAX + 1) * SCH_KC;
 
 // Exclusive prefix sum over the 1024 threads of a block; `total` = sum of all values.
@@ -180,7 +179,7 @@ __device__ void identity_schedule(int32_t* __restrict__ tiles, int B, int T) {
 // (unpadded) and <= 32 graphs, or opens a new one.  Identical graphs are placed in bulk, which gives
 // exactly what first-fit gives one at a time: a stable counting sort by class (warps 1..31) runs
 // beside warp 0, which walks the classes in order and gives every tile, lowest first, as many graphs
-// of the class as still fit.  Batches outside the shared-memory path, with K > KMAX or with an
+// of the class as still fit.  Batches outside the shared-memory path, with K > LNB_CONV_MAX_K or with an
 // n_eff > 128 (shapes the stack kernel does not run) get the next-fit tiles in graph order instead.
 template <bool in_smem>
 __global__ void __launch_bounds__(1024)
@@ -317,7 +316,7 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
   }
   __syncthreads();                                   // table done; the shared arrays above are dead
   if (B < 2) return;                                 // no room for a schedule: the kernel runs the table
-  if (K > KMAX) {
+  if (K > LNB_CONV_MAX_K) {
     identity_schedule(tiles, B, run_n);
     return;
   }
@@ -341,7 +340,7 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
     if (b < B) {
       const int n = gext[b * 2];
       big |= n > RMAX;
-      c = (RMAX - min(n, RMAX)) * SCH_KC + (KMAX - min(gext[b * 2 + 1], K));
+      c = (RMAX - min(n, RMAX)) * SCH_KC + (LNB_CONV_MAX_K - min(gext[b * 2 + 1], K));
       key[b] = c;
     }
     const unsigned peers = __match_any_sync(0xffffffffu, c);
@@ -394,7 +393,7 @@ tile_assign_kernel(const int32_t* __restrict__ gext, int B, int K, int32_t* __re
         c_first = hist[c];
         c_count = (i0 + lane + 1 < ncls ? hist[cls[i0 + lane + 1]] : B) - c_first;
         c_n = RMAX - c / SCH_KC;
-        c_k = KMAX - c % SCH_KC;
+        c_k = LNB_CONV_MAX_K - c % SCH_KC;
       }
       const int c_rn = c_n ? (65536 + c_n - 1) / c_n : 0, c_rk = c_k ? (65536 + c_k - 1) / c_k : 0;
       const int c_ce = max(1, min(GMAX, min(c_n ? RMAX / c_n : GMAX, c_k ? RMAX / c_k : GMAX)));
@@ -500,7 +499,6 @@ struct SpectralPolicyT {
   static constexpr bool kLongScales = kVariant == STACK_PLAIN;    // GraphSAGE runs S = 0: no step 0
   static constexpr int kStagesB = 2;      // k-block i + 1 is produced and its W tile loaded during MMA i
   static constexpr int kStagesA = 2;      // 64 KB: also holds Z (Ztot <= 128 rows x H <= 128) in one pass
-  static constexpr int LMAX = 8;          // layers run by one launch
   // Two producer warpgroups take alternate k-blocks: producing a k-block (an ELL gather or U, then
   // the hi / lo split) takes one group about as long as the MMAs that consume it
   static constexpr int kProducerGroups = 2;
@@ -527,7 +525,7 @@ struct SpectralPolicyT {
     float* score;           // [B, P]
     int P, emb_rows;
     int L;                  // number of layers in this launch
-    int Din[LMAX];          // input width of each layer (Din[l>0] == H)
+    int Din[LNB_CONV_MAX_LAYERS];          // input width of each layer (Din[l>0] == H)
     int B, N, E1, K, S, H, relu;
     int LB;                 // ELL lines (channel, t) that fit in shared memory
     int write_pad;          // also write the constant rows of padded nodes of `out`
@@ -597,8 +595,8 @@ struct SpectralPolicyT {
     int ng, Rtot, Ztot, nquads, nzquads, nlines;
     int gid[GMAX];                                  // graph ids of the tile's graphs
     int nbase[GMAX + 1], kbase[GMAX + 1], gn[GMAX], gk[GMAX];
-    int cnt_e[EMAX], base_e[EMAX], tmax_e[EMAX];
-    uint8_t emax[GMAX][EMAX];
+    int cnt_e[LNB_MAX_E1], base_e[LNB_MAX_E1], tmax_e[LNB_MAX_E1];
+    uint8_t emax[GMAX][LNB_MAX_E1];
     uint8_t row_g[RMAX], row_n[RMAX], z_g[RMAX], z_k[RMAX];
     uint8_t q_g[RMAX / 4 + GMAX], q_n0[RMAX / 4 + GMAX];     // node-row quads
     uint8_t zq_g[RMAX / 4 + GMAX], zq_k0[RMAX / 4 + GMAX];   // Ritz-row quads
@@ -676,12 +674,12 @@ struct SpectralPolicyT {
     const int nquads = __shfl_sync(0xffffffffu, pq, 31), nzquads = __shfl_sync(0xffffffffu, pz, 31);
     // per-channel maximum row length over the tile's graphs, per-graph row lengths
     // (all loads issued before the first reduction: one global round trip instead of E1)
-    int em[EMAX];
+    int em[LNB_MAX_E1];
 #pragma unroll
-    for (int e = 0; e < EMAX; ++e)
+    for (int e = 0; e < LNB_MAX_E1; ++e)
       em[e] = (e < E1 && lane < ng) ? __ldg(p.ell_max + g * E1 + e) : 0;
 #pragma unroll
-    for (int e = 0; e < EMAX; ++e) {
+    for (int e = 0; e < LNB_MAX_E1; ++e) {
       if (e < E1) {
         int m = em[e];
         if (lane < ng) tb->emax[lane][e] = (uint8_t)m;
@@ -1200,7 +1198,7 @@ int lnb_graph_prepare(lnb_stream_t stream, const float* L, const float* Q, int B
                       int32_t* rowmap, int32_t* nrows, int flags) {
   LNB_REQUIRE(L && Q && ell_val && ell_idx && ell_max && gext && tiles, "graph_prepare: null pointer");
   LNB_REQUIRE((rowmap == nullptr) == (nrows == nullptr), "graph_prepare: rowmap and nrows go together");
-  LNB_REQUIRE(B >= 0 && N >= 1 && N <= 255 && E1 >= 1 && E1 <= EMAX && K >= 1,
+  LNB_REQUIRE(B >= 0 && N >= 1 && N <= LNB_MAX_N_ELL && E1 >= 1 && E1 <= LNB_MAX_E1 && K >= 1,
               "graph_prepare: bad dims B=%d N=%d E1=%d K=%d", B, N, E1, K);
   if (B == 0) return LNB_OK;
   cudaStream_t s = (cudaStream_t)stream;
@@ -1237,12 +1235,13 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
                   (d.coeff || d.S == 0),
               "%s: null pointer", who);
   LNB_REQUIRE(d.B >= 0 && d.N >= 1 && d.E1 >= 1 && d.K >= 1 && d.S >= 0 && d.H >= 1 &&
-                  d.num_layers >= 1 && d.num_layers <= Pol::LMAX,
+                  d.num_layers >= 1 && d.num_layers <= LNB_CONV_MAX_LAYERS,
               "%s: bad dims", who);
   LNB_REQUIRE(!d.score || (d.W_out && d.b_out && d.w_att && d.b_att && d.P >= 1 && d.P <= 48),
               "%s: readout needs W_out, b_out, w_att, b_att and 1 <= P <= 48", who);
   int dmax = 0;
-  bool ok = d.N <= RMAX && d.K <= KMAX && d.K % 4 == 0 && d.H % 4 == 0 && d.H <= tcg::BN && d.E1 <= EMAX;
+  bool ok = d.N <= LNB_MAX_N && d.K <= LNB_CONV_MAX_K && d.K % 4 == 0 && d.H % 4 == 0 && d.H <= LNB_MAX_WIDTH &&
+            d.E1 <= LNB_MAX_E1;
   for (int l = 0; l < d.num_layers; ++l) {
     ok = ok && d.Din[l] % 32 == 0 && d.Din[l] >= 32 && (l == 0 || d.Din[l] == d.H);
     dmax = d.Din[l] > dmax ? d.Din[l] : dmax;
@@ -1251,7 +1250,7 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
   if (!ok) {
     lnb::set_err("%s: unsupported shape N=%d K=%d H=%d E1=%d (needs N<=128, Din%%32==0, inner "
                  "layers Din==H, K%%4==0, K<=%d, H%%4==0, H<=128, E1<=%d)", who, d.N, d.K, d.H, d.E1,
-                 KMAX, EMAX);
+                 LNB_CONV_MAX_K, LNB_MAX_E1);
     return LNB_ERR_UNSUPPORTED;
   }
   if ((d.bias && (reinterpret_cast<uintptr_t>(d.bias) & 15)) || (reinterpret_cast<uintptr_t>(d.Q) & 15) ||
@@ -1262,12 +1261,12 @@ static int launch_stack(lnb_stream_t stream, const lnb_spectral_stack& d, const 
   if (d.B == 0) return LNB_OK;
   size_t smem = tcg::core_smem(Pol::kStagesB, Pol::kStagesA) + 1024 +
                 Pol::smem_fixed(dmax, d.K, d.H);
-  if (smem > 227 * 1024) {
+  if (smem > lnb::SMEM_MAX) {
     lnb::set_err("%s: tile state (Din=%d, K=%d, H=%d) needs %zu B of shared memory", who, dmax, d.K,
                  d.H, smem);
     return LNB_ERR_UNSUPPORTED;
   }
-  int lb = (int)((227 * 1024 - smem) / Pol::ell_line_bytes());
+  int lb = (int)((lnb::SMEM_MAX - smem) / Pol::ell_line_bytes());
   if (lb > 255) lb = 255;
   // The readout scratch (at most 56 KiB: P = 48, H = 128, N = 128) fits the A ring (64 KiB), which
   // is idle after the last drain, at every shape accepted above; the check keeps it that way.

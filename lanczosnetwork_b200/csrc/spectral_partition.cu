@@ -28,7 +28,6 @@ namespace {
 
 using namespace eigs;
 
-constexpr int SP_PMIN = 2, SP_PMAX = 16;
 constexpr int SP_ITERS = 300;                 // KMeans' max_iter
 constexpr double SP_TIE = 1e-9;
 
@@ -232,7 +231,7 @@ struct Kmeans {
   // _relocate_empty_clusters_dense: each empty cluster (ascending) takes the next point farthest from
   // its centre (descending distance, ties by the lower index), which leaves its old cluster
   __device__ void relocate_empty() {
-    int far[SP_PMAX];
+    int far[LNB_PARTITION_MAX_P];
     int taken = 0;
     for (int j = 0; j < P; ++j) {
       if (wic[j] != 0.0) continue;
@@ -365,7 +364,7 @@ spectral_partition_kernel(const PartParams p) {
              km + 2 * P * P + 2 * P + N, km + 2 * P * P + 2 * P + 2 * N, lab, canon};
     const int iters = k.run(p.draws, p.T);
     if (lane == 0) {
-      int map[SP_PMAX], next = 0;
+      int map[LNB_PARTITION_MAX_P], next = 0;
       for (int j = 0; j < P; ++j) map[j] = -1;
       for (int i = 0; i < N; ++i) {
         if (!linked[i]) { canon[i] = -1; continue; }
@@ -447,9 +446,9 @@ spectral_partition_kernel(const PartParams p) {
   }
 }
 
-static_assert(sizeof(double) * part_doubles(GE_NMAX, 4, SP_PMAX, true) <= 227 * 1024,
+static_assert(sizeof(double) * part_doubles(LNB_MAX_N, 4, LNB_PARTITION_MAX_P, true) <= lnb::SMEM_MAX,
               "spectral_partition: N = 128, P = 16 must fit one CTA's shared memory");
-static_assert(4 * sizeof(double) * part_doubles(32, 1, SP_PMAX, true) <= 227 * 1024,
+static_assert(4 * sizeof(double) * part_doubles(32, 1, LNB_PARTITION_MAX_P, true) <= lnb::SMEM_MAX,
               "spectral_partition: four N = 32 graphs per CTA");
 
 template <bool SPARSE>
@@ -477,16 +476,17 @@ int launch(lnb_stream_t stream, const PartParams& p, const char* what) {
 extern "C" {
 
 int lnb_spectral_partition_draws(int P) {
-  if (P < SP_PMIN || P > SP_PMAX) return 0;
+  if (P < LNB_PARTITION_MIN_P || P > LNB_PARTITION_MAX_P) return 0;
   return 1 + (P - 1) * (2 + (int)log((double)P));
 }
 
 int lnb_spectral_partition(lnb_stream_t stream, const float* L, int64_t elem_stride, int B, int N, int P,
                            const double* inv_sqrt_deg, const double* draws, int32_t* labels, float* L_cluster,
                            float* L_cut, int32_t* status) {
-  if (!(B >= 0 && N >= 1 && N <= GE_NMAX && P >= SP_PMIN && P <= SP_PMAX && P < N && elem_stride >= 1)) {
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && P >= LNB_PARTITION_MIN_P && P <= LNB_PARTITION_MAX_P && P < N &&
+        elem_stride >= 1)) {
     lnb::set_err("spectral_partition: B=%d N=%d P=%d stride=%lld outside 1 <= N <= %d, %d <= P <= %d, P < N",
-                 B, N, P, (long long)elem_stride, GE_NMAX, SP_PMIN, SP_PMAX);
+                 B, N, P, (long long)elem_stride, LNB_MAX_N, LNB_PARTITION_MIN_P, LNB_PARTITION_MAX_P);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;
@@ -504,9 +504,10 @@ int lnb_spectral_partition_sparse(lnb_stream_t stream, const int32_t* sizes, con
                                   const double* draws, int32_t* labels, int32_t* status, float* ell_val,
                                   uint8_t* ell_idx, int32_t* ell_max, int32_t* gext, float* L_cluster,
                                   float* L_cut) {
-  if (!(B >= 0 && N >= 1 && N <= GE_NMAX && P >= SP_PMIN && P <= SP_PMAX && P < N && E >= 1 && E <= 32)) {
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && P >= LNB_PARTITION_MIN_P && P <= LNB_PARTITION_MAX_P && P < N &&
+        E >= 1 && E <= LNB_EIGS_MAX_E)) {
     lnb::set_err("spectral_partition_sparse: B=%d N=%d E=%d P=%d outside 1 <= N <= %d, %d <= P <= %d, P < N, "
-                 "1 <= E <= 32", B, N, E, P, GE_NMAX, SP_PMIN, SP_PMAX);
+                 "1 <= E <= 32", B, N, E, P, LNB_MAX_N, LNB_PARTITION_MIN_P, LNB_PARTITION_MAX_P);
     return LNB_ERR_UNSUPPORTED;
   }
   if (B == 0) return LNB_OK;

@@ -36,6 +36,7 @@
 namespace tcg {
 
 constexpr int BM = 128, BN = 128, BK = 32;
+static_assert(LNB_MAX_WIDTH <= BN, "a row of the widest layer fits one output tile");
 constexpr int TILE_B_BYTES = BN * BK * 4;          // 16 KB per hi or lo tile
 constexpr int STAGE_B_BYTES = 2 * TILE_B_BYTES;    // [W_hi tile | W_lo tile] = 256 rows x 128 B
 constexpr int TILE_A_BYTES = BM * BK * 4;          // 16 KB per hi or lo A block

@@ -53,6 +53,13 @@ def _opt(obj, name, default):
   return getattr(obj, name) if hasattr(obj, name) else default
 
 
+def _check_records_shape(N, E1):
+  """N and E+1 of a records or packed batch within the limits of the records producers."""
+  if not (1 <= N <= ops.MAX_N and 2 <= E1 <= ops.MAX_E1):
+    raise ValueError('forward_sparse: N=%d, E+1=%d outside 1 <= N <= %d, 2 <= E+1 <= %d'
+                     % (N, E1, ops.MAX_N, ops.MAX_E1))
+
+
 def loss_function(name):
   """The loss module of the config's ``model.loss`` (model/lanczos_net.py:64-71 and the other models)."""
   if name == 'CrossEntropy':
@@ -287,8 +294,7 @@ class SpectralNetBase(nn.Module):
       raise ValueError('forward_sparse: the batch lacks %s (data.sparse_collate records)' % ', '.join(missing))
     N, B = int(batch['N']), int(batch['sizes'].shape[0])
     E1 = self.num_edgetype + 1
-    if not (1 <= N <= 128 and 2 <= E1 <= 16):
-      raise ValueError('forward_sparse: N=%d, E+1=%d outside 1 <= N <= 128, 2 <= E+1 <= 16' % (N, E1))
+    _check_records_shape(N, E1)
     for k in ('sizes', 'node_ptr', 'node_feat', 'edge_ptr'):
       if k == 'node_feat' and feature_dim is not None:
         nf = batch[k]
@@ -321,8 +327,7 @@ class SpectralNetBase(nn.Module):
       raise ValueError('forward_sparse: blob must be a flat uint8 tensor of at least 64 bytes')
     B, N, K = int(batch['B']), int(batch['N']), int(batch['K'])
     E1 = self.num_edgetype + 1
-    if not (1 <= N <= 128 and 2 <= E1 <= 16):
-      raise ValueError('forward_sparse: N=%d, E+1=%d outside 1 <= N <= 128, 2 <= E+1 <= 16' % (N, E1))
+    _check_records_shape(N, E1)
     if B < 1 or K < 1:
       raise ValueError('forward_sparse: packed batch with B=%d, K=%d' % (B, K))
     eigs = batch.get('eigs')
@@ -569,7 +574,7 @@ class SpectralNetBase(nn.Module):
     first = 0
     while first < nl and not ok[first]:
       first += 1
-    stack_ok = uniform and first < nl and all(ok[first:]) and nl - first <= 8
+    stack_ok = uniform and first < nl and all(ok[first:]) and nl - first <= ops.CONV_MAX_LAYERS
     binarize = getattr(self, '_binarize_operators', False)
     if binarize and not (stack_ok and first == 0):
       L = (L != 0).to(L.dtype)          # shapes off the fused path read the dense operators
@@ -659,7 +664,7 @@ class SpectralNetBase(nn.Module):
     dims = [din0] + list(self.hidden_dim)
     ok = all(ops.fused_conv_supported(N, dims[t], K, dims[t + 1], len(self.short_diffusion_dist), False, S, E1)
              for t in range(self.num_layer))
-    return ok and all(d == dims[1] for d in dims[1:]) and self.num_layer <= 8
+    return ok and all(d == dims[1] for d in dims[1:]) and self.num_layer <= ops.CONV_MAX_LAYERS
 
   def _readout(self, state, mask):
     head = self.filter[self.num_layer]

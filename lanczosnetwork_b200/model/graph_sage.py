@@ -94,7 +94,7 @@ class GraphSAGE(SpectralNetBase):
     hidden width, every layer within the kernel's shapes (N <= 128, widths % 32, H <= 128) and at most
     48 outputs."""
     layers = self.num_layer - 1
-    if layers < 1 or layers > 8 or self.filter[self.num_layer].weight.shape[0] > 48:
+    if layers < 1 or layers > ops.CONV_MAX_LAYERS or self.filter[self.num_layer].weight.shape[0] > 48:
       return False
     dims = [self.embedding.weight.shape[1]] + list(self.hidden_dim[:layers])
     H = dims[1]

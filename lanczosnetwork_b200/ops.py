@@ -16,7 +16,8 @@ __all__ = [
     'graph_prepare_sparse', 'graph_prepare_sparse_features', 'graph_prepare_sparse_packed', 'records_unpack',
     'graph_eigs_sparse', 'sym_eigs',
     'spectral_partition', 'spectral_partition_sparse', 'spectral_partition_supported', 'partition_draws', 'gat_bias_sparse',
-    'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'embedding_rows', 'ritz_power_table', 'readout',
+    'fused_conv_supported', 'spectral_stack_forward', 'ritz_rowmap', 'ritz_filter_mlp', 'ritz_filter_mlp_supported', 'embedding_rows',
+    'ritz_power_table', 'readout',
     'gat_attention', 'gat_attention_supported', 'gat_attention_backward', 'gat_attention_backward_supported',
     'check_dropout_key', 'gat_attention_dropout', 'gat_attention_dropout_backward', 'gat_dropout_project',
     'gat_dropout_project_backward', 'gat_dropout_project_supported',
@@ -29,6 +30,34 @@ __all__ = [
     'tridiag_powers_backward', 'tridiag_powers_backward_supported', 'ada_start_vector', 'check_start_key',
     'lanczos_tridiag_train', 'lanczos_tridiag_backward', 'lanczos_tridiag_train_supported', 'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
+
+# The kernels' shape limits: the LNB_* limits of include/lanczosnet_b200.h under the same names without the
+# prefix, and SMEM_MAX of csrc/common.cuh.  The *_supported predicates and the argument checks read these.
+MAX_N = 128
+MAX_N_ELL = 255
+MAX_E1 = 16
+MAX_WIDTH = 128
+PREPARE_MAX_F = 4096
+CONV_MAX_K = 32
+CONV_MAX_LAYERS = 8
+FILTER_MLP_MAX_S = 32
+GAT_MAX_WIDTH = 128
+GAT_MAX_HEADS = 32
+SET2VEC_MAX_P = 128
+CHAIN_MAX_N = 32
+CHAIN_MAX_STEPS = 64
+MESSAGES_MAX_N = 32
+MESSAGES_MAX_K = 32
+MESSAGES_MAX_S = 8
+LANCZOS_FUSED_MAX_N = 1024
+LANCZOS_MAX_K = 64
+LANCZOS_TRAIN_MAX_N = 128
+TRIDIAG_POWERS_MAX_S = 32
+EIGS_MAX_K = 128
+EIGS_MAX_E = 32
+PARTITION_MIN_P = 2
+PARTITION_MAX_P = 16
+SMEM_MAX = 227 * 1024
 
 
 def _need_cuda(*tensors):
@@ -302,7 +331,7 @@ def graph_prepare_sparse_features(sizes, node_ptr, node_x, edge_ptr, edges, V_ro
   """graph_prepare_sparse for records with float node features (lnb_graph_prepare_sparse_features):
   node_x [>= node_ptr[B], F] float32 holds the feature rows of the real nodes instead of atom ids, and the
   padded features X [B,N,F] (real rows bit for bit, padded rows 0) come back instead of node ids.
-  1 <= F <= 4096.  Returns (GraphPrep, X [B,N,F], mask [B,N] uint8, V [B,N,K], L [B,N,N,E1] or None)."""
+  1 <= F <= PREPARE_MAX_F.  Returns (GraphPrep, X [B,N,F], mask [B,N] uint8, V [B,N,K], L [B,N,N,E1] or None)."""
   for name, t in (('sizes', sizes), ('node_ptr', node_ptr), ('edge_ptr', edge_ptr)):
     if t.dtype != torch.int32:
       raise ValueError('graph_prepare_sparse_features: %s must be int32; got %s' % (name, t.dtype))
@@ -314,9 +343,9 @@ def graph_prepare_sparse_features(sizes, node_ptr, node_x, edge_ptr, edges, V_ro
   if V_rows.dtype != torch.float32 or V_rows.dim() != 2 or not V_rows.is_contiguous():
     raise ValueError('graph_prepare_sparse_features: V_rows must be a contiguous float32 [rows, K] tensor')
   F = int(node_x.shape[1])
-  if not (1 <= int(N) <= 128 and 2 <= int(E1) <= 16 and 1 <= F <= 4096):
-    raise ValueError('graph_prepare_sparse_features: N=%d, E1=%d, F=%d outside 1 <= N <= 128, 2 <= E1 <= 16, '
-                     '1 <= F <= 4096' % (int(N), int(E1), F))
+  if not (1 <= int(N) <= MAX_N and 2 <= int(E1) <= MAX_E1 and 1 <= F <= PREPARE_MAX_F):
+    raise ValueError('graph_prepare_sparse_features: N=%d, E1=%d, F=%d outside 1 <= N <= %d, 2 <= E1 <= %d, '
+                     '1 <= F <= %d' % (int(N), int(E1), F, MAX_N, MAX_E1, PREPARE_MAX_F))
   _need_cuda(sizes, node_ptr, node_x, edge_ptr, edges, V_rows)
   dev = sizes.device
   B = sizes.shape[0]
@@ -468,10 +497,6 @@ def sym_eigs(A, sizes, K):
   return D, V, status
 
 
-PARTITION_MAX_N = 128
-PARTITION_P_RANGE = (2, 16)
-
-
 def partition_draws(N, P, seed=1234):
   """The draws scikit-learn's k-means++ seeding takes from a fresh ``RandomState(seed)`` for N points and
   P clusters, as one fp64 numpy array: ``choice(N, p=ones(N)/N)``, then ``uniform(size=2 + int(log P))``
@@ -512,9 +537,9 @@ def spectral_partition(L, num_partition, seed=1234):
     raise ValueError('spectral_partition: L must be [B,N,N] or [B,N,N,E1]; got %s' % (tuple(L.shape),))
   P, N = int(num_partition), int(L.shape[1])
   assert P < N - 1, 'spectral_partition: num_partition=%d needs more than %d nodes (N=%d)' % (P, P + 1, N)
-  if not (PARTITION_P_RANGE[0] <= P <= PARTITION_P_RANGE[1]) or N > PARTITION_MAX_N:
+  if not (PARTITION_MIN_P <= P <= PARTITION_MAX_P) or N > MAX_N:
     raise ValueError('spectral_partition: N=%d, num_partition=%d outside N <= %d, %d <= num_partition <= %d'
-                     % ((N, P, PARTITION_MAX_N) + PARTITION_P_RANGE))
+                     % (N, P, MAX_N, PARTITION_MIN_P, PARTITION_MAX_P))
   _need_cuda(L)
   A = L[..., 0] if L.dim() == 4 else L
   if A.dtype != torch.float32:
@@ -545,9 +570,12 @@ def _check_records(who, sizes, edge_ptr, edges):
 
 
 def spectral_partition_supported(N, num_partition):
-  """The envelope of spectral_partition and spectral_partition_sparse: N <= 128, 2 <= P <= 16, P < N - 1."""
+  """The envelope of spectral_partition and spectral_partition_sparse: N <= MAX_N,
+  PARTITION_MIN_P <= P <= PARTITION_MAX_P, P < N - 1."""
   P, N = int(num_partition), int(N)
-  return PARTITION_P_RANGE[0] <= P <= PARTITION_P_RANGE[1] and 1 <= N <= PARTITION_MAX_N and P < N - 1
+  # the kernels take P < N; P < N - 1 is the reference's own assertion in spectral_clustering
+  # (utils/spectral_graph_partition.py), so only partitions the reference can compute are accepted
+  return PARTITION_MIN_P <= P <= PARTITION_MAX_P and 1 <= N <= MAX_N and P < N - 1
 
 
 def spectral_partition_sparse(sizes, edge_ptr, edges, N, num_partition, num_edgetype, seed=1234,
@@ -562,9 +590,9 @@ def spectral_partition_sparse(sizes, edge_ptr, edges, N, num_partition, num_edge
   P, N, E = int(num_partition), int(N), int(num_edgetype)
   if not spectral_partition_supported(N, P):
     raise ValueError('spectral_partition_sparse: N=%d, num_partition=%d outside N <= %d, %d <= num_partition <= %d, '
-                     'num_partition < N - 1' % ((N, P, PARTITION_MAX_N) + PARTITION_P_RANGE))
-  if not 1 <= E <= 32:
-    raise ValueError('spectral_partition_sparse: num_edgetype=%d outside 1..32' % E)
+                     'num_partition < N - 1' % (N, P, MAX_N, PARTITION_MIN_P, PARTITION_MAX_P))
+  if not 1 <= E <= EIGS_MAX_E:
+    raise ValueError('spectral_partition_sparse: num_edgetype=%d outside 1..%d' % (E, EIGS_MAX_E))
   _check_records('spectral_partition_sparse', sizes, edge_ptr, edges)
   dev = sizes.device
   B = sizes.shape[0]
@@ -590,8 +618,8 @@ def gat_bias_sparse(sizes, edge_ptr, edges, N, E1):
   bit data.gat_bias of the collated operators (-0.0 on the diagonal and on the channel's bonds, -1e9
   elsewhere)."""
   N, E1 = int(N), int(E1)
-  if not (1 <= N <= 128 and 2 <= E1 <= 16):
-    raise ValueError('gat_bias_sparse: N=%d, E1=%d outside 1 <= N <= 128, 2 <= E1 <= 16' % (N, E1))
+  if not (1 <= N <= MAX_N and 2 <= E1 <= MAX_E1):
+    raise ValueError('gat_bias_sparse: N=%d, E1=%d outside 1 <= N <= %d, 2 <= E1 <= %d' % (N, E1, MAX_N, MAX_E1))
   _check_records('gat_bias_sparse', sizes, edge_ptr, edges)
   B = sizes.shape[0]
   bias = torch.empty((B, N, N, E1), device=sizes.device, dtype=torch.float32)
@@ -604,11 +632,11 @@ def gat_bias_sparse(sizes, edge_ptr, edges, N, E1):
 def fused_conv_supported(N, Din, K, H, n_short, dense_filter, S=8, E1=7):
   """Shapes the fused wgmma convolution kernel handles (others use the unfused ops);
   mirrors the checks of lnb_spectral_conv_fused."""
-  if (n_short or dense_filter or N > 128 or Din % 32 or K > 32 or K % 4 or H % 4 or H > 128 or
-      E1 > 16):
+  if (n_short or dense_filter or N > MAX_N or Din % 32 or K > CONV_MAX_K or K % 4 or H % 4 or H > MAX_WIDTH or
+      E1 > MAX_E1):
     return False
   smem = 4 * 32768 + 256 + 1024 + 128 * (max(Din, H) + 4) * 4 + 128 * K * 4 + 4096
-  return smem <= 227 * 1024
+  return smem <= SMEM_MAX
 
 
 def spectral_conv_fused(X, Q, coeff, prep, w_hi, w_lo, bias, relu=True, write_pad=True):
@@ -693,9 +721,9 @@ def sage_sample_sparse(sizes, node_ptr, node_feat, edge_ptr, edges, sample_key, 
     raise ValueError('sage_sample_sparse: sample_key must be a contiguous int64 tensor of shape (2,); got %s %s'
                      % (sample_key.dtype, tuple(sample_key.shape)))
   B = sizes.shape[0]
-  if not (1 <= N <= 128 and 2 <= E1 <= 16 and K >= 1 and B * N * E1 < 2 ** 31):
-    raise ValueError('sage_sample_sparse: B=%d N=%d E1=%d K=%d outside 1 <= N <= 128, 2 <= E1 <= 16, K >= 1, '
-                     'B*N*E1 < 2^31' % (B, N, E1, K))
+  if not (1 <= N <= MAX_N and 2 <= E1 <= MAX_E1 and K >= 1 and B * N * E1 < 2 ** 31):
+    raise ValueError('sage_sample_sparse: B=%d N=%d E1=%d K=%d outside 1 <= N <= %d, 2 <= E1 <= %d, K >= 1, '
+                     'B*N*E1 < 2^31' % (B, N, E1, K, MAX_N, MAX_E1))
   if want_ell_t and not want_ell:
     raise ValueError('sage_sample_sparse: want_ell_t needs want_ell')
   dev = sizes.device
@@ -808,6 +836,11 @@ def ritz_rowmap(gext, K):
   return rowmap, nrows
 
 
+def ritz_filter_mlp_supported(S, hidden):
+  """Shapes lnb_ritz_filter_mlp accepts: S scales and a hidden width of ``hidden``."""
+  return S <= FILTER_MLP_MAX_S and hidden % 32 == 0 and hidden <= MAX_WIDTH
+
+
 def ritz_filter_mlp(table, w_hi, w_lo, bias_all, num_layers, rowmap=None, nrows=None, ctas=0):
   """coeff[l, r, :] = MLP_l(table[r, :]) for all layers in one persistent kernel.
   table [R, S]; w_hi/w_lo [L*(3*Hd+S), Hd] stacked split weights; returns coeff [L, R, S]
@@ -867,7 +900,7 @@ def readout(state, W_out, b_out, w_att, b_att, mask=None):
 
 def gat_attention_supported(N, F, E1, heads):
   """Shapes lnb_gat_attention accepts (mirrors its checks)."""
-  return N <= 128 and F % 4 == 0 and F <= 128 and E1 <= 16 and heads <= 32
+  return N <= MAX_N and F % 4 == 0 and F <= GAT_MAX_WIDTH and E1 <= MAX_E1 and heads <= GAT_MAX_HEADS
 
 
 def gat_attention(Wh, bias, a1, a2, c1, c2, state_bias, last=False):
@@ -1000,7 +1033,7 @@ def gat_attention_dropout_backward(gout, Wh, bias, a1, a2, c1, c2, state_bias, d
 
 def gat_dropout_project_supported(Din, F):
   """Shapes lnb_gat_dropout_project(_backward) accept (mirrors their checks)."""
-  return Din % 4 == 0 and F % 4 == 0 and F <= 128
+  return Din % 4 == 0 and F % 4 == 0 and F <= GAT_MAX_WIDTH
 
 
 def _project_dims(who, X, W, C):
@@ -1049,7 +1082,7 @@ def gat_dropout_project_backward(X, W, gWh, C, dropout_key, p, t):
 
 def ggnn_update_supported(N, D, E1):
   """Shapes lnb_ggnn_update accepts (mirrors its checks)."""
-  return 1 <= N <= 255 and D % 32 == 0 and 32 <= D <= 128 and 1 <= E1 <= 16
+  return 1 <= N <= MAX_N_ELL and D % 32 == 0 and 32 <= D <= MAX_WIDTH and 1 <= E1 <= MAX_E1
 
 
 def ggnn_update(M, h, prep, w_hi, w_lo, bias, avg, out=None):
@@ -1078,7 +1111,7 @@ def ggnn_update(M, h, prep, w_hi, w_lo, bias, avg, out=None):
 
 def sage_lstm_step_supported(D, E1, K):
   """Shapes lnb_sage_lstm_step accepts (mirrors its checks)."""
-  return D % 32 == 0 and 32 <= D <= 128 and 1 <= E1 <= 16 and K >= 1
+  return D % 32 == 0 and 32 <= D <= MAX_WIDTH and 1 <= E1 <= MAX_E1 and K >= 1
 
 
 def sage_lstm_step(state, nn_idx, nonempty, h, c, w_hi, w_lo, bias, t, out):
@@ -1131,7 +1164,7 @@ def sage_lstm_messages(state, nn_idx, nonempty, w_hi, w_lo, bias):
 
 def gpnn_partition_update_supported(N, H):
   """Shapes lnb_gpnn_partition_update accepts (mirrors its checks)."""
-  return 1 <= N <= 255 and H % 32 == 0 and 32 <= H <= 128
+  return 1 <= N <= MAX_N_ELL and H % 32 == 0 and 32 <= H <= MAX_WIDTH
 
 
 def _rows_view(who, t, rows, H):
@@ -1193,7 +1226,7 @@ MPNN_EDGE_HIDDEN = 64      # width of the edge network's hidden layer, fixed in 
 
 def mpnn_update_supported(N, D, E1):
   """Shapes lnb_mpnn_update accepts (mirrors its checks)."""
-  return 1 <= N <= 255 and D % 32 == 0 and 32 <= D <= 128 and 1 <= E1 <= 16
+  return 1 <= N <= MAX_N_ELL and D % 32 == 0 and 32 <= D <= MAX_WIDTH and 1 <= E1 <= MAX_E1
 
 
 def mpnn_update(PQ, h, prep, w_hi, w_lo, bias, avg, out=None):
@@ -1223,7 +1256,7 @@ def mpnn_update(PQ, h, prep, w_hi, w_lo, bias, avg, out=None):
 
 def mpnn_edge_aggregate_supported(N, E1):
   """Shapes lnb_mpnn_edge_aggregate and its backward accept (mirrors their checks)."""
-  return 1 <= N <= 255 and 1 <= E1 <= 16
+  return 1 <= N <= MAX_N_ELL and 1 <= E1 <= MAX_E1
 
 
 def _check_pq(who, PQ, prep):
@@ -1263,10 +1296,6 @@ def mpnn_edge_aggregate_backward(PQ, gS, prep, prep_t, avg):
   return gPQ
 
 
-ELL_MAX_N = 128
-ELL_MAX_E1 = 16
-
-
 def _ell_operator(who, prep, c0, nc):
   """(B, N, E1, nc) of the ELL rows ``prep`` for the channels [c0, c0 + nc), or ValueError."""
   if len(prep) < 4:
@@ -1275,8 +1304,8 @@ def _ell_operator(who, prep, c0, nc):
   if val.dim() != 4 or val.shape[2] != val.shape[3]:
     raise ValueError('%s: ell_val must be [B, E1, N, N]; got %s' % (who, tuple(val.shape)))
   B, E1, N = val.shape[0], val.shape[1], val.shape[2]
-  if not (1 <= N <= ELL_MAX_N and 1 <= E1 <= ELL_MAX_E1):
-    raise ValueError('%s: N=%d, E1=%d outside 1 <= N <= %d, 1 <= E1 <= %d' % (who, N, E1, ELL_MAX_N, ELL_MAX_E1))
+  if not (1 <= N <= MAX_N and 1 <= E1 <= MAX_E1):
+    raise ValueError('%s: N=%d, E1=%d outside 1 <= N <= %d, 1 <= E1 <= %d' % (who, N, E1, MAX_N, MAX_E1))
   if (val.dtype != torch.float32 or idx.dtype != torch.uint8 or emax.dtype != torch.int32 or
       gext.dtype != torch.int32):
     raise ValueError('%s: ELL rows must be float32 / uint8 / int32 / int32 (ell_val, ell_idx, ell_max, gext)' % who)
@@ -1389,7 +1418,7 @@ def ell_messages_adjoint(G, prep_t, D, c0=0, nc=None, w=None, out=None):
 
 def set2vec_supported(N, D, P):
   """Shapes lnb_set2vec accepts (mirrors its checks)."""
-  return 1 <= N <= 128 and D % 32 == 0 and 32 <= D <= 128 and 1 <= P <= 128
+  return 1 <= N <= MAX_N and D % 32 == 0 and 32 <= D <= MAX_WIDTH and 1 <= P <= SET2VEC_MAX_P
 
 
 def set2vec(X, mask, WgT, bg, W1, W2, W_out, b_out, steps):
@@ -1420,7 +1449,7 @@ def set2vec(X, mask, WgT, bg, W1, W2, W_out, b_out, steps):
 
 
 def operator_chain_supported(N, steps):
-  return N <= 32 and steps <= 64
+  return N <= CHAIN_MAX_N and steps <= CHAIN_MAX_STEPS
 
 
 def operator_chain(L, X, steps, block_of_step, out, out_col0, chebyshev=False):
@@ -1441,7 +1470,8 @@ def operator_chain(L, X, steps, block_of_step, out, out_col0, chebyshev=False):
 
 
 def graph_messages_supported(N, K, E1, S, max_short):
-  return N <= 32 and (S == 0 or K <= 32) and E1 <= 16 and S <= 8 and max_short <= 64
+  return (N <= MESSAGES_MAX_N and (S == 0 or K <= MESSAGES_MAX_K) and E1 <= MAX_E1 and S <= MESSAGES_MAX_S and
+          max_short <= CHAIN_MAX_STEPS)
 
 
 def graph_messages(L, X, Q, filt, dense_filter, short_dist, out):
@@ -1565,12 +1595,12 @@ def tridiag_powers(T, powers):
 
 
 def tridiag_powers_backward_supported(K, powers):
-  """True when lnb_tridiag_powers_backward takes K and these powers: at most 32, positive and strictly
-  increasing, (6 K + (max power + 1) K^2) floats within 227 KB of shared memory."""
+  """True when lnb_tridiag_powers_backward takes K and these powers: at most TRIDIAG_POWERS_MAX_S, positive
+  and strictly increasing, (6 K + (max power + 1) K^2) floats within SMEM_MAX bytes of shared memory."""
   powers = [int(p) for p in powers]
-  return (1 <= len(powers) <= 32 and K >= 1 and powers[0] >= 1 and
+  return (1 <= len(powers) <= TRIDIAG_POWERS_MAX_S and K >= 1 and powers[0] >= 1 and
           all(a < b for a, b in zip(powers, powers[1:])) and
-          (6 * K + (powers[-1] + 1) * K * K) * 4 <= 227 * 1024)
+          (6 * K + (powers[-1] + 1) * K * K) * 4 <= SMEM_MAX)
 
 
 def tridiag_powers_backward(T, gOut, powers):
@@ -1580,8 +1610,8 @@ def tridiag_powers_backward(T, gOut, powers):
   S = len(powers)
   if not tridiag_powers_backward_supported(K, powers):
     raise ValueError('tridiag_powers_backward: K=%d with powers up to %d outside the shared-memory envelope '
-                     '((6 K + (max power + 1) K^2) * 4 bytes <= 227 KB, at most 32 powers)'
-                     % (K, max(powers) if powers else 0))
+                     '((6 K + (max power + 1) K^2) * 4 bytes <= %d KB, at most %d powers)'
+                     % (K, max(powers) if powers else 0, SMEM_MAX // 1024, TRIDIAG_POWERS_MAX_S))
   if tuple(gOut.shape) != (B, K, S, K):
     raise ValueError('tridiag_powers_backward: gOut must be [B,K,S,K] = %s; got %s'
                      % ((B, K, S, K), tuple(gOut.shape)))
@@ -1595,14 +1625,16 @@ def tridiag_powers_backward(T, gOut, powers):
 
 
 def lanczos_tridiag_train_supported(N, K):
-  """True when lnb_lanczos_tridiag_train / _backward take N and K: 1 <= N <= 128, 1 <= K <= 64."""
-  return 1 <= int(N) <= 128 and 1 <= int(K) <= 64
+  """True when lnb_lanczos_tridiag_train / _backward take N and K: 1 <= N <= LANCZOS_TRAIN_MAX_N,
+  1 <= K <= LANCZOS_MAX_K."""
+  return 1 <= int(N) <= LANCZOS_TRAIN_MAX_N and 1 <= int(K) <= LANCZOS_MAX_K
 
 
 def _lanczos_train_args(who, A, mask, q1, K):
   B, N = A.shape[0], A.shape[1]
   if not lanczos_tridiag_train_supported(N, K):
-    raise ValueError('%s: N=%d K=%d outside 1 <= N <= 128, 1 <= K <= 64' % (who, N, K))
+    raise ValueError('%s: N=%d K=%d outside 1 <= N <= %d, 1 <= K <= %d' % (who, N, K, LANCZOS_TRAIN_MAX_N,
+                                                                          LANCZOS_MAX_K))
   _need_cuda(A, mask, q1)
   A = _f32c(A)
   q1 = _f32c(q1).reshape(B, N)

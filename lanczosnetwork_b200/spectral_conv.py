@@ -156,7 +156,7 @@ def ritz_filter_coefficients(D, powers, mlp_layers, cache, gext=None, table=None
   nl = len(mlp_layers)
   flat = table.reshape(B * K, S)
   hd = mlp_layers[0][0][1].shape[0]
-  if S <= 32 and hd % 32 == 0 and hd <= 128:
+  if ops.ritz_filter_mlp_supported(S, hd):
     # all layers, all four stages in ONE persistent kernel, activations on chip; with the
     # extents of graph_prepare only the rows of non-zero Ritz vectors are evaluated
     w_hi, w_lo, bias_all = cache.split_mlp_chain('spectral_filter.chain', mlp_layers)

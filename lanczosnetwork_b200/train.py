@@ -995,7 +995,8 @@ def lanczos_tridiag(A, mask, q1, K):
   q1 [B,N] or [B,N,1] -> (T [B,K,K], Q [B,N,K]).  ValueError outside ops.lanczos_tridiag_train_supported."""
   B, N = A.shape[0], A.shape[1]
   if not ops.lanczos_tridiag_train_supported(N, K):
-    raise ValueError('lanczos_tridiag: N=%d K=%d outside 1 <= N <= 128, 1 <= K <= 64' % (N, K))
+    raise ValueError('lanczos_tridiag: N=%d K=%d outside 1 <= N <= %d, 1 <= K <= %d'
+                     % (N, K, ops.LANCZOS_TRAIN_MAX_N, ops.LANCZOS_MAX_K))
   q1 = q1.reshape(B, N).float().contiguous()
   if mask is not None:
     mask = (mask != 0).to(torch.uint8).contiguous()
