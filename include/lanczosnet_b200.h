@@ -741,27 +741,6 @@ int lnb_gaussian_laplacian(lnb_stream_t stream, const float* x, const float* L, 
                            int Dx, int E1, float* out /* [B,N,N] */);
 
 /* ---------------------------------------------------------------------------------------
- * Batched K-step Lanczos tridiagonalisation with full double re-orthogonalisation and the
- * reference's masking rules (model/ada_lanczos_net.py:139-247).  q1 is the raw start vector
- * (the randn draw of :161); mask (uint8, may be NULL) zeroes padded nodes.
- * Outputs: T [B,K,K] dense tridiagonal, Q [B,N,K], alpha [B,K], beta [B,K] (beta[b,K-1]=0),
- * idx [B] int32 = number of retained Krylov directions (:208-211).
- * ------------------------------------------------------------------------------------- */
-int lnb_lanczos_tridiag(lnb_stream_t stream, const float* A, const uint8_t* mask, const float* q1,
-                        int B, int N, int K, float* T, float* Q, float* alpha, float* beta,
-                        int32_t* idx);
-
-/* ---------------------------------------------------------------------------------------
- * Ritz pairs of the Lanczos tridiagonal: implicit-shift QL on (alpha, beta) with the
- * rotations applied to Q, so ritz_vec = Q S directly.  Ordered by descending |theta|
- * (the reference's Ritz ordering, utils/data_helper.py:217-223); ties keep ascending index.
- * status[b] = 0 ok, >0 = QL sweeps exhausted on that graph.
- * ------------------------------------------------------------------------------------- */
-int lnb_tridiag_ritz(lnb_stream_t stream, const float* alpha, const float* beta, const float* Q,
-                     int B, int N, int K, float* theta /* [B,K] */, float* ritz_vec /* [B,N,K] */,
-                     int32_t* status /* [B] */);
-
-/* ---------------------------------------------------------------------------------------
  * Exact eigenpairs of every graph's simple-graph operator, in fp64: the reference's offline
  * preprocessing (utils/data_helper.py:169-226 dense eigh branch, dataset/get_qm8_data.py:63-83,
  * truncated / zero padded to K at collate, dataset/qm8.py:265-291) on the device.  Householder
@@ -845,23 +824,26 @@ int lnb_gat_bias_sparse(lnb_stream_t stream, const int32_t* sizes, const int32_t
                         int B, int N, int E1, float* bias /* [B,N,N,E1] */);
 
 /* ---------------------------------------------------------------------------------------
- * The north-star pipeline in ONE launch: operator -> K-step Lanczos (rules of
- * model/ada_lanczos_net.py:139-247, as lnb_lanczos_tridiag) -> implicit-shift QL on (alpha, beta)
+ * The north-star pipeline in ONE launch: operator -> K-step Lanczos with full double
+ * re-orthogonalisation (rules of model/ada_lanczos_net.py:139-247) -> implicit-shift QL on (alpha, beta)
  * -> Ritz vectors V = Q S ordered by descending |theta| (utils/data_helper.py:217-223) -- the pair
  * (theta, V) is what utils/data_helper.py:169-226 + dataset/qm8.py:265-291 hand to
- * LanczosNet.forward as (D, V).  One group of 32..512 threads per graph; the dense padded operator
+ * LanczosNet.forward as (D, V).  q1 is the raw start vector (the randn draw of :161); mask (uint8, may
+ * be NULL) zeroes padded nodes.  One group of 32..512 threads per graph; the dense padded operator
  * A [B,N,N] is read from HBM exactly once (its non-zeros are packed into shared memory, exact zeros
  * contribute nothing to A q); the Krylov basis, (alpha, beta) and the QL rotations never leave the
- * SM.  T, Q may be NULL (not written).  theta / ritz_vec / status may be NULL together: then only
- * the tridiagonalisation is produced (AdaLanczosNet).  status[b]: bit 0 = QL sweeps exhausted,
- * bit 1 = the graph's non-zeros did not fit on chip and its rows were streamed per iteration.
+ * SM.  Outputs: T [B,K,K] dense tridiagonal, Q [B,N,K], alpha [B,K], beta [B,K] (beta[b,K-1]=0),
+ * idx [B] int32 = number of retained Krylov directions (:208-211).  T, Q may be NULL (not written).
+ * theta / ritz_vec / status may be NULL together: then only the tridiagonalisation is produced
+ * (AdaLanczosNet).  status[b]: bit 0 = QL sweeps exhausted, bit 1 = the graph's non-zeros did not fit
+ * on chip and its rows were streamed per iteration.
  * flags: 0 = the reference's masking rules (idx = min(#valid betas, #real nodes) directions and node
  * rows kept; the alpha of the breakdown step dropped, ada_lanczos_net.py:207-237);
  * LNB_LANCZOS_PROPER = the textbook Krylov factorisation (m = #valid + 1 vectors, T_m with m alphas
  * and m-1 betas, no row masking; idx[b] = m) whose Ritz values are eigenvalues of A -- the mode of
  * the online (D, V) provider.
  * Limits: N <= LNB_LANCZOS_FUSED_MAX_N, K <= LNB_LANCZOS_MAX_K and a basis of K*(N+1) floats within shared memory
- * (LNB_ERR_UNSUPPORTED otherwise: use lnb_lanczos_tridiag + lnb_tridiag_ritz).
+ * (LNB_ERR_UNSUPPORTED otherwise, nothing launched).
  * ------------------------------------------------------------------------------------- */
 #define LNB_LANCZOS_PROPER 1
 int lnb_lanczos_ritz(lnb_stream_t stream, const float* A, const uint8_t* mask, const float* q1,

@@ -143,10 +143,6 @@ SIGNATURES = {
     'lnb_graph_messages': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_int,
                                    c_int, c_int, c_int, ctypes.POINTER(c_int), c_int, c_f32p, c_i64, c_i64]),
     'lnb_gaussian_laplacian': (c_int, [c_stream, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_f32p]),
-    'lnb_lanczos_tridiag': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_int, c_int, c_int,
-                                    c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_void_p]),
-    'lnb_tridiag_ritz': (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_f32p,
-                                 c_f32p, ctypes.c_void_p]),
     'lnb_lanczos_ritz': (c_int, [c_stream, c_f32p, ctypes.c_void_p, c_f32p, c_int, c_int, c_int, c_int,
                                  c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, c_f32p, c_f32p,
                                  ctypes.c_void_p]),

@@ -12,6 +12,10 @@ namespace lnb {
 // dynamic shared memory one CTA may opt in to on sm_90a
 constexpr int SMEM_MAX = 227 * 1024;
 
+// the reference's Lanczos constants, shared by the inference and training kernels
+constexpr float LANCZOS_EPS = 1.1920928955078125e-07f;  // np.finfo(np.float32).eps (ada_lanczos_net.py:8)
+constexpr float LANCZOS_BETA_LOWER_BOUND = 1.0e-4f;     // ada_lanczos_net.py:169
+
 // thread-local error text + launch counter (no other global mutable state)
 char* err_buf();
 void set_err(const char* fmt, ...);

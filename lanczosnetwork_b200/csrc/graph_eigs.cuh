@@ -3,8 +3,8 @@
 //
 //   1. Householder tridiagonalisation of the leading n x n block (lower triangle, packed in shared
 //      memory; the reflectors overwrite the columns they annihilate, as LAPACK's dsptrd does),
-//   2. implicit-shift QL on the tridiagonal with the rotations accumulated into Z (the pattern of
-//      tridiag_ritz_kernel, in fp64),
+//   2. implicit-shift QL on the tridiagonal with the rotations accumulated into Z (the QL stage of
+//      lanczos_fused.cu, in fp64),
 //   3. the reference's ordering: descending |lambda|, ties by ascending lambda (np.argsort(-|w|,
 //      kind='mergesort') over eigh's ascending order), then the first kk,
 //   4. the back-transform Q Z of only those columns.

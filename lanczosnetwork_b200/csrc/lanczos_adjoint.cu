@@ -134,8 +134,6 @@ size_t powers_backward_smem(int K, int pmax) {
 // ------------------------------------------------------------------------------------------------------
 constexpr int LZ_THREADS = 128;
 static_assert(LNB_LANCZOS_TRAIN_MAX_N <= LZ_THREADS, "thread n owns node n");
-constexpr float kLzEps = 1.1920928955078125e-07f;   // np.finfo(np.float32).eps (ada_lanczos_net.py:8)
-constexpr float kLzBetaLowerBound = 1.0e-4f;        // ada_lanczos_net.py:169
 
 __device__ __forceinline__ float lz_block_sum(float v, float* red) {
   v = lnb::warp_sum(v);
@@ -249,18 +247,18 @@ __global__ void __launch_bounds__(LZ_THREADS) lanczos_train_kernel(const LzParam
   const float q0 = v / nrm;
   if (act) Qs[n] = q0;
   const float qq0 = lz_block_sum(act ? q0 * q0 : 0.f, red);
-  if (n == 0) iqs[0] = 1.f / (qq0 + kLzEps);
+  if (n == 0) iqs[0] = 1.f / (qq0 + lnb::LANCZOS_EPS);
 
   float bprev = 0.f, okv = 1.f;
   int count = 0;
   for (int i = 0; i < iters; ++i) {
     const LzStep st = lz_step(i, n, N, As, lda, Qs, iqs, bprev, zs, pr1, pr2, red);
-    okv = (st.b >= kLzBetaLowerBound) ? okv : 0.f;
+    okv = (st.b >= lnb::LANCZOS_BETA_LOWER_BOUND) ? okv : 0.f;
     count += (okv != 0.f) ? 1 : 0;
-    const float qn = act ? (st.z2 * okv) / (st.b + kLzEps) : 0.f;
+    const float qn = act ? (st.z2 * okv) / (st.b + lnb::LANCZOS_EPS) : 0.f;
     if (act) Qs[(i + 1) * N + n] = qn;
     const float qq = lz_block_sum(qn * qn, red);
-    if (n == 0) { iqs[i + 1] = 1.f / (qq + kLzEps); al[i] = st.a; be[i] = st.b; okf[i] = okv; }
+    if (n == 0) { iqs[i + 1] = 1.f / (qq + lnb::LANCZOS_EPS); al[i] = st.a; be[i] = st.b; okf[i] = okv; }
     bprev = st.b;
     __syncthreads();
   }
@@ -315,7 +313,7 @@ __global__ void __launch_bounds__(LZ_THREADS) lanczos_train_kernel(const LzParam
     // q_{i+1} is final: add the gradient through s_{i+1} = 1 / (q.q + EPS)
     const float sn = iqs[i + 1];
     const float qbn = act ? Qb[(i + 1) * N + n] - 2.f * sn * sn * sbar[i + 1] * qnext : 0.f;
-    const float ok = okf[i], inv = 1.f / (st.b + kLzEps);
+    const float ok = okf[i], inv = 1.f / (st.b + lnb::LANCZOS_EPS);
     float zb = qbn * ok * inv;
     const float t = lz_block_sum(qbn * st.z2, red);
     const float bb = bbar[i] - ok * t * inv * inv;

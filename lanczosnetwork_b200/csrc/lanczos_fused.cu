@@ -25,8 +25,6 @@
 
 namespace {
 
-constexpr float kEps = 1.1920928955078125e-07f;  // np.finfo(np.float32).eps (ada_lanczos_net.py:8)
-constexpr float kBetaLowerBound = 1.0e-4f;       // ada_lanczos_net.py:169
 constexpr unsigned kFull = 0xffffffffu;
 
 struct FusedParams {
@@ -322,7 +320,7 @@ lanczos_ritz_kernel(const FusedParams P) {
     for (int kk = 0; kk < NPT; ++kk) { pa = fmaf(q[kk], z[kk], pa); pq = fmaf(q[kk], q[kk], pq); }
     const float2 aq = gsum2<TPG>(pa, pq, red, flip, grp, wg, lane);
     const float alpha = aq.x;
-    if (t == 0) iq[i] = 1.f / (aq.y + kEps);    // first read by the projections of step i+1
+    if (t == 0) iq[i] = 1.f / (aq.y + lnb::LANCZOS_EPS);    // first read by the projections of step i+1
 #pragma unroll
     for (int kk = 0; kk < NPT; ++kk) z[kk] = z[kk] - alpha * q[kk] - beta_prev * qp[kk];
     if (i > 0) {
@@ -412,12 +410,12 @@ lanczos_ritz_kernel(const FusedParams P) {
 #pragma unroll
     for (int kk = 0; kk < NPT; ++kk) pb = fmaf(z[kk], z[kk], pb);
     const float beta = sqrtf(gsum2<TPG>(pb, 0.f, red, flip, grp, wg, lane).x);
-    valid = (beta >= kBetaLowerBound) ? valid : 0.f;
+    valid = (beta >= lnb::LANCZOS_BETA_LOWER_BOUND) ? valid : 0.f;
     count += (valid != 0.f) ? 1 : 0;
     if (t == 0) { al[i] = alpha; be[i] = beta; }
 #pragma unroll
     for (int kk = 0; kk < NPT; ++kk) {
-      const float qn = (z[kk] * valid) / (beta + kEps);
+      const float qn = (z[kk] * valid) / (beta + lnb::LANCZOS_EPS);
       qp[kk] = q[kk]; q[kk] = qn;
       if (i + 1 < iters) Qs[(size_t)(i + 1) * NS + t + kk * TPG] = qn;
     }

@@ -26,7 +26,7 @@ __all__ = [
     'ggnn_update_supported', 'gpnn_partition_update', 'gpnn_partition_update_supported', 'mpnn_update', 'mpnn_update_supported', 'mpnn_edge_aggregate',
     'mpnn_edge_aggregate_backward', 'mpnn_edge_aggregate_supported', 'ell_messages', 'ell_messages_adjoint',
     'set2vec', 'set2vec_supported',
-    'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_tridiag', 'lanczos_ritz', 'tridiag_ritz', 'tridiag_powers',
+    'operator_chain', 'operator_chain_supported', 'graph_messages', 'graph_messages_supported', 'gaussian_laplacian', 'lanczos_ritz', 'tridiag_powers',
     'tridiag_powers_backward', 'tridiag_powers_backward_supported', 'ada_start_vector', 'check_start_key',
     'lanczos_tridiag_train', 'lanczos_tridiag_backward', 'lanczos_tridiag_train_supported', 'symmetrize_filters', 'segment_sum_forward', 'segment_sum_backward', 'launch_count',
 ]
@@ -1510,41 +1510,6 @@ def gaussian_laplacian(x, L):
     _lib.check(_lib.load().lnb_gaussian_laplacian(_stream(x), _ptr(x), _ptr(L), B, N, Dx, E1,
                                                   _ptr(out)), 'lnb_gaussian_laplacian')
   return out
-
-
-def lanczos_tridiag(A, mask, q1, K):
-  """Returns dict(T [B,K,K], Q [B,N,K], alpha [B,K], beta [B,K], idx [B] int32)."""
-  _need_cuda(A, mask, q1)
-  A = _f32c(A)
-  B, N = A.shape[0], A.shape[1]
-  q1 = _f32c(q1).reshape(B, N)
-  if mask is not None:
-    mask = (mask != 0).to(torch.uint8).contiguous()
-  dev = A.device
-  T = torch.empty((B, K, K), device=dev, dtype=torch.float32)
-  Q = torch.empty((B, N, K), device=dev, dtype=torch.float32)
-  alpha = torch.empty((B, K), device=dev, dtype=torch.float32)
-  beta = torch.empty((B, K), device=dev, dtype=torch.float32)
-  idx = torch.empty((B,), device=dev, dtype=torch.int32)
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_lanczos_tridiag(_stream(A), _ptr(A), _ptr(mask), _ptr(q1), B, N, K,
-                                               _ptr(T), _ptr(Q), _ptr(alpha), _ptr(beta),
-                                               _ptr(idx)), 'lnb_lanczos_tridiag')
-  return {'T': T, 'Q': Q, 'alpha': alpha, 'beta': beta, 'idx': idx}
-
-
-def tridiag_ritz(alpha, beta, Q):
-  """Ritz values (descending |theta|) and vectors V = Q S.  Returns (theta, V, status)."""
-  _need_cuda(alpha, beta, Q)
-  alpha, beta, Q = _f32c(alpha), _f32c(beta), _f32c(Q)
-  B, N, K = Q.shape
-  theta = torch.empty((B, K), device=Q.device, dtype=torch.float32)
-  V = torch.empty((B, N, K), device=Q.device, dtype=torch.float32)
-  status = torch.empty((B,), device=Q.device, dtype=torch.int32)
-  with torch.cuda.device(Q.device):
-    _lib.check(_lib.load().lnb_tridiag_ritz(_stream(Q), _ptr(alpha), _ptr(beta), _ptr(Q), B, N, K,
-                                            _ptr(theta), _ptr(V), _ptr(status)), 'lnb_tridiag_ritz')
-  return theta, V, status
 
 
 def lanczos_ritz(A, mask, q1, K, want_ritz=True, want_T=True, want_Q=True, proper=False):

@@ -1,22 +1,20 @@
-"""Measurements of the BASELINE.json configs other than the bench.py headline (profiling aid;
-numbers are printed).  Run on an H100:  python tools/bench_configs.py"""
+"""Measurements of the BASELINE.json model configs other than the bench.py headline (profiling aid;
+numbers are printed; the Lanczos configs are in tools/time_lanczos.py).  Run on an H100:
+python tools/bench_configs.py"""
 import json
 import os
 import sys
 
-import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 from helpers import deterministic_state_dict  # noqa: E402
-from lanczosnetwork_b200 import configs, data, ops  # noqa: E402
+from lanczosnetwork_b200 import configs, data  # noqa: E402
 from lanczosnetwork_b200.model import AdaLanczosNet, LanczosNetGeneral  # noqa: E402
 
 dev = torch.device('cuda:0')
-PEAK = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))) if os.path.exists(
-    os.path.join(ROOT, 'MEASURED_PEAKS.json')) else {'hbm_gbs': 3350.0, 'bf16_tflops_sustained': 989.0}
 
 
 def timeit(fn, iters=10, warm=3):
@@ -30,51 +28,6 @@ def timeit(fn, iters=10, warm=3):
   b.record()
   torch.cuda.synchronize()
   return a.elapsed_time(b) / iters
-
-
-def lanczos_sweep(out):
-  """Config #5: N in {64,256,1024}, K=40, L4 of G(N,p) with p=min(0.5, 8/N), n_b=N."""
-  import networkx as nx
-  for N, G in [(64, 10000), (256, 10000), (1024, 2000)]:
-    K = 40
-    rng = np.random.RandomState(1234)
-    base = []
-    for i in range(8):            # 8 distinct graphs tiled to G (generation cost), all dense reads
-      g = nx.fast_gnp_random_graph(N, min(0.5, 8.0 / N), seed=int(rng.randint(10 ** 6)))
-      base.append(data.get_laplacian(np.asarray(nx.to_numpy_array(g))).astype(np.float32))
-    A = torch.from_numpy(np.stack(base)).to(dev)
-    A = A.repeat((G + 7) // 8, 1, 1)[:G].contiguous()
-    q1 = torch.randn(G, N, generator=torch.Generator().manual_seed(1234)).to(dev)
-    lz = ops.lanczos_tridiag(A, None, q1, K)
-    t_l = timeit(lambda: ops.lanczos_tridiag(A, None, q1, K), iters=3, warm=1)
-    t_r = timeit(lambda: ops.tridiag_ritz(lz['alpha'], lz['beta'], lz['Q']), iters=3, warm=1)
-    bytes_alg = 4 * N * N + 4 * N + 4 * N * K + 4 * (2 * K - 1) + 4 * K * K
-    bytes_ritz = 4 * N * K * 2 + 4 * K * 3
-    rec = {
-        'N': N, 'K': K, 'graphs': G,
-        'lanczos_ms': t_l, 'lanczos_graphs_per_s': G / (t_l * 1e-3),
-        'lanczos_alg_GBs': G * bytes_alg / (t_l * 1e-3) / 1e9,
-        'lanczos_frac_hbm': G * bytes_alg / (t_l * 1e-3) / 1e9 / PEAK['hbm_gbs'],
-        'lanczos_gflops': G * (2.0 * K * N * N + 6.0 * N * K * K + 8.0 * N * K) / (t_l * 1e-3) / 1e9,
-        'ritz_ms': t_r, 'ritz_graphs_per_s': G / (t_r * 1e-3),
-        'ritz_alg_GBs': G * bytes_ritz / (t_r * 1e-3) / 1e9,
-    }
-    out.append(('lanczos_sweep', rec))
-    print(json.dumps(rec), flush=True)
-
-
-def qm8_lanczos_ritz(out):
-  batch = data.synthetic_qm8_batch(1024, seed=1)
-  A = torch.from_numpy(batch['L'][..., 0].copy()).to(dev)
-  mask = torch.from_numpy(batch['node_mask']).to(dev)
-  q1 = torch.randn(1024, 26, generator=torch.Generator().manual_seed(1)).to(dev)
-  lz = ops.lanczos_tridiag(A, mask, q1, 20)
-  t_l = timeit(lambda: ops.lanczos_tridiag(A, mask, q1, 20))
-  t_r = timeit(lambda: ops.tridiag_ritz(lz['alpha'], lz['beta'], lz['Q']))
-  rec = {'config': 'QM8-shaped B=1024 N=26 K=20', 'lanczos_us': t_l * 1e3, 'ritz_us': t_r * 1e3,
-         'lanczos_graphs_per_s': 1024 / (t_l * 1e-3), 'ritz_graphs_per_s': 1024 / (t_r * 1e-3)}
-  out.append(('qm8_lanczos', rec))
-  print(json.dumps(rec), flush=True)
 
 
 def ada_forward(out):
@@ -112,12 +65,8 @@ def general_forward(out):
 
 if __name__ == '__main__':
   res = []
-  which = sys.argv[1:] or ['qm8', 'general', 'sweep', 'ada']
-  if 'qm8' in which:
-    qm8_lanczos_ritz(res)
+  which = sys.argv[1:] or ['general', 'ada']
   if 'general' in which:
     general_forward(res)
-  if 'sweep' in which:
-    lanczos_sweep(res)
   if 'ada' in which:
     ada_forward(res)

@@ -35,8 +35,6 @@ if 'qm8' in which:
   for kw in ([] if PHASES_ONLY else [{}, {'want_ritz': False}, {'want_T': False, 'want_Q': False}]):
     t = bench.time_events(lambda: ops.lanczos_ritz(A, mask, q1, 20, **kw), 20, 5)
     report('qm8 %s' % kw, t, 1024, 26, 20, o['status'])
-  t = 0.0 if PHASES_ONLY else bench.time_events(lambda: ops.lanczos_tridiag(A, mask, q1, 20), 20, 5)
-  print('old lanczos_tridiag qm8 ms', t)
 for N, G in ((64, 10000), (256, 10000), (1024, 10000)):
   if str(N) not in which:
     continue
