@@ -83,6 +83,15 @@ def _stream(t):
   return ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
 
 
+def _launch(name, on, *args):
+  """Runs library entry `name` with `on`'s device current, on that device's current stream (the
+  entry's first argument); tensors in `args` are passed as their data pointers, None as NULL, and
+  everything else as given.  RuntimeError('<name> failed (status s): <text>') on a non-zero status."""
+  with torch.cuda.device(on.device):
+    _lib.check(getattr(_lib.load(), name)(
+        _stream(on), *[_ptr(a) if a is None or isinstance(a, torch.Tensor) else a for a in args]), name)
+
+
 def _ints(vals):
   arr = (ctypes.c_int * len(vals))(*[int(v) for v in vals])
   return arr
@@ -99,7 +108,6 @@ def bgemm(A, a_str, Bm, b_str, C, c_str, batch, nz, M, N, K, kscale=None, s_str=
   """C[b,z] = act(alpha * (A[b,z] * kscale[b,z]) @ B[b,z] + beta * addend[b,z] + bias); strides in
   elements, *_off element offsets into the (fp32, CUDA) storage of A / B / C / addend."""
   _need_cuda(A, Bm, C, kscale, bias)
-  lib = _lib.load()
   d = GemmDesc()
   d.A = A.data_ptr() + 4 * a_off
   d.a_sb, d.a_sz, d.a_sm, d.a_sk = [int(v) for v in a_str]
@@ -115,8 +123,7 @@ def bgemm(A, a_str, Bm, b_str, C, c_str, batch, nz, M, N, K, kscale=None, s_str=
   d.alpha, d.beta = float(alpha), float(beta)
   d.addend = addend.data_ptr() + 4 * add_off if addend is not None else None
   d.d_sb, d.d_sz, d.d_sm, d.d_sn = [int(v) for v in add_str]
-  with torch.cuda.device(C.device):
-    _lib.check(lib.lnb_batched_gemm(_stream(C), ctypes.byref(d)), 'lnb_batched_gemm')
+  _launch('lnb_batched_gemm', C, ctypes.byref(d))
   return C
 
 
@@ -126,9 +133,7 @@ def split_tf32(x):
   x = _f32c(x)
   hi = torch.empty_like(x)
   lo = torch.empty_like(x)
-  with torch.cuda.device(x.device):
-    _lib.check(_lib.load().lnb_split_tf32(_stream(x), _ptr(x), x.numel(), _ptr(hi), _ptr(lo)),
-               'lnb_split_tf32')
+  _launch('lnb_split_tf32', x, x, x.numel(), hi, lo)
   return hi, lo
 
 
@@ -154,16 +159,12 @@ def linear_tf32x3(x, w_hi, w_lo, bias=None, relu=False, out=None):
     splits = min(_sm_count(x.device) // tiles, 8, nkb // 16)
     while splits > 1 and ((nkb + splits - 1) // splits) * (splits - 1) >= nkb:
       splits -= 1
-  with torch.cuda.device(x.device):
-    if splits > 1:
-      ws, counters = _splitk_workspace(x.device, tiles * splits * 128 * 128, tiles)
-      _lib.check(_lib.load().lnb_linear_tf32x3_splitk(
-          _stream(x), _ptr(x), _ptr(w_hi), _ptr(w_lo), _ptr(bias), M, N, K, int(bool(relu)),
-          _ptr(out), splits, _ptr(ws), _ptr(counters)), 'lnb_linear_tf32x3_splitk')
-    else:
-      _lib.check(_lib.load().lnb_linear_tf32x3(_stream(x), _ptr(x), _ptr(w_hi), _ptr(w_lo),
-                                               _ptr(bias), M, N, K, int(bool(relu)), _ptr(out)),
-                 'lnb_linear_tf32x3')
+  if splits > 1:
+    ws, counters = _splitk_workspace(x.device, tiles * splits * 128 * 128, tiles)
+    _launch('lnb_linear_tf32x3_splitk', x, x, w_hi, w_lo, bias, M, N, K, int(bool(relu)), out, splits, ws,
+            counters)
+  else:
+    _launch('lnb_linear_tf32x3', x, x, w_hi, w_lo, bias, M, N, K, int(bool(relu)), out)
   return out
 
 
@@ -207,11 +208,7 @@ def linear_tf32x3_grouped(x, w_hi, w_lo, bias, groups, relu=False):
   N = w_hi.shape[0] // groups
   assert x.shape[1] == groups * K and w_hi.shape[0] == groups * N
   out = torch.empty((M, groups * N), device=x.device, dtype=torch.float32)
-  with torch.cuda.device(x.device):
-    _lib.check(_lib.load().lnb_linear_tf32x3_grouped(_stream(x), _ptr(x), _ptr(w_hi), _ptr(w_lo),
-                                                     _ptr(bias), M, groups, N, K,
-                                                     int(bool(relu)), _ptr(out)),
-               'lnb_linear_tf32x3_grouped')
+  _launch('lnb_linear_tf32x3_grouped', x, x, w_hi, w_lo, bias, M, groups, N, K, int(bool(relu)), out)
   return out
 
 
@@ -228,9 +225,7 @@ def tile_assign(prep, K):
   """Writes the tile table and schedule of a GraphPrep built with defer_tiles (lnb_tile_assign) on
   the current stream; they equal what graph_prepare without defer_tiles writes."""
   gext, tiles = prep[3], prep[4]
-  with torch.cuda.device(gext.device):
-    _lib.check(_lib.load().lnb_tile_assign(_stream(gext), _ptr(gext), gext.shape[0], int(K), _ptr(tiles)),
-               'lnb_tile_assign')
+  _launch('lnb_tile_assign', gext, gext, gext.shape[0], int(K), tiles)
   prep.tiles_pending = False
 
 
@@ -258,12 +253,8 @@ def graph_prepare(L, Q=None, binarize=False, defer_tiles=False):
   tiles = torch.empty((4 * B + 2,), device=dev, dtype=torch.int32)   # tile table + scratch
   rowmap = torch.empty((B * K,), device=dev, dtype=torch.int32)
   nrows = torch.empty((1,), device=dev, dtype=torch.int32)
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_graph_prepare(_stream(L), _ptr(L), _ptr(Q), B, N, E1, K,
-                                             _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max),
-                                             _ptr(gext), _ptr(tiles), _ptr(rowmap), _ptr(nrows),
-                                             (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0)),
-               'lnb_graph_prepare')
+  _launch('lnb_graph_prepare', L, L, Q, B, N, E1, K, ell_val, ell_idx, ell_max, gext, tiles, rowmap, nrows,
+          (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0))
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows, prep.tiles_pending = rowmap, nrows, bool(defer_tiles) and B > 0
   return prep
@@ -313,14 +304,10 @@ def graph_prepare_sparse(sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N,
   mask = torch.empty((B, N), device=dev, dtype=torch.uint8)
   V = torch.empty((B, N, K), device=dev, dtype=torch.float32)
   L = torch.empty((B, N, N, E1), device=dev, dtype=torch.float32) if want_dense else None
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_graph_prepare_sparse(
-        _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(node_feat), _ptr(edge_ptr), _ptr(edges),
-        _ptr(V_rows), _ptr(_inv_sqrt_deg_table(dev)), B, int(N), int(E1), int(K),
-        (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0), _ptr(ell_val), _ptr(ell_idx),
-        _ptr(ell_max), _ptr(gext), _ptr(tiles),
-        _ptr(rowmap), _ptr(nrows), _ptr(node_ids), _ptr(mask), _ptr(V), _ptr(L)),
-               'lnb_graph_prepare_sparse')
+  _launch('lnb_graph_prepare_sparse', sizes, sizes, node_ptr, node_feat, edge_ptr, edges, V_rows,
+          _inv_sqrt_deg_table(dev), B, int(N), int(E1), int(K),
+          (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0), ell_val, ell_idx, ell_max, gext, tiles,
+          rowmap, nrows, node_ids, mask, V, L)
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows, prep.tiles_pending = rowmap, nrows, bool(defer_tiles) and B > 0
   return prep, node_ids, mask, V, L
@@ -361,13 +348,10 @@ def graph_prepare_sparse_features(sizes, node_ptr, node_x, edge_ptr, edges, V_ro
   mask = torch.empty((B, N), device=dev, dtype=torch.uint8)
   V = torch.empty((B, N, K), device=dev, dtype=torch.float32)
   L = torch.empty((B, N, N, E1), device=dev, dtype=torch.float32) if want_dense else None
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_graph_prepare_sparse_features(
-        _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(node_x), _ptr(edge_ptr), _ptr(edges),
-        _ptr(V_rows), _ptr(_inv_sqrt_deg_table(dev)), B, int(N), int(E1), int(K), F,
-        (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0), _ptr(ell_val), _ptr(ell_idx),
-        _ptr(ell_max), _ptr(gext), _ptr(tiles), _ptr(rowmap), _ptr(nrows), _ptr(X), _ptr(mask), _ptr(V), _ptr(L)),
-               'lnb_graph_prepare_sparse_features')
+  _launch('lnb_graph_prepare_sparse_features', sizes, sizes, node_ptr, node_x, edge_ptr, edges, V_rows,
+          _inv_sqrt_deg_table(dev), B, int(N), int(E1), int(K), F,
+          (1 if binarize else 0) | (PREP_DEFER_TILES if defer_tiles else 0), ell_val, ell_idx, ell_max, gext, tiles,
+          rowmap, nrows, X, mask, V, L)
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows, prep.tiles_pending = rowmap, nrows, bool(defer_tiles) and B > 0
   return prep, X, mask, V, L
@@ -398,12 +382,9 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
   mask = torch.empty((B, N), device=dev, dtype=torch.uint8)
   V = torch.empty((B, N, K), device=dev, dtype=torch.float32)
   L = torch.empty((B, N, N, E1), device=dev, dtype=torch.float32) if want_dense else None
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_graph_prepare_sparse_packed(
-        _stream(blob), _ptr(blob), _ptr(_inv_sqrt_deg_table(dev)), int(B), int(N), int(E1), int(K),
-        (1 if binarize else 0) | (PACKED_HOST_TILES if host_tiles else 0), _ptr(ell_val), _ptr(ell_idx),
-        _ptr(ell_max), _ptr(gext), _ptr(tiles), _ptr(rowmap), _ptr(nrows), _ptr(node_ids), _ptr(mask), _ptr(V), _ptr(L)),
-               'lnb_graph_prepare_sparse_packed')
+  _launch('lnb_graph_prepare_sparse_packed', blob, blob, _inv_sqrt_deg_table(dev), int(B), int(N), int(E1), int(K),
+          (1 if binarize else 0) | (PACKED_HOST_TILES if host_tiles else 0), ell_val, ell_idx, ell_max, gext, tiles,
+          rowmap, nrows, node_ids, mask, V, L)
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows = rowmap, nrows
   return prep, node_ids, mask, V, L
@@ -438,15 +419,13 @@ def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False, label_dim=0):
   D = torch.empty((B, K), device=dev, dtype=torch.float32) if eigs else None
   V_rows = torch.empty((cap_rows, K), device=dev, dtype=torch.float32) if eigs else None
   status = torch.empty((1,), **i32)
-  args = (_stream(blob), _ptr(blob), blob.numel(), B, K, cap_rows, cap_edges, _ptr(sizes), _ptr(node_ptr),
-          _ptr(node_feat), _ptr(edge_ptr), _ptr(edges), _ptr(D), _ptr(V_rows), _ptr(status))
+  args = (blob, blob.numel(), B, K, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows,
+          status)
   if not P:
-    with torch.cuda.device(dev):
-      _lib.check(_lib.load().lnb_records_unpack(*args), 'lnb_records_unpack')
+    _launch('lnb_records_unpack', blob, *args)
     return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, status
   label = torch.empty((B, P), device=dev, dtype=torch.float32)
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_records_unpack_labels(*args, P, _ptr(label)), 'lnb_records_unpack_labels')
+  _launch('lnb_records_unpack_labels', blob, *args, P, label)
   return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, label, status
 
 
@@ -467,10 +446,8 @@ def graph_eigs_sparse(sizes, node_ptr, edge_ptr, edges, N, K, num_edgetype=32, r
   D = torch.empty((B, int(K)), device=dev, dtype=torch.float32)
   V_rows = torch.empty((int(rows), int(K)), device=dev, dtype=torch.float32)
   status = torch.empty((B,), device=dev, dtype=torch.int32)
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_graph_eigs_sparse(
-        _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(edge_ptr), _ptr(edges), _ptr(_inv_sqrt_deg_table(dev)),
-        B, int(N), int(num_edgetype), int(K), _ptr(D), _ptr(V_rows), _ptr(status)), 'lnb_graph_eigs_sparse')
+  _launch('lnb_graph_eigs_sparse', sizes, sizes, node_ptr, edge_ptr, edges, _inv_sqrt_deg_table(dev),
+          B, int(N), int(num_edgetype), int(K), D, V_rows, status)
   return D, V_rows, status
 
 
@@ -491,9 +468,7 @@ def sym_eigs(A, sizes, K):
   D = torch.empty((B, int(K)), device=A.device, dtype=torch.float32)
   V = torch.empty((B, N, int(K)), device=A.device, dtype=torch.float32)
   status = torch.empty((B,), device=A.device, dtype=torch.int32)
-  with torch.cuda.device(A.device):
-    _lib.check(_lib.load().lnb_sym_eigs(_stream(A), _ptr(A), int(es), _ptr(sizes), B, N, int(K), _ptr(D), _ptr(V),
-                                        _ptr(status)), 'lnb_sym_eigs')
+  _launch('lnb_sym_eigs', A, A, int(es), sizes, B, N, int(K), D, V, status)
   return D, V, status
 
 
@@ -553,11 +528,9 @@ def spectral_partition(L, num_partition, seed=1234):
   L_cluster = torch.empty((B, N, N), device=dev, dtype=torch.float32)
   L_cut = torch.empty((B, N, N), device=dev, dtype=torch.float32)
   status = torch.empty((B,), device=dev, dtype=torch.int32)
-  with torch.cuda.device(dev):
-    draws = _partition_draws_table(dev, N, P, seed)
-    _lib.check(_lib.load().lnb_spectral_partition(
-        _stream(A), _ptr(A), int(es), B, N, P, _ptr(_inv_sqrt_deg_table(dev)), _ptr(draws), _ptr(labels),
-        _ptr(L_cluster), _ptr(L_cut), _ptr(status)), 'lnb_spectral_partition')
+  draws = _partition_draws_table(dev, N, P, seed)
+  _launch('lnb_spectral_partition', A, A, int(es), B, N, P, _inv_sqrt_deg_table(dev), draws, labels, L_cluster, L_cut,
+          status)
   return labels, L_cluster, L_cut, status
 
 
@@ -604,12 +577,9 @@ def spectral_partition_sparse(sizes, edge_ptr, edges, N, num_partition, num_edge
   gext = torch.empty((B, 2), device=dev, dtype=torch.int32)
   L_cluster = torch.empty((B, N, N), device=dev, dtype=torch.float32) if want_dense else None
   L_cut = torch.empty((B, N, N), device=dev, dtype=torch.float32) if want_dense else None
-  with torch.cuda.device(dev):
-    draws = _partition_draws_table(dev, N, P, seed)
-    _lib.check(_lib.load().lnb_spectral_partition_sparse(
-        _stream(sizes), _ptr(sizes), _ptr(edge_ptr), _ptr(edges), _ptr(_inv_sqrt_deg_table(dev)), B, N, E, P,
-        _ptr(draws), _ptr(labels), _ptr(status), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(gext),
-        _ptr(L_cluster), _ptr(L_cut)), 'lnb_spectral_partition_sparse')
+  draws = _partition_draws_table(dev, N, P, seed)
+  _launch('lnb_spectral_partition_sparse', sizes, sizes, edge_ptr, edges, _inv_sqrt_deg_table(dev), B, N, E, P, draws,
+          labels, status, ell_val, ell_idx, ell_max, gext, L_cluster, L_cut)
   return labels, status, GraphPrep((ell_val, ell_idx, ell_max, gext, None)), L_cluster, L_cut
 
 
@@ -623,9 +593,7 @@ def gat_bias_sparse(sizes, edge_ptr, edges, N, E1):
   _check_records('gat_bias_sparse', sizes, edge_ptr, edges)
   B = sizes.shape[0]
   bias = torch.empty((B, N, N, E1), device=sizes.device, dtype=torch.float32)
-  with torch.cuda.device(sizes.device):
-    _lib.check(_lib.load().lnb_gat_bias_sparse(_stream(sizes), _ptr(sizes), _ptr(edge_ptr), _ptr(edges), B, N, E1,
-                                               _ptr(bias)), 'lnb_gat_bias_sparse')
+  _launch('lnb_gat_bias_sparse', sizes, sizes, edge_ptr, edges, B, N, E1, bias)
   return bias
 
 
@@ -657,11 +625,8 @@ def spectral_conv_fused(X, Q, coeff, prep, w_hi, w_lo, bias, relu=True, write_pa
   H = w_hi.shape[0]
   assert w_hi.shape[1] == (S + E1) * Din, (w_hi.shape, S, E1, Din)
   out = torch.empty((B, N, H), device=X.device, dtype=torch.float32)
-  with torch.cuda.device(X.device):
-    _lib.check(_lib.load().lnb_spectral_conv_fused(
-        _stream(X), _ptr(X), _ptr(Q), _ptr(coeff), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max),
-        _ptr(gext), _ptr(tiles), _ptr(w_hi), _ptr(w_lo), _ptr(bias), B, N, Din, E1, K, S, H,
-        int(bool(relu)), int(bool(write_pad)), _ptr(out)), 'lnb_spectral_conv_fused')
+  _launch('lnb_spectral_conv_fused', X, X, Q, coeff, ell_val, ell_idx, ell_max, gext, tiles, w_hi, w_lo, bias,
+          B, N, Din, E1, K, S, H, int(bool(relu)), int(bool(write_pad)), out)
   return out
 
 
@@ -676,9 +641,7 @@ def sage_operators(nn_idx, nonempty):
     raise ValueError('sage_operators: nonempty %s does not match nn_idx %s'
                      % (tuple(nonempty.shape), tuple(nn_idx.shape)))
   out = torch.empty((B, N, N, E1), device=nn_idx.device, dtype=torch.float32)
-  with torch.cuda.device(nn_idx.device):
-    _lib.check(_lib.load().lnb_sage_operators(_stream(nn_idx), _ptr(nn_idx), _ptr(nonempty), B, N, K, E1,
-                                              _ptr(out)), 'lnb_sage_operators')
+  _launch('lnb_sage_operators', nn_idx, nn_idx, nonempty, B, N, K, E1, out)
   return out
 
 
@@ -692,10 +655,7 @@ def neighbour_max(X, prep):
   E1 = ell_val.shape[1]
   out = torch.empty((B, N, E1 * D), device=X.device, dtype=torch.float32)
   arg = torch.empty((B, N, E1, D), device=X.device, dtype=torch.int32)
-  with torch.cuda.device(X.device):
-    _lib.check(_lib.load().lnb_neighbour_max(_stream(X), _ptr(X), _ptr(ell_val), _ptr(ell_idx),
-                                             _ptr(ell_max), B, N, E1, D, _ptr(out), _ptr(arg)),
-               'lnb_neighbour_max')
+  _launch('lnb_neighbour_max', X, X, ell_val, ell_idx, ell_max, B, N, E1, D, out, arg)
   return out, arg
 
 
@@ -740,11 +700,8 @@ def sage_sample_sparse(sizes, node_ptr, node_feat, edge_ptr, edges, sample_key, 
   rows_t = ell() if want_ell_t else (None,) * 4
   flags = ((SAGE_SAMPLE_NN_IDX if want_nn_idx else 0) | (SAGE_SAMPLE_ELL if want_ell else 0) |
            (SAGE_SAMPLE_ELL_T if want_ell_t else 0))
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_sage_sample_sparse(
-        _stream(sizes), _ptr(sizes), _ptr(node_ptr), _ptr(node_feat), _ptr(edge_ptr), _ptr(edges),
-        _ptr(sample_key), B, N, E1, K, flags, _ptr(node_ids), _ptr(mask), _ptr(nonempty), _ptr(nn_idx),
-        *[_ptr(t) for t in rows + rows_t]), 'lnb_sage_sample_sparse')
+  _launch('lnb_sage_sample_sparse', sizes, sizes, node_ptr, node_feat, edge_ptr, edges, sample_key, B, N, E1, K,
+          flags, node_ids, mask, nonempty, nn_idx, *rows, *rows_t)
   prep = prep_t = None
   if want_ell:
     prep = GraphPrep(rows + (torch.empty((4 * B + 2,), device=dev, dtype=torch.int32),))
@@ -811,16 +768,12 @@ def spectral_stack_forward(prep, Q, w_hi, w_lo, bias, dins, H, S, coeff=None, co
     d.Din[i] = int(v)
   d.num_layers, d.Kw, d.write_pad = len(dins), int(w_hi.shape[1]), int(bool(write_pad))
   d.B, d.N, d.E1, d.K, d.S, d.H, d.relu = B, N, E1, K, int(S), int(H), int(bool(relu))
-  with torch.cuda.device(dev):
-    if sage is None:
-      _lib.check(_lib.load().lnb_spectral_stack_forward(_stream(Q), ctypes.byref(d)),
-                 'lnb_spectral_stack_forward')
-    else:
-      if sage not in ('Mean', 'Max'):
-        raise ValueError('spectral_stack_forward: sage=%r (Mean or Max)' % (sage,))
-      _lib.check(_lib.load().lnb_sage_stack_forward(_stream(Q), ctypes.byref(d),
-                                                    SAGE_MAX if sage == 'Max' else 0),
-                 'lnb_sage_stack_forward')
+  if sage is None:
+    _launch('lnb_spectral_stack_forward', Q, ctypes.byref(d))
+  elif sage not in ('Mean', 'Max'):
+    raise ValueError('spectral_stack_forward: sage=%r (Mean or Max)' % (sage,))
+  else:
+    _launch('lnb_sage_stack_forward', Q, ctypes.byref(d), SAGE_MAX if sage == 'Max' else 0)
   return state, score
 
 
@@ -830,9 +783,7 @@ def ritz_rowmap(gext, K):
   B = gext.shape[0]
   rowmap = torch.empty((B * K,), device=gext.device, dtype=torch.int32)
   nrows = torch.empty((1,), device=gext.device, dtype=torch.int32)
-  with torch.cuda.device(gext.device):
-    _lib.check(_lib.load().lnb_ritz_rowmap(_stream(gext), _ptr(gext), B, int(K), _ptr(rowmap),
-                                           _ptr(nrows)), 'lnb_ritz_rowmap')
+  _launch('lnb_ritz_rowmap', gext, gext, B, int(K), rowmap, nrows)
   return rowmap, nrows
 
 
@@ -850,11 +801,8 @@ def ritz_filter_mlp(table, w_hi, w_lo, bias_all, num_layers, rowmap=None, nrows=
   R, S = table.shape
   Hd = w_hi.shape[1]
   coeff = torch.empty((num_layers, R, S), device=table.device, dtype=torch.float32)
-  with torch.cuda.device(table.device):
-    _lib.check(_lib.load().lnb_ritz_filter_mlp_ctas(_stream(table), _ptr(table), _ptr(rowmap),
-                                                    _ptr(nrows), _ptr(w_hi), _ptr(w_lo),
-                                                    _ptr(bias_all), R, int(num_layers), S, Hd,
-                                                    _ptr(coeff), int(ctas)), 'lnb_ritz_filter_mlp')
+  _launch('lnb_ritz_filter_mlp_ctas', table, table, rowmap, nrows, w_hi, w_lo, bias_all, R, int(num_layers), S, Hd,
+          coeff, int(ctas))
   return coeff
 
 
@@ -864,10 +812,7 @@ def embedding_rows(idx, table):
   table = _f32c(table)
   rows = idx.numel()
   out = torch.empty(tuple(idx.shape) + (table.shape[1],), device=table.device, dtype=torch.float32)
-  with torch.cuda.device(table.device):
-    _lib.check(_lib.load().lnb_embedding_rows(_stream(table), _ptr(idx), _ptr(table), rows,
-                                              table.shape[0], table.shape[1], _ptr(out)),
-               'lnb_embedding_rows')
+  _launch('lnb_embedding_rows', table, idx, table, rows, table.shape[0], table.shape[1], out)
   return out
 
 
@@ -877,9 +822,7 @@ def ritz_power_table(D, powers):
   D = _f32c(D)
   S = len(powers)
   out = torch.empty(tuple(D.shape) + (S,), device=D.device, dtype=torch.float32)
-  with torch.cuda.device(D.device):
-    _lib.check(_lib.load().lnb_ritz_power_table(_stream(D), _ptr(D), D.numel(), _ints(powers), S,
-                                                _ptr(out)), 'lnb_ritz_power_table')
+  _launch('lnb_ritz_power_table', D, D, D.numel(), _ints(powers), S, out)
   return out
 
 
@@ -891,10 +834,8 @@ def readout(state, W_out, b_out, w_att, b_att, mask=None):
   if mask is not None:
     mask = (mask != 0).to(torch.uint8).contiguous()
   out = torch.empty((B, P), device=state.device, dtype=torch.float32)
-  with torch.cuda.device(state.device):
-    _lib.check(_lib.load().lnb_readout(_stream(state), _ptr(state), _ptr(_f32c(W_out)),
-                                       _ptr(_f32c(b_out)), _ptr(_f32c(w_att)), _ptr(_f32c(b_att)),
-                                       _ptr(mask), B, N, H, P, _ptr(out)), 'lnb_readout')
+  _launch('lnb_readout', state, state, _f32c(W_out), _f32c(b_out), _f32c(w_att), _f32c(b_att), mask, B, N, H, P,
+          out)
   return out
 
 
@@ -917,10 +858,7 @@ def gat_attention(Wh, bias, a1, a2, c1, c2, state_bias, last=False):
     raise ValueError('gat_attention: Wh %s, bias %s, a1 %s, state_bias %s do not agree'
                      % (tuple(Wh.shape), tuple(bias.shape), tuple(a1.shape), tuple(state_bias.shape)))
   out = torch.empty((B, N, F if last else C * F), device=Wh.device, dtype=torch.float32)
-  with torch.cuda.device(Wh.device):
-    _lib.check(_lib.load().lnb_gat_attention(
-        _stream(Wh), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
-        B, N, E1, heads, F, int(bool(last)), _ptr(out)), 'lnb_gat_attention')
+  _launch('lnb_gat_attention', Wh, Wh, bias, a1, a2, c1, c2, state_bias, B, N, E1, heads, F, int(bool(last)), out)
   return out
 
 
@@ -952,10 +890,8 @@ def gat_attention_backward(gout, Wh, bias, a1, a2, c1, c2, state_bias, out=None,
     z = torch.zeros((C, F), device=Wh.device, dtype=torch.float32)
     return gWh, z, z.clone(), z[:, 0].clone(), z[:, 0].clone(), z.clone()
   gpar = torch.empty((B, C, 3 * F + 2), device=Wh.device, dtype=torch.float32)
-  with torch.cuda.device(Wh.device):
-    _lib.check(_lib.load().lnb_gat_attention_backward(
-        _stream(Wh), _ptr(gout), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
-        B, N, E1, heads, F, int(bool(last)), _ptr(gWh), _ptr(gpar)), 'lnb_gat_attention_backward')
+  _launch('lnb_gat_attention_backward', Wh, gout, Wh, bias, a1, a2, c1, c2, state_bias, B, N, E1, heads, F,
+          int(bool(last)), gWh, gpar)
   g = gpar.sum(dim=0)
   return (gWh, g[:, :F].contiguous(), g[:, F:2 * F].contiguous(), g[:, 3 * F].contiguous(),
           g[:, 3 * F + 1].contiguous(), g[:, 2 * F:3 * F].contiguous())
@@ -994,10 +930,8 @@ def gat_attention_dropout(Wh, bias, a1, a2, c1, c2, state_bias, dropout_key, p, 
     raise ValueError('gat_attention_dropout: Wh %s, bias %s, a1 %s, state_bias %s do not agree'
                      % (tuple(Wh.shape), tuple(bias.shape), tuple(a1.shape), tuple(state_bias.shape)))
   out = torch.empty((B, N, F if last else C * F), device=Wh.device, dtype=torch.float32)
-  with torch.cuda.device(Wh.device):
-    _lib.check(_lib.load().lnb_gat_attention_dropout(
-        _stream(Wh), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
-        B, N, E1, heads, F, int(bool(last)), _ptr(key), p, t, _ptr(out)), 'lnb_gat_attention_dropout')
+  _launch('lnb_gat_attention_dropout', Wh, Wh, bias, a1, a2, c1, c2, state_bias, B, N, E1, heads, F,
+          int(bool(last)), key, p, t, out)
   return out
 
 
@@ -1021,11 +955,8 @@ def gat_attention_dropout_backward(gout, Wh, bias, a1, a2, c1, c2, state_bias, d
     z = torch.zeros((C, F), device=Wh.device, dtype=torch.float32)
     return gWh, z, z.clone(), z[:, 0].clone(), z[:, 0].clone(), z.clone()
   gpar = torch.empty((B, C, 3 * F + 2), device=Wh.device, dtype=torch.float32)
-  with torch.cuda.device(Wh.device):
-    _lib.check(_lib.load().lnb_gat_attention_dropout_backward(
-        _stream(Wh), _ptr(gout), _ptr(Wh), _ptr(bias), _ptr(a1), _ptr(a2), _ptr(c1), _ptr(c2), _ptr(state_bias),
-        B, N, E1, heads, F, int(bool(last)), _ptr(key), p, t, _ptr(gWh), _ptr(gpar)),
-        'lnb_gat_attention_dropout_backward')
+  _launch('lnb_gat_attention_dropout_backward', Wh, gout, Wh, bias, a1, a2, c1, c2, state_bias, B, N, E1, heads, F,
+          int(bool(last)), key, p, t, gWh, gpar)
   g = gpar.sum(dim=0)
   return (gWh, g[:, :F].contiguous(), g[:, F:2 * F].contiguous(), g[:, 3 * F].contiguous(),
           g[:, 3 * F + 1].contiguous(), g[:, 2 * F:3 * F].contiguous())
@@ -1052,9 +983,7 @@ def gat_dropout_project(X, W, C, dropout_key, p, t):
   X, W = _f32c(X), _f32c(W)
   M, Din, F = _project_dims('gat_dropout_project', X, W, int(C))
   Wh = torch.empty((M, W.shape[0]), device=X.device, dtype=torch.float32)
-  with torch.cuda.device(X.device):
-    _lib.check(_lib.load().lnb_gat_dropout_project(_stream(X), _ptr(X), _ptr(W), M, Din, int(C), F, _ptr(key), p,
-                                                   t, _ptr(Wh)), 'lnb_gat_dropout_project')
+  _launch('lnb_gat_dropout_project', X, X, W, M, Din, int(C), F, key, p, t, Wh)
   return Wh
 
 
@@ -1068,15 +997,11 @@ def gat_dropout_project_backward(X, W, gWh, C, dropout_key, p, t):
   M, Din, F = _project_dims('gat_dropout_project_backward', X, W, C)
   if tuple(gWh.shape) != (M, C * F):
     raise ValueError('gat_dropout_project_backward: gWh %s, expected %s' % (tuple(gWh.shape), (M, C * F)))
-  lib = _lib.load()
-  slabs = max(int(lib.lnb_gat_dropout_project_slabs(M, Din, C, F)), 1)
+  slabs = max(int(_lib.load().lnb_gat_dropout_project_slabs(M, Din, C, F)), 1)
   gX = torch.empty_like(X)
   gW = torch.empty_like(W)
   work = torch.empty((slabs, C * F, Din), device=X.device, dtype=torch.float32)
-  with torch.cuda.device(X.device):
-    _lib.check(lib.lnb_gat_dropout_project_backward(_stream(X), _ptr(X), _ptr(W), _ptr(gWh), M, Din, C, F, _ptr(key),
-                                                    p, t, _ptr(gX), _ptr(gW), _ptr(work)),
-               'lnb_gat_dropout_project_backward')
+  _launch('lnb_gat_dropout_project_backward', X, X, W, gWh, M, Din, C, F, key, p, t, gX, gW, work)
   return gX, gW
 
 
@@ -1102,10 +1027,7 @@ def ggnn_update(M, h, prep, w_hi, w_lo, bias, avg, out=None):
                      % (tuple(M.shape), tuple(h.shape), tuple(w_hi.shape), tuple(bias.shape), B, N, E1))
   if out is None:
     out = torch.empty_like(h)
-  with torch.cuda.device(h.device):
-    _lib.check(_lib.load().lnb_ggnn_update(
-        _stream(h), _ptr(M), _ptr(h), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi), _ptr(w_lo),
-        _ptr(bias), B, N, D, E1, int(bool(avg)), _ptr(out)), 'lnb_ggnn_update')
+  _launch('lnb_ggnn_update', h, M, h, ell_val, ell_idx, ell_max, w_hi, w_lo, bias, B, N, D, E1, int(bool(avg)), out)
   return out
 
 
@@ -1135,10 +1057,7 @@ def sage_lstm_step(state, nn_idx, nonempty, h, c, w_hi, w_lo, bias, t, out):
   for name, x in (('state', state), ('nonempty', nonempty), ('h', h), ('c', c), ('out', out), ('bias', bias)):
     if x is not None and (x.dtype != torch.float32 or not x.is_contiguous()):
       raise ValueError('sage_lstm_step: %s must be a contiguous float32 tensor' % name)
-  with torch.cuda.device(state.device):
-    _lib.check(_lib.load().lnb_sage_lstm_step(
-        _stream(state), _ptr(state), _ptr(nn_idx), _ptr(nonempty), _ptr(h), _ptr(c), _ptr(w_hi), _ptr(w_lo),
-        _ptr(bias), B, N, K, E1, D, int(t), _ptr(out)), 'lnb_sage_lstm_step')
+  _launch('lnb_sage_lstm_step', state, state, nn_idx, nonempty, h, c, w_hi, w_lo, bias, B, N, K, E1, D, int(t), out)
   return out
 
 
@@ -1212,12 +1131,8 @@ def gpnn_partition_update(parts, prep, w_hi, w_lo, bias, avg, h_copy=None):
   if any(len(s) != 1 for s in strides.values()):
     raise ValueError('gpnn_partition_update: one row stride each for M, h and out, got %s' % strides)
   ldm, ldh, ldo = strides['M'].pop(), strides['h'].pop(), strides['out'].pop()
-  dev = live[0][1].device
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_gpnn_partition_update(
-        _stream(live[0][1]), *[_ptr(t) for t in ptrs], _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi),
-        _ptr(w_lo), _ptr(bias), _ptr(h_copy), B, N, H, ldm, ldh, ldo, int(bool(avg))),
-               'lnb_gpnn_partition_update')
+  _launch('lnb_gpnn_partition_update', live[0][1], *ptrs, ell_val, ell_idx, ell_max, w_hi, w_lo, bias, h_copy,
+          B, N, H, ldm, ldh, ldo, int(bool(avg)))
   return [None if pt is None else pt[2] for pt in parts]
 
 
@@ -1247,10 +1162,7 @@ def mpnn_update(PQ, h, prep, w_hi, w_lo, bias, avg, out=None):
                      % (tuple(PQ.shape), tuple(h.shape), tuple(w_hi.shape), tuple(bias.shape), B, N, E1))
   if out is None:
     out = torch.empty_like(h)
-  with torch.cuda.device(h.device):
-    _lib.check(_lib.load().lnb_mpnn_update(
-        _stream(h), _ptr(PQ), _ptr(h), _ptr(ell_val), _ptr(ell_idx), _ptr(ell_max), _ptr(w_hi), _ptr(w_lo),
-        _ptr(bias), B, N, D, E1, int(bool(avg)), _ptr(out)), 'lnb_mpnn_update')
+  _launch('lnb_mpnn_update', h, PQ, h, ell_val, ell_idx, ell_max, w_hi, w_lo, bias, B, N, D, E1, int(bool(avg)), out)
   return out
 
 
@@ -1272,10 +1184,7 @@ def mpnn_edge_aggregate(PQ, prep, avg):
   PQ = _f32c(PQ)
   B, N, E1 = _check_pq('mpnn_edge_aggregate', PQ, prep)
   S = torch.empty((B * N, E1 * MPNN_EDGE_HIDDEN), device=PQ.device, dtype=torch.float32)
-  with torch.cuda.device(PQ.device):
-    _lib.check(_lib.load().lnb_mpnn_edge_aggregate(
-        _stream(PQ), _ptr(PQ), _ptr(prep[0]), _ptr(prep[1]), _ptr(prep[2]), B, N, E1, int(bool(avg)), _ptr(S)),
-               'lnb_mpnn_edge_aggregate')
+  _launch('lnb_mpnn_edge_aggregate', PQ, PQ, prep[0], prep[1], prep[2], B, N, E1, int(bool(avg)), S)
   return S
 
 
@@ -1289,10 +1198,8 @@ def mpnn_edge_aggregate_backward(PQ, gS, prep, prep_t, avg):
     raise ValueError('mpnn_edge_aggregate_backward: gS %s / transposed ELL %s do not agree with B=%d N=%d E1=%d'
                      % (tuple(gS.shape), tuple(prep_t[0].shape), B, N, E1))
   gPQ = torch.empty_like(PQ)
-  with torch.cuda.device(PQ.device):
-    _lib.check(_lib.load().lnb_mpnn_edge_aggregate_backward(
-        _stream(PQ), _ptr(PQ), _ptr(gS), _ptr(prep[0]), _ptr(prep[1]), _ptr(prep[2]), _ptr(prep_t[0]),
-        _ptr(prep_t[1]), _ptr(prep_t[2]), B, N, E1, int(bool(avg)), _ptr(gPQ)), 'lnb_mpnn_edge_aggregate_backward')
+  _launch('lnb_mpnn_edge_aggregate_backward', PQ, PQ, gS, prep[0], prep[1], prep[2], prep_t[0], prep_t[1], prep_t[2],
+          B, N, E1, int(bool(avg)), gPQ)
   return gPQ
 
 
@@ -1383,10 +1290,8 @@ def ell_messages(X, prep, c0=0, nc=None, w=None, out=None, col0=0):
   if out is None:
     out = torch.empty((B * N, col0 + nc * D), device=dev, dtype=torch.float32)
   ldo = _ell_rows('ell_messages', 'out', out, B * N, col0 + nc * D, dev)
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_ell_messages(
-        _stream(X), _ptr(X), ldx, _ptr(prep[0]), _ptr(prep[1]), _ptr(prep[2]), _ptr(prep[3]), _ptr(w), B, N, E1,
-        int(c0), nc, D, _ptr(out), ldo, col0), 'lnb_ell_messages')
+  _launch('lnb_ell_messages', X, X, ldx, prep[0], prep[1], prep[2], prep[3], w, B, N, E1, int(c0), nc, D, out, ldo,
+          col0)
   return out
 
 
@@ -1409,10 +1314,8 @@ def ell_messages_adjoint(G, prep_t, D, c0=0, nc=None, w=None, out=None):
   if out is None:
     out = torch.empty((B * N, D), device=dev, dtype=torch.float32)
   ldgx = _ell_rows('ell_messages_adjoint', 'out', out, B * N, D, dev)
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_ell_messages_adjoint(
-        _stream(G), _ptr(G), ldg, _ptr(prep_t[0]), _ptr(prep_t[1]), _ptr(prep_t[2]), _ptr(prep_t[3]), _ptr(w),
-        B, N, E1, int(c0), nc, D, _ptr(out), ldgx), 'lnb_ell_messages_adjoint')
+  _launch('lnb_ell_messages_adjoint', G, G, ldg, prep_t[0], prep_t[1], prep_t[2], prep_t[3], w, B, N, E1, int(c0), nc,
+          D, out, ldgx)
   return out
 
 
@@ -1441,10 +1344,7 @@ def set2vec(X, mask, WgT, bg, W1, W2, W_out, b_out, steps):
     if tuple(mask.shape) != (B, N):
       raise ValueError('set2vec: mask %s does not match X %s' % (tuple(mask.shape), tuple(X.shape)))
   out = torch.empty((B, P), device=X.device, dtype=torch.float32)
-  with torch.cuda.device(X.device):
-    _lib.check(_lib.load().lnb_set2vec(
-        _stream(X), _ptr(X), _ptr(mask), _ptr(WgT), _ptr(bg), _ptr(W1), _ptr(W2), _ptr(W_out), _ptr(b_out),
-        B, N, D, P, int(steps), _ptr(out)), 'lnb_set2vec')
+  _launch('lnb_set2vec', X, X, mask, WgT, bg, W1, W2, W_out, b_out, B, N, D, P, int(steps), out)
   return out
 
 
@@ -1461,11 +1361,8 @@ def operator_chain(L, X, steps, block_of_step, out, out_col0, chebyshev=False):
   E1 = L.shape[3]
   assert out.dtype == torch.float32 and out.is_contiguous() and out.shape[:2] == (B, N)
   sel = (ctypes.c_int * steps)(*[int(v) for v in block_of_step])
-  with torch.cuda.device(X.device):
-    _lib.check(_lib.load().lnb_operator_chain(_stream(X), _ptr(L), _ptr(X), B, N, E1, D, int(steps),
-                                              1 if chebyshev else 0, sel, _ptr(out),
-                                              out.stride(0), out.stride(1), int(out_col0)),
-               'lnb_operator_chain')
+  _launch('lnb_operator_chain', X, L, X, B, N, E1, D, int(steps), 1 if chebyshev else 0, sel, out, out.stride(0),
+          out.stride(1), int(out_col0))
   return out
 
 
@@ -1492,11 +1389,8 @@ def graph_messages(L, X, Q, filt, dense_filter, short_dist, out):
   sel = [steps.index(s) if s in steps else -1 for s in range(1, max_short + 1)]
   arr = (ctypes.c_int * max(1, max_short))(*([int(v) for v in sel] or [0]))
   assert out.dtype == torch.float32 and out.is_contiguous()
-  with torch.cuda.device(X.device):
-    _lib.check(_lib.load().lnb_graph_messages(
-        _stream(X), _ptr(L), _ptr(X), _ptr(Q), _ptr(filt), B, N, E1, D, K, S,
-        1 if dense_filter else 0, max_short, arr, len(steps), _ptr(out), out.stride(0), out.stride(1)),
-               'lnb_graph_messages')
+  _launch('lnb_graph_messages', X, L, X, Q, filt, B, N, E1, D, K, S, 1 if dense_filter else 0, max_short, arr,
+          len(steps), out, out.stride(0), out.stride(1))
   return out
 
 
@@ -1506,9 +1400,7 @@ def gaussian_laplacian(x, L):
   B, N, Dx = x.shape
   E1 = L.shape[3]
   out = torch.empty((B, N, N), device=x.device, dtype=torch.float32)
-  with torch.cuda.device(x.device):
-    _lib.check(_lib.load().lnb_gaussian_laplacian(_stream(x), _ptr(x), _ptr(L), B, N, Dx, E1,
-                                                  _ptr(out)), 'lnb_gaussian_laplacian')
+  _launch('lnb_gaussian_laplacian', x, x, L, B, N, Dx, E1, out)
   return out
 
 
@@ -1537,12 +1429,8 @@ def lanczos_ritz(A, mask, q1, K, want_ritz=True, want_T=True, want_Q=True, prope
     out['theta'] = torch.empty((B, K), device=dev, dtype=torch.float32)
     out['V'] = torch.empty((B, N, K), device=dev, dtype=torch.float32)
     out['status'] = torch.empty((B,), device=dev, dtype=torch.int32)
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_lanczos_ritz(
-        _stream(A), _ptr(A), _ptr(mask), _ptr(q1), B, N, K, 1 if proper else 0,
-        _ptr(out.get('T')), _ptr(out.get('Q')),
-        _ptr(out['alpha']), _ptr(out['beta']), _ptr(out['idx']), _ptr(out.get('theta')),
-        _ptr(out.get('V')), _ptr(out.get('status'))), 'lnb_lanczos_ritz')
+  _launch('lnb_lanczos_ritz', A, A, mask, q1, B, N, K, 1 if proper else 0, out.get('T'), out.get('Q'), out['alpha'],
+          out['beta'], out['idx'], out.get('theta'), out.get('V'), out.get('status'))
   return out
 
 
@@ -1553,9 +1441,7 @@ def tridiag_powers(T, powers):
   B, K = T.shape[0], T.shape[1]
   S = len(powers)
   out = torch.empty((B, K, S, K), device=T.device, dtype=torch.float32)
-  with torch.cuda.device(T.device):
-    _lib.check(_lib.load().lnb_tridiag_powers(_stream(T), _ptr(T), B, K, _ints(powers), S,
-                                              _ptr(out)), 'lnb_tridiag_powers')
+  _launch('lnb_tridiag_powers', T, T, B, K, _ints(powers), S, out)
   return out
 
 
@@ -1583,9 +1469,7 @@ def tridiag_powers_backward(T, gOut, powers):
   _need_cuda(T, gOut)
   T, gOut = _f32c(T), _f32c(gOut)
   gT = torch.empty((B, K, K), device=T.device, dtype=torch.float32)
-  with torch.cuda.device(T.device):
-    _lib.check(_lib.load().lnb_tridiag_powers_backward(_stream(T), _ptr(T), _ptr(gOut), B, K, _ints(powers),
-                                                       S, _ptr(gT)), 'lnb_tridiag_powers_backward')
+  _launch('lnb_tridiag_powers_backward', T, T, gOut, B, K, _ints(powers), S, gT)
   return gT
 
 
@@ -1618,10 +1502,8 @@ def lanczos_tridiag_train(A, mask, q1, K):
          'alpha': torch.empty((B, K), device=dev, dtype=torch.float32),
          'beta': torch.empty((B, K), device=dev, dtype=torch.float32),
          'idx': torch.empty((B,), device=dev, dtype=torch.int32)}
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_lanczos_tridiag_train(
-        _stream(A), _ptr(A), _ptr(mask), _ptr(q1), B, N, int(K), _ptr(out['T']), _ptr(out['Q']),
-        _ptr(out['alpha']), _ptr(out['beta']), _ptr(out['idx'])), 'lnb_lanczos_tridiag_train')
+  _launch('lnb_lanczos_tridiag_train', A, A, mask, q1, B, N, int(K), out['T'], out['Q'], out['alpha'], out['beta'],
+          out['idx'])
   return out
 
 
@@ -1638,10 +1520,7 @@ def lanczos_tridiag_backward(A, mask, q1, K, gT, gQ, want_tape=False):
   gA = torch.empty((B, N, N), device=dev, dtype=torch.float32)
   T = torch.empty((B, K, K), device=dev, dtype=torch.float32) if want_tape else None
   Q = torch.empty((B, N, K), device=dev, dtype=torch.float32) if want_tape else None
-  with torch.cuda.device(dev):
-    _lib.check(_lib.load().lnb_lanczos_tridiag_backward(
-        _stream(A), _ptr(A), _ptr(mask), _ptr(q1), B, N, int(K), _ptr(gT), _ptr(gQ), _ptr(gA), _ptr(T),
-        _ptr(Q)), 'lnb_lanczos_tridiag_backward')
+  _launch('lnb_lanczos_tridiag_backward', A, A, mask, q1, B, N, int(K), gT, gQ, gA, T, Q)
   return (gA, T, Q) if want_tape else gA
 
 
@@ -1662,9 +1541,7 @@ def ada_start_vector(start_key, B, N):
     raise ValueError('ada_start_vector: bad dims B=%d N=%d' % (B, N))
   key = start_key.contiguous()
   q1 = torch.empty((B, N), device=key.device, dtype=torch.float32)
-  with torch.cuda.device(key.device):
-    _lib.check(_lib.load().lnb_ada_start_vector(_stream(key), _ptr(key), B, N, _ptr(q1)),
-               'lnb_ada_start_vector')
+  _launch('lnb_ada_start_vector', key, key, B, N, q1)
   return q1
 
 
@@ -1674,9 +1551,7 @@ def symmetrize_filters(Y, K, S):
   Y = _f32c(Y)
   B = Y.shape[0]
   G = torch.empty((B, S, K, K), device=Y.device, dtype=torch.float32)
-  with torch.cuda.device(Y.device):
-    _lib.check(_lib.load().lnb_symmetrize_filters(_stream(Y), _ptr(Y), B, K, S, _ptr(G)),
-               'lnb_symmetrize_filters')
+  _launch('lnb_symmetrize_filters', Y, Y, B, K, S, G)
   return G
 
 
@@ -1687,10 +1562,7 @@ def segment_sum_forward(data, segment_index, num_segments, output=None):
   B, d1, d2 = data.shape
   if output is None:
     output = torch.zeros((B, num_segments, d2), device=data.device, dtype=torch.float32)
-  with torch.cuda.device(data.device):
-    _lib.check(_lib.load().lnb_unsorted_segment_sum_forward(
-        _stream(data), _ptr(data), _ptr(seg), _ints([B, d1, d2]), int(num_segments), _ptr(output)),
-               'lnb_unsorted_segment_sum_forward')
+  _launch('lnb_unsorted_segment_sum_forward', data, data, seg, _ints([B, d1, d2]), int(num_segments), output)
   return output
 
 
@@ -1701,8 +1573,6 @@ def segment_sum_backward(grad_output, segment_index, data_shape, grad_data=None)
   B, d1, d2 = [int(v) for v in data_shape]
   if grad_data is None:
     grad_data = torch.empty((B, d1, d2), device=grad_output.device, dtype=torch.float32)
-  with torch.cuda.device(grad_output.device):
-    _lib.check(_lib.load().lnb_unsorted_segment_sum_backward(
-        _stream(grad_output), _ptr(grad_output), _ptr(seg), _ints([B, d1, d2]),
-        int(grad_output.shape[1]), _ptr(grad_data)), 'lnb_unsorted_segment_sum_backward')
+  _launch('lnb_unsorted_segment_sum_backward', grad_output, grad_output, seg, _ints([B, d1, d2]),
+          int(grad_output.shape[1]), grad_data)
   return grad_data

@@ -125,16 +125,11 @@ def _check(out, ref64, ref32, floor, what):
 def _conv_raw(X, Q, coeff, prep, w_hi, w_lo, bias, relu, write_pad, out):
   """lnb_spectral_conv_fused into a caller-provided output (ops.spectral_conv_fused allocates its
   own), so rows the kernel must not write can be checked against a sentinel."""
-  from lanczosnetwork_b200 import _lib
-  o = ops()
   ell_val, ell_idx, ell_max, gext, tiles = prep
   B, N, Din = X.shape
   S = 0 if coeff is None else coeff.shape[2]
-  _lib.check(_lib.load().lnb_spectral_conv_fused(
-      o._stream(X), o._ptr(X), o._ptr(Q), o._ptr(coeff), o._ptr(ell_val), o._ptr(ell_idx),
-      o._ptr(ell_max), o._ptr(gext), o._ptr(tiles), o._ptr(w_hi), o._ptr(w_lo), o._ptr(bias), B, N,
-      Din, ell_val.shape[1], Q.shape[2], S, w_hi.shape[0], int(relu), int(write_pad), o._ptr(out)),
-      'lnb_spectral_conv_fused')
+  ops()._launch('lnb_spectral_conv_fused', X, X, Q, coeff, ell_val, ell_idx, ell_max, gext, tiles, w_hi, w_lo, bias,
+                B, N, Din, ell_val.shape[1], Q.shape[2], S, w_hi.shape[0], int(relu), int(write_pad), out)
   torch.cuda.synchronize()
   return out
 
@@ -374,13 +369,9 @@ def _mlp_layers(g, nl, S, Hd):
 
 
 def _mlp_raw(table, w_hi, w_lo, bias_all, nl, rowmap, nrows, coeff):
-  from lanczosnetwork_b200 import _lib
-  o = ops()
   R, S = table.shape
-  _lib.check(_lib.load().lnb_ritz_filter_mlp(o._stream(table), o._ptr(table), o._ptr(rowmap),
-                                             o._ptr(nrows), o._ptr(w_hi), o._ptr(w_lo),
-                                             o._ptr(bias_all), R, nl, S, w_hi.shape[1], o._ptr(coeff)),
-             'lnb_ritz_filter_mlp')
+  ops()._launch('lnb_ritz_filter_mlp', table, table, rowmap, nrows, w_hi, w_lo, bias_all, R, nl, S, w_hi.shape[1],
+                coeff)
   torch.cuda.synchronize()
   return coeff
 

@@ -20,7 +20,7 @@ import pytest
 import torch
 
 from helpers import deterministic_state_dict
-from lanczosnetwork_b200 import _lib, configs, data, ops
+from lanczosnetwork_b200 import configs, data, ops
 from lanczosnetwork_b200.model import LanczosNet
 from lanczosnetwork_b200.train import GraphedStep
 from test_gpu_train_envelope import MULT, _deep_floor
@@ -92,24 +92,20 @@ def _plain_c(x, w_hi, w_lo, b, relu, out, M=None, K=None):
   """lnb_linear_tf32x3 through the C ABI (never split-K, whatever the shape)."""
   M = x.shape[0] if M is None else M
   K = x.shape[1] if K is None else K
-  _lib.check(_lib.load().lnb_linear_tf32x3(ops._stream(out), ops._ptr(x), ops._ptr(w_hi), ops._ptr(w_lo),
-                                           ops._ptr(b), M, w_hi.shape[0], K, int(relu), ops._ptr(out)),
-             'lnb_linear_tf32x3')
+  ops._launch('lnb_linear_tf32x3', out, x, w_hi, w_lo, b, M, w_hi.shape[0], K, int(relu), out)
 
 
 def _splitk_c(x, w_hi, w_lo, b, relu, out, splits, ws, counters, M=None, K=None):
   M = x.shape[0] if M is None else M
   K = x.shape[1] if K is None else K
-  _lib.check(_lib.load().lnb_linear_tf32x3_splitk(
-      ops._stream(out), ops._ptr(x), ops._ptr(w_hi), ops._ptr(w_lo), ops._ptr(b), M, w_hi.shape[0], K,
-      int(relu), ops._ptr(out), splits, ops._ptr(ws), ops._ptr(counters)), 'lnb_linear_tf32x3_splitk')
+  ops._launch('lnb_linear_tf32x3_splitk', out, x, w_hi, w_lo, b, M, w_hi.shape[0], K, int(relu), out, splits, ws,
+              counters)
 
 
 def _grouped_c(x, w_hi, w_lo, b, groups, relu, out, M=None):
   M = x.shape[0] if M is None else M
-  _lib.check(_lib.load().lnb_linear_tf32x3_grouped(
-      ops._stream(out), ops._ptr(x), ops._ptr(w_hi), ops._ptr(w_lo), ops._ptr(b), M, groups,
-      w_hi.shape[0] // groups, w_hi.shape[1], int(relu), ops._ptr(out)), 'lnb_linear_tf32x3_grouped')
+  ops._launch('lnb_linear_tf32x3_grouped', out, x, w_hi, w_lo, b, M, groups, w_hi.shape[0] // groups, w_hi.shape[1],
+              int(relu), out)
 
 
 def _tiles(M, N):

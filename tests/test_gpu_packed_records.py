@@ -2,13 +2,11 @@
 malformed headers included), and forward_sparse of every drop-in with a records entry on packed batches,
 bit-equal to forward_sparse on the records they pack -- pinned-host and device-resident blobs, with and
 without eigenpairs, several batches from one captured graph."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
-from lanczosnetwork_b200 import _lib, configs, data, ops
+from lanczosnetwork_b200 import configs, data, ops
 from lanczosnetwork_b200.model import (DCNN, GAT, GCN, GCNFP, GGNN, GPNN, MPNN, ChebyNet, KeyedGAT, LanczosNet,
                                        SampledGraphSAGE, TrainableGAT)
 
@@ -91,12 +89,8 @@ def _unpack_raw(blob, B, Kb, cap_rows, cap_edges, eigs, slack=64):
       'V_rows': fill((4 * ((cap_rows + slack) * Kb),), torch.float32) if eigs else None,
   }
   status = torch.full((1,), -1, device=dev(), dtype=torch.int32)
-  p = lambda t: ctypes.c_void_p(t.data_ptr() if t is not None else 0)
-  stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-  _lib.check(_lib.load().lnb_records_unpack(
-      stream, p(blob), blob.numel(), B, Kb, cap_rows, cap_edges, p(out['sizes']), p(out['node_ptr']),
-      p(out['node_feat']), p(out['edge_ptr']), p(out['edges']), p(out['D']), p(out['V_rows']), p(status)),
-      'lnb_records_unpack')
+  ops._launch('lnb_records_unpack', blob, blob, blob.numel(), B, Kb, cap_rows, cap_edges, out['sizes'],
+              out['node_ptr'], out['node_feat'], out['edge_ptr'], out['edges'], out['D'], out['V_rows'], status)
   torch.cuda.synchronize()
   return {k: (v.cpu().numpy() if v is not None else None) for k, v in out.items()}, int(status.item())
 

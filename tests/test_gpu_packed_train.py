@@ -2,13 +2,11 @@
 status without the label segment or with another P), inference unchanged by a label segment, and
 GraphedStep(packed=True) against GraphedStep(sparse=True) on the same batches for every model it trains --
 one capture for every batch of a shape, and refusals that leave the model untouched."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
-from lanczosnetwork_b200 import _lib, configs, data, ops, train
+from lanczosnetwork_b200 import configs, data, ops, train
 from lanczosnetwork_b200.model import (DCNN, GCN, GCNFP, GGNN, GPNN, MPNN, ChebyNet, KeyedGAT, LanczosNet,
                                        SampledGraphSAGE, TrainableGAT)
 
@@ -66,14 +64,12 @@ def _unpack_raw(blob, B, cap_rows, cap_edges, P, labels=True, slack=64):
          'edge_ptr': fill(B + 1 + slack, torch.int32), 'node_feat': fill(cap_rows + slack, torch.int32),
          'edges': fill(cap_edges + slack, torch.uint8).view(-1, 4), 'label': fill(B * P + slack, torch.float32)}
   status = torch.full((1,), -1, device=dev(), dtype=torch.int32)
-  p = lambda t: ctypes.c_void_p(t.data_ptr())
-  args = (ctypes.c_void_p(torch.cuda.current_stream().cuda_stream), p(blob), blob.numel(), B, K, cap_rows, cap_edges,
-          p(out['sizes']), p(out['node_ptr']), p(out['node_feat']), p(out['edge_ptr']), p(out['edges']), None, None,
-          p(status))
+  args = (blob, blob.numel(), B, K, cap_rows, cap_edges, out['sizes'], out['node_ptr'], out['node_feat'],
+          out['edge_ptr'], out['edges'], None, None, status)
   if labels:
-    _lib.check(_lib.load().lnb_records_unpack_labels(*args, P, p(out['label'])), 'lnb_records_unpack_labels')
+    ops._launch('lnb_records_unpack_labels', blob, *args, P, out['label'])
   else:
-    _lib.check(_lib.load().lnb_records_unpack(*args), 'lnb_records_unpack')
+    ops._launch('lnb_records_unpack', blob, *args)
   torch.cuda.synchronize()
   return {k: v.cpu().numpy() for k, v in out.items()}, int(status.item())
 
