@@ -223,7 +223,12 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
  * LABEL and P: the labels of a training batch (data.pack_sparse(..., label=True),
  * data.PackedMolecules(..., labels=True)), the last segment, behind the bonds; every other offset is that
  * of the same batch without labels, and TOTAL counts the segment.  Both are 0 when the batch carries no
- * labels.  Only lnb_records_unpack_labels reads the segment. */
+ * labels.  Only lnb_records_unpack_labels reads the segment.
+ * F: the width of the node rows.  0 = atom ids, NODE_FEAT is int32 [sum n]; F > 0 = float feature rows
+ * (LanczosNetGeneral's GraphData records), NODE_FEAT is float32 [sum n, F], 4 F bytes per node.  Every other
+ * segment and offset rule is the same for both.  Atom-id batches are read by lnb_graph_prepare_sparse_packed
+ * and lnb_records_unpack(_labels), feature batches by lnb_graph_prepare_sparse_features_packed and
+ * lnb_records_unpack_features. */
 #define LNB_PACK_MAGIC 0x4c4e4231   /* "LNB1" */
 #define LNB_PACK_HDR_BYTES 64
 #define LNB_PACK_HDR_MAGIC 0        /* LNB_PACK_MAGIC */
@@ -241,6 +246,7 @@ int lnb_graph_prepare_sparse(lnb_stream_t stream, const int32_t* sizes, const in
 #define LNB_PACK_HDR_KROW 12        /* offset of krow_ptr [B+1] i32 */
 #define LNB_PACK_HDR_LABEL 13       /* offset of label [B, P] f32 */
 #define LNB_PACK_HDR_P 14
+#define LNB_PACK_HDR_F 15           /* width of the node rows: 0 = atom ids, F > 0 = float32 [sum n, F] */
 /* The kernel derives its input pointers from the header on the device.  flags bit 1
  * (LNB_PACKED_HOST_TILES): the host knows every graph's extents, so it ships the tiles (the same
  * next-fit table and first-fit-decreasing schedule as lnb_graph_prepare, in the same layout) and the
@@ -271,6 +277,7 @@ int lnb_graph_prepare_sparse_packed(lnb_stream_t stream, const uint8_t* blob, co
 #define LNB_UNPACK_EDGES_OVER 16    /* edge_ptr[B] > cap_edges */
 #define LNB_UNPACK_NO_EIGS 32       /* D or V_rows requested from a batch without eigenpairs */
 #define LNB_UNPACK_NO_LABELS 64     /* lnb_records_unpack_labels: no label segment of that P in the body */
+#define LNB_UNPACK_BAD_FEATURES 128 /* the header's F differs from the caller's (0 for the atom-id entries) */
 int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K,
                        int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
                        int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
@@ -284,6 +291,16 @@ int lnb_records_unpack_labels(lnb_stream_t stream, const uint8_t* blob, int64_t 
                               int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
                               int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
                               int32_t* status, int P, float* label);
+
+/* The same split of a batch of float feature rows (header slot F > 0): node_x [cap_rows, F] float32 takes the
+ * NODE_FEAT segment, 4 F bytes per node, in place of node_feat; P >= 1 also copies the labels into label
+ * [B, P], as lnb_records_unpack_labels does, and P = 0 (label NULL) leaves them.  A header whose F is not the
+ * caller's adds LNB_UNPACK_BAD_FEATURES, with every graph empty and nothing copied.  One launch of the kernel
+ * of lnb_records_unpack.  Limits: 1 <= F <= LNB_PREPARE_MAX_F. */
+int lnb_records_unpack_features(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K, int F,
+                                int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
+                                float* node_x, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
+                                int32_t* status, int P, float* label);
 
 /* Float-feature variant (LanczosNetGeneral's GraphData records, node features instead of atom ids): the
  * same records and outputs as lnb_graph_prepare_sparse, except that node_x [node_ptr[B], F] fp32 holds the
@@ -300,6 +317,19 @@ int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes,
                                       int K, int F, int flags, float* ell_val, uint8_t* ell_idx,
                                       int32_t* ell_max, int32_t* gext, int32_t* tiles, int32_t* rowmap,
                                       int32_t* nrows, float* X, uint8_t* mask, float* V, float* L_dense);
+
+/* lnb_graph_prepare_sparse_features on a packed batch of float feature rows with eigenpairs (header slot
+ * F > 0): the input pointers come from the header on the device, as in lnb_graph_prepare_sparse_packed, and
+ * flags takes LNB_PACKED_HOST_TILES the same way (the tiles and krow_ptr come with the batch, the kernel
+ * expands the Ritz row list and no tile-assignment launch follows).  Outputs as
+ * lnb_graph_prepare_sparse_features: X [B,N,F], mask, V, the ELL rows and, when L_dense != NULL, the dense
+ * operators.  A batch whose header slot F is not the caller's F is read as B empty graphs.  Same kernel as
+ * lnb_graph_prepare_sparse_features.  Limits: those of lnb_graph_prepare_sparse_features. */
+int lnb_graph_prepare_sparse_features_packed(lnb_stream_t stream, const uint8_t* blob, const double* inv_sqrt_deg,
+                                             int B, int N, int E1, int K, int F, int flags, float* ell_val,
+                                             uint8_t* ell_idx, int32_t* ell_max, int32_t* gext, int32_t* tiles,
+                                             int32_t* rowmap, int32_t* nrows, float* X, uint8_t* mask, float* V,
+                                             float* L_dense);
 
 /* ---------------------------------------------------------------------------------------
  * The whole convolution stack (and optionally the embedding gather in front and the readout

@@ -82,6 +82,10 @@ SIGNATURES = {
                                   [ctypes.c_void_p] * 8 + [c_int, ctypes.c_void_p]),
     'lnb_graph_prepare_sparse_features': (c_int, [c_stream] + [ctypes.c_void_p] * 7 + [c_int] * 6 +
                                           [ctypes.c_void_p] * 11),
+    'lnb_graph_prepare_sparse_features_packed': (c_int, [c_stream] + [ctypes.c_void_p] * 2 + [c_int] * 6 +
+                                                 [ctypes.c_void_p] * 11),
+    'lnb_records_unpack_features': (c_int, [c_stream, ctypes.c_void_p, c_i64, c_int, c_int, c_int, c_i64, c_i64] +
+                                    [ctypes.c_void_p] * 8 + [c_int, ctypes.c_void_p]),
     'lnb_spectral_conv_fused':
         (c_int, [c_stream, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p,
                  ctypes.c_void_p, ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int,

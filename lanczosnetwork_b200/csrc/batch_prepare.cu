@@ -28,8 +28,9 @@ struct SparseBatchParams {
   const uint8_t* edges;        // [edge_ptr[B]][4] = {u, v, bond type, 0}, undirected, listed once
   const float* V_rows;         // [node_ptr[B], K] Ritz vectors, rows of real nodes only
   const double* inv_sqrt_deg;  // [LNB_INV_SQRT_DEG_LEN] deg^-1/2 in fp64 (entry 0 = 0)
-  const uint8_t* blob;         // packed batch (lnb_graph_prepare_sparse_packed): the pointers above are derived
-                               // from its header on the device, so ONE H2D copy ships a whole batch
+  const uint8_t* blob;         // packed batch (lnb_graph_prepare_sparse_packed / _features_packed): the pointers
+                               // above, and node_x, are derived from its header on the device, so ONE H2D copy
+                               // ships a whole batch
   int B, N, E1, K, flags;
   float* ell_val; uint8_t* ell_idx; int32_t* ell_max; int32_t* gext;
   int64_t* node_ids; uint8_t* mask; float* V;     // padded [B,N], [B,N], [B,N,K]
@@ -70,7 +71,7 @@ __device__ __forceinline__ void copy_feature_rows(const float* __restrict__ src,
 }
 
 // kFeat = false: atom ids -> node_ids (lnb_graph_prepare_sparse / _packed); kFeat = true: float feature rows
-// -> X (lnb_graph_prepare_sparse_features, never packed).  Everything else is the same code.
+// -> X (lnb_graph_prepare_sparse_features / _features_packed).  Everything else is the same code.
 template <bool kFeat>
 __global__ void __launch_bounds__(BP_THREADS)
 batch_prepare_sparse_kernel(const SparseBatchParams P) {
@@ -81,12 +82,14 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
   const int N = P.N, E1 = P.E1, E = E1 - 1, K = P.K;
   const int32_t* sizes = P.sizes; const int32_t* node_ptr = P.node_ptr; const int32_t* node_feat = P.node_feat;
   const int32_t* edge_ptr = P.edge_ptr; const uint8_t* edges = P.edges; const float* V_rows = P.V_rows;
-  if (!kFeat && P.blob) {                        // header: byte offsets of the segments (see the C header)
+  bool other_width = false;                      // a feature batch of another F: read as empty graphs
+  if (P.blob) {                                  // header: byte offsets of the segments (see the C header)
     const int32_t* header = reinterpret_cast<const int32_t*>(P.blob);
     sizes = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_SIZES]);
     node_ptr = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_NODE_PTR]);
     edge_ptr = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_EDGE_PTR]);
-    node_feat = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_NODE_FEAT]);
+    if (kFeat) other_width = header[LNB_PACK_HDR_F] != P.F;   // node_x is derived where it is read
+    else node_feat = reinterpret_cast<const int32_t*>(P.blob + header[LNB_PACK_HDR_NODE_FEAT]);
     V_rows = reinterpret_cast<const float*>(P.blob + header[LNB_PACK_HDR_V_ROWS]);
     edges = P.blob + header[LNB_PACK_HDR_EDGES];
     if ((P.flags & LNB_PACKED_HOST_TILES) && header[LNB_PACK_HDR_KROW] > 0 && P.rowmap) {
@@ -98,7 +101,7 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
       if (b == 0 && threadIdx.x == 0) P.nrows[0] = krow[P.B];
     }
   }
-  const int nb = min(max(sizes[b], 0), N);
+  const int nb = other_width ? 0 : min(max(sizes[b], 0), N);
   uint32_t* rowmask = reinterpret_cast<uint32_t*>(bp_smem);              // [E][NMAX][NW]
   double* scale = reinterpret_cast<double*>(rowmask + (size_t)E * LNB_MAX_N * BP_NW);   // [E1][NMAX]
   uint8_t* cnt_s = reinterpret_cast<uint8_t*>(scale + (size_t)E1 * LNB_MAX_N);          // [N*E1]
@@ -177,7 +180,11 @@ batch_prepare_sparse_kernel(const SparseBatchParams P) {
     if (!kFeat) P.node_ids[(int64_t)b * N + n] = (n < nb) ? (int64_t)node_feat[r0 + n] : 0;
     P.mask[(int64_t)b * N + n] = (n < nb) ? 1 : 0;
   }
-  if (kFeat) copy_feature_rows(P.node_x + (int64_t)r0 * P.F, P.X + (int64_t)b * N * P.F, nb, N, P.F, tid);
+  if (kFeat) {
+    const float* node_x = P.blob ? reinterpret_cast<const float*>(
+        P.blob + reinterpret_cast<const int32_t*>(P.blob)[LNB_PACK_HDR_NODE_FEAT]) : P.node_x;
+    copy_feature_rows(node_x + (int64_t)r0 * P.F, P.X + (int64_t)b * N * P.F, nb, N, P.F, tid);
+  }
   int ke = 0;
   for (int i = tid; i < N * K; i += BP_THREADS) {
     const int n = i / K, k = i - n * K;
@@ -338,6 +345,35 @@ int lnb_graph_prepare_sparse_features(lnb_stream_t stream, const int32_t* sizes,
   p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.gext = gext;
   p.node_ids = nullptr; p.mask = mask; p.V = V; p.L = L_dense;
   p.node_x = node_x; p.X = X; p.F = F;
+  return launch_sparse<true>(stream, p, tiles, rowmap, nrows);
+}
+
+int lnb_graph_prepare_sparse_features_packed(lnb_stream_t stream, const uint8_t* blob, const double* inv_sqrt_deg,
+                                             int B, int N, int E1, int K, int F, int flags, float* ell_val,
+                                             uint8_t* ell_idx, int32_t* ell_max, int32_t* gext, int32_t* tiles,
+                                             int32_t* rowmap, int32_t* nrows, float* X, uint8_t* mask, float* V,
+                                             float* L_dense) {
+  if (!(B >= 0 && N >= 1 && N <= LNB_MAX_N && E1 >= 2 && E1 <= LNB_MAX_E1 && K >= 1 && F >= 1 &&
+        F <= LNB_PREPARE_MAX_F)) {
+    lnb::set_err("graph_prepare_sparse_features_packed: B=%d N=%d E1=%d K=%d F=%d outside 1 <= N <= %d, "
+                 "2 <= E1 <= %d, K >= 1, 1 <= F <= %d", B, N, E1, K, F, LNB_MAX_N, LNB_MAX_E1, LNB_PREPARE_MAX_F);
+    return LNB_ERR_UNSUPPORTED;
+  }
+  if (B == 0) return LNB_OK;
+  LNB_REQUIRE(blob && inv_sqrt_deg && ell_val && ell_idx && ell_max && gext &&
+                  (tiles || (flags & LNB_PACKED_HOST_TILES)) && X && mask && V,
+              "graph_prepare_sparse_features_packed: null pointer");
+  LNB_REQUIRE((reinterpret_cast<uintptr_t>(blob) & 15) == 0,
+              "graph_prepare_sparse_features_packed: blob must be 16-byte aligned");
+  LNB_REQUIRE((rowmap == nullptr) == (nrows == nullptr),
+              "graph_prepare_sparse_features_packed: rowmap and nrows go together");
+  SparseBatchParams p;
+  p.sizes = nullptr; p.node_ptr = nullptr; p.node_feat = nullptr; p.edge_ptr = nullptr;
+  p.edges = nullptr; p.V_rows = nullptr; p.inv_sqrt_deg = inv_sqrt_deg; p.blob = blob;
+  p.B = B; p.N = N; p.E1 = E1; p.K = K; p.flags = flags;
+  p.ell_val = ell_val; p.ell_idx = ell_idx; p.ell_max = ell_max; p.gext = gext;
+  p.node_ids = nullptr; p.mask = mask; p.V = V; p.L = L_dense;
+  p.node_x = nullptr; p.X = X; p.F = F;
   return launch_sparse<true>(stream, p, tiles, rowmap, nrows);
 }
 

@@ -3,7 +3,8 @@
 // (lnb_graph_prepare_sparse, lnb_gat_bias_sparse, lnb_spectral_partition_sparse, lnb_sage_sample_sparse,
 // lnb_graph_eigs_sparse) then run unchanged behind it, so every drop-in with a records entry takes the
 // one-H2D-copy format at the cost of one D2D copy of the blob's bytes.  lnb_records_unpack_labels also
-// copies the label segment [B, P] of a training batch (the same launch, an eighth segment).
+// copies the label segment [B, P] of a training batch (the same launch, an eighth segment);
+// lnb_records_unpack_features reads a batch of float feature rows, whose node segment is 4 F bytes per node.
 //
 // The segment offsets change from batch to batch, so they are read here, on the device: one captured
 // graph serves every batch of a (B, N, K) whose rows fit the capacities.  Every block validates the
@@ -16,14 +17,15 @@
 namespace {
 
 constexpr int RU_THREADS = 256;
-constexpr int RU_SEGS = 8;          // sizes, node_ptr, edge_ptr, node_feat, edges, D, V_rows, label
+constexpr int RU_SEGS = 8;          // sizes, node_ptr, edge_ptr, node_feat (ids or rows), edges, D, V_rows, label
 
 struct UnpackParams {
   const uint8_t* blob;
   int64_t blob_bytes;
   int B, K;
   int64_t cap_rows, cap_edges;
-  int32_t* sizes; int32_t* node_ptr; int32_t* node_feat; int32_t* edge_ptr; uint8_t* edges;
+  int F;                               // width of the node rows: 0 = atom ids, F > 0 = float feature rows
+  int32_t* sizes; int32_t* node_ptr; uint8_t* node_feat; int32_t* edge_ptr; uint8_t* edges;
   float* D; float* V_rows;
   int P; float* label;                 // label [B, P] of lnb_records_unpack_labels, else 0 / NULL
   int32_t* status;
@@ -44,6 +46,8 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
     int st = 0;
     if (header[LNB_PACK_HDR_MAGIC] != LNB_PACK_MAGIC) st |= LNB_UNPACK_BAD_MAGIC;
     if (header[LNB_PACK_HDR_B] != P.B || header[LNB_PACK_HDR_K] != P.K) st |= LNB_UNPACK_BAD_SHAPE;
+    if (header[LNB_PACK_HDR_F] != P.F) st |= LNB_UNPACK_BAD_FEATURES;
+    const int64_t row_bytes = 4 * (int64_t)(P.F ? P.F : 1);    // one atom id or F floats per node
     const int64_t total = header[LNB_PACK_HDR_TOTAL];
     int64_t rows = 0, nedge = 0;
     const bool eigs = header[LNB_PACK_HDR_D] != 0 || header[LNB_PACK_HDR_V_ROWS] != 0;
@@ -59,7 +63,7 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
         rows = np_[B];
         nedge = ep_[B];
         if (np_[0] != 0 || ep_[0] != 0 || rows < 0 || nedge < 0 ||
-            !seg_ok(header[LNB_PACK_HDR_NODE_FEAT], 4 * rows, total) ||
+            !seg_ok(header[LNB_PACK_HDR_NODE_FEAT], row_bytes * rows, total) ||
             !seg_ok(header[LNB_PACK_HDR_EDGES], 4 * nedge, total))
           st |= LNB_UNPACK_BAD_SEGMENT;
         else if (eigs && (!seg_ok(header[LNB_PACK_HDR_D], 4 * B * K, total) ||
@@ -79,11 +83,11 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
                                     header[LNB_PACK_HDR_EDGE_PTR], header[LNB_PACK_HDR_NODE_FEAT],
                                     header[LNB_PACK_HDR_EDGES], header[LNB_PACK_HDR_D],
                                     header[LNB_PACK_HDR_V_ROWS], P.label ? header[LNB_PACK_HDR_LABEL] : 0};
-      const int64_t bytes[RU_SEGS] = {4 * B, 4 * (B + 1), 4 * (B + 1), 4 * rows, 4 * nedge,
+      const int64_t bytes[RU_SEGS] = {4 * B, 4 * (B + 1), 4 * (B + 1), row_bytes * rows, 4 * nedge,
                                       P.D ? 4 * B * K : 0, P.V_rows ? 4 * rows * K : 0,
                                       P.label ? 4 * B * P.P : 0};
       uint8_t* dst[RU_SEGS] = {reinterpret_cast<uint8_t*>(P.sizes), reinterpret_cast<uint8_t*>(P.node_ptr),
-                               reinterpret_cast<uint8_t*>(P.edge_ptr), reinterpret_cast<uint8_t*>(P.node_feat),
+                               reinterpret_cast<uint8_t*>(P.edge_ptr), P.node_feat,
                                P.edges, reinterpret_cast<uint8_t*>(P.D), reinterpret_cast<uint8_t*>(P.V_rows),
                                reinterpret_cast<uint8_t*>(P.label)};
       // every segment is a whole number of 4-byte words: 16-byte vectors, then up to three words
@@ -124,8 +128,8 @@ __global__ void __launch_bounds__(RU_THREADS) records_unpack_kernel(const Unpack
   }
 }
 
-int launch_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K, int64_t cap_rows,
-                  int64_t cap_edges, int32_t* sizes, int32_t* node_ptr, int32_t* node_feat, int32_t* edge_ptr,
+int launch_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K, int F, int64_t cap_rows,
+                  int64_t cap_edges, int32_t* sizes, int32_t* node_ptr, void* node_feat, int32_t* edge_ptr,
                   uint8_t* edges, float* D, float* V_rows, int P, float* label, int32_t* status) {
   LNB_REQUIRE(B >= 1 && K >= 1 && cap_rows >= 0 && cap_edges >= 0 && blob_bytes >= LNB_PACK_HDR_BYTES,
               "records_unpack: bad dims B=%d K=%d cap_rows=%lld cap_edges=%lld blob_bytes=%lld", B, K,
@@ -138,10 +142,11 @@ int launch_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, 
     LNB_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, "records_unpack: buffers must be 16-byte aligned");
   UnpackParams p;
   p.blob = blob; p.blob_bytes = blob_bytes; p.B = B; p.K = K; p.cap_rows = cap_rows; p.cap_edges = cap_edges;
-  p.sizes = sizes; p.node_ptr = node_ptr; p.node_feat = node_feat; p.edge_ptr = edge_ptr; p.edges = edges;
+  p.F = F; p.sizes = sizes; p.node_ptr = node_ptr; p.node_feat = static_cast<uint8_t*>(node_feat);
+  p.edge_ptr = edge_ptr; p.edges = edges;
   p.D = D; p.V_rows = V_rows; p.P = P; p.label = label; p.status = status;
   // the grid depends on the capacities only (a captured launch serves every batch that fits them)
-  const int64_t max_bytes = 12 * (int64_t)B + 8 + 4 * cap_rows + 4 * cap_edges +
+  const int64_t max_bytes = 12 * (int64_t)B + 8 + 4 * (int64_t)(F ? F : 1) * cap_rows + 4 * cap_edges +
                             (D ? 4 * (int64_t)B * K : 0) + (V_rows ? 4 * cap_rows * K : 0) +
                             (label ? 4 * (int64_t)B * P : 0);
   int dev = 0, sms = 132;
@@ -162,7 +167,7 @@ int lnb_records_unpack(lnb_stream_t stream, const uint8_t* blob, int64_t blob_by
                        int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
                        int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
                        int32_t* status) {
-  return launch_unpack(stream, blob, blob_bytes, B, K, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr,
+  return launch_unpack(stream, blob, blob_bytes, B, K, 0, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr,
                        edges, D, V_rows, 0, nullptr, status);
 }
 
@@ -171,7 +176,18 @@ int lnb_records_unpack_labels(lnb_stream_t stream, const uint8_t* blob, int64_t 
                               int32_t* node_feat, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
                               int32_t* status, int P, float* label) {
   LNB_REQUIRE(P >= 1 && label, "records_unpack_labels: P=%d, label %p", P, (const void*)label);
-  return launch_unpack(stream, blob, blob_bytes, B, K, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr,
+  return launch_unpack(stream, blob, blob_bytes, B, K, 0, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr,
+                       edges, D, V_rows, P, label, status);
+}
+
+int lnb_records_unpack_features(lnb_stream_t stream, const uint8_t* blob, int64_t blob_bytes, int B, int K, int F,
+                                int64_t cap_rows, int64_t cap_edges, int32_t* sizes, int32_t* node_ptr,
+                                float* node_x, int32_t* edge_ptr, uint8_t* edges, float* D, float* V_rows,
+                                int32_t* status, int P, float* label) {
+  LNB_REQUIRE(F >= 1 && F <= LNB_PREPARE_MAX_F && P >= 0 && (P == 0) == (label == nullptr),
+              "records_unpack_features: F=%d (1 <= F <= %d), P=%d, label %p", F, LNB_PREPARE_MAX_F, P,
+              (const void*)label);
+  return launch_unpack(stream, blob, blob_bytes, B, K, F, cap_rows, cap_edges, sizes, node_ptr, node_x, edge_ptr,
                        edges, D, V_rows, P, label, status);
 }
 

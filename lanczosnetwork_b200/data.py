@@ -264,7 +264,7 @@ PACK_MAGIC = 0x4c4e4231          # "LNB1"
 
 # the int32 slots of a packed batch's header in slot order: LNB_PACK_HDR_* of include/lanczosnet_b200.h
 PackHeader = collections.namedtuple('PackHeader', 'magic B K sizes node_ptr edge_ptr D node_feat V_rows edges '
-                                                  'total tiles krow label P')
+                                                  'total tiles krow label P F')
 PackedOffsets = collections.namedtuple('PackedOffsets', 'sizes node_ptr edge_ptr D var tiles krow')
 
 
@@ -285,29 +285,37 @@ def packed_offsets(B, K):
   return PackedOffsets(off_sizes, off_node_ptr, off_edge_ptr, off_D, off_var, off_tiles, off_krow)
 
 
-def packed_layout(B, K, rows, nedges, eigs, P=0):
+def packed_layout(B, K, rows, nedges, eigs, P=0, F=0):
   """The PackHeader of a packed batch of B graphs with ``rows`` nodes and ``nedges`` bonds in all.  Without
   ``eigs`` there is no D, V_rows, tiles or krow segment, and the node ids start where D would.  P > 0: a label
-  segment [B, P] float32 behind the bonds."""
+  segment [B, P] float32 behind the bonds.  F > 0: the node segment holds float32 feature rows [rows, F]
+  instead of int32 atom ids; every other rule is the same."""
   o = packed_offsets(B, K)
+  node_bytes = 4 * rows * (F if F else 1)
   if eigs:
     D, node_feat, tiles, krow = o.D, o.var, o.tiles, o.krow
-    V_rows = node_feat + _align16(4 * rows)
+    V_rows = node_feat + _align16(node_bytes)
     edges = V_rows + _align16(4 * rows * K)
   else:
     D, node_feat, V_rows, tiles, krow = 0, o.D, 0, 0, 0
-    edges = node_feat + _align16(4 * rows)
+    edges = node_feat + _align16(node_bytes)
   label = edges + _align16(4 * nedges)
   total = label + _align16(4 * B * P)
   return PackHeader(PACK_MAGIC, B, K, o.sizes, o.node_ptr, o.edge_ptr, D, node_feat, V_rows, edges, total, tiles,
-                    krow, label if P else 0, P)
+                    krow, label if P else 0, P, F)
 
 
-def packed_capacity(B, N, K, eigs, nbytes, label_dim=0):
-  """Static size of a packed batch's blob under graph replay: the blob of any B molecules of at most N
-  nodes and 4 N bonds each, or the blob's own ``nbytes`` when that is larger.  ``label_dim`` = P > 0 counts a
-  label segment [B, P] float32 (pack_sparse(..., label=True))."""
-  return max(packed_layout(B, K, B * N, 4 * B * N, eigs, int(label_dim)).total, int(nbytes))
+def packed_capacity(B, N, K, eigs, nbytes, label_dim=0, feature_dim=0, num_edgetype=1):
+  """Static size of a packed batch's blob under graph replay, or the blob's own ``nbytes`` when that is
+  larger.  ``label_dim`` = P > 0 counts a label segment [B, P] float32 (pack_sparse(..., label=True)).
+
+  Atom ids (``feature_dim`` = 0): the blob of any B molecules of at most N nodes and 4 N bonds each.  Float
+  feature rows (``feature_dim`` = F > 0, GraphData graphs such as G(n, 0.5), far denser than molecules): the
+  blob of ANY B graphs of at most N nodes, whose bond lists hold each (u <= v, bond type) pair at most once,
+  as prepare_graph writes them: ``num_edgetype`` * N (N + 1) / 2 bonds per graph."""
+  F = int(feature_dim)
+  bonds = int(num_edgetype) * N * (N + 1) // 2 if F else 4 * N
+  return max(packed_layout(B, K, B * N, B * bonds, eigs, int(label_dim), F).total, int(nbytes))
 
 
 def read_packed_header(blob):
@@ -444,13 +452,17 @@ def pack_sparse(sp, label=False):
   eigs=False)``) give a blob without D, Ritz rows, tiles and Ritz-row offsets (their header offsets are 0):
   the node ids start where D would.  ``label=True``: the records' labels [B, P] float32 follow the bonds as
   one more segment (slots label and P), for training from the blob (train.GraphedStep(..., packed=True));
-  every other byte is that of the blob without them.  Returns dict(blob, B, N, K, num_edgetype, eigs[, label])."""
+  every other byte is that of the blob without them.  Records whose ``node_feat`` is 2-D (float feature rows
+  [sum n, F], sparse_collate of GraphData samples) give a blob of feature rows: header slot F, 4 F bytes per node
+  in the node segment, everything else as for atom ids.  Returns dict(blob, B, N, K, num_edgetype, eigs, F[, label])
+  with F = 0 for atom ids."""
   eigs = 'D' in sp
+  F = int(sp['node_feat'].shape[1]) if sp['node_feat'].ndim == 2 else 0
   if label and 'label' not in sp:
     raise ValueError('pack_sparse: label=True needs records with labels (samples with a label)')
   B, K = sp['D'].shape if eigs else (len(sp['sizes']), int(sp['K']))
   lab = np.ascontiguousarray(sp['label'], np.float32).reshape(B, -1) if label else None
-  h = packed_layout(B, K, len(sp['node_feat']), len(sp['edges']), eigs, lab.shape[1] if label else 0)
+  h = packed_layout(B, K, len(sp['node_feat']), len(sp['edges']), eigs, lab.shape[1] if label else 0, F)
   segs = [(h.sizes, sp['sizes']), (h.node_ptr, sp['node_ptr']), (h.edge_ptr, sp['edge_ptr']),
           (h.node_feat, sp['node_feat']), (h.edges, sp['edges'])]
   if eigs:
@@ -468,7 +480,7 @@ def pack_sparse(sp, label=False):
     raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
     blob[off:off + raw.size] = raw
   out = {'blob': blob, 'B': int(B), 'N': int(sp['N']), 'K': int(K), 'num_edgetype': int(sp['num_edgetype']),
-         'eigs': eigs}
+         'eigs': eigs, 'F': F}
   if 'label' in sp:
     out['label'] = sp['label']
   return out
@@ -488,7 +500,10 @@ class PackedMolecules(object):
   of 4 (K + 1), and the device computes the eigenpairs where a model reads them.
 
   ``labels=True`` writes each batch's labels into the blob, as ``pack_sparse(..., label=True)`` does: the
-  batches train.GraphedStep(..., packed=True) trains from."""
+  batches train.GraphedStep(..., packed=True) trains from.
+
+  Samples with float feature rows (GraphData records, ``node_feat`` [n, F]) give blobs of feature rows, those
+  of ``pack_sparse`` for such records (header slot F = the feature width)."""
 
   def __init__(self, samples, num_eigs, eigs=True, labels=False):
     sp = sparse_collate(samples, num_eigs, eigs=eigs)
@@ -502,6 +517,7 @@ class PackedMolecules(object):
     self.node_feat, self.edges, self.V_rows, self.D = sp['node_feat'], sp['edges'], sp.get('V_rows'), sp.get('D')
     self.k_eff = ritz_extents(self.V_rows, self.node_ptr) if eigs else None
     self.label = sp.get('label')
+    self.F = int(self.node_feat.shape[1]) if self.node_feat.ndim == 2 else 0
 
   def __len__(self):
     return len(self.sizes)
@@ -520,7 +536,7 @@ class PackedMolecules(object):
     buffer): an index list may repeat the largest molecule B times."""
     P = self.label.shape[1] if self.labels else 0
     return packed_layout(B, self.K, B * int(self.sizes.max()), B * int(np.diff(self.edge_ptr).max()), self.eigs,
-                         P).total
+                         P, self.F).total
 
   def batch(self, idx, out=None):
     """Packed batch of the molecules ``idx`` (order kept).  ``out``: optional uint8 buffer (e.g. the numpy
@@ -537,7 +553,9 @@ class PackedMolecules(object):
     rows = self._ranges(self.node_ptr[idx], n_len)
     erow = self._ranges(self.edge_ptr[idx], e_len)
     P = self.label.shape[1] if self.labels else 0
-    h = packed_layout(B, K, len(rows), len(erow), self.eigs, P)
+    F = self.F
+    node_bytes = 4 * len(rows) * (F if F else 1)
+    h = packed_layout(B, K, len(rows), len(erow), self.eigs, P, F)
     if out is None:
       blob = np.zeros(h.total, np.uint8)
     else:
@@ -545,7 +563,7 @@ class PackedMolecules(object):
         raise ValueError('PackedMolecules.batch: out must be a flat uint8 buffer of >= %d bytes' % h.total)
       blob = out[:h.total]
       blob[:h.node_feat] = 0                         # header + fixed segments (alignment gaps stay zero)
-      body = [(off, n) for off, n in ((h.node_feat, 4 * len(rows)), (h.V_rows, 4 * len(rows) * K),
+      body = [(off, n) for off, n in ((h.node_feat, node_bytes), (h.V_rows, 4 * len(rows) * K),
                                       (h.edges, 4 * len(erow)), (h.label, 4 * B * P)) if off]
       for (off, n), end in zip(body, [off for off, _ in body[1:]] + [h.total]):
         blob[off + n:end] = 0                        # the alignment gap behind each segment
@@ -567,12 +585,16 @@ class PackedMolecules(object):
     put(h.sizes, sizes)
     put(h.node_ptr, node_ptr)
     put(h.edge_ptr, edge_ptr)
-    np.take(self.node_feat, rows, out=blob[h.node_feat:h.node_feat + 4 * len(rows)].view(np.int32))
+    if F:
+      np.take(self.node_feat, rows, axis=0,
+              out=blob[h.node_feat:h.node_feat + node_bytes].view(np.float32).reshape(len(rows), F))
+    else:
+      np.take(self.node_feat, rows, out=blob[h.node_feat:h.node_feat + node_bytes].view(np.int32))
     np.take(self.edges, erow, axis=0, out=blob[h.edges:h.edges + 4 * len(erow)].reshape(len(erow), 4))
     if self.labels:
       np.take(self.label, idx, axis=0, out=blob[h.label:h.label + 4 * B * P].view(np.float32).reshape(B, P))
     res = {'blob': blob, 'B': int(B), 'N': int(sizes.max()) if B else 0, 'K': K, 'num_edgetype': self.num_edgetype,
-           'eigs': self.eigs}
+           'eigs': self.eigs, 'F': F}
     if self.label is not None:
       res['label'] = self.label[idx]
     return res

@@ -93,6 +93,10 @@ def init_cell(cell):
 class SpectralNetBase(nn.Module):
   """Common constructor pieces; subclasses define the embedding and the long-scale operator."""
 
+  # True: the records' node_feat holds float feature rows [rows, input_dim] (SparseLanczosNetGeneral), so a
+  # packed batch must carry rows of that width (header slot F = input_dim); False: int32 atom ids (F = 0)
+  _feature_records = False
+
   def _setup_fields(self, config, num_edgetype):
     """The config fields every drop-in keeps; ``num_atom`` where the dataset has atom types."""
     m = config.model
@@ -309,16 +313,51 @@ class SpectralNetBase(nn.Module):
 
   PACKED_KEYS = ('blob', 'B', 'N', 'K')
 
+  def _packed_width(self):
+    """The width F of the node rows this model reads from a packed batch: input_dim for float feature rows,
+    0 for atom ids."""
+    return int(self.input_dim) if self._feature_records else 0
+
+  @staticmethod
+  def _blob_width(batch):
+    """The node-row width F a packed batch names: batch['F'], else its blob's header slot (a device blob with a
+    small synchronous copy); None when neither can be read."""
+    if 'F' in batch:
+      return int(batch['F'])
+    blob = batch.get('blob')
+    if (not torch.is_tensor(blob) or blob.dtype != torch.uint8 or blob.dim() != 1 or blob.numel() < 64 or
+        (blob.is_cuda and torch.cuda.is_current_stream_capturing())):
+      return None
+    return data_mod.read_packed_header(blob).F
+
+  def _check_packed_width(self, F):
+    """A packed batch's node-row width F against the model's: an atom-id blob given to a feature model raises
+    NotImplementedError, a feature blob given to an atom-id model or one of another width ValueError."""
+    want = self._packed_width()
+    if F == want:
+      return
+    if want and not F:
+      raise NotImplementedError('%s takes packed batches of float feature rows (F = %d), not packed batches of '
+                                'atom ids' % (type(self).__name__, want))
+    if not want:
+      raise ValueError('forward_sparse: %s reads atom ids; the packed batch holds float feature rows (F = %d)'
+                       % (type(self).__name__, F))
+    raise ValueError('forward_sparse: the packed batch holds feature rows of width F = %d; %s reads input_dim = %d'
+                     % (F, type(self).__name__, want))
+
   def _check_packed_batch(self, batch):
     """forward_sparse's checks of a packed batch (data.pack_sparse / data.PackedMolecules.batch), before any
     device work: the keys, a flat uint8 blob, N and E+1 within the prepare kernel's limits, and the blob's
-    header -- magic, B and K against the batch's, the total size, node_ptr[B] <= B * N -- which also says
-    whether the blob carries eigenpairs.  A host blob is read in place.  A device blob is read with two
-    small synchronous copies unless the batch says ``eigs`` (pack_sparse and PackedMolecules.batch do):
-    then nothing is read on the host, ``eigs`` is trusted -- LanczosNet runs an eigenpair blob through
-    lnb_graph_prepare_sparse_packed, which reads the Ritz rows, so it must be right -- and the header is
+    header -- magic, B and K against the batch's, the total size, node_ptr[B] <= B * N, the node-row width F
+    against the model's -- which also says whether the blob carries eigenpairs.  A host blob is read in place.
+    A device blob is read with two small synchronous copies unless the batch says both ``eigs`` and ``F``
+    (pack_sparse and PackedMolecules.batch do; for an atom-id model a missing ``F`` means 0): then nothing is
+    read on the host, both are trusted -- LanczosNet runs an eigenpair blob through
+    lnb_graph_prepare_sparse_packed, which reads the Ritz rows, so ``eigs`` must be right -- and the header is
     checked by lnb_records_unpack on the device only; a batch that fails there gives the scores of empty
     graphs.  Returns (B, N, K, eigs, header): the data.PackHeader read, None when nothing was read."""
+    if self._feature_records and self._blob_width(batch) == 0:
+      self._check_packed_width(0)                # an atom-id blob is refused first, whatever else it lacks
     missing = [k for k in self.PACKED_KEYS if k not in batch]
     if missing:
       raise ValueError('forward_sparse: the packed batch lacks %s (data.pack_sparse)' % ', '.join(missing))
@@ -331,11 +370,14 @@ class SpectralNetBase(nn.Module):
     if B < 1 or K < 1:
       raise ValueError('forward_sparse: packed batch with B=%d, K=%d' % (B, K))
     eigs = batch.get('eigs')
-    if blob.is_cuda and eigs is not None:
+    F = batch.get('F', None if self._feature_records else 0)
+    if F is not None:
+      self._check_packed_width(int(F))
+    if blob.is_cuda and eigs is not None and F is not None:
       return B, N, K, bool(eigs), None
     if blob.is_cuda and torch.cuda.is_current_stream_capturing():
-      raise ValueError("forward_sparse: a device blob under stream capture needs batch['eigs'] (its header "
-                       "cannot be read on the host there)")
+      raise ValueError("forward_sparse: a device blob under stream capture needs batch['eigs'] and batch['F'] (its "
+                       "header cannot be read on the host there)")
 
     hdr = data_mod.read_packed_header(blob)
     if hdr.magic != data_mod.PACK_MAGIC:
@@ -344,6 +386,9 @@ class SpectralNetBase(nn.Module):
     if (hdr.B, hdr.K) != (B, K):
       raise ValueError('forward_sparse: blob header has B=%d, K=%d; the batch says B=%d, K=%d'
                        % (hdr.B, hdr.K, B, K))
+    if 'F' in batch and hdr.F != int(batch['F']):
+      raise ValueError("forward_sparse: batch['F'] is %d, the blob header says F=%d" % (int(batch['F']), hdr.F))
+    self._check_packed_width(hdr.F)
     if not 64 <= hdr.total <= blob.numel():
       raise ValueError('forward_sparse: blob header total %d bytes outside [64, %d]' % (hdr.total, blob.numel()))
     if not (64 <= hdr.node_ptr and hdr.node_ptr % 16 == 0 and hdr.node_ptr + 4 * (B + 1) <= hdr.total):
@@ -365,12 +410,16 @@ class SpectralNetBase(nn.Module):
     B, N, K, eigs, _ = self._check_packed_batch(batch)
     self._check_runnable(N, self.num_edgetype + 1)
     blob = batch['blob']
-    return (Ragged(blob, packed_capacity(B, N, K, eigs, blob.shape[0])),
+    return (Ragged(blob, self._packed_capacity(B, N, K, eigs, blob.shape[0])),
             lambda b_: self._unpack(b_, B, N, K)[0], ('packed_records', B, N, K))
 
-  def _takes_packed_training(self):
-    """True when ``train.GraphedStep(..., packed=True)`` trains this model: it has a training entry from records
-    and its ``forward_sparse`` takes packed batches."""
+  def _packed_capacity(self, B, N, K, eigs, nbytes, label_dim=0):
+    """data.packed_capacity of this model's packed batches (node rows of its width, its bond types)."""
+    return packed_capacity(B, N, K, eigs, nbytes, label_dim, self._packed_width(), self.num_edgetype)
+
+  def _takes_packed_training(self, batch):
+    """True when ``train.GraphedStep(..., packed=True)`` trains this model from ``batch``: it has a training
+    entry from records and its ``forward_sparse`` takes packed batches."""
     return hasattr(self, '_train_records') and hasattr(self, '_forward_records')
 
   def _check_packed_train(self, batch):
@@ -402,7 +451,7 @@ class SpectralNetBase(nn.Module):
     the bytes past D's offset hold (the bonds lie behind it, with or without eigenpairs); P > 0 adds the labels.
     Returns (SparseRecords, D, V_rows[, label [B, P]], status), D and V_rows None without ``eigs``."""
     cap_edges = (blob.shape[0] - data_mod.packed_offsets(B, K).D) // 4
-    out = ops.records_unpack(blob, B, K, B * N, cap_edges, eigs=eigs, label_dim=P)
+    out = ops.records_unpack(blob, B, K, B * N, cap_edges, eigs=eigs, label_dim=P, feature_dim=self._packed_width())
     return (SparseRecords(*out[:5], N=N, K=K),) + tuple(out[5:])
 
   def _check_runnable(self, N=None, E1=None):
@@ -684,19 +733,15 @@ class RitzRecords(object):
   lnb_graph_eigs_sparse launch in front of the batch construction, inside the same CUDA graph -- no host
   eigh, no eigenvector bytes on the bus).  ``_feature_records`` is the one difference between the users:
   False, ``node_feat`` holds atom ids and the stack gathers the embedding (LanczosNet); True, it holds float
-  feature rows [rows, input_dim] that the prepare kernel pads into X (SparseLanczosNetGeneral)."""
-
-  _feature_records = False
+  feature rows [rows, input_dim] that the prepare kernel pads into X (SparseLanczosNetGeneral).  Packed
+  batches (data.pack_sparse) hold the same node rows: atom ids, or feature rows of width F = input_dim."""
 
   def _sparse_inputs(self, batch):
     feat = self._feature_records
     if 'blob' in batch:
-      if feat:
-        raise NotImplementedError('%s takes data.sparse_collate records, not packed batches'
-                                  % type(self).__name__)
       # a packed batch (data.pack_sparse) crosses PCIe as ONE copy of exactly the bytes present
       B, N, K, eigs, _ = self._check_packed_batch(batch)
-      inputs = (Ragged(batch['blob'], packed_capacity(B, N, K, eigs, batch['blob'].shape[0])),)
+      inputs = (Ragged(batch['blob'], self._packed_capacity(B, N, K, eigs, batch['blob'].shape[0])),)
       if not eigs:
         # without eigenpairs: records_unpack, then the path of records without them
         return (inputs, lambda b_: self._forward_sparse_eigs_impl(N, K, *self._unpack(b_, B, N, K)[0][:5]),
@@ -730,8 +775,10 @@ class RitzRecords(object):
       raise ValueError('forward_sparse: V_rows must be float32 [rows, K] and D float32 [B, K]; got %s %s and %s %s'
                        % (V_rows.dtype, tuple(V_rows.shape), D.dtype, tuple(D.shape)))
 
-  def _takes_packed_training(self):
-    return not self._feature_records            # float feature rows have no packed layout
+  def _takes_packed_training(self, batch):
+    """A feature model trains from blobs of feature rows only: given an atom-id blob (or no packed batch) it is
+    outside GraphedStep(packed=True)'s list, which names it."""
+    return not self._feature_records or bool(self._blob_width(batch))
 
   def _train_packed(self, batch, P):
     """A labelled blob with eigenpairs trains on its D and V_rows; one without gets them from
@@ -744,6 +791,18 @@ class RitzRecords(object):
     """(GraphPrep, node ids or padded features X, mask, V, L or None) of the records."""
     prepare = ops.graph_prepare_sparse_features if self._feature_records else ops.graph_prepare_sparse
     return prepare(sizes, node_ptr, node_feat, edge_ptr, edges, V_rows, N, self.num_edgetype + 1, **kw)
+
+  def _forward_packed_impl(self, B, N, K, blob):
+    """The forward of a device blob with eigenpairs: one lnb_graph_prepare_sparse(_features)_packed launch reads
+    the segments in place, D at its fixed offset, and the tiles come with the blob."""
+    E1 = self.num_edgetype + 1
+    F = self._packed_width()
+    dense = not self._sparse_stack_ok(N, E1, K, F or None)
+    off_D = data_mod.packed_offsets(B, K).D
+    D = blob[off_D:off_D + 4 * B * K].view(torch.float32).reshape(B, K)     # fixed address in the buffer
+    prep, x, mask, V, L = ops.graph_prepare_sparse_packed(
+        blob, B, N, E1, K, binarize=getattr(self, '_binarize_operators', False), want_dense=dense, feature_dim=F)
+    return self._ritz_conv_stack(*self._ritz_inputs(x), L, D, V, mask, prep=prep, dims_hint=(N, E1))
 
   def _ritz_inputs(self, x):
     """(state, node_ids) of _ritz_conv_stack / ritz_stack_train for the prepare kernel's node output."""

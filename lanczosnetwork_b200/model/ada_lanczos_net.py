@@ -172,7 +172,7 @@ class KeyedAdaLanczosNet(AdaLanczosNet):
     return (inputs + (key,), lambda *a: self._forward_records(SparseRecords(*a[:5], N=N), a[5]),
             ('keyed', N))
 
-  def _takes_packed_training(self):
+  def _takes_packed_training(self, batch):
     return False                                   # packed batches are refused (_sparse_inputs)
 
   def _records_inputs(self, recs, key):

@@ -1,11 +1,8 @@
 """Drop-in for the reference ``model.LanczosNet`` (model/lanczos_net.py:13-199): same
 constructor, parameter names and ``forward(node_feat, L, D, V, label=None, mask=None)``;
 the forward runs in hand-written sm_90a CUDA (no CPU path)."""
-import torch
 import torch.nn as nn
 
-from .. import data as data_mod
-from .. import ops
 from ._common import RitzRecords, SpectralNetBase
 
 __all__ = ['LanczosNet']
@@ -38,12 +35,3 @@ class LanczosNet(RitzRecords, SpectralNetBase):
   def _forward_impl(self, node_feat, L, D, V, mask):
     return self._ritz_conv_stack(None, node_feat.long(), L.float().contiguous(),
                                  D.float().contiguous(), V.float().contiguous(), mask)
-
-  def _forward_packed_impl(self, B, N, K, blob):
-    E1 = self.num_edgetype + 1
-    dense = not self._sparse_stack_ok(N, E1, K)
-    off_D = data_mod.packed_offsets(B, K).D
-    D = blob[off_D:off_D + 4 * B * K].view(torch.float32).reshape(B, K)     # fixed address in the buffer
-    prep, node_ids, mask, V, L = ops.graph_prepare_sparse_packed(
-        blob, B, N, E1, K, binarize=getattr(self, '_binarize_operators', False), want_dense=dense)
-    return self._ritz_conv_stack(None, node_ids, L, D, V, mask, prep=prep, dims_hint=(N, E1))

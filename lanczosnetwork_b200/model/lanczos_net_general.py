@@ -50,6 +50,13 @@ class SparseLanczosNetGeneral(RitzRecords, LanczosNetGeneral):
   in front of it.  Layer 0 (input width 10 in the config) is not a fused-stack shape, so the prepare kernel
   also writes the dense operators on the device for it, as ``forward`` reads them; they never cross PCIe.
   Scores from records with eigenpairs equal ``forward`` on ``data.collate`` of the same samples, bit for
-  bit.  Packed batches are not taken."""
+  bit.
+
+  Packed batches of float feature rows (``data.pack_sparse`` of such records, ``data.PackedMolecules`` of
+  GraphData samples; header slot F = input_dim) are taken too, by ``forward_sparse`` and by
+  ``GraphedStep(packed=True)`` with labels in the blob: one copy per step.  A blob with eigenpairs runs
+  lnb_graph_prepare_sparse_features_packed on the blob in place; one without them, and every training step, is
+  split by lnb_records_unpack_features first.  The scores are those of the same records.  A packed batch of atom
+  ids raises NotImplementedError, one of another feature width ValueError."""
 
   _feature_records = True

@@ -357,13 +357,20 @@ def graph_prepare_sparse_features(sizes, node_ptr, node_x, edge_ptr, edges, V_ro
   return prep, X, mask, V, L
 
 
-def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=False, host_tiles=True):
+def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=False, host_tiles=True,
+                                feature_dim=0):
   """graph_prepare_sparse on a packed batch (data.pack_sparse: one contiguous uint8 buffer, see
   lnb_graph_prepare_sparse_packed).  host_tiles: the batch carries the tile table and the Ritz-row
   prefix sums (data.pack_sparse always writes them), so no tile-assignment kernel is launched and the
-  stack kernel reads the table in place.  Returns (GraphPrep, node_ids, mask, V, L or None)."""
+  stack kernel reads the table in place.  Returns (GraphPrep, node_ids, mask, V, L or None).
+
+  ``feature_dim`` = F > 0: a batch of float feature rows (header slot F, lnb_graph_prepare_sparse_features_packed)
+  whose padded features X [B,N,F] come back in place of node_ids; a batch of another F gives B empty graphs."""
   _need_cuda(blob)
   assert blob.dtype == torch.uint8 and blob.is_contiguous()
+  F = int(feature_dim)
+  if not 0 <= F <= PREPARE_MAX_F:
+    raise ValueError('graph_prepare_sparse_packed: feature_dim=%d outside [0, %d]' % (F, PREPARE_MAX_F))
   dev = blob.device
   ell_val = torch.empty((B, E1, N, N), device=dev, dtype=torch.float32)
   ell_idx = torch.empty((B, E1, N, N), device=dev, dtype=torch.uint8)
@@ -378,19 +385,24 @@ def graph_prepare_sparse_packed(blob, B, N, E1, K, binarize=False, want_dense=Fa
     tiles = torch.empty((4 * B + 2,), device=dev, dtype=torch.int32)
   rowmap = torch.empty((B * K,), device=dev, dtype=torch.int32)
   nrows = torch.empty((1,), device=dev, dtype=torch.int32)
-  node_ids = torch.empty((B, N), device=dev, dtype=torch.int64)
   mask = torch.empty((B, N), device=dev, dtype=torch.uint8)
   V = torch.empty((B, N, K), device=dev, dtype=torch.float32)
   L = torch.empty((B, N, N, E1), device=dev, dtype=torch.float32) if want_dense else None
-  _launch('lnb_graph_prepare_sparse_packed', blob, blob, _inv_sqrt_deg_table(dev), int(B), int(N), int(E1), int(K),
-          (1 if binarize else 0) | (PACKED_HOST_TILES if host_tiles else 0), ell_val, ell_idx, ell_max, gext, tiles,
-          rowmap, nrows, node_ids, mask, V, L)
+  flags = (1 if binarize else 0) | (PACKED_HOST_TILES if host_tiles else 0)
+  if F:
+    x = torch.empty((B, N, F), device=dev, dtype=torch.float32)
+    _launch('lnb_graph_prepare_sparse_features_packed', blob, blob, _inv_sqrt_deg_table(dev), int(B), int(N),
+            int(E1), int(K), F, flags, ell_val, ell_idx, ell_max, gext, tiles, rowmap, nrows, x, mask, V, L)
+  else:
+    x = torch.empty((B, N), device=dev, dtype=torch.int64)
+    _launch('lnb_graph_prepare_sparse_packed', blob, blob, _inv_sqrt_deg_table(dev), int(B), int(N), int(E1), int(K),
+            flags, ell_val, ell_idx, ell_max, gext, tiles, rowmap, nrows, x, mask, V, L)
   prep = GraphPrep((ell_val, ell_idx, ell_max, gext, tiles))
   prep.rowmap, prep.nrows = rowmap, nrows
-  return prep, node_ids, mask, V, L
+  return prep, x, mask, V, L
 
 
-def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False, label_dim=0):
+def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False, label_dim=0, feature_dim=0):
   """A packed batch (data.pack_sparse / data.PackedMolecules: a 16-byte aligned uint8 CUDA buffer) split
   into the records of data.sparse_collate by lnb_records_unpack, one launch whose segment offsets come from
   the header on the device.  cap_rows / cap_edges: rows of node_feat / edges (at least node_ptr[B] /
@@ -401,30 +413,40 @@ def records_unpack(blob, B, K, cap_rows, cap_edges, eigs=False, label_dim=0):
 
   ``label_dim`` = P > 0: also unpack the batch's labels (data.pack_sparse(..., label=True)) through
   lnb_records_unpack_labels, in the same launch; a batch without them, or with another P, sets status bit 64.
-  Returns (sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, label [B, P] float32, status)."""
+  Returns (sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, label [B, P] float32, status).
+
+  ``feature_dim`` = F > 0: a batch of float feature rows (header slot F), through lnb_records_unpack_features;
+  node_feat is then float32 [cap_rows, F], and labels come as above.  A header whose F differs from the
+  caller's (F = 0 for atom ids) sets status bit 128, with every graph empty."""
   _need_cuda(blob)
   if blob.dtype != torch.uint8 or blob.dim() != 1 or not blob.is_contiguous() or blob.numel() < 64:
     raise ValueError('records_unpack: blob must be a contiguous 1-D uint8 tensor of >= 64 bytes')
   if blob.data_ptr() % 16:
     raise ValueError('records_unpack: blob must be 16-byte aligned')
-  B, K, cap_rows, cap_edges, P = int(B), int(K), int(cap_rows), int(cap_edges), int(label_dim)
-  if B < 1 or K < 1 or cap_rows < 0 or cap_edges < 0 or P < 0:
-    raise ValueError('records_unpack: B=%d, K=%d, cap_rows=%d, cap_edges=%d, label_dim=%d'
-                     % (B, K, cap_rows, cap_edges, P))
+  B, K, cap_rows, cap_edges, P, F = int(B), int(K), int(cap_rows), int(cap_edges), int(label_dim), int(feature_dim)
+  if B < 1 or K < 1 or cap_rows < 0 or cap_edges < 0 or P < 0 or not 0 <= F <= PREPARE_MAX_F:
+    raise ValueError('records_unpack: B=%d, K=%d, cap_rows=%d, cap_edges=%d, label_dim=%d, feature_dim=%d'
+                     % (B, K, cap_rows, cap_edges, P, F))
   dev = blob.device
   i32 = dict(device=dev, dtype=torch.int32)
   sizes, node_ptr, edge_ptr = torch.empty((B,), **i32), torch.empty((B + 1,), **i32), torch.empty((B + 1,), **i32)
-  node_feat = torch.empty((cap_rows,), **i32)
+  node_feat = (torch.empty((cap_rows, F), device=dev, dtype=torch.float32) if F else
+               torch.empty((cap_rows,), **i32))
   edges = torch.empty((cap_edges, 4), device=dev, dtype=torch.uint8)
   D = torch.empty((B, K), device=dev, dtype=torch.float32) if eigs else None
   V_rows = torch.empty((cap_rows, K), device=dev, dtype=torch.float32) if eigs else None
   status = torch.empty((1,), **i32)
+  label = torch.empty((B, P), device=dev, dtype=torch.float32) if P else None
+  if F:
+    _launch('lnb_records_unpack_features', blob, blob, blob.numel(), B, K, F, cap_rows, cap_edges, sizes, node_ptr,
+            node_feat, edge_ptr, edges, D, V_rows, status, P, label)
+    out = (sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows)
+    return out + ((label, status) if P else (status,))
   args = (blob, blob.numel(), B, K, cap_rows, cap_edges, sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows,
           status)
   if not P:
     _launch('lnb_records_unpack', blob, *args)
     return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, status
-  label = torch.empty((B, P), device=dev, dtype=torch.float32)
   _launch('lnb_records_unpack_labels', blob, *args, P, label)
   return sizes, node_ptr, node_feat, edge_ptr, edges, D, V_rows, label, status
 

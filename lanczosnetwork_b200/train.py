@@ -1078,9 +1078,11 @@ class GraphedStep:
     split on the device (lnb_records_unpack_labels) and the model's training entry from records runs on it,
     with ``model.loss_func`` on the unpacked labels.  One capture serves every batch with the same (B, N, K,
     P, eigs).  Keys (``sample_key``, ``dropout_key``) travel beside the blob, as in ``sparse=True``.  For GCN,
-    GCNFP, DCNN, ChebyNet, TrainableGAT, KeyedGAT, GGNN, MPNN, GPNN, SampledGraphSAGE and LanczosNet (blobs
-    with or without eigenpairs).  Every call checks the header on the host before copying (a pinned blob in
-    place, a device blob with a small synchronous copy) and raises ValueError, leaving parameters and optimizer
+    GCNFP, DCNN, ChebyNet, TrainableGAT, KeyedGAT, GGNN, MPNN, GPNN, SampledGraphSAGE and LanczosNet (blobs of
+    atom ids, with or without eigenpairs) and SparseLanczosNetGeneral (blobs of float feature rows,
+    data.PackedMolecules of GraphData samples: lnb_records_unpack_features splits them).  Every call checks the
+    header on the host before copying (a pinned blob in place, a device blob with a small synchronous copy) and
+    raises ValueError, leaving parameters and optimizer
     state untouched, rather than step on a batch the device would refuse.  ``step.status`` is the unpack's
     status (device int32 [1], 0 = copied).  ``step.input_consumed`` is a new CUDA event per call, recorded
     after that call's copy: a loader refills the host buffer it passed only once that event has completed
@@ -1090,9 +1092,10 @@ class GraphedStep:
       if sparse:
         raise ValueError('GraphedStep: sparse=True and packed=True exclude each other')
       takes = getattr(model, '_takes_packed_training', None)
-      if takes is None or not takes():
+      if takes is None or not takes(args[0] if len(args) == 1 and isinstance(args[0], dict) else {}):
         raise TypeError('GraphedStep(packed=True) trains GCN, GCNFP, DCNN, ChebyNet, TrainableGAT, KeyedGAT, GGNN, '
-                        'MPNN, GPNN, SampledGraphSAGE and LanczosNet from packed batches; %s is not among them'
+                        'MPNN, GPNN, SampledGraphSAGE and LanczosNet from packed batches of atom ids, and '
+                        'SparseLanczosNetGeneral from packed batches of float feature rows; %s is not among them'
                         % type(model).__name__)
       self._check_packed_args(args, kwargs)
       checked = model._check_packed_train(args[0])
@@ -1220,12 +1223,11 @@ class GraphedStep:
       raise ValueError('GraphedStep(packed=True): the labels travel in the blob; got %s=' % ', '.join(sorted(kwargs)))
 
   def _static_packed(self, batch, dev, hdr, N, eigs):
-    from .data import packed_capacity
     self._packed_shape = (hdr.B, N, hdr.K, eigs, hdr.P)
-    blob = torch.zeros(packed_capacity(hdr.B, N, hdr.K, eigs, hdr.total, label_dim=hdr.P), dtype=torch.uint8,
-                       device=dev)
+    blob = torch.zeros(self.model._packed_capacity(hdr.B, N, hdr.K, eigs, hdr.total, label_dim=hdr.P),
+                       dtype=torch.uint8, device=dev)
     blob[:hdr.total].copy_(batch['blob'][:hdr.total])
-    out = {'blob': blob, 'B': hdr.B, 'N': N, 'K': hdr.K, 'eigs': eigs}
+    out = {'blob': blob, 'B': hdr.B, 'N': N, 'K': hdr.K, 'eigs': eigs, 'F': hdr.F}
     for k in self._PACKED_KEYS:
       if k in batch:
         out[k] = self._static(batch[k], dev)
