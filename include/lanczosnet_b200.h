@@ -81,6 +81,25 @@ int lnb_unsorted_segment_sum_backward(lnb_stream_t stream, const float* grad_out
                                       const int64_t* segment_ids, const int* data_shape,
                                       int num_segments, float* grad_data);
 
+/* The forward's sum made exact and order-independent: the same arguments and semantics (output
+ * accumulated into, batch stride num_segments*dim2, ids outside [0, num_segments) skipped, empty data:
+ * nothing launched), but the result's bits do not depend on row order, grid size or scheduling, so
+ * repeated runs are bit-identical.  lnb_unsorted_segment_sum_forward adds with fp32 atomics instead.
+ * Workspace, one word of each per output element [B, num_segments, dim2], zeroed by the caller:
+ * acc int64, exp int32, flags int32.  Three launches, integer atomics only.  For each output element
+ * with terms x_i (out_in: its value on entry):
+ *   1. e_max = the largest ilogb|x_i| over the finite nonzero terms; flags record NaN, +Inf, -Inf;
+ *   2. k = 61 - H - e_max, H = the bit length of dim1;  acc = sum of rint(x_i * 2^k) (ties to even),
+ *      each product exact in double and the sum exact in int64 (|acc| < 2^62);
+ *   3. out = out_in + s, with s = NaN if a NaN or both infinities occurred, else +-Inf if one sign of
+ *      infinity occurred, else 0 if there was no finite nonzero term, else
+ *      ldexpf(__ll2float_rn(acc), -k): acc rounded to float, then scaled by 2^-k (correctly rounded).
+ * Against the exact sum of c terms, s errs by at most c * 2^(e_max - 62 + H) plus its final rounding:
+ * below half an ulp of the largest term whenever c * 2^H < 2^38. */
+int lnb_unsorted_segment_sum_exact(lnb_stream_t stream, const float* data, const int64_t* segment_ids,
+                                   const int* data_shape, int num_segments, int64_t* acc, int32_t* exp,
+                                   int32_t* flags, float* output);
+
 /* ---------------------------------------------------------------------------------------
  * Generic strided batched fp32 GEMM
  *     C[b,z] = act( alpha * (A[b,z] * kscale[b,z]) @ B[b,z] + beta * D[b,z] + bias )

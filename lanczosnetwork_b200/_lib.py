@@ -59,6 +59,9 @@ SIGNATURES = {
         (c_int, [c_stream, c_f32p, ctypes.c_void_p, ctypes.POINTER(c_int), c_int, c_f32p]),
     'lnb_unsorted_segment_sum_backward':
         (c_int, [c_stream, c_f32p, ctypes.c_void_p, ctypes.POINTER(c_int), c_int, c_f32p]),
+    'lnb_unsorted_segment_sum_exact':
+        (c_int, [c_stream, c_f32p, ctypes.c_void_p, ctypes.POINTER(c_int), c_int, ctypes.c_void_p,
+                 ctypes.c_void_p, ctypes.c_void_p, c_f32p]),
     'lnb_batched_gemm': (c_int, [c_stream, ctypes.POINTER(GemmDesc)]),
     'lnb_split_tf32': (c_int, [c_stream, c_f32p, c_i64, c_f32p, c_f32p]),
     'lnb_linear_tf32x3':

@@ -1577,14 +1577,28 @@ def symmetrize_filters(Y, K, S):
   return G
 
 
-def segment_sum_forward(data, segment_index, num_segments, output=None):
+def segment_sum_forward(data, segment_index, num_segments, output=None, exact=None):
+  """output[b, ids[b, c], :] += data[b, c, :] for data [B, d1, d2] and ids [B, d1] in [0, num_segments)
+  (other ids are skipped); output defaults to zeros [B, num_segments, d2].  ``exact=True`` sums in
+  lnb_unsorted_segment_sum_exact, whose bits do not depend on row order or scheduling; ``exact=False`` in
+  the fp32-atomic lnb_unsorted_segment_sum_forward.  ``exact=None`` follows
+  torch.are_deterministic_algorithms_enabled(), read at each call (so at capture in a CUDA graph)."""
   _need_cuda(data, segment_index, output)
   data = _f32c(data)
   seg = segment_index.contiguous().long()
   B, d1, d2 = data.shape
   if output is None:
     output = torch.zeros((B, num_segments, d2), device=data.device, dtype=torch.float32)
-  _launch('lnb_unsorted_segment_sum_forward', data, data, seg, _ints([B, d1, d2]), int(num_segments), output)
+  if exact is None:
+    exact = torch.are_deterministic_algorithms_enabled()
+  if exact:
+    n = B * int(num_segments) * d2
+    ws = torch.zeros((2, n), device=data.device, dtype=torch.int64)   # acc [n], then exp [n] and flags [n] int32
+    words = ws[1].view(torch.int32)
+    _launch('lnb_unsorted_segment_sum_exact', data, data, seg, _ints([B, d1, d2]), int(num_segments), ws[0],
+            words[:n], words[n:], output)
+  else:
+    _launch('lnb_unsorted_segment_sum_forward', data, data, seg, _ints([B, d1, d2]), int(num_segments), output)
   return output
 
 

@@ -12,8 +12,10 @@ forward and of its adjoint goes through the C ABI:
   * operator products ``L_e X``, ``L_e^T G`` (channel-innermost operators read in place through
     their strides), ``V^T X``, ``V diag(f) U`` and their adjoints: the strided batched GEMM
     (lnb_batched_gemm);
-  * the embedding gradient: the scatter-add of the reference's own ``unsorted_segment_sum`` op
-    (lnb_unsorted_segment_sum_forward).
+  * the embedding gradient, GraphSAGE Max's gradient and the LSTM aggregator's row gather adjoint: the
+    scatter-add of the reference's own ``unsorted_segment_sum`` op (ops.segment_sum_forward): fp32 atomics
+    (lnb_unsorted_segment_sum_forward), or, under ``torch.use_deterministic_algorithms(True)``, the exact
+    order-independent sum (lnb_unsorted_segment_sum_exact), which makes every training step bit-reproducible.
 
 PyTorch supplies what it supplies everywhere in this package -- tensor memory, streams, the autograd
 tape -- plus the pointwise glue of the adjoint (ReLU masks, sigmoid gate, masked mean, the loss).
@@ -1063,7 +1065,10 @@ class GraphedStep:
   ``AdamW`` get ``capturable=True`` here; plain SGD needs nothing).  The warm-up iterations torch needs
   before capture are rolled back (parameters and optimizer state restored in place), so constructing
   the object does not advance training.  Not for AdaLanczosNet (its start vector is drawn on the
-  host each call); KeyedAdaLanczosNet draws it on the device and is captured like the others."""
+  host each call); KeyedAdaLanczosNet draws it on the device and is captured like the others.  The
+  segment sums of the backward read ``torch.are_deterministic_algorithms_enabled()`` when the step is
+  captured: a step captured under ``torch.use_deterministic_algorithms(True)`` replays the exact,
+  order-independent sum whatever the flag is at replay, and one captured without it replays the atomic sum."""
 
   def __init__(self, model, optimizer, args, kwargs=None, warmup=3, sparse=False, edge_capacity=None,
                packed=False):
